@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- pdgstrf3d factorization GFlop/s (FP64) of the B200-native path, with its roofline,
+"""bench.py -- pdgstrf3d factorization GFlop/s (FP64) of the CUDA path, with its roofline,
 end-to-end (host buffers) figure and the reference's CPU path timed beside it.
 
-    python bench.py [--gpus N --steps K --warmup W] [--grid G] [--impl reference]
+    python bench.py [--gpus N --steps K --warmup W] [--grid G] [--impl reference] [--dump-outputs DIR]
 
 One "step" = one numeric factorization (pdgstrf3d) of the 3D 7-point Poisson matrix on a G^3 grid
 (BASELINE.json configs[1] shape; geometric nested dissection as MY_PERMC, NOROWPERM, no
@@ -18,6 +18,8 @@ stat->ops[FACT] (pdgstrf2.c:578,590; trfAux.c:2303; sec_structs.c:692-693).
 N > 1 (torchrun): 1 x 1 x N process grid -- Z-forests + NCCL ancestor reduction; same matrix, so
 "scaling" is "strong".  Every line carries residual_probe = ||(LU - A) x|| / ||A x|| of the factors the
 e2e call returned (N > 1: every rank applies the supernodes it finally owns, partial vectors all-reduced).
+--dump-outputs DIR: after the timed steps, the factors the last timed step left in HBM (rank 0), as a fixed, seeded
+sample of the L and U value arrays: DIR/lval_sample.npy, DIR/uval_sample.npy (float64) and the sampled positions.
 """
 import argparse
 import json
@@ -59,7 +61,7 @@ def parse():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--workload", default=os.environ.get("SLU_BENCH_WORKLOAD", "fem3"), choices=["poisson", "fem3"],
                     help="fem3: audikw_1-shaped 27-pt, 3 dof/node, G^3 nodes (BASELINE configs[2], default G=68: n=943,296, "
-                         "nnz=74.2M); poisson: 7-pt Laplacian G^3 (configs[1] shape; 200^3 does not fit one B200, default G=128)")
+                         "nnz=74.2M); poisson: 7-pt Laplacian G^3 (configs[1] shape; default G=128: 47 GB of L+U, fits one 80 GB H100)")
     ap.add_argument("--grid", type=int, default=int(os.environ.get("SLU_BENCH_GRID", "0")))
     ap.add_argument("--cpu-grid", type=int, default=int(os.environ.get("SLU_BENCH_CPU_GRID", "0")))
     ap.add_argument("--maxsup", type=int, default=256)
@@ -72,8 +74,10 @@ def parse():
     ap.add_argument("--e2e-steps", type=int, default=2)
     ap.add_argument("--schur-variant", type=int, default=int(os.environ.get("SLU_SCHUR_VARIANT", "0")))
     ap.add_argument("--tc-slices", type=int, default=int(os.environ.get("SLU_BENCH_TC_SLICES", "0")),
-                    help="tcgen05 path for wide supernodes: int8 slices per operand (0: library default, -1: off, 5..8)")
-    ap.add_argument("--tc-min-ns", type=int, default=0, help="narrowest supernode on the tcgen05 path (0: library default)")
+                    help="int8 tensor-core path for wide supernodes: int8 slices per operand (0: library default, -1: off, 5..8)")
+    ap.add_argument("--tc-min-ns", type=int, default=0, help="narrowest supernode on the int8 tensor-core path (0: library default)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write a fixed, seeded sample of the factors of the last timed step to DIR/*.npy")
     ap.add_argument("--no-lookahead", type=int, default=0)
     ap.add_argument("--no-coop", type=int, default=0)
     ap.add_argument("--overlap-d2h", type=int, default=1, help="e2e through slu_b200_factor_host (download overlapped)")
@@ -81,7 +85,7 @@ def parse():
                     help="opt-in: level-by-level arena, factor_host also overlaps the upload (options.reserved[3])")
     ap.add_argument("--ref-mode", default=os.environ.get("SLU_BENCH_REF_MODE", "full"), choices=["sample", "full"],
                     help="--impl reference: full (default) = ONE factorization of the full-size workload (the like-for-like "
-                         "number: 96 s on the 16 host cores of a B200 box, 142 s with its setup); sample = K + W steps on --cpu-grid")
+                         "number); sample = K + W steps on --cpu-grid")
     ap.add_argument("--device-fill", type=int, default=0,
                     help="1: distribute A on the device (slu_b200_fill_csr) instead of uploading host panels, check through "
                          "slu_b200_solve (no host copy of L/U at all: the mode of the largest runs); e2e is not measured")
@@ -203,7 +207,7 @@ def cpu_baseline(args, tmp):
 def main_reference(args):
     """The reference arm: the UNMODIFIED reference pdgstrf3d (CPU path, oracle/_ref) on the box's host cores, same
     metric / unit / config as the b200 arm.  --ref-mode full (default): ONE factorization of the full-size matrix
-    (~2.5 minutes with its symbolic phase on a B200 box; steps_run says 1) -- the like-for-like number: CPU supernodal
+    (minutes with its symbolic phase; steps_run says 1) -- the like-for-like number: CPU supernodal
     LU gets more efficient with size (356 GFlop/s at 68^3 against 147 on the 36^3 sample, profiles/r02_*).
     --ref-mode sample: every step factors the bounded sample (--cpu-grid), K + W steps."""
     rank = int(os.environ.get("RANK", "0"))
@@ -244,7 +248,7 @@ def main_reference(args):
 
 # ---------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         self.rows, self.proc, self.index = [], None, index
@@ -281,6 +285,23 @@ class ClockSampler:
         pw = [float(r[2]) for r in self.rows if len(r) > 2 and r[2].replace(".", "").isdigit()]
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": reasons, "power_w_max": max(pw) if pw else None, "samples": len(sm)}
+
+
+DUMP_SAMPLE = 1 << 20      # entries sampled per factor array: values + positions of L and U, 4 x 8 MiB in float64
+
+
+def dump_factors(h, lay, out_dir):
+    """What the timed path computed: the L and U values the last timed factorization left in HBM, downloaded into the
+    host layer and sampled at fixed positions (seed 0), so that two builds can be compared entry by entry."""
+    h.download()
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.default_rng(0)
+    for name in ("lval", "uval"):
+        vals = np.asarray(getattr(lay, name))
+        n = min(DUMP_SAMPLE, vals.size)
+        pos = np.sort(rng.choice(vals.size, size=n, replace=False)) if n < vals.size else np.arange(vals.size)
+        np.save(os.path.join(out_dir, f"{name}_sample.npy"), np.ascontiguousarray(vals[pos], dtype=np.float64))
+        np.save(os.path.join(out_dir, f"{name}_positions.npy"), pos.astype(np.float64))
 
 
 def per_update_roofline_ms(prob, peak_tflops, hbm_gbs):
@@ -417,6 +438,8 @@ def main():
     sampler.start()
     step_s = [allmax(one_step()) for _ in range(args.steps)]
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_factors(h, lay, args.dump_outputs)
     st = h.stats()
     total_ops = allsum(st.ops_fact)
     t_step = float(np.mean(step_s))
@@ -565,7 +588,7 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        hbm_peak = peaks.get("hbm_gbs", 6650.0)
+        hbm_peak = peaks.get("hbm_gbs", 3350.0)           # H100 SXM data sheet
         try:
             roof_ms, cshare = per_update_roofline_ms(prob, peak, hbm_peak)
         except Exception as exc:      # an accounting extra must never cost the bench line
@@ -580,11 +603,11 @@ def main():
                 pass
         S_tc = int(sp.reserved[3])
         tc_share = allsum(sp.reserved[1]) / max(ops_schur, 1.0)
-        bf16_peak = peaks.get("bf16_tflops_sustained") or peaks.get("bf16_tflops") or 1590.0
+        bf16_peak = peaks.get("bf16_tflops_sustained") or peaks.get("bf16_tflops") or 989.0   # H100 SXM data sheet, dense
         tc_extra = None
         if S_tc > 0:
-            # executed int8 work of the tcgen05 kernel: S(S+1)/2 int8 products per FP64 product; the int8 pipe runs at twice
-            # the bf16 rate (B200_PROFILING.md: 4.5 vs 2.25 PFLOP/s nominal), so its measured peak = 2 x MEASURED_PEAKS bf16
+            # executed int8 work of the int8 tensor-core kernel: S(S+1)/2 int8 products per FP64 product; the int8 pipe runs
+            # at twice the bf16 rate (H100 SXM data sheet: 1979 vs 989 TOPS dense), so its peak = 2 x the bf16 peak
             prod = S_tc * (S_tc + 1) // 2
             tc_extra = {"slices": S_tc, "schur_flop_share": round(tc_share, 4), "int8_products_per_fp64_product": prod,
                         "int8_tops_executed": round(ach * tc_share * prod, 1),
@@ -593,7 +616,7 @@ def main():
                         "slice_workspace_bytes_rank0": int(sp.reserved[2]),
                         "note": "frac above is FP64-equivalent TF/s over the cuBLAS FP64 GEMM rate: > 1 means faster than the FP64 pipe"}
         roof = {"bound": "tensor",
-                "kernel": ("schur_kernel_tc (tcgen05.mma.kind::i8 on int8 slices, TMEM accumulators, bulk-copy staged tiles, fused scatter) + "
+                "kernel": ("schur_kernel_tc (wgmma s8 on int8 slices, register accumulators, bulk-copy staged tiles, fused scatter) + "
                            "schur_kernel (DMMA) for supernodes < 128 columns") if S_tc > 0 else "schur_kernel (DMMA m8n8k4 GEMM + fused scatter)",
                 "achieved": round(ach, 3), "peak": round(peak, 3), "unit": "TFLOP/s", "frac": round(ach / peak, 4),
                 "peak_source": "cuBLAS FP64 GEMM 8192x8192x256 measured live on this GPU (FP64 pipe; MEASURED_PEAKS.json has bf16/HBM only)",
@@ -628,8 +651,8 @@ def main():
             "config": bench_config(args),
             "problem": {"n": prob.n, "nsupers": prob.nsupers, "grid": f"1x1x{world}", "factor_flops": total_ops,
                         "lu_bytes_rank0": h2d, "amalg": args.amalg, "host_setup_s": round(t_setup, 1),
-                        "note": "BASELINE configs[1] (Poisson 200^3, ~280 GB of L+U) does not fit one 180 GB B200; it runs "
-                                "on 1x1x8 (profiles/r02_*); scaled single-GPU instances: --workload poisson --grid 128|160"},
+                        "note": "BASELINE configs[1] (Poisson 200^3, ~280 GB of L+U) does not fit one 80 GB H100; "
+                                "scaled single-GPU instance: --workload poisson --grid 128"},
             "clocks": clocks, "e2e": e2e, "e2e_handle": e2e_handle, "e2e_csr_to_solution": e2e_csr, "gpu_launches": int(st.gpu_launches), "nlevels": int(st.nlevels),
             "residual_probe": resid if resid is not None else (solve_check or {}).get("residual_Ax_b_over_b"),
             "solve_check": solve_check, "roofline": roof, "cpu_baseline": cb}))

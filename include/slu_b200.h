@@ -1,5 +1,5 @@
 /*
- * slu_b200.h -- C-ABI of libslu_b200.so: a B200-native (sm_100a) implementation of
+ * slu_b200.h -- C-ABI of libslu_b200.so: an H100-native (sm_90a) implementation of
  * SuperLU_DIST's 3D supernodal numeric factorization hot path `pdgstrf3d`.
  *
  * Boundary.  The reference reaches a non-C factorization backend through an opaque handle
@@ -209,8 +209,8 @@ int slu_b200_k_rerun_schur(slu_b200_handle_t h, int level, int reps, float *ms);
  * only to keep one struct; n, nsupr, lda ... count complex elements.  Supernodes up to 256 columns.
  * stats.ops_fact follows the reference's own complex accounting (pzgstrf2.c:578,590 for the diagonal blocks,
  * the precision-independent 2*m*n*k for the Schur update, sec_structs.c:692-693).
- * Validated on a B200 (GPUTEST_r01.json: kernels vs NumPy, cg20 vs the reference's pzgstrf3d factors, pzdrive3d
- * drop-in); gating tests in tests/test_gpu_variants_complex.py. */
+ * Checked on an H100 by tests/test_gpu_variants_complex.py: kernels vs NumPy, cg20 vs the reference's pzgstrf3d
+ * factors, pzdrive3d drop-in. */
 typedef struct slu_b200_zhandle_s *slu_b200_zhandle_t;
 int slu_b200_z_create(slu_b200_zhandle_t *h, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt);
 int slu_b200_z_upload(slu_b200_zhandle_t h);

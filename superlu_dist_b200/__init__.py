@@ -1,4 +1,4 @@
-"""superlu_dist_b200 -- a B200-native (sm_100a) `pdgstrf3d` for SuperLU_DIST.
+"""superlu_dist_b200 -- an H100-native (sm_90a) `pdgstrf3d` for SuperLU_DIST.
 
 The product is the C-ABI shared library ``lib/libslu_b200.so`` (hand-written CUDA kernels + host
 orchestration, ``include/slu_b200.h``).  This Python package is only the thin host-side mirror

@@ -1,4 +1,4 @@
-// slu_api.cu -- C-ABI (include/slu_b200.h) and host orchestration of the B200 pdgstrf3d.
+// slu_api.cu -- C-ABI (include/slu_b200.h) and host orchestration of the CUDA pdgstrf3d.
 //
 // The level loop mirrors pdgstrf3d (SRC/double/pdgstrf3d.c:333-385): for every Z-tree level this
 // rank takes part in, factor its elimination sub-forest, combining the replicated ancestor copies
@@ -195,7 +195,7 @@ struct LevelPlan {
     int64_t slab_begin = 0, slab_end = 0;  // val range of this level's panels (contiguous in cooperative forests)
     int big_count = 0, small_count = 0;
     int64_t big_nodes = 0, big_prefix = 0, big_ctas = 0, small_nodes = 0, small_prefix = 0, small_ctas = 0;
-    // tcgen05 path: the wide supernodes of the level (slu_ozaki.cu)
+    // int8 tensor-core path: the wide supernodes of the level (slu_ozaki.cu)
     int tc_count = 0;
     int64_t tc_nodes = 0, tc_prefix = 0, tc_ctas = 0, tc_urg_prefix = 0, tc_urg_ctas = 0, tc_bulk_prefix = 0, tc_bulk_ctas = 0;
     int64_t tc_p_rt = 0, tc_n_rt = 0, tc_p_ak = 0, tc_n_ak = 0, tc_p_b = 0, tc_n_b = 0;
@@ -224,11 +224,11 @@ struct slu_b200_handle_s {
     DevBuf<UBlk> d_ublk;
     DevBuf<RowInfo> d_rowinfo;
     DevBuf<ColInfo> d_colinfo;
-    DevBuf<int8_t> d_oz_i8;               // tcgen05 path: int8 slice workspace (two level parities)
+    DevBuf<int8_t> d_oz_i8;               // int8 tensor-core path: int8 slice workspace (two level parities)
     DevBuf<double> d_oz_scale;
     DevBuf<int> d_oz_rexp;
-    int tc_slices = 0, tc_min_ns = 0;     // 0 slices: tcgen05 path off
-    bool tc_force_off = false, tc_alloc_failed = false;   // slice workspace did not fit: analysed again without the tcgen05 path
+    int tc_slices = 0, tc_min_ns = 0;     // 0 slices: int8 tensor-core path off
+    bool tc_force_off = false, tc_alloc_failed = false;   // slice workspace did not fit: analysed again without the int8 tensor-core path
     int tc_nonatomic = 0;                 // plain load/store scatter for destinations only one supernode of a level updates
     DevBuf<double> d_x, d_x2;             // triangular solve: right-hand sides / solution
     std::vector<int64_t> z_nodes_off;     // [zl] offset into d_pool_i32 of the forest's node list (solve masks)
@@ -577,7 +577,7 @@ int analyze(slu_b200_handle_s *H)
     int64_t ws_oz_i8_max = 0, ws_oz_s_max = 0;
     double ops_tc = 0;
 #ifndef SLU_COMPLEX
-    // tcgen05 path (slu_ozaki.cu): options.reserved[4] = int8 slices per operand (0: default, < 0: off),
+    // int8 tensor-core path (slu_ozaki.cu): options.reserved[4] = int8 slices per operand (0: default, < 0: off),
     // options.reserved[5] = narrowest supernode that takes it (0: default)
     H->tc_slices = H->opt.reserved[4] < 0 ? 0 : (H->opt.reserved[4] == 0 ? (OZ_DEFAULT_ON ? OZ_DEFAULT_SLICES : 0) : std::min(8, std::max(5, (int)H->opt.reserved[4])));
     H->tc_min_ns = H->opt.reserved[5] > 0 ? H->opt.reserved[5] : OZ_DEFAULT_MIN_NS;
@@ -595,7 +595,7 @@ int analyze(slu_b200_handle_s *H)
         for (auto &nodes : by) {
             if (nodes.empty()) continue;
             LevelPlan L;
-            L.zlvl = zl; L.count = (int)nodes.size(); L.atomic = 1;  // RED.ADD.F64 beats a load/store read-modify-write here (profiles/r01_notes.md)
+            L.zlvl = zl; L.count = (int)nodes.size(); L.atomic = 1;  // RED.ADD.F64 beats a load/store read-modify-write here
             L.nodes_off = (int64_t)pool_i32.size();
             pool_i32.insert(pool_i32.end(), nodes.begin(), nodes.end());
             // which destination panels are updated by MORE than one supernode of this level?  Only those need atomic
@@ -759,7 +759,7 @@ int analyze(slu_b200_handle_s *H)
         (H->d_oz_i8.alloc((size_t)ws_oz_i8_max * 2) || H->d_oz_scale.alloc((size_t)ws_oz_s_max * 2) || H->d_oz_rexp.alloc((size_t)ws_oz_s_max * 2))) {
         H->tc_alloc_failed = true;
         H->d_oz_i8.release(); H->d_oz_scale.release(); H->d_oz_rexp.release();
-        return fail("tcgen05 path: cannot allocate %.1f GB of int8 slice workspace (options.reserved[4] = -1 turns the path off): %s",
+        return fail("int8 tensor-core path: cannot allocate %.1f GB of int8 slice workspace (options.reserved[4] = -1 turns the path off): %s",
                     2e-9 * ws_oz_i8_max, g_err.c_str());
     }
     lap("device alloc + index upload");
@@ -778,7 +778,7 @@ int analyze(slu_b200_handle_s *H)
     st.ops_fact = ops; st.ops_schur = ops_schur; st.schur_bytes = bytes_schur;
     st.nnz_l = nnz_l; st.nnz_u = nnz_u; st.nlevels = (int)H->levels.size();
     st.lu_device_bytes = (int64_t)H->val.bytes();
-    st.reserved[1] = ops_tc;                                   // Schur flops taken by the tcgen05 path
+    st.reserved[1] = ops_tc;                                   // Schur flops taken by the int8 tensor-core path
     st.reserved[2] = (double)(H->d_oz_i8.bytes() + H->d_oz_scale.bytes() + H->d_oz_rexp.bytes());
     st.reserved[3] = (double)H->tc_slices;
     st.index_device_bytes = (int64_t)(H->d_nodes.bytes() + H->d_xsup.bytes() + H->d_supno.bytes() + H->d_lrows.bytes() * 3 +
@@ -1367,7 +1367,7 @@ int slu_b200_create(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, const 
     }
     if (gather_structure(H)) { slu_b200_destroy(H); return -1; }
     if (analyze(H)) {
-        // the int8 slice workspace of the tcgen05 path did not fit beside the L/U arena: plan again without it (FP64 DMMA only)
+        // the int8 slice workspace of the int8 tensor-core path did not fit beside the L/U arena: plan again without it (FP64 DMMA only)
         if (!H->tc_alloc_failed) { slu_b200_destroy(H); return -1; }
         cudaGetLastError();
         H->tc_force_off = true;
@@ -1489,7 +1489,7 @@ static int factor_impl(slu_b200_handle_t H, int *info, bool pipelined, bool up_p
             const int32_t *bign = H->d_pool_i32.p + L.big_nodes;
             if (lookahead || pipelined) CU(cudaEventRecord(H->ev_panel[li], s));
             if (pipelined && pipe_download_level(H, li)) return -1;
-            // non-atomic scatter of exclusive destinations (tcgen05 path): this level's updates must not overlap the bulk
+            // non-atomic scatter of exclusive destinations (int8 tensor-core path): this level's updates must not overlap the bulk
             // update of the level before (it targets the same ancestors); the panel work above still did
             const int tc_na = (H->tc_nonatomic && !up_pipe) ? 1 : 0;
             if (tc_na && lookahead && li >= first + 1 && (L.tc_count > 0 || H->levels[li - 1].tc_count > 0))
@@ -1945,7 +1945,7 @@ int slu_b200_k_gemm_sub(int m, int n, int k, const double *a, int lda, const dou
         if (variant_ >= 100) return launch_gemm_sub_ozaki(m_, n_, k_, a_, lda_, b_, ldb_, c_, ldc_, variant_, s_);
         return SLU_NS::launch_gemm_sub(m_, n_, k_, a_, lda_, b_, ldb_, c_, ldc_, variant_, s_);
     };
-    if (variant >= 100 && k > 512) return fail("the tcgen05 path handles k <= 512 (MAX_SUPER_SIZE)");
+    if (variant >= 100 && k > 512) return fail("the int8 tensor-core path handles k <= 512 (MAX_SUPER_SIZE)");
 #endif
     launch_gemm_sub(m, n, k, da.p, lda, db.p, ldb, dc.p, ldc, variant, 0);
     CU(cudaDeviceSynchronize());

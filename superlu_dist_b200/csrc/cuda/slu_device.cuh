@@ -1,4 +1,4 @@
-// slu_device.cuh -- data structures shared by the host orchestration (slu_api.cu) and the sm_100a
+// slu_device.cuh -- data structures shared by the host orchestration (slu_api.cu) and the sm_90a
 // kernels (slu_kernels.cu) of libslu_b200.so.
 //
 // HBM layout (DESIGN.md section 3).  One value arena `val` (double) holds, per Z-tree level of the
@@ -48,7 +48,7 @@ struct NodeDesc {            // one per supernode (indexed by global supernode i
     int64_t ws_inv;          // offset into the per-level workspace of inverted 16x16 diagonal blocks
     int32_t urg_rows, urg_cols;  // look-ahead: leading rows / packed columns whose destination is factored at
                                  // the NEXT level (the parent supernode); tiles touching them are "urgent"
-    // tcgen05 path (slu_ozaki.cu): per-level workspace of this supernode's int8 slices and scales
+    // int8 tensor-core path (slu_ozaki.cu): per-level workspace of this supernode's int8 slices and scales
     int64_t ws_oza, ws_ozb;      // byte offsets into oz_i8: A tiles [rt][ks][s][4096], B tiles [ct][ks][s][OZ_NT*32]
     int64_t ws_ozs;              // element offset into oz_scale / oz_rexp: row scales [0, 128*RT), column scales after
 };
@@ -89,7 +89,7 @@ struct DeviceLU {            // everything the kernels need, passed by value
     RowInfo *rowinfo;
     ColInfo *colinfo;
     int32_t *lrel, *urel;
-    int8_t *oz_i8;           // tcgen05 path: int8 slice tiles of the level's wide supernodes
+    int8_t *oz_i8;           // int8 tensor-core path: int8 slice tiles of the level's wide supernodes
     double *oz_scale;        //   2^(e-6) back-scales of their rows / columns
     int *oz_rexp;            //   row exponents (between the two slicing passes)
     int *info;               // min over zero pivots of (1-based global column); INT_MAX if none
@@ -158,16 +158,16 @@ int launch_solve_mask(const DeviceLU &d, const int32_t *nodes, int count, double
 // device-side distribution of a CSR matrix (device arrays) into the arena; *err counts entries without a slot
 int launch_fill_csr(const DeviceLU &d, int n, const int32_t *rowptr, const int32_t *colind, const double *aval, const int32_t *perm,
                     const int8_t *active, int *err, cudaStream_t s);
-// slu_ozaki.cu: the Schur update of wide supernodes on tcgen05 (int8 slices, exact int32 accumulation in TMEM)
-constexpr int OZ_NT = 32;             // columns of one CTA's tcgen05 Schur tile (rows: 128)
-constexpr int OZ_CL = 1;              // CTAs per cluster sharing the A operand by multicast (2 and 4 measured SLOWER: r02_notes.md)
+// slu_ozaki.cu: the Schur update of wide supernodes on wgmma (int8 slices, exact int32 accumulation in registers)
+constexpr int OZ_NT = 32;             // columns of one CTA's int8 Schur tile (rows: 128)
+constexpr int OZ_CL = 1;              // CTAs per cluster sharing the A operand by multicast
 constexpr int OZ_NT_HOST = OZ_NT * OZ_CL;  // columns of the tile unit the host enumerates
-constexpr int OZ_KSTEP = 32;          // int8 k per MMA instruction and per pipeline stage
+constexpr int OZ_KSTEP = 32;          // int8 k per wgmma instruction and per pipeline stage
 constexpr int OZ_DEFAULT_SLICES = 7;  // 48 bits per operand: error ~1e-15 * k * rowmax * colmax (scripts/ozaki_emulate.py)
 constexpr int OZ_DEFAULT_MIN_NS = 128;
-constexpr bool OZ_PERSIST_DEFAULT = false;     // persistent warp-specialised tcgen05 Schur kernel (SLU_B200_TC_PERSIST=1|0)
+constexpr bool OZ_PERSIST_DEFAULT = false;     // persistent int8 Schur kernel (SLU_B200_TC_PERSIST=1|0)
 constexpr bool OZ_NONATOMIC_DEFAULT = false;   // SLU_B200_TC_NONATOMIC=1|0 overrides
-constexpr bool OZ_DEFAULT_ON = true;  // validated on hardware: profiles/r02_notes.md (options.reserved[4] = -1 / SLU_B200_TC_SLICES=0: off)
+constexpr bool OZ_DEFAULT_ON = true;  // options.reserved[4] = -1 / SLU_B200_TC_SLICES=0: off
 inline int64_t oz_a_bytes(int m, int ns, int S) { return (int64_t)((m + 127) / 128) * ((ns + OZ_KSTEP - 1) / OZ_KSTEP) * S * 4096; }
 inline int64_t oz_b_bytes(int n, int ns, int S) { return (int64_t)((n + OZ_NT - 1) / OZ_NT) * ((ns + OZ_KSTEP - 1) / OZ_KSTEP) * S * OZ_NT * OZ_KSTEP; }
 inline int64_t oz_scale_elems(int m, int n) { return (int64_t)((m + 127) / 128) * 128 + (int64_t)((n + OZ_NT - 1) / OZ_NT) * OZ_NT; }
@@ -179,7 +179,7 @@ int launch_oz_slice(const DeviceLU &d, const int32_t *nodes, int count, const in
 // the caller must then order this level's updates after ALL earlier levels' (no bulk update of level l-1 in flight)
 int launch_oz_schur(const DeviceLU &d, const Batch &b, int64_t ctas, int mode, int split_n, int split_i, int S, int nonatomic,
                     cudaStream_t s);
-// slu_ozaki.cu: C -= A*B through int8 slices on tcgen05 (variants 120..142: slices and tile width)
+// slu_ozaki.cu: C -= A*B through int8 slices on wgmma (variants 110..149: slices, stages, cluster)
 int launch_gemm_sub_ozaki(int m, int n, int k, const double *a, int lda, const double *b, int ldb, double *c, int ldc,
                           int variant, cudaStream_t s);
 #endif

@@ -1,4 +1,4 @@
-// slu_kernels.cu -- the sm_100a kernels of the pdgstrf3d hot path.
+// slu_kernels.cu -- the sm_90a kernels of the pdgstrf3d hot path.
 //
 //   diag_lu_kernel      unpivoted LU of the diagonal block      (Local_Dgstrf2, SRC/double/pdgstrf2.c:508-601)
 //   trsm_kernel<false>  L(below,k) <- L(below,k) U_kk^-1         (dLPanelTrSolve, SRC/double/dtrfCommWrapper.c:120-223)
@@ -11,8 +11,8 @@
 //   u_expand / u_pack   skyline <-> dense-packed U at the boundary (dRgather_U, SRC/double/dgather.c:256-398)
 //   axpy_kernel         ancestor reduction add                  (dzRecvLPanel/UPanel, SRC/double/pd3dcomm.c:224-331)
 //
-// tcgen05.mma has no f64 kind (kinds: tf32/f16/i8/f8f6f4/mx*), so the native FP64 tensor path on
-// sm_100a is the warp-level DMMA fed from shared memory; tiles are staged with cp.async (LDGSTS).
+// wgmma has no f64 kind, so the native FP64 tensor path on
+// sm_90a is the warp-level DMMA fed from shared memory; tiles are staged with cp.async (LDGSTS).
 #include "slu_device.cuh"
 #include "slu_kernels_common.cuh"
 
@@ -132,7 +132,7 @@ __global__ void __launch_bounds__(512) diag_lu_kernel(DeviceLU d, Batch b, int r
 // diagonal block LU, Crout form on the FP64 tensor cores (opt-in: SLU_B200_DIAG_V3=1, supernodes <= 256 columns).
 // The right-looking kernel above streams the whole trailing block through L2 at every 16-column step and factors
 // the 16x16 pivot block through shared memory; on a 252-column block it takes 0.54 ms -- at every level of the
-// elimination tree, replicated on every rank of a cooperative group (profiles/r01_notes.md).  Here step j forms only
+// elimination tree, replicated on every rank of a cooperative group.  Here step j forms only
 //   panel  P = A(j0:, j0:j0+16)     - L(j0:, 0:j0)      U(0:j0, j0:j0+16)      (rem x 16, K = j0)
 //   rows   R = A(j0:j0+16, j0+16:)  - L(j0:j0+16, 0:j0) U(0:j0, j0+16:)        (16 x ncr, K = j0)
 // as DMMA products (16 warps: two 8-row tiles each for P, two 8-column tiles each for R; the operand every warp
@@ -939,7 +939,7 @@ __device__ __forceinline__ void gemm_tile(const double *__restrict__ A, int lda,
     cp_async_wait<0>();
 }
 
-// Same tile product with a strength-reduced loader (profiles/r01_notes.md, "where the Schur kernel's time goes": the
+// Same tile product with a strength-reduced loader ("where the Schur kernel's time goes": the
 // general loader above spends ~300 instructions per k-step on 64-bit address arithmetic and predicates, 30 % of a
 // warp's main-loop time, and a warp alone cannot keep the DMMA pipe busy while its sibling CTA is in its epilogue).
 // Interior tiles (no M/N edge) and full k-steps use running pointers: every warp copies whole 32-row column
@@ -1154,8 +1154,7 @@ int launch_schur(const DeviceLU &d, const Batch &b, int64_t ctas, int big, int a
                  int split_i, int wide, cudaStream_t s)
 {
     if (b.count <= 0 || ctas <= 0) return 0;
-    // default since round 2: the running-pointer loader (gemm_tile_v2).  Measured on the default bench workload
-    // (profiles/r02_notes.md): Schur phase 1385 -> 1134 ms, 0.75 -> 0.92 of the live cuBLAS FP64 GEMM rate.
+    // default: the running-pointer loader (gemm_tile_v2).
     // variant 6 = the round-1 general loader, kept for A/B runs.
     if (variant == 0) variant = 4;
     if (variant == 6) variant = 0;
@@ -1295,7 +1294,7 @@ int launch_axpy(double *dst, const double *src, int64_t n, cudaStream_t s)
 {
     if (n <= 0) return 0;
     int64_t blocks = (n + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     axpy_kernel<<<(unsigned)blocks, 256, 0, s>>>(dst, src, n);
     return 1;
 }
@@ -1309,7 +1308,7 @@ int launch_axpy_atomic(double *dst, const double *src, int64_t n, cudaStream_t s
 {
     if (n <= 0) return 0;
     int64_t blocks = (n + 255) / 256;
-    if (blocks > 148 * 4) blocks = 148 * 4;  // a few CTAs per SM: it shares the GPU with the factorization
+    if (blocks > 132 * 4) blocks = 132 * 4;  // a few CTAs per SM: it shares the GPU with the factorization
     axpy_atomic_kernel<<<(unsigned)blocks, 256, 0, s>>>(dst, src, n);
     return 1;
 }

@@ -1,4 +1,4 @@
-// slu_kernels_z.cu -- the sm_100a kernels of the doublecomplex hot path (pzgstrf3d, SURVEY 8a row a15:
+// slu_kernels_z.cu -- the sm_90a kernels of the doublecomplex hot path (pzgstrf3d, SURVEY 8a row a15:
 // SRC/complex16/pzgstrf3d.c:120, Local_Zgstrf2 pzgstrf2.c:508-601, zscatter_l/zblock_gemm_scatter).
 // Same batched level-synchronous structure and HBM layout as slu_kernels.cu; elements are (re, im) pairs.
 //
@@ -628,7 +628,7 @@ int launch_axpy(zd *dst, const zd *src, int64_t n, cudaStream_t s)
     if (n <= 0) return 0;
     const int64_t nd2 = 2 * n;  // (re, im) pairs add component-wise
     int64_t blocks = (nd2 + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     axpy_kernel<<<(unsigned)blocks, 256, 0, s>>>(reinterpret_cast<double *>(dst), reinterpret_cast<const double *>(src), nd2);
     return 1;
 }
@@ -643,7 +643,7 @@ int launch_axpy_atomic(zd *dst, const zd *src, int64_t n, cudaStream_t s)
     if (n <= 0) return 0;
     const int64_t nd2 = 2 * n;
     int64_t blocks = (nd2 + 255) / 256;
-    if (blocks > 148 * 4) blocks = 148 * 4;
+    if (blocks > 132 * 4) blocks = 132 * 4;
     axpy_atomic_kernel<<<(unsigned)blocks, 256, 0, s>>>(reinterpret_cast<double *>(dst), reinterpret_cast<const double *>(src), nd2);
     return 1;
 }

@@ -1,37 +1,37 @@
-// slu_ozaki.cu -- the Schur-complement GEMM of wide supernodes on the 5th-generation tensor cores (tcgen05).
+// slu_ozaki.cu -- the Schur-complement GEMM of wide supernodes on the int8 tensor cores (Hopper wgmma).
 //
-// tcgen05.mma has no f64 kind, so V = L(below,k) * U(k,:) (dblock_gemm_scatter, SRC/double/dscatter3d.c:82-189) is
-// computed EXACTLY-ROUNDED-EQUIVALENT from int8 slices (Ozaki scheme): every row i of the L operand is scaled by a
-// power of two 2^-e_i so that |a| < 1 and cut into S signed base-128 digits
+// The tensor cores have no FP64 kind fast enough to matter beside int8, so V = L(below,k) * U(k,:) (dblock_gemm_scatter,
+// SRC/double/dscatter3d.c:82-189) is computed EXACTLY-ROUNDED-EQUIVALENT from int8 slices (Ozaki scheme): every row i
+// of the L operand is scaled by a power of two 2^-e_i so that |a| < 1 and cut into S signed base-128 digits
 //        a = 2^e_i * sum_s d_s * 2^(-6-7s),   |d_s| <= 64            (S = 8: 55 bits >= the 53 of a double)
 // and likewise every column j of the U operand (2^f_j, digits t).  Then
 //        (A B)_ij = 2^(e_i+f_j-12) * sum_g 2^(-7g) * sum_{s+t=g} (A_s B_t)_ij
 // where each A_s B_t is an int8 x int8 -> int32 product, exact on the tensor cores (|sum| <= 8*512*2^12 < 2^31).
 // Products with s + t >= S are dropped: the result carries a NORMWISE error like a DGEMM's, at worst
 // k * (S+2) * 2^(4-7S) * max_p|a_ip| * max_p|b_pj| (2.6e-13 for the default S = 7, 2.2e-15 for S = 8), typically one to two
-// orders below (1.3e-15 measured at k = 256, S = 7) -- bounds and cases in tests/test_gpu_ozaki.py.
+// orders below -- bounds and cases in tests/test_gpu_ozaki.py.
 //
-// Mapping onto tcgen05 (one CTA = one 128 x NT tile of V, 128 threads, 2 CTAs per SM so that one CTA's epilogue
-// overlaps the other's MMAs):
+// Mapping onto wgmma (one CTA = one 128 x NT tile of V; two consumer warpgroups, one per 64-row half, and one producer
+// warpgroup that hands its registers to them with setmaxnreg):
 //   * operands are pre-sliced ONCE per supernode by oz_slice_* into int8 tiles that already have the shared-memory
-//     image UMMA wants (K-major "core matrices" of 8 rows x 16 bytes, no swizzle: LBO = 128 B between the two
+//     image wgmma wants (K-major "core matrices" of 8 rows x 16 bytes, no swizzle: LBO = 128 B between the two
 //     16-byte K chunks, SBO = 256 B between 8-row groups), so a pipeline stage (all S slices of a 128-row x 32-k
 //     A tile and of an NT-column x 32-k B tile) is TWO contiguous bulk copies (cp.async.bulk, the TMA engine's 1-D
 //     mode) completing on an mbarrier;
-//   * the S column-slices of B sit one under the other in shared memory, so ONE tcgen05.mma.kind::i8 of A_s against
-//     the first (S-s)*NT rows of that stack yields A_s*B_t for every t <= S-1-s, landing in TMEM columns
-//     [s*NT, S*NT): the accumulator of digit group g = s+t lives at columns [g*NT, (g+1)*NT).  S instructions per
-//     32-k step (N = S*NT ... NT) instead of S(S+1)/2, all with M = 128;
-//   * accumulators: S*NT = 256 of the 512 TMEM columns; the epilogue reads them back with tcgen05.ld (32 lanes x
-//     32 bit: thread = row), recombines the groups in FP64 (Horner in 2^-7), scales by 2^(e_i-6) * 2^(f_j-6) and
-//     subtract-scatters with RED.ADD.F64 exactly like the DMMA kernel -- but with thread = row, so one warp
-//     instruction covers 32 consecutive rows of one destination column (coalesced).
-// One thread issues the bulk copies, one thread issues the MMAs (tcgen05 is single-thread issue); mbarriers carry
-// smem-full / smem-empty / accumulator-ready.  Every wait is bounded (trap after ~1 s) so a protocol bug cannot hang
-// the GPU.
+//   * the S column-slices of B sit one under the other in shared memory, so ONE wgmma m64nNk32 of A_s against the
+//     first (S-s)*NT rows of that stack yields A_s*B_t for every t <= S-1-s, landing in accumulator columns
+//     [s*NT, S*NT): the accumulator of digit group g = s+t holds columns [g*NT, (g+1)*NT).  S instructions per
+//     32-k step (N = S*NT ... NT) instead of S(S+1)/2;
+//   * accumulators: S*NT/2 registers per consumer thread (112 for S = 7); the epilogue recombines the groups in FP64
+//     (Horner in 2^-7), scales by 2^(e_i-6) * 2^(f_j-6) and subtract-scatters with RED.ADD.F64 exactly like the DMMA
+//     kernel.
+// One producer lane issues the bulk copies; the consumers release a stage (mbarrier arrive, one per warpgroup) once
+// wgmma.wait_group shows the MMAs that read it are complete.  Every wait is bounded (trap after ~1 s) so a protocol
+// bug cannot hang the GPU.
 #include "slu_device.cuh"
 #define SLU_COMMON_HELPERS_ONLY
 #include "slu_kernels_common.cuh"
+#include "slu_wgmma.cuh"
 
 #include <cstdio>
 #include <cstdlib>
@@ -39,9 +39,11 @@
 namespace slu {
 namespace oz {
 
-constexpr int TM = 128;                 // rows of a tile = UMMA M
-constexpr int KSTEP = 32;               // int8 k per tcgen05.mma.kind::i8 = k per pipeline stage
+constexpr int TM = 128;                 // rows of a tile: two wgmma M = 64 halves
+constexpr int KSTEP = 32;               // int8 k per wgmma = k per pipeline stage
 constexpr int A_SLICE_BYTES = TM * KSTEP;  // one slice of one A tile stage
+constexpr int CONSUMERS = 256;          // two warpgroups: tile rows [0, 64) and [64, 128)
+constexpr int THREADS = CONSUMERS + 128; // + the producer warpgroup (one lane issues the copies)
 
 // ---------------------------------------------------------------------------------------------------------------
 // PTX wrappers
@@ -94,56 +96,36 @@ __device__ __forceinline__ uint32_t cluster_ctarank()
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
     return r;
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_slot, uint32_t ncols)
+__device__ __forceinline__ void mbar_arrive(uint32_t bar)
 {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_slot), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols)
+// arrive on the mbarrier at the same CTA-relative offset in CTA `cta` of the cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta)
 {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// the same arrive on the mbarrier at this offset in every CTA of ctamask (frees a multicast stage cluster-wide)
-__device__ __forceinline__ void umma_commit_multicast(uint32_t bar, uint16_t ctamask)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(bar), "h"(ctamask)
+    asm volatile("{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
+                 "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(bar), "r"(cta)
                  : "memory");
 }
-// D[tmem] (+)= A[smem] * B[smem], int8 x int8 -> int32, M = 128, N and the operand formats in idesc
-__device__ __forceinline__ void umma_i8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// register budget of the 384-thread CTA: the producer warpgroup gives back what the accumulators of the consumers need
+__device__ __forceinline__ void producer_regs() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory"); }
+__device__ __forceinline__ void consumer_regs() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory"); }
+__device__ __forceinline__ void consumer_bar_sync()   // the 256 consumer threads only (named barrier 1)
 {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-                 : "memory");
+    asm volatile("bar.sync 1, 256;" ::: "memory");
 }
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&r)[8])
-{
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// shared-memory matrix descriptor, K-major, no swizzle (cute::UMMA::SmemDescriptor: start >> 4 at [0,14), LBO >> 4 at
-// [16,30), SBO >> 4 at [32,46), version 1 at [46,48), layout type 0 at [61,64))
+// shared-memory matrix descriptor, K-major, no swizzle: start >> 4 at [0,14), LBO >> 4 at [16,30) (128 B between the two
+// 16-byte K chunks), SBO >> 4 at [32,46) (256 B between 8-row groups), base offset 0, layout type 0 at [62,64)
 __device__ __forceinline__ uint64_t smem_desc(uint32_t addr)
 {
-    return (uint64_t)((addr & 0x3FFFF) >> 4) | ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(256 >> 4) << 32) | (1ull << 46);
+    return (uint64_t)((addr & 0x3FFFF) >> 4) | ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(256 >> 4) << 32);
 }
-// instruction descriptor (cute::UMMA::InstrDescriptor): c_format S32 = 2 at [4,6), a/b_format INT8 = 1 at [7,10)/[10,13),
-// K-major A and B (bits 15, 16 = 0), N >> 3 at [17,23), M >> 4 at [24,29)
-__device__ __forceinline__ uint32_t instr_desc(int n)
-{
-    return (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-}
+
 
 // ---------------------------------------------------------------------------------------------------------------
 // slicing
@@ -248,67 +230,49 @@ __device__ __forceinline__ void b_slice_col(const double *__restrict__ B, int ld
     for (int s = 0; s < S; ++s) *reinterpret_cast<uint4 *>(base + (size_t)s * (NT * KSTEP)) = dg[s];
 }
 
+
 // ---------------------------------------------------------------------------------------------------------------
-// the tile product: all 128 threads call it; returns the TMEM base once the S accumulator groups are complete
+// the tile product
 // ---------------------------------------------------------------------------------------------------------------
 template <int S, int NT, int STAGES>
 struct TileCfg {
     static constexpr int A_STAGE = S * A_SLICE_BYTES, B_STAGE = S * NT * KSTEP, STAGE = A_STAGE + B_STAGE;
-    static constexpr int TMEM_COLS = (S * NT <= 32) ? 32 : (S * NT <= 64) ? 64 : (S * NT <= 128) ? 128 : (S * NT <= 256) ? 256 : 512;
-    static constexpr size_t SMEM = (size_t)STAGES * STAGE + 8 * (2 * STAGES + 1) + 16 + 1024;  // + alignment slack
-    static_assert(S * NT <= 512, "accumulator groups exceed TMEM");
-    static_assert(NT % 16 == 0, "UMMA N must be a multiple of 16 at M = 128");
+    static constexpr int ACC = S * NT / 2;   // accumulator registers per consumer thread
+    static constexpr size_t SMEM = (size_t)STAGES * STAGE + 8 * 2 * STAGES + 1024;  // + alignment slack
+    static_assert(S * NT <= 256, "accumulator groups exceed the widest wgmma (N = 256)");
+    static_assert(NT % 32 == 0, "wgmma N of every slice instruction must be a multiple of 32");
 };
 
+// Stage ring at the 1 KB aligned start of dynamic shared memory: STAGES stages, then full[STAGES], empty[STAGES].
 // CL > 1: the CL CTAs of a cluster work on CL neighbouring column tiles of the SAME row tile.  The A stage (S slices
-// of 128 rows x 32 k, 7/8 of the operand bytes) is fetched from L2 once per cluster: CTA r copies the r-th 1/CL of it
+// of 128 rows x 32 k, 4/5 of the operand bytes) is fetched from L2 once per cluster: CTA r copies the r-th 1/CL of it
 // with a multicast bulk copy that lands in every CTA's shared memory and counts on every CTA's full barrier; a stage
-// is re-used only when the MMAs of ALL CTAs have read it (empty barrier: CL arrivals, each CTA's commit is multicast).
-// WAIT = false: return right after the role loops; the caller overlaps its own work (destination prefetch) with the
-// MMAs still in flight and then calls tile_wait<STAGES, S, NT>() before touching TMEM.
-template <int S, int NT, int STAGES>
-__device__ __forceinline__ void tile_wait(uint8_t *smem_raw)
-{
+// is re-used only when the MMAs of ALL CTAs have read it (empty barrier: 2 * CL arrivals, one per warpgroup of the
+// cluster).
+template <int S, int NT, int STAGES, int CL>
+struct Pipe {
     using C = TileCfg<S, NT, STAGES>;
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    __syncwarp();
-    mbar_wait(smem_u32(smem) + STAGES * C::STAGE + 8 * 2 * STAGES, 0);
-    tc_fence_after();
-}
-
-template <int S, int NT, int STAGES, int CL, bool WAIT = true>
-__device__ __forceinline__ uint32_t tile_product(const int8_t *__restrict__ ga, const int8_t *__restrict__ gb, int ksteps,
-                                                 uint8_t *smem_raw)
-{
-    using C = TileCfg<S, NT, STAGES>;
-    static_assert(C::A_STAGE % (16 * CL) == 0, "A stage must split into 16-byte aligned parts");
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const uint32_t sbase = smem_u32(smem);
-    const uint32_t bar0 = sbase + STAGES * C::STAGE;  // full[STAGES], empty[STAGES], accfull
-    auto full = [&](int st) { return bar0 + 8 * st; };
-    auto empty = [&](int st) { return bar0 + 8 * (STAGES + st); };
-    const uint32_t accfull = bar0 + 8 * 2 * STAGES;
-    uint32_t *slot = reinterpret_cast<uint32_t *>(smem + STAGES * C::STAGE + 8 * (2 * STAGES + 1));
-    const int warp = threadIdx.x >> 5;
-    const uint32_t crank = CL > 1 ? cluster_ctarank() : 0;
-    constexpr uint16_t MASK = (uint16_t)((1u << CL) - 1);
-    constexpr int A_PART = C::A_STAGE / CL;
-
-    if (threadIdx.x == 0) {
-        for (int st = 0; st < STAGES; ++st) { mbar_init(full(st), 1); mbar_init(empty(st), CL); }
-        mbar_init(accfull, 1);
+    uint32_t sbase;
+    __device__ __forceinline__ explicit Pipe(uint8_t *smem_raw)
+        : sbase(smem_u32(reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023))) {}
+    __device__ __forceinline__ uint32_t full(int st) const { return sbase + STAGES * C::STAGE + 8 * st; }
+    __device__ __forceinline__ uint32_t empty(int st) const { return sbase + STAGES * C::STAGE + 8 * (STAGES + st); }
+    // thread 0; the caller then synchronises the CTA (CL > 1: the cluster) before anybody uses the barriers
+    __device__ __forceinline__ void init() const
+    {
+        for (int st = 0; st < STAGES; ++st) { mbar_init(full(st), 1); mbar_init(empty(st), 2 * CL); }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(smem_u32(slot), C::TMEM_COLS);
-    tc_fence_before();
-    if (CL > 1) cluster_sync_all(); else __syncthreads();   // CL > 1: nobody multicasts before every barrier exists
-    tc_fence_after();
-    const uint32_t tmem = *slot;
-
-    if (threadIdx.x == 0) {  // producer
-        for (int ks = 0; ks < ksteps; ++ks) {
-            const int st = ks % STAGES;
-            if (ks >= STAGES) mbar_wait(empty(st), ((ks / STAGES) - 1) & 1);
+    // producer lane: the ksteps stages of one tile; g counts k-steps over the CTA's life (ring slot and parity)
+    __device__ __forceinline__ uint32_t load(const int8_t *ga, const int8_t *gb, int ksteps, uint32_t g) const
+    {
+        constexpr uint16_t MASK = (uint16_t)((1u << CL) - 1);
+        constexpr int A_PART = C::A_STAGE / CL;
+        static_assert(C::A_STAGE % (16 * CL) == 0, "A stage must split into 16-byte aligned parts");
+        const uint32_t crank = CL > 1 ? cluster_ctarank() : 0;
+        for (int ks = 0; ks < ksteps; ++ks, ++g) {
+            const int st = g % STAGES;
+            if (g >= (uint32_t)STAGES) mbar_wait(empty(st), ((g / STAGES) - 1) & 1);
             mbar_expect_tx(full(st), C::STAGE);
             const uint32_t a0 = sbase + st * C::STAGE;
             if (CL > 1)
@@ -317,27 +281,50 @@ __device__ __forceinline__ uint32_t tile_product(const int8_t *__restrict__ ga, 
                 bulk_g2s(a0, ga + (size_t)ks * C::A_STAGE, C::A_STAGE, full(st));
             bulk_g2s(a0 + C::A_STAGE, gb + (size_t)ks * C::B_STAGE, C::B_STAGE, full(st));
         }
-    } else if (threadIdx.x == 32) {  // MMA issuer
-        for (int ks = 0; ks < ksteps; ++ks) {
-            const int st = ks % STAGES;
-            mbar_wait(full(st), (ks / STAGES) & 1);
-            tc_fence_after();
-            const uint32_t a0 = sbase + st * C::STAGE, b0 = a0 + C::A_STAGE;
-            const uint64_t bdesc = smem_desc(b0);
+        return g;
+    }
+    __device__ __forceinline__ void release(int st) const
+    {
+        if ((threadIdx.x & 127) != 0) return;    // one arrival per warpgroup
+        if (CL == 1) {
+            mbar_arrive(empty(st));
+        } else {
 #pragma unroll
-            for (int s = 0; s < S; ++s)
-                umma_i8(tmem + s * NT, smem_desc(a0 + s * A_SLICE_BYTES), bdesc, instr_desc((S - s) * NT), (ks | s) != 0);
-            if (CL > 1) umma_commit_multicast(empty(st), MASK); else umma_commit(empty(st));  // stage free when read
+            for (int r = 0; r < CL; ++r) mbar_arrive_cluster(empty(st), r);
         }
-        umma_commit(accfull);
     }
-    if (WAIT) {
-        __syncwarp();
-        mbar_wait(accfull, 0);
-        tc_fence_after();
+    // consumer warpgroups: acc = the S accumulator groups of this warpgroup's 64 x NT half of the tile
+    __device__ __forceinline__ uint32_t mma(int ksteps, uint32_t g, uint32_t (&acc)[C::ACC]) const
+    {
+        const uint32_t half = (threadIdx.x >> 7) * (A_SLICE_BYTES / 2);   // rows [64 wg, 64 wg + 64) of each slice
+        for (int ks = 0; ks < ksteps; ++ks, ++g) {
+            const int st = g % STAGES;
+            mbar_wait(full(st), (g / STAGES) & 1);
+            const uint32_t a0 = sbase + st * C::STAGE;
+            wgmma_fence();
+            issue<0>(acc, smem_desc(a0 + half), smem_desc(a0 + C::A_STAGE), ks != 0);
+            wgmma_commit();
+            wgmma_wait<1>();                      // the previous k-step's MMAs are done: its stage is free
+            if (ks > 0) release((g - 1) % STAGES);
+        }
+        wgmma_wait<0>();
+        if (ksteps > 0) release((g - 1) % STAGES);
+        return g;
     }
-    return tmem;
-}
+    template <int s>
+    __device__ __forceinline__ static void issue(uint32_t (&acc)[C::ACC], uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
+    {
+        if constexpr (s < S) {
+            Wgmma<(S - s) * NT>::mma(acc + s * (NT / 2), adesc + (uint64_t)(s * (A_SLICE_BYTES >> 4)), bdesc, accumulate | s);
+            issue<s + 1>(acc, adesc, bdesc, accumulate);
+        }
+    }
+};
+
+// Where a consumer thread's accumulator elements sit in the 128 x NT tile: register 4c + 2h + e of every group is
+// (row tile_row(h), column 8c + 2 (lane % 4) + e).
+__device__ __forceinline__ int tile_row(int h) { return ((threadIdx.x >> 5) << 4) + ((threadIdx.x & 31) >> 2) + 8 * h; }
+__device__ __forceinline__ int tile_col(int c, int e) { return 8 * c + 2 * (threadIdx.x & 3) + e; }
 
 // int32 -> double without the (slow) I2F.F64 path: 2^52 + 2^31 + x is exact in a double whose low word is x ^ 2^31
 __device__ __forceinline__ double i2d(uint32_t x)
@@ -345,44 +332,34 @@ __device__ __forceinline__ double i2d(uint32_t x)
     return __hiloint2double(0x43300000, (int)(x ^ 0x80000000u)) - 4503601774854144.0;  // 2^52 + 2^31
 }
 
-// FP64 value (before the row/column scales) of 8 consecutive columns [8*jc, 8*jc+8) of this thread's row.
+// FP64 value (before the row/column scales) of accumulator element idx (0 <= idx < NT/2) of this thread.
 // PAIRS (k-steps <= 8, i.e. supernodes <= 256 columns: |acc_g| <= 8*256*2^12 = 2^23): neighbouring groups are first
 // combined exactly in int32 (acc_hi * 128 + acc_lo < 2^31), halving the conversions.
 template <int S, int NT, bool PAIRS>
-__device__ __forceinline__ void read_chunk(uint32_t tmem, int jc, double (&v)[8])
+__device__ __forceinline__ double combine(const uint32_t *acc, int idx)
 {
-    const uint32_t lane_base = tmem + ((uint32_t)((threadIdx.x >> 5) & 3) << 21);  // lanes [32q, 32q+32): q << (16 + 5)
-    uint32_t r[S][8];
+    auto r = [&](int g) { return acc[g * (NT / 2) + idx]; };
+    if constexpr (PAIRS) {
+        // sum_g acc_g 2^(-7g): pair (g-1, g), g odd, is P = acc_(g-1) * 128 + acc_g with weight 2^(-7g); Horner over
+        // the pairs in 2^-14, a leading single group (S odd) pre-scaled by 2^7, the common 2^-7 applied last
+        double acc_d;
+        if constexpr (S % 2 == 1) acc_d = i2d(r(S - 1)) * 128.0;
+        else acc_d = i2d((uint32_t)((int)r(S - 2) * 128 + (int)r(S - 1)));
 #pragma unroll
-    for (int g = 0; g < S; ++g) tmem_ld8(lane_base + g * NT + jc * 8, r[g]);
-    tmem_ld_wait();
+        for (int g = (S % 2 == 1) ? S - 2 : S - 3; g >= 1; g -= 2)
+            acc_d = fma(acc_d, 6.103515625e-05, i2d((uint32_t)((int)r(g - 1) * 128 + (int)r(g))));
+        return acc_d * 0.0078125;
+    } else {
+        double acc_d = i2d(r(S - 1));
 #pragma unroll
-    for (int e = 0; e < 8; ++e) {
-        if constexpr (PAIRS) {
-            // sum_g acc_g 2^(-7g): pair (g-1, g), g odd, is P = acc_(g-1) * 128 + acc_g with weight 2^(-7g); Horner over
-            // the pairs in 2^-14, a leading single group (S odd) pre-scaled by 2^7, the common 2^-7 applied last
-            double acc;
-            if constexpr (S % 2 == 1) acc = i2d(r[S - 1][e]) * 128.0;
-            else acc = i2d((uint32_t)((int)r[S - 2][e] * 128 + (int)r[S - 1][e]));
-#pragma unroll
-            for (int g = (S % 2 == 1) ? S - 2 : S - 3; g >= 1; g -= 2)
-                acc = fma(acc, 6.103515625e-05, i2d((uint32_t)((int)r[g - 1][e] * 128 + (int)r[g][e])));
-            v[e] = acc * 0.0078125;
-        } else {
-            double acc = i2d(r[S - 1][e]);
-#pragma unroll
-            for (int g = S - 2; g >= 0; --g) acc = fma(acc, 0.0078125, i2d(r[g][e]));
-            v[e] = acc;
-        }
+        for (int g = S - 2; g >= 0; --g) acc_d = fma(acc_d, 0.0078125, i2d(r(g)));
+        return acc_d;
     }
 }
-
-template <int S, int NT, int STAGES, int CL>
-__device__ __forceinline__ void tile_teardown(uint32_t tmem)
+template <int S, int NT>
+__device__ __forceinline__ double combine(const uint32_t *acc, int idx, int ks)
 {
-    tc_fence_before();
-    if (CL > 1) cluster_sync_all(); else __syncthreads();   // CL > 1: peers may still signal my barriers until they are done
-    if ((threadIdx.x >> 5) == 1) tmem_dealloc(tmem, TileCfg<S, NT, STAGES>::TMEM_COLS);
+    return ks <= 8 ? combine<S, NT, true>(acc, idx) : combine<S, NT, false>(acc, idx);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -406,39 +383,50 @@ __global__ void __launch_bounds__(128) dense_slice_b_kernel(const double *B, int
     if (j < ncol_pad) b_slice_col<S, NT>(B, ldb, k, n, KS, j, threadIdx.x & 31, cscale, out);
 }
 
+
 // EPI: 0 = subtract with RED.ADD.F64 (the real thing), 1 = plain store of -V (timing only), 2 = no output (timing only)
 template <int S, int NT, int STAGES, int CL, int EPI>
-__global__ void __launch_bounds__(128, 2)
+__global__ void __launch_bounds__(THREADS, 1)
     dense_gemm_kernel(const int8_t *As, const int8_t *Bs, const double *rscale, const double *cscale, int M, int N, int KS,
                       double *Cm, int ldc)
 {
     using C = TileCfg<S, NT, STAGES>;
     extern __shared__ uint8_t oz_smem[];
+    const Pipe<S, NT, STAGES, CL> pipe(oz_smem);
     const int tiles_m = (M + TM - 1) / TM, tiles_n = (N + NT - 1) / NT;
     // a cluster takes CL neighbouring column tiles of one row tile
     const int cid = blockIdx.x / CL, cr = blockIdx.x % CL;
     const int tm = cid % tiles_m, tn = (cid / tiles_m) * CL + cr;
     const int tnb = min(tn, tiles_n - 1);          // a column tile past the edge still takes part in the cluster protocol
-    const uint32_t tmem = tile_product<S, NT, STAGES, CL>(As + (size_t)tm * KS * C::A_STAGE, Bs + (size_t)tnb * KS * C::B_STAGE, KS, oz_smem);
-    const int i = tm * TM + (threadIdx.x & 127);  // warp q of the CTA reads TMEM lanes [32q, 32q+32) = rows
-    const double rs = i < M ? rscale[i] : 0.0;
-    if (EPI != 2 && tn < tiles_n) {
-#pragma unroll 1
-        for (int jc = 0; jc < NT / 8; ++jc) {
-            double v[8];
-            __syncwarp();
-            if (KS <= 8) read_chunk<S, NT, true>(tmem, jc, v); else read_chunk<S, NT, false>(tmem, jc, v);
+    if (threadIdx.x == 0) pipe.init();
+    if (CL > 1) cluster_sync_all(); else __syncthreads();   // CL > 1: nobody multicasts before every barrier exists
+    if (threadIdx.x >= CONSUMERS) {
+        producer_regs();
+        if (threadIdx.x == CONSUMERS) pipe.load(As + (size_t)tm * KS * C::A_STAGE, Bs + (size_t)tnb * KS * C::B_STAGE, KS, 0);
+    } else {
+        consumer_regs();
+        uint32_t acc[C::ACC];
+        pipe.mma(KS, 0, acc);
+        if (EPI != 2 && tn < tiles_n) {
 #pragma unroll
-            for (int e = 0; e < 8; ++e) {
-                const int j = tn * NT + jc * 8 + e;
-                if (i < M && j < N) {
-                    if (EPI == 0) atomicAdd(Cm + (size_t)j * ldc + i, -(v[e] * rs * cscale[j]));
-                    else Cm[(size_t)j * ldc + i] = -(v[e] * rs * cscale[j]);
-                }
+            for (int h = 0; h < 2; ++h) {
+                const int i = tm * TM + tile_row(h);
+                if (i >= M) continue;
+                const double rs = rscale[i];
+#pragma unroll
+                for (int c = 0; c < NT / 8; ++c)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int j = tn * NT + tile_col(c, e);
+                        if (j >= N) continue;
+                        const double v = combine<S, NT>(acc, 4 * c + 2 * h + e, KS) * rs * cscale[j];
+                        if (EPI == 0) atomicAdd(Cm + (size_t)j * ldc + i, -v);
+                        else Cm[(size_t)j * ldc + i] = -v;
+                    }
             }
         }
     }
-    tile_teardown<S, NT, STAGES, CL>(tmem);
+    if (CL > 1) cluster_sync_all();   // peers may still signal my barriers until they are done
 }
 
 struct DenseWs {          // scratch of the dense entry (per process, grows on demand)
@@ -495,13 +483,13 @@ static int launch_dense_t(int m, int n, int k, const double *a, int lda, const d
     ensure_dyn_smem(dense_gemm_kernel<S, NT, STAGES, CL, EPI>, (int)C::SMEM, attr);
     const int grid = RT * ((CT + CL - 1) / CL) * CL;
     if (CL == 1) {
-        dense_gemm_kernel<S, NT, STAGES, CL, EPI><<<grid, 128, C::SMEM, s>>>(w.a, w.b, w.rs, w.cs, m, n, KS, c, ldc);
+        dense_gemm_kernel<S, NT, STAGES, CL, EPI><<<grid, THREADS, C::SMEM, s>>>(w.a, w.b, w.rs, w.cs, m, n, KS, c, ldc);
     } else {
         const int8_t *pa = w.a, *pb = w.b;
         const double *prs = w.rs, *pcs = w.cs;
         int KSv = KS;
         void *args[] = {&pa, &pb, &prs, &pcs, &m, &n, &KSv, &c, &ldc};
-        launch_clustered(dense_gemm_kernel<S, NT, STAGES, CL, EPI>, dim3(grid), 128, C::SMEM, CL, s, args);
+        launch_clustered(dense_gemm_kernel<S, NT, STAGES, CL, EPI>, dim3(grid), THREADS, C::SMEM, CL, s, args);
     }
     return 4;
 }
@@ -537,22 +525,89 @@ __global__ void __launch_bounds__(128) schur_slice_b_kernel(DeviceLU d, const in
                               d.oz_scale + nd.ws_ozs + mpad, d.oz_i8 + nd.ws_ozb);
 }
 
+// Destinations of a consumer thread's 2 x NT/4 elements of tile (tm, tn) of supernode nd (column descriptors of the
+// tile in shared memory: sc_*); off = -1: no destination.  excl bit q: exclusive destination, plain load/store.
+struct Dest {
+    long long off[2][OZ_NT / 4];
+    double rs[2];
+    unsigned excl;
+};
+template <int NT>
+__device__ __forceinline__ void dest_offsets(const DeviceLU &d, const NodeDesc &nd, int tm, int tn, bool tile_ok, int nonatomic,
+                                             const int *sc_jb, const int *sc_pad, const long long *sc_lbase,
+                                             const long long *sc_lrel, Dest &D)
+{
+    static_assert(NT == OZ_NT, "Dest holds OZ_NT / 4 columns per row");
+    D.excl = 0;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int i = tm * TM + tile_row(h);
+        D.rs[h] = 0.0;
+#pragma unroll
+        for (int q = 0; q < NT / 4; ++q) D.off[h][q] = -1;
+        if (!tile_ok || i >= nd.m) continue;
+        const RowInfo ri = d.rowinfo[nd.ws_row + i];
+        D.rs[h] = d.oz_scale[nd.ws_ozs + i];
+        long long last_off = -1;
+        int lpos = -1;
+#pragma unroll
+        for (int q = 0; q < NT / 4; ++q) {
+            const int c = tile_col(q >> 1, q & 1), jb = sc_jb[c];
+            if (jb < 0) continue;
+            if (ri.ib >= jb) {   // destination in L panel jb: row position of my row there
+                if (sc_lrel[c] != last_off) { last_off = sc_lrel[c]; lpos = d.lrel[last_off + i]; }
+                if (lpos >= 0) { D.off[h][q] = sc_lbase[c] + lpos; if (nonatomic && !sc_pad[c]) D.excl |= 1u << (h * 16 + q); }
+            } else {             // destination in U panel ib: packed column position of column j there
+                const int p = d.urel[ri.urel_off + tn * NT + c];
+                if (p >= 0) { D.off[h][q] = ri.ubase + (long long)p * ri.ldu; if (nonatomic && !ri.shared) D.excl |= 1u << (h * 16 + q); }
+            }
+        }
+    }
+}
+// recombine, scale, subtract-scatter
+template <int S, int NT>
+__device__ __forceinline__ void scatter(const DeviceLU &d, const uint32_t *acc, int ks, const Dest &D, const double *sc_scale)
+{
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int q = 0; q < NT / 4; ++q) {
+            const long long o = D.off[h][q];
+            if (o < 0) continue;
+            const int c = tile_col(q >> 1, q & 1);
+            const double val = flip_sign(combine<S, NT>(acc, 2 * (q >> 1) * 2 + 2 * h + (q & 1), ks) * D.rs[h] * sc_scale[c]);
+            if (D.excl >> (h * 16 + q) & 1) __stcg(d.val + o, __ldcg(d.val + o) + val);
+            else atomicAdd(d.val + o, val);
+        }
+}
+template <int NT>
+__device__ __forceinline__ void load_col_desc(const DeviceLU &d, const NodeDesc &nd, int tn, bool tile_ok, int c, int *sc_jb,
+                                              int *sc_pad, long long *sc_lbase, long long *sc_lrel, double *sc_scale)
+{
+    const int j = tn * NT + c, mpad = (nd.m + TM - 1) / TM * TM;
+    if (tile_ok && j < nd.ncols) {
+        const ColInfo cj = d.colinfo[nd.ws_col + j];
+        sc_jb[c] = cj.jb; sc_pad[c] = cj.pad; sc_lbase[c] = cj.lbase; sc_lrel[c] = cj.lrel_off;
+        sc_scale[c] = d.oz_scale[nd.ws_ozs + mpad + j];
+    } else {
+        sc_jb[c] = -1; sc_pad[c] = 0; sc_lbase[c] = 0; sc_lrel[c] = -1; sc_scale[c] = 0.0;
+    }
+}
+
 // Tiles are enumerated in units of 128 x (CL * NT) "cluster tiles" (the host counts them with OZ_NT_HOST = CL * NT
 // columns); the CL CTAs of a cluster take its CL column tiles and share the A operand through multicast.
-//
-// 256 threads: thread 0 produces, thread 32 issues the MMAs, and ALL eight warps are the epilogue -- warps w and w + 4
-// read the same 32 TMEM lanes (rows) and split the tile's 32 columns 16 / 16.  While the MMAs run, every thread works
-// out where its 16 elements go (destination panel, row / column position, exclusive or shared): that index chase is
-// two dependent L2 round trips per element group and used to sit, un-overlapped, behind the accumulator wait.
+// The destination offsets are worked out after the MMAs: held across the k-loop beside the S * NT / 2 accumulators
+// they would spill.  Two consumer warpgroups per SM and the producer's prefetch cover part of that index chase.
 template <int S, int NT, int STAGES, int CL>
-__global__ void __launch_bounds__(256, 2) schur_kernel_tc(DeviceLU d, Batch b, int mode, int split_n, int split_i, int nonatomic)
+__global__ void __launch_bounds__(THREADS, 1) schur_kernel_tc(DeviceLU d, Batch b, int mode, int split_n, int split_i, int nonatomic)
 {
     using C = TileCfg<S, NT, STAGES>;
     extern __shared__ uint8_t oz_smem[];
     __shared__ int sc_jb[NT], sc_pad[NT];
     __shared__ long long sc_lbase[NT], sc_lrel[NT];
     __shared__ double sc_scale[NT];
-    constexpr int NTC = NT * CL, HALF = NT / 2;
+    constexpr int NTC = NT * CL;
+    const Pipe<S, NT, STAGES, CL> pipe(oz_smem);
     const int cr = blockIdx.x % CL;
     const int64_t gt = (int64_t)(blockIdx.x / CL) * split_n + split_i;  // cooperative ancestors: tiles dealt round-robin
     if (gt >= b.prefix[b.count]) return;                              // the whole cluster leaves
@@ -577,99 +632,30 @@ __global__ void __launch_bounds__(256, 2) schur_kernel_tc(DeviceLU d, Batch b, i
     const int tiles_n = (nd.ncols + NT - 1) / NT;
     const int tn = tnc * CL + cr, tnb = min(tn, tiles_n - 1);   // a column tile past the edge still runs the protocol
     const int KS = (nd.ns + KSTEP - 1) / KSTEP;
-    const int mpad = tiles_m * TM;
-    // the tile's 32 column descriptors -> shared memory (visible after the barrier inside tile_product)
-    if (threadIdx.x >= 64 && threadIdx.x < 64 + NT) {
-        const int c = threadIdx.x - 64, j = tn * NT + c;
-        if (tn < tiles_n && j < nd.ncols) {
-            const ColInfo cj = d.colinfo[nd.ws_col + j];
-            sc_jb[c] = cj.jb; sc_pad[c] = cj.pad; sc_lbase[c] = cj.lbase; sc_lrel[c] = cj.lrel_off;
-            sc_scale[c] = d.oz_scale[nd.ws_ozs + mpad + j];
-        } else {
-            sc_jb[c] = -1; sc_pad[c] = 0; sc_lbase[c] = 0; sc_lrel[c] = -1; sc_scale[c] = 0.0;
-        }
-    }
-    const uint32_t tmem = tile_product<S, NT, STAGES, CL, false>(d.oz_i8 + nd.ws_oza + (size_t)tm * KS * C::A_STAGE,
-                                                                 d.oz_i8 + nd.ws_ozb + (size_t)tnb * KS * C::B_STAGE, KS, oz_smem);
-
-    // ---- while the MMAs run: destinations of my 16 elements (row i, columns c0 .. c0 + 15) ----------------------------
-    const int i = tm * TM + (threadIdx.x & 127);
-    const int c0 = (threadIdx.x >> 7) * HALF;
-    const bool rok = i < nd.m && tn < tiles_n;
-    long long off[HALF];
-    unsigned excl = 0;
-    double rs = 0.0;
-    if (rok) {
-        const RowInfo ri = d.rowinfo[nd.ws_row + i];
-        rs = d.oz_scale[nd.ws_ozs + i];
-        long long last_off = -1;
-        int lpos = -1;
-#pragma unroll
-        for (int e = 0; e < HALF; ++e) {
-            const int c = c0 + e, jb = sc_jb[c];
-            off[e] = -1;
-            if (jb < 0) continue;
-            if (ri.ib >= jb) {   // destination in L panel jb: row position of my row there
-                if (sc_lrel[c] != last_off) { last_off = sc_lrel[c]; lpos = d.lrel[last_off + i]; }
-                if (lpos >= 0) { off[e] = sc_lbase[c] + lpos; if (nonatomic && !sc_pad[c]) excl |= 1u << e; }
-            } else {             // destination in U panel ib: packed column position of column j there
-                const int q = d.urel[ri.urel_off + tn * NT + c];
-                if (q >= 0) { off[e] = ri.ubase + (long long)q * ri.ldu; if (nonatomic && !ri.shared) excl |= 1u << e; }
-            }
-        }
+    if (threadIdx.x == 0) pipe.init();
+    if (threadIdx.x < NT) load_col_desc<NT>(d, nd, tn, tn < tiles_n, threadIdx.x, sc_jb, sc_pad, sc_lbase, sc_lrel, sc_scale);
+    if (CL > 1) cluster_sync_all(); else __syncthreads();   // CL > 1: nobody multicasts before every barrier exists
+    if (threadIdx.x >= CONSUMERS) {
+        producer_regs();
+        if (threadIdx.x == CONSUMERS)
+            pipe.load(d.oz_i8 + nd.ws_oza + (size_t)tm * KS * C::A_STAGE, d.oz_i8 + nd.ws_ozb + (size_t)tnb * KS * C::B_STAGE, KS, 0);
     } else {
-#pragma unroll
-        for (int e = 0; e < HALF; ++e) off[e] = -1;
+        consumer_regs();
+        uint32_t acc[C::ACC];
+        pipe.mma(KS, 0, acc);
+        Dest D;
+        dest_offsets<NT>(d, nd, tm, tn, tn < tiles_n, nonatomic, sc_jb, sc_pad, sc_lbase, sc_lrel, D);
+        scatter<S, NT>(d, acc, KS, D, sc_scale);
     }
-
-    tile_wait<S, NT, STAGES>(oz_smem);
-    // ---- epilogue: recombine the S groups, scale, subtract-scatter ---------------------------------------------------
-    if (tn < tiles_n) {
-#pragma unroll
-        for (int h = 0; h < HALF / 8; ++h) {
-            double v[8];
-            __syncwarp();        // tcgen05.ld is .sync.aligned
-            if (KS <= 8) read_chunk<S, NT, true>(tmem, c0 / 8 + h, v); else read_chunk<S, NT, false>(tmem, c0 / 8 + h, v);
-            double old[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e)
-                if (off[h * 8 + e] >= 0 && (excl >> (h * 8 + e) & 1)) old[e] = __ldcg(d.val + off[h * 8 + e]);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-                const long long o = off[h * 8 + e];
-                if (o < 0) continue;
-                const double val = flip_sign(v[e] * rs * sc_scale[c0 + h * 8 + e]);
-                if (excl >> (h * 8 + e) & 1) __stcg(d.val + o, old[e] + val);
-                else atomicAdd(d.val + o, val);
-            }
-        }
-    }
-    tile_teardown<S, NT, STAGES, CL>(tmem);
+    if (CL > 1) cluster_sync_all();   // peers may still signal my barriers until they are done
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Persistent, warp-specialised form of the same tile product (profiles/r02_notes.md: the one-tile-per-CTA kernel keeps
-// the int8 tensor pipe only ~45 % busy in the dense test and ~20 % inside the factorization -- every tile pays CTA
-// launch, barrier init, TMEM allocation, the first L2 round trip and an epilogue nobody overlaps).
-// Here a CTA lives for many tiles (grid = 2 x #SMs, tile t -> CTA t mod grid):
-//   warp 0  producer   one lane; keeps the STAGES-deep bulk-copy ring full ACROSS tiles (the next tile's operands
-//                      arrive during the current tile's epilogue);
-//   warp 1  MMA        one lane; waits for the accumulators to be drained (acc_empty), issues S MMAs per k-step,
-//                      commits stage-free and accumulator-ready barriers; owns the TMEM allocation for the CTA's life;
-//   warps 2-5 epilogue thread = row; per tile: column descriptors -> shared memory (double-buffered by tile parity),
-//                      destination offsets of the row's 32 elements (while the MMAs run), wait acc_full, read TMEM,
-//                      recombine, scatter, arrive on acc_empty.
-// The two CTAs of an SM alternate between MMA and epilogue, so the tensor pipe sees back-to-back tiles.
+// Persistent form of the same tile product: a CTA lives for many tiles (tile t -> CTA t / tiles_per_cta) so that CTA
+// launch and barrier set-up are paid once and the producer warp keeps the bulk-copy ring full ACROSS tiles (the next
+// tile's operands arrive during the current tile's epilogue).  Column descriptors in shared memory are
+// double-buffered by tile parity.
 // ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void mbar_arrive(uint32_t bar)
-{
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void epi_bar_sync()   // the 128 epilogue threads only (named barrier 1)
-{
-    asm volatile("bar.sync 1, 128;" ::: "memory");
-}
-
 struct TileDesc {     // what the roles need to know about tile gt
     const int8_t *ga, *gb;
     int ks, k, tm, tn;
@@ -710,180 +696,73 @@ __device__ __forceinline__ bool decode_tile(const DeviceLU &d, const Batch &b, i
 }
 
 template <int S, int NT, int STAGES>
-__global__ void __launch_bounds__(192, 2) schur_kernel_tc_persist(DeviceLU d, Batch b, int mode, int split_n, int split_i, int nonatomic,
-                                                                  int tiles_per_cta, long long mine)
+__global__ void __launch_bounds__(THREADS, 1) schur_kernel_tc_persist(DeviceLU d, Batch b, int mode, int split_n, int split_i, int nonatomic,
+                                                                      int tiles_per_cta, long long mine)
 {
     using C = TileCfg<S, NT, STAGES>;
     extern __shared__ uint8_t oz_smem[];
     __shared__ int sc_jb[2][NT], sc_pad[2][NT];
     __shared__ long long sc_lbase[2][NT], sc_lrel[2][NT];
     __shared__ double sc_scale[2][NT];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(oz_smem) + 1023) & ~(uintptr_t)1023);
-    const uint32_t sbase = smem_u32(smem);
-    const uint32_t bar0 = sbase + STAGES * C::STAGE;  // full[STAGES], empty[STAGES], acc_full, acc_empty
-    auto full = [&](int st) { return bar0 + 8 * st; };
-    auto empty = [&](int st) { return bar0 + 8 * (STAGES + st); };
-    const uint32_t acc_full = bar0 + 8 * 2 * STAGES, acc_empty = acc_full + 8;
-    uint32_t *slot_tm = reinterpret_cast<uint32_t *>(smem + STAGES * C::STAGE + 8 * (2 * STAGES + 2));
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-    if (threadIdx.x == 0) {
-        for (int st = 0; st < STAGES; ++st) { mbar_init(full(st), 1); mbar_init(empty(st), 1); }
-        mbar_init(acc_full, 1);
-        mbar_init(acc_empty, 4);          // one arrival per epilogue warp
-        fence_barrier_init();
-    }
-    if (warp == 1) tmem_alloc(smem_u32(slot_tm), C::TMEM_COLS);
-    tc_fence_before();
+    const Pipe<S, NT, STAGES, 1> pipe(oz_smem);
+    if (threadIdx.x == 0) pipe.init();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *slot_tm;
     // this rank's tiles are gt = q * split_n + split_i, q < mine (cooperative ancestors); CTA c takes the tiles_per_cta
     // consecutive q from c * tiles_per_cta.  A CTA lives for a bounded number of tiles so that the kernels of the
     // high-priority stream (the next level's panel work) still find free SMs quickly -- CTAs are not preempted.
     const long long q0 = (long long)blockIdx.x * tiles_per_cta, q1 = min(q0 + tiles_per_cta, mine);
-
-    if (warp == 0) {
-        if (lane == 0) {  // ---- producer ----------------------------------------------------------------------------
-            int slot_cache = -1;
-            uint32_t g = 0;
+    int slot_cache = -1;
+    uint32_t g = 0;
+    if (threadIdx.x >= CONSUMERS) {
+        producer_regs();
+        if (threadIdx.x == CONSUMERS) {   // ---- producer ----
             for (long long q = q0; q < q1; ++q) {
                 TileDesc t;
                 if (!decode_tile<S, NT>(d, b, mode, q * split_n + split_i, slot_cache, t)) break;
-                for (int ks = 0; ks < t.ks; ++ks, ++g) {
-                    const int st = g % STAGES;
-                    if (g >= (uint32_t)STAGES) mbar_wait(empty(st), ((g / STAGES) - 1) & 1);
-                    mbar_expect_tx(full(st), C::STAGE);
-                    const uint32_t a0 = sbase + st * C::STAGE;
-                    bulk_g2s(a0, t.ga + (size_t)ks * C::A_STAGE, C::A_STAGE, full(st));
-                    bulk_g2s(a0 + C::A_STAGE, t.gb + (size_t)ks * C::B_STAGE, C::B_STAGE, full(st));
-                }
+                g = pipe.load(t.ga, t.gb, t.ks, g);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {  // ---- MMA issuer --------------------------------------------------------------------------
-            int slot_cache = -1;
-            uint32_t g = 0, it = 0;
-            for (long long q = q0; q < q1; ++q, ++it) {
-                TileDesc t;
-                if (!decode_tile<S, NT>(d, b, mode, q * split_n + split_i, slot_cache, t)) break;
-                if (it > 0) mbar_wait(acc_empty, (it - 1) & 1);   // the epilogue has read the previous tile out of TMEM
-                tc_fence_after();
-                for (int ks = 0; ks < t.ks; ++ks, ++g) {
-                    const int st = g % STAGES;
-                    mbar_wait(full(st), (g / STAGES) & 1);
-                    tc_fence_after();
-                    const uint32_t a0 = sbase + st * C::STAGE, b0 = a0 + C::A_STAGE;
-                    const uint64_t bdesc = smem_desc(b0);
-#pragma unroll
-                    for (int s = 0; s < S; ++s)
-                        umma_i8(tmem + s * NT, smem_desc(a0 + s * A_SLICE_BYTES), bdesc, instr_desc((S - s) * NT), (ks | s) != 0);
-                    umma_commit(empty(st));
-                }
-                umma_commit(acc_full);
-            }
-        }
-    } else {
-        // ---- epilogue warps 2..5: TMEM lane quarter = warp & 3, thread = row -------------------------------------------
-        const int et = threadIdx.x - 64;                 // 0..127
-        const int rloc = ((warp & 3) << 5) | lane;       // row of the tile this thread reads from TMEM
-        int slot_cache = -1;
-        uint32_t it = 0;
-        for (long long q = q0; q < q1; ++q, ++it) {
-            TileDesc t;
-            if (!decode_tile<S, NT>(d, b, mode, q * split_n + split_i, slot_cache, t)) break;
-            const NodeDesc nd = d.nodes[t.k];
-            const int par = it & 1;
-            const int mpad = (nd.m + TM - 1) / TM * TM;
-            if (et < NT) {   // column descriptors of this tile -> shared memory
-                const int j = t.tn * NT + et;
-                if (j < nd.ncols) {
-                    const ColInfo cj = d.colinfo[nd.ws_col + j];
-                    sc_jb[par][et] = cj.jb; sc_pad[par][et] = cj.pad; sc_lbase[par][et] = cj.lbase; sc_lrel[par][et] = cj.lrel_off;
-                    sc_scale[par][et] = d.oz_scale[nd.ws_ozs + mpad + j];
-                } else {
-                    sc_jb[par][et] = -1; sc_pad[par][et] = 0; sc_lbase[par][et] = 0; sc_lrel[par][et] = -1; sc_scale[par][et] = 0.0;
-                }
-            }
-            epi_bar_sync();
-            // destinations of my row's NT elements (overlaps the MMAs of this tile)
-            const int i = t.tm * TM + rloc;
-            const bool rok = i < nd.m;
-            long long off[NT];
-            unsigned excl = 0;
-            double rs = 0.0;
-            if (rok) {
-                const RowInfo ri = d.rowinfo[nd.ws_row + i];
-                rs = d.oz_scale[nd.ws_ozs + i];
-                long long last_off = -1;
-                int lpos = -1;
-#pragma unroll
-                for (int e = 0; e < NT; ++e) {
-                    const int jb = sc_jb[par][e];
-                    off[e] = -1;
-                    if (jb < 0) continue;
-                    if (ri.ib >= jb) {
-                        if (sc_lrel[par][e] != last_off) { last_off = sc_lrel[par][e]; lpos = d.lrel[last_off + i]; }
-                        if (lpos >= 0) { off[e] = sc_lbase[par][e] + lpos; if (nonatomic && !sc_pad[par][e]) excl |= 1u << e; }
-                    } else {
-                        const int qq = d.urel[ri.urel_off + t.tn * NT + e];
-                        if (qq >= 0) { off[e] = ri.ubase + (long long)qq * ri.ldu; if (nonatomic && !ri.shared) excl |= 1u << e; }
-                    }
-                }
-            } else {
-#pragma unroll
-                for (int e = 0; e < NT; ++e) off[e] = -1;
-            }
-            __syncwarp();
-            mbar_wait(acc_full, it & 1);
-            tc_fence_after();
-#pragma unroll
-            for (int h = 0; h < NT / 8; ++h) {
-                double v[8];
-                __syncwarp();
-                if (t.ks <= 8) read_chunk<S, NT, true>(tmem, h, v); else read_chunk<S, NT, false>(tmem, h, v);
-                if (h == NT / 8 - 1) {     // TMEM is drained for this warp: let the next tile's MMAs start
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(acc_empty);
-                }
-#pragma unroll
-                for (int e = 0; e < 8; ++e) {
-                    const long long o = off[h * 8 + e];
-                    if (o < 0) continue;
-                    const double val = flip_sign(v[e] * rs * sc_scale[par][h * 8 + e]);
-                    if (excl >> (h * 8 + e) & 1) __stcg(d.val + o, __ldcg(d.val + o) + val);
-                    else atomicAdd(d.val + o, val);
-                }
-            }
-        }
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem, C::TMEM_COLS);
+    consumer_regs();
+    uint32_t it = 0;
+    for (long long q = q0; q < q1; ++q, ++it) {   // ---- consumers: MMA and epilogue of each tile ----
+        TileDesc t;
+        if (!decode_tile<S, NT>(d, b, mode, q * split_n + split_i, slot_cache, t)) break;
+        const NodeDesc nd = d.nodes[t.k];
+        const int par = it & 1;
+        if (threadIdx.x < NT)
+            load_col_desc<NT>(d, nd, t.tn, true, threadIdx.x, sc_jb[par], sc_pad[par], sc_lbase[par], sc_lrel[par], sc_scale[par]);
+        consumer_bar_sync();
+        uint32_t acc[C::ACC];
+        g = pipe.mma(t.ks, g, acc);
+        Dest D;
+        dest_offsets<NT>(d, nd, t.tm, t.tn, true, nonatomic, sc_jb[par], sc_pad[par], sc_lbase[par], sc_lrel[par], D);
+        scatter<S, NT>(d, acc, t.ks, D, sc_scale[par]);
+    }
 }
 
 template <int S>
 static int launch_schur_tc_persist_t(const DeviceLU &d, const Batch &b, int64_t ctas, int mode, int split_n, int split_i, int nonatomic,
                                      cudaStream_t s)
 {
-    constexpr int STAGES = S <= 7 ? 3 : 2;     // two CTAs must share an SM's 227 KB
+    constexpr int STAGES = 4;
     using C = TileCfg<S, OZ_NT, STAGES>;
     static std::atomic<unsigned long long> attr{0};
-    ensure_dyn_smem(schur_kernel_tc_persist<S, OZ_NT, STAGES>, (int)(C::SMEM + 16), attr);
+    ensure_dyn_smem(schur_kernel_tc_persist<S, OZ_NT, STAGES>, (int)C::SMEM, attr);
     static int nsm = 0, tmax = 0;
     if (!nsm) {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
-        if (nsm <= 0) nsm = 148;
+        if (nsm <= 0) nsm = 132;
         tmax = getenv("SLU_B200_TC_TILES_PER_CTA") ? std::max(1, atoi(getenv("SLU_B200_TC_TILES_PER_CTA"))) : 16;
     }
     const long long mine = (ctas + split_n - 1) / split_n;
-    // enough CTAs for ~4 waves over 2 x #SMs slots, at most tmax tiles each
+    // enough CTAs for ~8 waves over #SMs slots, at most tmax tiles each
     const int per = (int)std::max<long long>(1, std::min<long long>(tmax, mine / (8LL * nsm)));
     const long long grid = (mine + per - 1) / per;
-    schur_kernel_tc_persist<S, OZ_NT, STAGES><<<(unsigned)grid, 192, C::SMEM + 16, s>>>(d, b, mode, split_n, split_i, nonatomic, per, mine);
+    schur_kernel_tc_persist<S, OZ_NT, STAGES><<<(unsigned)grid, THREADS, C::SMEM, s>>>(d, b, mode, split_n, split_i, nonatomic, per, mine);
     return 1;
 }
 
@@ -899,19 +778,19 @@ static int launch_slice_t(const DeviceLU &d, const int32_t *nodes, int count, co
 template <int S>
 static int launch_schur_tc_t(const DeviceLU &d, const Batch &b, int64_t ctas, int mode, int split_n, int split_i, int nonatomic, cudaStream_t s)
 {
-    // two stages (a third did not help: r02_notes.md) so that two CTAs always share an SM
-    constexpr int CL = OZ_CL, STAGES = 2;
+    // one CTA per SM (the S * NT / 2 accumulator registers per consumer thread rule out two): a four-deep ring
+    constexpr int CL = OZ_CL, STAGES = 4;
     using C = TileCfg<S, OZ_NT, STAGES>;
     static std::atomic<unsigned long long> attr{0};
     ensure_dyn_smem(schur_kernel_tc<S, OZ_NT, STAGES, CL>, (int)C::SMEM, attr);
     const int64_t grid = (ctas + split_n - 1) / split_n * CL;
     if (CL == 1) {
-        schur_kernel_tc<S, OZ_NT, STAGES, CL><<<(unsigned)grid, 256, C::SMEM, s>>>(d, b, mode, split_n, split_i, nonatomic);
+        schur_kernel_tc<S, OZ_NT, STAGES, CL><<<(unsigned)grid, THREADS, C::SMEM, s>>>(d, b, mode, split_n, split_i, nonatomic);
     } else {
         DeviceLU dd = d;
         Batch bb = b;
         void *args[] = {&dd, &bb, &mode, &split_n, &split_i, &nonatomic};
-        launch_clustered(schur_kernel_tc<S, OZ_NT, STAGES, CL>, dim3((unsigned)grid), 256, C::SMEM, CL, s, args);
+        launch_clustered(schur_kernel_tc<S, OZ_NT, STAGES, CL>, dim3((unsigned)grid), THREADS, C::SMEM, CL, s, args);
     }
     return 1;
 }

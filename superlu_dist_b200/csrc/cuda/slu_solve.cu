@@ -208,7 +208,7 @@ int launch_solve_update(const DeviceLU &d, const Batch &b, int64_t ctas, bool up
 int launch_solve_mask(const DeviceLU &d, const int32_t *nodes, int count, double *x, int n, int nrhs, const double *src, cudaStream_t s)
 {
     if (count <= 0) return 0;
-    solve_mask_kernel<<<std::min(count, 148 * 8), 128, 0, s>>>(d, nodes, count, x, n, nrhs, src);
+    solve_mask_kernel<<<std::min(count, 132 * 8), 128, 0, s>>>(d, nodes, count, x, n, nrhs, src);
     return 1;
 }
 

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -23,7 +23,7 @@ def pytest_collection_modifyitems(config, items):
             return False
     gpu_items = [it for it in items if it.get_closest_marker("gpu")]
     if gpu_items and not have_gpu():
-        skip = pytest.mark.skip(reason="no CUDA device / libslu_b200.so: gpu tests need the B200 box")
+        skip = pytest.mark.skip(reason="no CUDA device / libslu_b200.so: gpu tests need an H100")
         for it in gpu_items:
             it.add_marker(skip)
 

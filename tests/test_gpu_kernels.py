@@ -1,5 +1,5 @@
 """Kernel-level parity through the C-ABI (include/slu_b200.h, slu_b200_k_*): each hand-written
-sm_100a kernel against a NumPy/SciPy restatement of the same BLAS-level operation the reference
+sm_90a kernel against a NumPy/SciPy restatement of the same BLAS-level operation the reference
 calls (dger-based LU pdgstrf2.c:508-601, dtrsm dtrfCommWrapper.c:166-219 / pdgstrf2.c:832, dgemm
 dscatter3d.c:143).  FP64 tolerance 1e-12 relative to the result's magnitude times the size."""
 import numpy as np

@@ -1,10 +1,10 @@
-"""The tcgen05 path (slu_ozaki.cu): int8-slice GEMM on tcgen05.mma.kind::i8 with TMEM accumulators.
+"""The int8 tensor-core path (slu_ozaki.cu): int8-slice GEMM on wgmma (s8 x s8 -> s32) with register accumulators.
 
 Tolerances.  With S slices an operand row is known to 2^-(7S-1) of ITS power-of-two scale 2^e (max|row| <= 2^e < 2 max|row|),
 and the S cross terms of weight 2^-(7S+5) per (s, t) pair with s + t = S are dropped, so for every element
     |(C - A B)_ij - exact| <= k * (S + 2) * 2^(4-7S) * rowmax_i * colmax_j        (worst case, any data)
 = k * 2.9e-11 (S = 6), 2.6e-13 (S = 7, the default), 2.2e-15 (S = 8) in units of rowmax * colmax.  Typical data sit one to two
-orders below (measured on a B200 with k = 256: 1.5e-13 / 1.3e-15 / 4e-17, profiles/r02_notes.md); the worst case is approached
+orders below; the worst case is approached
 only for k of a few (no averaging).  Inside the factorization the parity bar of the other tests applies unchanged: entry-wise
 1e-10 relative to max|factor| against the oracle, residual probe <= 1e-12."""
 import os
@@ -67,7 +67,7 @@ _K3, _K4 = dict(N=8, leaf=4, relax=8, maxsup=200, fem=3), dict(N=20, leaf=32, re
 
 @pytest.mark.parametrize("kw,slices", [(_K1, 7), (_K2, 7), (_K3, 7), (_K4, 7), (_K2, 6), (_K2, 8), (_K4, 8)])
 def test_factorization_through_tcgen05(kw, slices):
-    """Whole pdgstrf3d with the wide supernodes (>= 64 columns here) on the tcgen05 path against the oracle: same bar as
+    """Whole pdgstrf3d with the wide supernodes (>= 64 columns here) on the int8 tensor-core path against the oracle: same bar as
     the FP64 path.  maxsup = 400 exercises more than 8 k-steps (no int32 pair recombination)."""
     prob, _ = poisson_problem(**kw)
     chk, _ = poisson_problem(**kw)

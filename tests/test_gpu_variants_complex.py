@@ -1,7 +1,7 @@
 """Kernel variants and the doublecomplex path (pzgstrf3d_b200, SURVEY 8a row a15): gating.
 
 Round 1 wrote these pieces after its GPU minutes were spent and kept them xfail(strict=False); all seven XPASSED on
-the driver's B200 (GPUTEST_r01.json), so they gate now.  Each group still runs in a child process
+the GPU, so they gate now.  Each group still runs in a child process
 (tests/optin_worker.py): several of them select a kernel through an environment variable that the library reads once
 per process."""
 import os

@@ -1,6 +1,6 @@
 """Supernodes up to MAX_SUPER_SIZE = 512 columns (SRC/include/superlu_defs.h:154; sp_ienv(3) may be raised to it by the
 caller through SUPERLU_MAXSUP): panel solves with 32-vector strips above 416 columns, the one-CTA diagonal LU, the FP64
-DMMA and the tcgen05 Schur paths with k up to 512, and the resident solve -- kernel level against SciPy, whole
+DMMA and the int8 tensor-core Schur paths with k up to 512, and the resident solve -- kernel level against SciPy, whole
 factorization against the oracle (same tolerances as test_gpu_kernels.py / test_gpu_parity.py)."""
 import numpy as np
 import pytest
@@ -57,7 +57,7 @@ _W2 = dict(N=24, leaf=32, relax=64, maxsup=512)          # 576-column top separa
 
 @pytest.mark.parametrize("kw,tc_slices", [(_W1, -1), (_W1, 7), (_W2, -1), (_W2, 7)])
 def test_factorization_with_wide_supernodes(kw, tc_slices):
-    """tc_slices = -1: FP64 DMMA Schur only; 7: the tcgen05 path (16 k-steps at 512 columns)."""
+    """tc_slices = -1: FP64 DMMA Schur only; 7: the int8 tensor-core path (16 k-steps at 512 columns)."""
     prob, _ = poisson_problem(**kw)
     chk, _ = poisson_problem(**kw)
     assert np.diff(np.asarray(prob.xsup)).max() == 512
