@@ -209,14 +209,21 @@ int slu_b200_k_rerun_schur(slu_b200_handle_t h, int level, int reps, float *ms);
  * only to keep one struct; n, nsupr, lda ... count complex elements.  Supernodes up to 256 columns.
  * stats.ops_fact follows the reference's own complex accounting (pzgstrf2.c:578,590 for the diagonal blocks,
  * the precision-independent 2*m*n*k for the Schur update, sec_structs.c:692-693).
+ * slu_b200_z_fill_csr and slu_b200_z_solve follow the same convention: val and x point at interleaved
+ * doublecomplex, and n, ldx, nnz count complex elements.  The solve (the role of pzgstrs3d,
+ * SRC/complex16/pzgstrs3d.c) has the restrictions of slu_b200_solve.
  * Checked on an H100 by tests/test_gpu_variants_complex.py: kernels vs NumPy, cg20 vs the reference's pzgstrf3d
- * factors, pzdrive3d drop-in. */
+ * factors, pzdrive3d drop-in; and by tests/test_gpu_solve_complex.py: solves on the resident factors, device-side
+ * distribution. */
 typedef struct slu_b200_zhandle_s *slu_b200_zhandle_t;
 int slu_b200_z_create(slu_b200_zhandle_t *h, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt);
 int slu_b200_z_upload(slu_b200_zhandle_t h);
 int slu_b200_z_factor(slu_b200_zhandle_t h, int *info);
 int slu_b200_z_factor_host(slu_b200_zhandle_t h, int *info);
 int slu_b200_z_download(slu_b200_zhandle_t h);
+int slu_b200_z_fill_csr(slu_b200_zhandle_t h, int n, const int32_t *rowptr, const int32_t *colind, const double *val,
+                        const int32_t *perm);
+int slu_b200_z_solve(slu_b200_zhandle_t h, double *x, int ldx, int nrhs);
 int slu_b200_z_get_stats(slu_b200_zhandle_t h, slu_b200_stats_t *out);
 int slu_b200_z_plan(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, slu_b200_stats_t *stats);
 void slu_b200_z_destroy(slu_b200_zhandle_t h);

@@ -15,35 +15,12 @@
 #define SLU_COMPLEX 1
 #include "slu_device.cuh"
 #include "slu_kernels_common.cuh"
+#include "slu_scalar.cuh"   // zd, zmul, zsubmul, zrecip ...
 
 #include <climits>
 
 namespace sluz {
 
-typedef double2 zd;
-__device__ __forceinline__ zd zmake(double r, double i) { return make_double2(r, i); }
-__device__ __forceinline__ zd zmul(zd a, zd b) { return zmake(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
-__device__ __forceinline__ void zsubmul(zd &acc, zd a, zd b)  // acc -= a * b
-{
-    acc.x -= a.x * b.x - a.y * b.y;
-    acc.y -= a.x * b.y + a.y * b.x;
-}
-__device__ __forceinline__ void zaddmul(zd &acc, zd a, zd b)  // acc += a * b
-{
-    acc.x += a.x * b.x - a.y * b.y;
-    acc.y += a.x * b.y + a.y * b.x;
-}
-__device__ __forceinline__ bool zzero(zd a) { return a.x == 0.0 && a.y == 0.0; }
-// 1 / a by Smith's scaling (no overflow of |a|^2); the reference's slud_z_div(&t, &one, &a), dcomplex.c
-__device__ __forceinline__ zd zrecip(zd a)
-{
-    if (fabs(a.x) >= fabs(a.y)) {
-        const double r = a.y / a.x, den = a.x + a.y * r;
-        return zmake(1.0 / den, -r / den);
-    }
-    const double r = a.x / a.y, den = a.y + a.x * r;
-    return zmake(r / den, -1.0 / den);
-}
 __device__ __forceinline__ void cp_async16(void *smem, const void *gmem, bool pred)
 {
     unsigned sa = (unsigned)__cvta_generic_to_shared(smem);
