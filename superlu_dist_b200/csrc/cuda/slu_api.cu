@@ -264,6 +264,12 @@ struct slu_b200_handle_s {
     std::vector<void *> gcomm;            // [zl] communicator of my Z group at level zl (2^zl ranks)
     slu_b200_stats_t st{};
     bool uploaded = false;
+    // batched handle (slu_b200_batch_create): `batch` members of one pattern share everything above except the value
+    // arena, d_inv and the info flags, which hold `batch` consecutive copies
+    int batch = 0;                        // 0: an ordinary handle
+    int64_t member_len = 0, inv_len = 0;  // elements of one member's arena / diag-inverse workspace
+    BatchedLU bdev{};
+    std::vector<int> member_info;         // info of every member after the last slu_b200_batch_factor
 };
 
 namespace {
@@ -745,7 +751,9 @@ int analyze(slu_b200_handle_s *H)
         }
     }
     // upload the index structures
-    if (H->val.alloc((size_t)voff)) return -1;
+    const int members = std::max(1, H->batch);
+    H->member_len = voff; H->inv_len = ws_inv_max;
+    if (H->val.alloc((size_t)voff * members)) return -1;
     if (H->d_nodes.upload(H->nodes) || H->d_xsup.upload(H->xsup) || H->d_supno.upload(supno) ||
         H->d_lrows.upload(lrows) || H->d_lsrow.upload(lsrow) || H->d_lspos.upload(lspos) ||
         H->d_ucols.upload(ucols) || H->d_ufst.upload(ufst) || H->d_useg.upload(useg) ||
@@ -753,8 +761,8 @@ int analyze(slu_b200_handle_s *H)
         H->d_pool_i64.upload(pool_i64))
         return -1;
     if (H->d_rowinfo.alloc((size_t)ws_row_max * 2) || H->d_colinfo.alloc((size_t)ws_col_max * 2) ||
-        H->d_lrel.alloc((size_t)ws_lrel_max * 2) || H->d_urel.alloc((size_t)ws_urel_max * 2) || H->d_flags.alloc(2) ||
-        H->d_inv.alloc((size_t)ws_inv_max) ||
+        H->d_lrel.alloc((size_t)ws_lrel_max * 2) || H->d_urel.alloc((size_t)ws_urel_max * 2) || H->d_flags.alloc((size_t)members + 1) ||
+        H->d_inv.alloc((size_t)ws_inv_max * members) ||
         H->d_tiny.alloc(1))
         return -1;
     if (ws_oz_i8_max > 0 &&
@@ -774,7 +782,7 @@ int analyze(slu_b200_handle_s *H)
     d.ucols = H->d_ucols.p; d.ufst = H->d_ufst.p; d.useg = H->d_useg.p;
     d.lblk = H->d_lblk.p; d.ublk = H->d_ublk.p; d.rowinfo = H->d_rowinfo.p; d.colinfo = H->d_colinfo.p;
     d.oz_i8 = H->d_oz_i8.p; d.oz_scale = H->d_oz_scale.p; d.oz_rexp = H->d_oz_rexp.p;
-    d.lrel = H->d_lrel.p; d.urel = H->d_urel.p; d.info = H->d_flags.p; d.err = H->d_flags.p + 1; d.tiny = H->d_tiny.p;
+    d.lrel = H->d_lrel.p; d.urel = H->d_urel.p; d.info = H->d_flags.p; d.err = H->d_flags.p + members; d.tiny = H->d_tiny.p;
 
     slu_b200_stats_t &st = H->st;
     st.ops_fact = ops; st.ops_schur = ops_schur; st.schur_bytes = bytes_schur;
@@ -981,7 +989,7 @@ int transfer_2d(slu_b200_handle_s *H, bool to_device)
 
 // copy a list of (device offset, host pointer, length) runs, merging neighbours
 struct Run { int64_t dev; val_t *host; int64_t len; };
-int copy_runs(slu_b200_handle_s *H, std::vector<Run> &runs, bool to_device)
+int copy_runs(slu_b200_handle_s *H, std::vector<Run> &runs, bool to_device, val_t *arena)
 {
     size_t i = 0;
     while (i < runs.size()) {
@@ -989,8 +997,8 @@ int copy_runs(slu_b200_handle_s *H, std::vector<Run> &runs, bool to_device)
         size_t j = i + 1;
         while (j < runs.size() && runs[j].dev == r.dev + r.len && runs[j].host == r.host + r.len) { r.len += runs[j].len; ++j; }
         if (r.len > 0) {
-            if (to_device) CU(cudaMemcpyAsync(H->val.p + r.dev, r.host, (size_t)r.len * sizeof(val_t), cudaMemcpyHostToDevice, H->stream));
-            else CU(cudaMemcpyAsync(r.host, H->val.p + r.dev, (size_t)r.len * sizeof(val_t), cudaMemcpyDeviceToHost, H->stream));
+            if (to_device) CU(cudaMemcpyAsync(arena + r.dev, r.host, (size_t)r.len * sizeof(val_t), cudaMemcpyHostToDevice, H->stream));
+            else CU(cudaMemcpyAsync(r.host, arena + r.dev, (size_t)r.len * sizeof(val_t), cudaMemcpyDeviceToHost, H->stream));
         }
         i = j;
     }
@@ -998,8 +1006,10 @@ int copy_runs(slu_b200_handle_s *H, std::vector<Run> &runs, bool to_device)
 }
 
 // skyline <-> dense-packed conversion of the U panels that are not already identical
-int convert_u(slu_b200_handle_s *H, bool to_device)
+int convert_u(slu_b200_handle_s *H, bool to_device, val_t *arena)
 {
+    DeviceLU d = H->dev;
+    d.val = arena;
     const size_t STAGE = (size_t)32 << 20;  // elements (256 MB of doubles) per round
     std::vector<int32_t> pend;
     for (auto &zn : H->znodes)
@@ -1031,9 +1041,9 @@ int convert_u(slu_b200_handle_s *H, bool to_device)
             for (size_t t = 0; t < nodes.size(); ++t)
                 CU(cudaMemcpyAsync(H->stage.p + soff[t], H->view.Unzval_br_ptr[nodes[t]], (size_t)H->sky_len[nodes[t]] * sizeof(val_t),
                                    cudaMemcpyHostToDevice, H->stream));
-            launch_u_convert(H->dev, b, prefix.back(), 0, H->stage.p, ds.p, H->stream);
+            launch_u_convert(d, b, prefix.back(), 0, H->stage.p, ds.p, H->stream);
         } else {
-            launch_u_convert(H->dev, b, prefix.back(), 1, H->stage.p, ds.p, H->stream);
+            launch_u_convert(d, b, prefix.back(), 1, H->stage.p, ds.p, H->stream);
             for (size_t t = 0; t < nodes.size(); ++t)
                 CU(cudaMemcpyAsync(H->view.Unzval_br_ptr[nodes[t]], H->stage.p + soff[t], (size_t)H->sky_len[nodes[t]] * sizeof(val_t),
                                    cudaMemcpyDeviceToHost, H->stream));
@@ -1045,9 +1055,11 @@ int convert_u(slu_b200_handle_s *H, bool to_device)
     return 0;
 }
 
-int transfer(slu_b200_handle_s *H, bool to_device)
+// member: which value arena of a batched handle (0 for an ordinary one)
+int transfer(slu_b200_handle_s *H, bool to_device, int member = 0)
 {
     if (H->P2 > 1) return transfer_2d(H, to_device);
+    val_t *arena = H->val.p + (int64_t)member * H->member_len;
     std::vector<Run> runs;
     for (auto &zn : H->znodes) {
         for (int k : zn) {
@@ -1061,8 +1073,8 @@ int transfer(slu_b200_handle_s *H, bool to_device)
     }
     for (auto &r : runs)
         if (r.len > 0 && !r.host) return fail("a held panel has a NULL value pointer");
-    if (copy_runs(H, runs, to_device)) return -1;
-    if (convert_u(H, to_device)) return -1;
+    if (copy_runs(H, runs, to_device, arena)) return -1;
+    if (convert_u(H, to_device, arena)) return -1;
     CU(cudaStreamSynchronize(H->stream));
     return 0;
 }
@@ -1233,6 +1245,12 @@ int upload_pipe_issue(slu_b200_handle_s *H)
     return 0;
 }
 
+// a batched handle (slu_b200_batch_create) only takes the slu_b200_batch_* calls, get_stats and destroy
+int refuse_batched(const slu_b200_handle_s *H, const char *fn)
+{
+    return H->batch ? fail("%s on a batched handle (%d members): use the slu_b200_batch_* calls", fn, H->batch) : 0;
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -1317,7 +1335,8 @@ void slu_b200_destroy(slu_b200_handle_t H)
     delete H;
 }
 
-int slu_b200_create(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt)
+// batch > 0: a batched handle (slu_b200_batch_create), 1 x 1 x 1 grid, FP64 DMMA kernels only
+static int create_impl(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, int batch)
 {
     if (!out || !lu || !opt) return fail("null argument");
     *out = nullptr;
@@ -1326,6 +1345,13 @@ int slu_b200_create(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, const 
     slu_b200_handle_s *H = new slu_b200_handle_s;
     H->view = *lu;
     H->opt = *opt;
+    H->batch = batch;
+    if (batch) {             // the int8 path and the opt-in Schur variants are not batched
+        H->opt.schur_variant = 0;
+        H->opt.reserved[3] = 0;
+        H->opt.reserved[4] = -1;
+        H->tc_force_off = true;
+    }
     H->coop = opt->world_size > 1 && !opt->reserved[1];
     H->P2 = lu->nprow * lu->npcol;
     double t0 = now_s();
@@ -1377,6 +1403,16 @@ int slu_b200_create(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, const 
         if (analyze(H)) { slu_b200_destroy(H); return -1; }
     }
     if (build_pieces(H)) { slu_b200_destroy(H); return -1; }
+    if (batch) {             // the stats describe the whole handle: every member's work
+        slu_b200_stats_t &st = H->st;
+        st.ops_fact *= batch; st.ops_schur *= batch; st.schur_bytes *= batch;
+        st.nnz_l *= batch; st.nnz_u *= batch;
+        static_cast<DeviceLU &>(H->bdev) = H->dev;
+        H->bdev.val_stride = H->member_len;
+        H->bdev.inv_stride = H->inv_len;
+        H->bdev.members = batch;
+        H->member_info.assign(batch, -1);
+    }
     {
         int lo = 0, hi = 0;
         cudaDeviceGetStreamPriorityRange(&lo, &hi);  // hi = numerically lowest = highest priority
@@ -1399,9 +1435,15 @@ int slu_b200_create(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, const 
     return 0;
 }
 
+int slu_b200_create(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt)
+{
+    return create_impl(out, lu, opt, 0);
+}
+
 int slu_b200_upload(slu_b200_handle_t H)
 {
     if (!H) return fail("null handle");
+    if (refuse_batched(H, "slu_b200_upload")) return -1;
     double t0 = now_s();
     H->factored = false;
     if (transfer(H, true)) return -1;
@@ -1413,6 +1455,7 @@ int slu_b200_upload(slu_b200_handle_t H)
 int slu_b200_download(slu_b200_handle_t H)
 {
     if (!H) return fail("null handle");
+    if (refuse_batched(H, "slu_b200_download")) return -1;
     double t0 = now_s();
     if (transfer(H, false)) return -1;
     H->st.t_download_s = now_s() - t0;
@@ -1422,6 +1465,7 @@ int slu_b200_download(slu_b200_handle_t H)
 static int factor_impl(slu_b200_handle_t H, int *info, bool pipelined, bool up_pipe = false)
 {
     if (!H || !info) return fail("null argument");
+    if (refuse_batched(H, "slu_b200_factor")) return -1;
     if (!H->uploaded) return fail("slu_b200_factor before slu_b200_upload");
     if (pipelined && pipe_prepare(H)) return -1;
     cudaStream_t s = H->stream;
@@ -1566,6 +1610,7 @@ int slu_b200_factor(slu_b200_handle_t H, int *info) { return factor_impl(H, info
 int slu_b200_factor_host(slu_b200_handle_t H, int *info)
 {
     if (!H || !info) return fail("null argument");
+    if (refuse_batched(H, "slu_b200_factor_host")) return -1;
     // The overlapped transfers move whole panels between the caller's arrays and the arena, which needs the U
     // skylines to equal their dense-packed form (symmetric patterns) and 1 x 1 x Pz pieces.  Anything else -- the
     // unsymmetric patterns SuperLU exists for, Pr x Pc pieces -- takes the plain path: upload (with the skyline
@@ -1602,6 +1647,7 @@ int slu_b200_factor_host(slu_b200_handle_t H, int *info)
 int slu_b200_fill_csr(slu_b200_handle_t H, int n, const int32_t *rowptr, const int32_t *colind, const double *val, const int32_t *perm)
 {
     if (!H || !rowptr || !colind || !val || !perm) return fail("null argument");
+    if (refuse_batched(H, "slu_b200_fill_csr")) return -1;
     if (n != H->n) return fail("matrix order %d does not match the handle's %d", n, H->n);
     if (H->P2 > 1) return fail("slu_b200_fill_csr handles 1 x 1 x Pz grids");
     double t0 = now_s();
@@ -1643,6 +1689,7 @@ int slu_b200_fill_csr(slu_b200_handle_t H, int n, const int32_t *rowptr, const i
 int slu_b200_solve(slu_b200_handle_t H, double *xh, int ldx, int nrhs)
 {
     if (!H || !xh) return fail("null argument");
+    if (refuse_batched(H, "slu_b200_solve")) return -1;
     if (!H->factored) return fail("slu_b200_solve needs a successful slu_b200_factor on this handle first");
     if (nrhs < 1 || ldx < H->n) return fail("bad nrhs / ldx");
     if (H->P2 > 1) return fail("slu_b200_solve: Pr x Pc > 1 is not supported yet (1 x 1 x Pz only)");
@@ -1727,6 +1774,7 @@ int slu_b200_solve(slu_b200_handle_t H, double *xh, int ldx, int nrhs)
 int slu_b200_k_level_export(slu_b200_handle_t H, int level, void *device_lu, int device_lu_bytes, int32_t *nodes, int max_nodes)
 {
     if (!H || level < 0 || level >= (int)H->levels.size()) return fail("bad handle / level");
+    if (refuse_batched(H, "slu_b200_k_level_export")) return -1;
     if (device_lu && device_lu_bytes == (int)sizeof(DeviceLU)) memcpy(device_lu, &H->dev, sizeof(DeviceLU));
     else if (device_lu) return fail("DeviceLU is %d bytes", (int)sizeof(DeviceLU));
     const LevelPlan &L = H->levels[level];
@@ -1744,6 +1792,7 @@ int slu_b200_k_level_export(slu_b200_handle_t H, int level, void *device_lu, int
 int slu_b200_k_rerun_schur(slu_b200_handle_t H, int level, int reps, float *ms)
 {
     if (!H || level < 0 || level >= (int)H->levels.size() || reps < 1 || !ms) return fail("bad argument");
+    if (refuse_batched(H, "slu_b200_k_rerun_schur")) return -1;
     const LevelPlan &L = H->levels[level];
     cudaStream_t s = H->stream;
     const DeviceLU &d = H->dev;
@@ -1766,6 +1815,183 @@ int slu_b200_k_rerun_schur(slu_b200_handle_t H, int level, int reps, float *ms)
     float t = 0;
     CU(cudaEventElapsedTime(&t, ev[0], ev[1]));
     *ms = t / reps;
+    return 0;
+}
+
+// ---- batched handles: many matrices of one sparsity pattern (pdgssvx3d_csc_batch, SRC/double/pdgssvx3d_csc_batch.c:81;
+// dsparseTreeFactorBatchGPU, SRC/CplusplusFactor/batch_factorize.cu:801) ------------------------------------------------
+// Everything the analysis builds is value-independent and shared by the members: the level plan and CTA prefixes, NodeDesc,
+// the LBlk/UBlk tables, the look-ahead split and the RowInfo/ColInfo/lrel/urel maps (built once per level by
+// schur_setup_kernel).  Each member has its own value arena, d_inv slice and info flag; every batched launch is the
+// unbatched one with gridDim.y = members, so a batched factorization takes exactly as many launches as one matrix.
+static int refuse_unbatched(const slu_b200_handle_s *H, const char *fn)
+{
+    return H->batch ? 0 : fail("%s on an unbatched handle: use the slu_b200_* calls without _batch", fn);
+}
+
+int slu_b200_batch_create(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, int batch)
+{
+    if (!out || !lu || !opt) return fail("null argument");
+    *out = nullptr;
+    if (batch < 1 || batch > 65535) return fail("slu_b200_batch_create: batch = %d, must be 1 ... 65535", batch);
+    if (lu->nprow != 1 || lu->npcol != 1 || lu->npdep != 1)
+        return fail("slu_b200_batch_create: batched handles need a 1 x 1 x 1 grid (got %d x %d x %d)", lu->nprow, lu->npcol, lu->npdep);
+    if (opt->world_size > 1) return fail("slu_b200_batch_create: batched handles are single-GPU (world_size = %d)", opt->world_size);
+    return create_impl(out, lu, opt, batch);
+}
+
+// rowptr / colind / perm as slu_b200_fill_csr, shared by the members; val = batch x nnz values, member-major
+int slu_b200_batch_fill_csr(slu_b200_handle_t H, int n, const int32_t *rowptr, const int32_t *colind, const double *val,
+                            const int32_t *perm)
+{
+    if (!H || !rowptr || !colind || !val || !perm) return fail("null argument");
+    if (refuse_unbatched(H, "slu_b200_batch_fill_csr")) return -1;
+    if (n != H->n) return fail("matrix order %d does not match the handle's %d", n, H->n);
+    double t0 = now_s();
+    const int B = H->batch;
+    const int64_t nnz = rowptr[n];
+    DevBuf<int32_t> drp, dci, dperm;
+    DevBuf<val_t> dv;
+    DevBuf<int8_t> dact;
+    std::vector<int8_t> act(H->nsupers, 0);
+    for (int k : H->znodes[0]) act[k] = 1;
+    if (drp.alloc((size_t)n + 1) || dci.alloc((size_t)nnz) || dv.alloc((size_t)nnz * B) || dperm.alloc((size_t)n) || dact.upload(act)) return -1;
+    cudaStream_t s = H->stream;
+    int *err = H->d_flags.p + B;
+    CU(cudaMemcpyAsync(drp.p, rowptr, ((size_t)n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(dci.p, colind, (size_t)nnz * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(dv.p, val, (size_t)nnz * B * sizeof(val_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(dperm.p, perm, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemsetAsync(H->val.p, 0, H->val.bytes(), s));
+    CU(cudaMemsetAsync(err, 0, sizeof(int), s));
+    launch_fill_csr(H->bdev, n, drp.p, dci.p, dv.p, dperm.p, dact.p, err, s);
+    int bad = 0;
+    CU(cudaMemcpyAsync(&bad, err, sizeof(int), cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    if (bad) return fail("%d entries of the members have no slot in the L/U structure (wrong permutation or symbolic structure)", bad);
+    H->st.t_upload_s = now_s() - t0;
+    H->uploaded = true;
+    H->member_info.assign(B, -1);
+    return 0;
+}
+
+// factor_impl's level loop on a 1 x 1 x 1 grid, every launch over all members (look-ahead streams and events as there:
+// the members advance in lockstep).  The destination maps are value-independent: one schur_setup launch per level.
+int slu_b200_batch_factor(slu_b200_handle_t H, int *info)
+{
+    if (!H || !info) return fail("null argument");
+    if (refuse_unbatched(H, "slu_b200_batch_factor")) return -1;
+    if (!H->uploaded) return fail("slu_b200_batch_factor before slu_b200_batch_fill_csr");
+    const int B = H->batch;
+    cudaStream_t s = H->stream, s2 = H->stream2;
+    const BatchedLU &d = H->bdev;
+    std::vector<int> flags(B + 1, INT_MAX);
+    flags[B] = 0;
+    CU(cudaMemcpyAsync(H->d_flags.p, flags.data(), flags.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    CU(cudaMemsetAsync(H->d_tiny.p, 0, sizeof(unsigned long long), s));
+    CU(cudaStreamSynchronize(s));   // `flags` is pageable host memory reused below
+    int64_t launches = 0;
+    const bool lookahead = !H->opt.reserved[0];
+    const int replace_tiny = H->opt.replace_tiny_pivot ? 1 : 0;
+    const int64_t *p64 = H->d_pool_i64.p;
+    CU(cudaEventRecord(H->ev0, s));
+    for (size_t li = 0; li < H->levels.size(); ++li) {
+        const LevelPlan &L = H->levels[li];
+        const int32_t *nodes = H->d_pool_i32.p + L.nodes_off, *bign = H->d_pool_i32.p + L.big_nodes;
+        const Batch small{H->d_pool_i32.p + L.small_nodes, p64 + L.small_prefix, L.small_count};
+        if (lookahead && li >= 2) CU(cudaStreamWaitEvent(s, H->ev_bulk[li - 2], 0));
+        launches += launch_diag_lu(d, Batch{nodes, p64 + L.trsml_prefix, L.count}, L.max_ns, replace_tiny, H->opt.thresh, s);
+        launches += launch_diag_inv(d, Batch{nodes, p64 + L.inv_prefix, L.count}, L.inv_ctas, H->d_inv.p, s);
+        launches += launch_trsm_l(d, Batch{nodes, p64 + L.trsml_prefix, L.count}, L.trsml_ctas, L.max_ns, H->d_inv.p, s);
+        launches += launch_trsm_u(d, Batch{nodes, p64 + L.trsmu_prefix, L.count}, L.trsmu_ctas, L.max_ns, H->d_inv.p, s);
+        launches += launch_schur_setup(H->dev, Batch{nodes, p64 + L.setup_prefix, L.count}, L.setup_ctas, s);
+        if (lookahead) {
+            CU(cudaEventRecord(H->ev_panel[li], s));
+            launches += launch_schur(d, Batch{bign, p64 + L.urg_prefix, L.big_count}, L.urg_ctas, 1, 1, s);
+            launches += launch_schur(d, small, L.small_ctas, 0, 0, s);
+            CU(cudaStreamWaitEvent(s2, H->ev_panel[li], 0));
+            launches += launch_schur(d, Batch{bign, p64 + L.bulk_prefix, L.big_count}, L.bulk_ctas, 1, 2, s2);
+            CU(cudaEventRecord(H->ev_bulk[li], s2));
+        } else {
+            launches += launch_schur(d, Batch{bign, p64 + L.big_prefix, L.big_count}, L.big_ctas, 1, 0, s);
+            launches += launch_schur(d, small, L.small_ctas, 0, 0, s);
+        }
+    }
+    const size_t nl = H->levels.size();
+    if (lookahead && nl > 0) {
+        CU(cudaStreamWaitEvent(s, H->ev_bulk[nl - 1], 0));
+        if (nl > 1) CU(cudaStreamWaitEvent(s, H->ev_bulk[nl - 2], 0));
+    }
+    CU(cudaEventRecord(H->ev1, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    float ms = 0;
+    CU(cudaEventElapsedTime(&ms, H->ev0, H->ev1));
+    H->st.t_factor_s = ms * 1e-3;
+    H->st.gpu_launches = launches;
+    unsigned long long tiny = 0;
+    CU(cudaMemcpy(flags.data(), H->d_flags.p, flags.size() * sizeof(int), cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(&tiny, H->d_tiny.p, sizeof tiny, cudaMemcpyDeviceToHost));
+    H->st.tiny_pivots = (int64_t)tiny;   // summed over the members
+    if (flags[B]) return fail("%d Schur-update destinations were not found in the L/U structure", flags[B]);
+    for (int j = 0; j < B; ++j) info[j] = H->member_info[j] = flags[j] == INT_MAX ? 0 : flags[j];
+    return 0;
+}
+
+// x: batch blocks, block j at x + j * ldx * nrhs, each n x nrhs column-major (ldx >= n): b on entry, the solution on return
+int slu_b200_batch_solve(slu_b200_handle_t H, double *xh, int ldx, int nrhs)
+{
+    if (!H || !xh) return fail("null argument");
+    if (refuse_unbatched(H, "slu_b200_batch_solve")) return -1;
+    const int B = H->batch, n = H->n;
+    for (int j = 0; j < B; ++j) {
+        if (H->member_info[j] < 0) return fail("slu_b200_batch_solve needs a slu_b200_batch_factor of the filled members first");
+        if (H->member_info[j] > 0) return fail("slu_b200_batch_solve: member %d has an exact zero pivot in column %d", j, H->member_info[j]);
+    }
+    if (nrhs < 1 || ldx < n) return fail("bad nrhs / ldx");
+    if ((int64_t)n * nrhs > INT_MAX) return fail("slu_b200_batch_solve: n * nrhs must stay below 2^31 per member");
+    const size_t len = (size_t)n * nrhs * B;
+    if (H->d_x.n < len && H->d_x.alloc(len)) return -1;
+    cudaStream_t s = H->stream;
+    const BatchedLU &d = H->bdev;
+    val_t *x = H->d_x.p;
+    double t0 = now_s();
+    // the B blocks are B * nrhs columns at pitch ldx: one 2D copy each way
+    CU(cudaMemcpy2DAsync(x, (size_t)n * sizeof(val_t), xh, (size_t)ldx * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs * B,
+                         cudaMemcpyHostToDevice, s));
+    const int64_t *p64 = H->d_pool_i64.p;
+    int launches = 0;
+    for (size_t li = 0; li < H->levels.size(); ++li) {          // forward: L y = b
+        const LevelPlan &L = H->levels[li];
+        const int32_t *nodes = H->d_pool_i32.p + L.nodes_off;
+        launches += launch_solve_diag(d, nodes, L.count, false, x, n, nrhs, s);
+        launches += launch_solve_update(d, Batch{nodes, p64 + L.sl_prefix, L.count}, L.sl_ctas, false, x, n, nrhs, s);
+    }
+    for (size_t li = H->levels.size(); li-- > 0;) {             // backward: U x = y
+        const LevelPlan &L = H->levels[li];
+        const int32_t *nodes = H->d_pool_i32.p + L.nodes_off;
+        launches += launch_solve_update(d, Batch{nodes, p64 + L.su_prefix, L.count}, L.su_ctas, true, x, n, nrhs, s);
+        launches += launch_solve_diag(d, nodes, L.count, true, x, n, nrhs, s);
+    }
+    CU(cudaMemcpy2DAsync(xh, (size_t)ldx * sizeof(val_t), x, (size_t)n * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs * B,
+                         cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    H->st.reserved[4] = now_s() - t0;
+    H->st.reserved[5] = (double)launches;
+    return 0;
+}
+
+// D2H of member `member`'s L and U into the view's Lnzval / Unzval, as slu_b200_download
+int slu_b200_batch_download(slu_b200_handle_t H, int member)
+{
+    if (!H) return fail("null handle");
+    if (refuse_unbatched(H, "slu_b200_batch_download")) return -1;
+    if (member < 0 || member >= H->batch) return fail("slu_b200_batch_download: member %d out of range (batch of %d)", member, H->batch);
+    double t0 = now_s();
+    if (transfer(H, false, member)) return -1;
+    H->st.t_download_s = now_s() - t0;
     return 0;
 }
 #endif

@@ -97,6 +97,15 @@ struct DeviceLU {            // everything the kernels need, passed by value
     int *err;                // debug: count of destination lookups that failed
 };
 
+// Several matrices of one sparsity pattern factored together (slu_b200_batch_*): every structure-only object of
+// DeviceLU is shared, each member has its own value arena, diag-inverse workspace and info flag.  A batched launch
+// has the grid of the unbatched one in x and the member in blockIdx.y (member_view, slu_kernels_common.cuh).
+struct BatchedLU : DeviceLU {
+    int64_t val_stride;      // elements between the value arenas of two members (val = member 0)
+    int64_t inv_stride;      // elements between their diag-inverse workspaces
+    int32_t members, pad;    // info = [members] flags
+};
+
 struct Batch {               // one kernel launch over several supernodes
     const int32_t *nodes;    // supernode ids
     const int64_t *prefix;   // [count+1] cumulative CTA counts
@@ -158,6 +167,21 @@ int launch_solve_mask(const DeviceLU &d, const int32_t *nodes, int count, val_t 
 // device-side distribution of a CSR matrix (device arrays) into the arena; *err counts entries without a slot
 int launch_fill_csr(const DeviceLU &d, int n, const int32_t *rowptr, const int32_t *colind, const val_t *aval, const int32_t *perm,
                     const int8_t *active, int *err, cudaStream_t s);
+
+#ifndef SLU_COMPLEX
+// batched launches: the same kernels over d.members matrices of one pattern (gridDim.y = members).  dinv = member 0's
+// workspace; in the solve x holds the members' n x nrhs blocks back to back, in fill_csr aval their nnz values.
+// Always the FP64 DMMA path with the default tile shapes: the opt-in kernel variants are not batched.
+int launch_diag_lu(const BatchedLU &d, const Batch &b, int max_ns, int replace_tiny, double thresh, cudaStream_t s);
+int launch_diag_inv(const BatchedLU &d, const Batch &b, int64_t ctas, val_t *dinv, cudaStream_t s);
+int launch_trsm_l(const BatchedLU &d, const Batch &b, int64_t ctas, int max_ns, const val_t *dinv, cudaStream_t s);
+int launch_trsm_u(const BatchedLU &d, const Batch &b, int64_t ctas, int max_ns, const val_t *dinv, cudaStream_t s);
+int launch_schur(const BatchedLU &d, const Batch &b, int64_t ctas, int big, int mode, cudaStream_t s);
+int launch_solve_diag(const BatchedLU &d, const int32_t *nodes, int count, bool upper, val_t *x, int n, int nrhs, cudaStream_t s);
+int launch_solve_update(const BatchedLU &d, const Batch &b, int64_t ctas, bool upper, val_t *x, int n, int nrhs, cudaStream_t s);
+int launch_fill_csr(const BatchedLU &d, int n, const int32_t *rowptr, const int32_t *colind, const val_t *aval, const int32_t *perm,
+                    const int8_t *active, int *err, cudaStream_t s);
+#endif
 
 #ifndef SLU_COMPLEX
 // slu_ozaki.cu: the Schur update of wide supernodes on wgmma (int8 slices, exact int32 accumulation in registers)

@@ -18,15 +18,18 @@
 
 #include <climits>
 #include <cstdlib>
+#include <type_traits>
 
 namespace slu {
 
 // ------------------------------------------------------------------------------------------------
 // diagonal block LU: one CTA per supernode, right-looking with NB-wide panels in shared memory
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(512) diag_lu_kernel(DeviceLU d, Batch b, int replace_tiny, double thresh, int skip_lo, int skip_hi)
+template <class LU>
+__global__ void __launch_bounds__(512) diag_lu_kernel(LU dd, Batch b, int replace_tiny, double thresh, int skip_lo, int skip_hi)
 {
     extern __shared__ double sm[];
+    const DeviceLU &d = member_view(dd);
     constexpr int NB = DIAG_NB;
     const int k = b.nodes[blockIdx.x];
     const NodeDesc nd = d.nodes[k];
@@ -354,9 +357,11 @@ __device__ __forceinline__ unsigned cluster_rank()
     return r;
 }
 
-__global__ void __cluster_dims__(DC_CL, 1, 1) __launch_bounds__(256) diag_lu_cluster_kernel(DeviceLU d, Batch b, int replace_tiny, double thresh)
+template <class LU>
+__global__ void __cluster_dims__(DC_CL, 1, 1) __launch_bounds__(256) diag_lu_cluster_kernel(LU dd, Batch b, int replace_tiny, double thresh)
 {
     extern __shared__ double sm[];
+    const DeviceLU &d = member_view(dd);
     double *S = sm;                        // my slab      S[c * DC_LD + r], r < ns, c < 32
     double *P = S + DC_W * DC_LD;          // L panel      P[c * DC_LD + i], i < rem (rows relative to j0)
     double *urow = P + DC_W * DC_LD;       // pivot rows, double buffered: urow[buf * 40 + c], [buf * 40 + 32] = 1 / pivot
@@ -489,31 +494,42 @@ static bool diag_v3_enabled()
     return on != 0;
 }
 
-int launch_diag_lu(const DeviceLU &d, const Batch &b, int max_ns, int replace_tiny, double thresh,
-                   cudaStream_t s)
+template <class LU>
+static int launch_diag_lu_t(const LU &d, const Batch &b, int max_ns, int replace_tiny, double thresh, cudaStream_t s)
 {
     if (b.count <= 0) return 0;
+    constexpr bool batched = std::is_same<LU, BatchedLU>::value;   // the opt-in v3 kernel is not batched
     int launched = 0, skip_lo = 1, skip_hi = 0;    // empty range: the one-CTA kernel takes every supernode
     if (max_ns >= DC_MIN_NS && diag_cluster_enabled()) {
         static std::atomic<unsigned long long> attrc{0};
-        ensure_dyn_smem(diag_lu_cluster_kernel, (int)DC_SMEM, attrc);
-        diag_lu_cluster_kernel<<<b.count * DC_CL, 256, DC_SMEM, s>>>(d, b, replace_tiny, thresh);
+        ensure_dyn_smem(diag_lu_cluster_kernel<LU>, (int)DC_SMEM, attrc);
+        diag_lu_cluster_kernel<LU><<<member_grid(d, b.count * DC_CL), 256, DC_SMEM, s>>>(d, b, replace_tiny, thresh);
         skip_lo = DC_MIN_NS; skip_hi = DC_MAX_NS;
         ++launched;
         if (b.count == 1 && max_ns <= DC_MAX_NS) return launched;   // the single supernode of a chain level went to the cluster
     }
-    if (max_ns <= D3_MAX_NS && diag_v3_enabled()) {
-        static std::atomic<unsigned long long> attr3_0{0};
-        ensure_dyn_smem(diag_lu_kernel_v3, (int)D3_SMEM, attr3_0);
-        diag_lu_kernel_v3<<<b.count, 512, D3_SMEM, s>>>(d, b, replace_tiny, thresh, skip_lo, skip_hi);
-        return launched + 1;
+    if constexpr (!batched) {
+        if (max_ns <= D3_MAX_NS && diag_v3_enabled()) {
+            static std::atomic<unsigned long long> attr3_0{0};
+            ensure_dyn_smem(diag_lu_kernel_v3, (int)D3_SMEM, attr3_0);
+            diag_lu_kernel_v3<<<b.count, 512, D3_SMEM, s>>>(d, b, replace_tiny, thresh, skip_lo, skip_hi);
+            return launched + 1;
+        }
     }
     size_t smem = sizeof(double) * 2 * DIAG_NB * (size_t)max_ns;
     static std::atomic<unsigned long long> attr_0{0};
-    ensure_dyn_smem(diag_lu_kernel, (int)(sizeof(double) * 2 * DIAG_NB * MAX_NS), attr_0);
+    ensure_dyn_smem(diag_lu_kernel<LU>, (int)(sizeof(double) * 2 * DIAG_NB * MAX_NS), attr_0);
     int threads = max_ns <= 32 ? 128 : (max_ns <= 128 ? 256 : 512);
-    diag_lu_kernel<<<b.count, threads, smem, s>>>(d, b, replace_tiny, thresh, skip_lo, skip_hi);
+    diag_lu_kernel<LU><<<member_grid(d, b.count), threads, smem, s>>>(d, b, replace_tiny, thresh, skip_lo, skip_hi);
     return launched + 1;
+}
+int launch_diag_lu(const DeviceLU &d, const Batch &b, int max_ns, int replace_tiny, double thresh, cudaStream_t s)
+{
+    return launch_diag_lu_t(d, b, max_ns, replace_tiny, thresh, s);
+}
+int launch_diag_lu(const BatchedLU &d, const Batch &b, int max_ns, int replace_tiny, double thresh, cudaStream_t s)
+{
+    return launch_diag_lu_t(d, b, max_ns, replace_tiny, thresh, s);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -529,9 +545,12 @@ int launch_diag_lu(const DeviceLU &d, const Batch &b, int max_ns, int replace_ti
 // ------------------------------------------------------------------------------------------------
 constexpr int TRSM_LD = TRSM_STRIP + 4;
 
-__global__ void __launch_bounds__(64) diag_inv_kernel(DeviceLU d, Batch b, double *dinv)
+template <class LU>
+__global__ void __launch_bounds__(64) diag_inv_kernel(LU dd, Batch b, double *dinv)
 {
     __shared__ double M[16 * 17];
+    const DeviceLU &d = member_view(dd);
+    dinv = member_inv(dd, dinv);
     const int slot = find_slot(b.prefix, b.count, blockIdx.x);
     const int k = b.nodes[slot];
     const NodeDesc nd = d.nodes[k];
@@ -575,11 +594,20 @@ __global__ void __launch_bounds__(64) diag_inv_kernel(DeviceLU d, Batch b, doubl
     }
 }
 
-int launch_diag_inv(const DeviceLU &d, const Batch &b, int64_t ctas, double *dinv, cudaStream_t s)
+template <class LU>
+static int launch_diag_inv_t(const LU &d, const Batch &b, int64_t ctas, double *dinv, cudaStream_t s)
 {
     if (b.count <= 0 || ctas <= 0) return 0;
-    diag_inv_kernel<<<(unsigned)ctas, 64, 0, s>>>(d, b, dinv);
+    diag_inv_kernel<LU><<<member_grid(d, (unsigned)ctas), 64, 0, s>>>(d, b, dinv);
     return 1;
+}
+int launch_diag_inv(const DeviceLU &d, const Batch &b, int64_t ctas, double *dinv, cudaStream_t s)
+{
+    return launch_diag_inv_t(d, b, ctas, dinv, s);
+}
+int launch_diag_inv(const BatchedLU &d, const Batch &b, int64_t ctas, double *dinv, cudaStream_t s)
+{
+    return launch_diag_inv_t(d, b, ctas, dinv, s);
 }
 
 template <bool UCASE, bool STAGED, int STRIP>
@@ -698,10 +726,12 @@ __device__ __forceinline__ void trsm_body(const DeviceLU &d, const NodeDesc &nd,
 // Supernodes wider than TRSM_WIDE_NS (up to MAX_SUPER_SIZE = 512) take 32-vector strips (4 of the 8 warps sweep, the
 // strip is 144 KB instead of 272 KB); they only occur with superlu_maxsup raised above its default 256 and always run
 // the un-staged variant.  The CTA prefix of the batch is built with trsm_strip_of(ns) (slu_api.cu).
-template <bool UCASE, bool STAGED>
-__global__ void __launch_bounds__(256) trsm_kernel(DeviceLU d, Batch b, const double *dinv)
+template <bool UCASE, bool STAGED, class LU>
+__global__ void __launch_bounds__(256) trsm_kernel(LU dd, Batch b, const double *dinv)
 {
     extern __shared__ double Ys[];
+    const DeviceLU &d = member_view(dd);
+    dinv = member_inv(dd, dinv);
     const int slot = find_slot(b.prefix, b.count, blockIdx.x);
     const NodeDesc nd = d.nodes[b.nodes[slot]];
     const int strip = (int)(blockIdx.x - b.prefix[slot]);
@@ -839,24 +869,27 @@ static bool trsm_rl_enabled()
     return on != 0;
 }
 
-template <bool UCASE>
-static int launch_trsm(const DeviceLU &d, const Batch &b, int64_t ctas, int max_ns, const double *dinv, cudaStream_t s)
+template <bool UCASE, class LU>
+static int launch_trsm(const LU &d, const Batch &b, int64_t ctas, int max_ns, const double *dinv, cudaStream_t s)
 {
     if (b.count <= 0 || ctas <= 0) return 0;
-    if (max_ns <= 256 && trsm_rl_enabled()) {
-        trsm_rl_kernel<UCASE><<<(unsigned)ctas, 256, 0, s>>>(d, b, dinv);
-        return 1;
+    if constexpr (!std::is_same<LU, BatchedLU>::value) {   // the opt-in register-blocked kernel is not batched
+        if (max_ns <= 256 && trsm_rl_enabled()) {
+            trsm_rl_kernel<UCASE><<<(unsigned)ctas, 256, 0, s>>>(d, b, dinv);
+            return 1;
+        }
     }
     static std::atomic<unsigned long long> attr_0{0};
-    ensure_dyn_smem(trsm_kernel<UCASE, false>, 227 * 1024, attr_0);
+    ensure_dyn_smem(trsm_kernel<UCASE, false, LU>, 227 * 1024, attr_0);
     static std::atomic<unsigned long long> attr_1{0};
-    ensure_dyn_smem(trsm_kernel<UCASE, true>, 227 * 1024, attr_1);
+    ensure_dyn_smem(trsm_kernel<UCASE, true, LU>, 227 * 1024, attr_1);
     const size_t nsp = (size_t)((max_ns + 15) & ~15);
     size_t smem = sizeof(double) * nsp * TRSM_LD, staged = smem + sizeof(double) * 2 * 16 * (nsp + 4);
     if (max_ns > TRSM_WIDE_NS)   // narrower supernodes of the same batch keep their 64-vector strips
         smem = std::max(sizeof(double) * TRSM_WIDE_NS * TRSM_LD, sizeof(double) * nsp * (TRSM_STRIP / 2 + 4));
-    if (max_ns <= TRSM_WIDE_NS && staged <= 227 * 1024) trsm_kernel<UCASE, true><<<(unsigned)ctas, 256, staged, s>>>(d, b, dinv);
-    else trsm_kernel<UCASE, false><<<(unsigned)ctas, 256, smem, s>>>(d, b, dinv);
+    const dim3 grid = member_grid(d, (unsigned)ctas);
+    if (max_ns <= TRSM_WIDE_NS && staged <= 227 * 1024) trsm_kernel<UCASE, true, LU><<<grid, 256, staged, s>>>(d, b, dinv);
+    else trsm_kernel<UCASE, false, LU><<<grid, 256, smem, s>>>(d, b, dinv);
     return 1;
 }
 int launch_trsm_l(const DeviceLU &d, const Batch &b, int64_t ctas, int max_ns, const double *dinv, cudaStream_t s)
@@ -864,6 +897,14 @@ int launch_trsm_l(const DeviceLU &d, const Batch &b, int64_t ctas, int max_ns, c
     return launch_trsm<false>(d, b, ctas, max_ns, dinv, s);
 }
 int launch_trsm_u(const DeviceLU &d, const Batch &b, int64_t ctas, int max_ns, const double *dinv, cudaStream_t s)
+{
+    return launch_trsm<true>(d, b, ctas, max_ns, dinv, s);
+}
+int launch_trsm_l(const BatchedLU &d, const Batch &b, int64_t ctas, int max_ns, const double *dinv, cudaStream_t s)
+{
+    return launch_trsm<false>(d, b, ctas, max_ns, dinv, s);
+}
+int launch_trsm_u(const BatchedLU &d, const Batch &b, int64_t ctas, int max_ns, const double *dinv, cudaStream_t s)
 {
     return launch_trsm<true>(d, b, ctas, max_ns, dinv, s);
 }
@@ -1037,12 +1078,13 @@ __device__ __forceinline__ void gemm_tile_v2(const double *__restrict__ A, int l
 // ------------------------------------------------------------------------------------------------
 // Schur-complement update of a batch of supernodes: GEMM tile + fused subtract-scatter epilogue
 // ------------------------------------------------------------------------------------------------
-template <int BM, int BN, int WARPS_M, int WARPS_N, bool ATOMIC, int BK = 16, int STAGES = 3, bool V2 = false>
+template <int BM, int BN, int WARPS_M, int WARPS_N, bool ATOMIC, int BK = 16, int STAGES = 3, bool V2 = false, class LU = DeviceLU>
 __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, (32 * WARPS_M * WARPS_N <= 256) ? 2 : 1)
-    schur_kernel(DeviceLU d, Batch b, int mode, int split_n, int split_i)
+    schur_kernel(LU dd, Batch b, int mode, int split_n, int split_i)
 {
     using C = GemmCfg<BM, BN, WARPS_M, WARPS_N, BK, STAGES>;
     extern __shared__ double sm[];
+    const DeviceLU &d = member_view(dd);
     // cooperative ancestors: the ranks of a Z group deal the tiles of the batch round-robin
     const int64_t gt = (int64_t)blockIdx.x * split_n + split_i;
     if (gt >= b.prefix[b.count]) return;
@@ -1139,14 +1181,14 @@ __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, (32 * WARPS_M * WARPS_
     }
 }
 
-template <int BM, int BN, int WARPS_M, int WARPS_N, bool ATOMIC, int BK = 16, int STAGES = 3, bool V2 = false>
-static int launch_schur_t(const DeviceLU &d, const Batch &b, int64_t ctas, int mode, int split_n, int split_i, cudaStream_t s)
+template <int BM, int BN, int WARPS_M, int WARPS_N, bool ATOMIC, int BK = 16, int STAGES = 3, bool V2 = false, class LU = DeviceLU>
+static int launch_schur_t(const LU &d, const Batch &b, int64_t ctas, int mode, int split_n, int split_i, cudaStream_t s)
 {
     using C = GemmCfg<BM, BN, WARPS_M, WARPS_N, BK, STAGES>;
     static std::atomic<unsigned long long> attr_0{0};
-    ensure_dyn_smem(schur_kernel<BM, BN, WARPS_M, WARPS_N, ATOMIC, BK, STAGES, V2>, (int)C::SMEM, attr_0);
+    ensure_dyn_smem(schur_kernel<BM, BN, WARPS_M, WARPS_N, ATOMIC, BK, STAGES, V2, LU>, (int)C::SMEM, attr_0);
     const int64_t grid = (ctas + split_n - 1) / split_n;
-    schur_kernel<BM, BN, WARPS_M, WARPS_N, ATOMIC, BK, STAGES, V2><<<(unsigned)grid, C::NT, C::SMEM, s>>>(d, b, mode, split_n, split_i);
+    schur_kernel<BM, BN, WARPS_M, WARPS_N, ATOMIC, BK, STAGES, V2, LU><<<member_grid(d, (unsigned)grid), C::NT, C::SMEM, s>>>(d, b, mode, split_n, split_i);
     return 1;
 }
 
@@ -1173,6 +1215,14 @@ int launch_schur(const DeviceLU &d, const Batch &b, int64_t ctas, int big, int a
     }
     return atomic ? launch_schur_t<SCHUR_BM_SMALL, SCHUR_BN_SMALL, 2, 2, true>(d, b, ctas, mode, split_n, split_i, s)
                   : launch_schur_t<SCHUR_BM_SMALL, SCHUR_BN_SMALL, 2, 2, false>(d, b, ctas, mode, split_n, split_i, s);
+}
+
+// batched: the default tiles of the launcher above (schur_variant 0, atomic scatter, no Z split)
+int launch_schur(const BatchedLU &d, const Batch &b, int64_t ctas, int big, int mode, cudaStream_t s)
+{
+    if (b.count <= 0 || ctas <= 0) return 0;
+    if (!big) return launch_schur_t<SCHUR_BM_SMALL, SCHUR_BN_SMALL, 2, 2, true, 16, 3, true>(d, b, ctas, mode, 1, 0, s);
+    return launch_schur_t<128, 64, 4, 2, true, 16, 3, true>(d, b, ctas, mode, 1, 0, s);
 }
 
 // plain C -= A*B with the same main loop (kernel-level test and micro-benchmark of tile configurations)

@@ -25,6 +25,26 @@ inline bool ensure_dyn_smem(K kernel, int bytes, std::atomic<unsigned long long>
 }
 
 // ------------------------------------------------------------------------------------------------
+// batched launches (BatchedLU): the member of a CTA is blockIdx.y.  For a plain DeviceLU these are the identity, so
+// the unbatched instantiations of a kernel templated on its DeviceLU type compile exactly as before.
+__device__ __forceinline__ const DeviceLU &member_view(const DeviceLU &d) { return d; }
+__device__ __forceinline__ DeviceLU member_view(const BatchedLU &d)
+{
+    DeviceLU m = d;
+    m.val += (int64_t)blockIdx.y * d.val_stride;
+    m.info += blockIdx.y;
+    return m;
+}
+// a per-member buffer of `stride` (< 2^32) elements per member
+template <class T> __device__ __forceinline__ T *member_ptr(const DeviceLU &, T *p, uint32_t) { return p; }
+template <class T> __device__ __forceinline__ T *member_ptr(const BatchedLU &, T *p, uint32_t stride) { return p + (size_t)blockIdx.y * stride; }
+template <class T> __device__ __forceinline__ T *member_inv(const DeviceLU &, T *dinv) { return dinv; }
+template <class T> __device__ __forceinline__ T *member_inv(const BatchedLU &d, T *dinv) { return dinv + (int64_t)blockIdx.y * d.inv_stride; }
+// launch grid: the unbatched x extent, one row per member
+inline dim3 member_grid(const DeviceLU &, unsigned x) { return dim3(x); }
+inline dim3 member_grid(const BatchedLU &d, unsigned x) { return dim3(x, (unsigned)d.members); }
+
+// ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ int find_slot(const int64_t *prefix, int count, int64_t bid)
 {
     int lo = 0, hi = count;  // prefix[lo] <= bid < prefix[hi]

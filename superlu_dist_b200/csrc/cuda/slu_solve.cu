@@ -20,16 +20,20 @@
 #include "slu_kernels_common.cuh"
 #include "slu_scalar.cuh"
 
+#include <type_traits>
+
 namespace SLU_NS {
 
 constexpr int SOLVE_ROWS = 256;   // rows of an L panel / columns of a U panel per CTA in the update kernels
 
 // x_k <- L_kk^-1 x_k (unit lower) or U_kk^-1 x_k (upper, non-unit): one CTA per supernode, column sweep in shared
 // memory.  16-column blocks: warp 0 finishes the block's 16 unknowns with shuffles, then all threads apply them.
-template <bool UPPER>
-__global__ void __launch_bounds__(256) solve_diag_kernel(DeviceLU d, const int32_t *nodes, val_t *x, int n, int nrhs)
+template <bool UPPER, class LU>
+__global__ void __launch_bounds__(256) solve_diag_kernel(LU dd, const int32_t *nodes, val_t *x, int n, int nrhs)
 {
     __shared__ val_t xs[MAX_NS_HELD];
+    const DeviceLU &d = member_view(dd);
+    x = member_ptr(dd, x, (uint32_t)(n * nrhs));   // the host keeps n * nrhs < 2^31
     const NodeDesc nd = d.nodes[nodes[blockIdx.x]];
     const int ns = nd.ns, lda = nd.nsupr, tid = threadIdx.x;
     const val_t *A = d.val + nd.lval;
@@ -85,9 +89,12 @@ __global__ void __launch_bounds__(256) solve_diag_kernel(DeviceLU d, const int32
 }
 
 // x[rows below] -= L(below, k) x_k: CTA = 256 rows of one panel, thread = row (coalesced down the columns)
-__global__ void __launch_bounds__(SOLVE_ROWS) solve_update_l_kernel(DeviceLU d, Batch b, val_t *x, int n, int nrhs)
+template <class LU>
+__global__ void __launch_bounds__(SOLVE_ROWS) solve_update_l_kernel(LU dd, Batch b, val_t *x, int n, int nrhs)
 {
     __shared__ val_t xs[MAX_NS_HELD];
+    const DeviceLU &d = member_view(dd);
+    x = member_ptr(dd, x, (uint32_t)(n * nrhs));   // the host keeps n * nrhs < 2^31
     const int slot = find_slot(b.prefix, b.count, blockIdx.x);
     const NodeDesc nd = d.nodes[b.nodes[slot]];
     const int i = (int)(blockIdx.x - b.prefix[slot]) * SOLVE_ROWS + threadIdx.x;
@@ -108,9 +115,12 @@ __global__ void __launch_bounds__(SOLVE_ROWS) solve_update_l_kernel(DeviceLU d, 
 }
 
 // x_k -= U(k, cols) x[cols]: CTA = 256 packed columns of one U panel; warp w sweeps columns w, w+8, ..., lanes over rows
-__global__ void __launch_bounds__(256) solve_update_u_kernel(DeviceLU d, Batch b, val_t *x, int n, int nrhs)
+template <class LU>
+__global__ void __launch_bounds__(256) solve_update_u_kernel(LU dd, Batch b, val_t *x, int n, int nrhs)
 {
     __shared__ val_t part[8][MAX_NS_HELD];
+    const DeviceLU &d = member_view(dd);
+    x = member_ptr(dd, x, (uint32_t)(n * nrhs));   // the host keeps n * nrhs < 2^31
     const int slot = find_slot(b.prefix, b.count, blockIdx.x);
     const NodeDesc nd = d.nodes[b.nodes[slot]];
     const int j0 = (int)(blockIdx.x - b.prefix[slot]) * SOLVE_ROWS, j1 = min(nd.ncols, j0 + SOLVE_ROWS);
@@ -163,12 +173,16 @@ __global__ void solve_mask_kernel(DeviceLU d, const int32_t *nodes, int count, v
 // factor-entry host arrays and their H2D.  One thread per row of A; an entry (i, j) of the permuted matrix belongs to
 // the L panel of supno(j) if i is at or below that supernode's first row, else to the U panel of supno(i).
 // `active[k]` = 0 for panels this rank does not hold or holds as zero-initialised replicated ancestors.
-__global__ void fill_csr_kernel(DeviceLU d, int n, const int32_t *__restrict__ rowptr, const int32_t *__restrict__ colind,
+// Batched: member blockIdx.y scatters its own nnz values (aval + member * nnz) into its own arena.
+template <class LU>
+__global__ void fill_csr_kernel(LU dd, int n, const int32_t *__restrict__ rowptr, const int32_t *__restrict__ colind,
                                 const val_t *__restrict__ aval, const int32_t *__restrict__ perm, const int8_t *__restrict__ active,
                                 int *err)
 {
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= n) return;
+    const DeviceLU &d = member_view(dd);
+    if constexpr (std::is_same<LU, BatchedLU>::value) aval += (int64_t)blockIdx.y * rowptr[n];
     const int pi = perm[r];
     for (int p = rowptr[r]; p < rowptr[r + 1]; ++p) {
         const int pj = perm[colind[p]];
@@ -191,27 +205,57 @@ __global__ void fill_csr_kernel(DeviceLU d, int n, const int32_t *__restrict__ r
         }
     }
 }
+template <class LU>
+static int launch_fill_csr_t(const LU &d, int n, const int32_t *rowptr, const int32_t *colind, const val_t *aval, const int32_t *perm,
+                             const int8_t *active, int *err, cudaStream_t s)
+{
+    fill_csr_kernel<LU><<<member_grid(d, (n + 127) / 128), 128, 0, s>>>(d, n, rowptr, colind, aval, perm, active, err);
+    return 1;
+}
+template <class LU>
+static int launch_solve_diag_t(const LU &d, const int32_t *nodes, int count, bool upper, val_t *x, int n, int nrhs, cudaStream_t s)
+{
+    if (count <= 0) return 0;
+    if (upper) solve_diag_kernel<true, LU><<<member_grid(d, count), 256, 0, s>>>(d, nodes, x, n, nrhs);
+    else solve_diag_kernel<false, LU><<<member_grid(d, count), 256, 0, s>>>(d, nodes, x, n, nrhs);
+    return 1;
+}
+template <class LU>
+static int launch_solve_update_t(const LU &d, const Batch &b, int64_t ctas, bool upper, val_t *x, int n, int nrhs, cudaStream_t s)
+{
+    if (b.count <= 0 || ctas <= 0) return 0;
+    if (upper) solve_update_u_kernel<LU><<<member_grid(d, (unsigned)ctas), 256, 0, s>>>(d, b, x, n, nrhs);
+    else solve_update_l_kernel<LU><<<member_grid(d, (unsigned)ctas), SOLVE_ROWS, 0, s>>>(d, b, x, n, nrhs);
+    return 1;
+}
 int launch_fill_csr(const DeviceLU &d, int n, const int32_t *rowptr, const int32_t *colind, const val_t *aval, const int32_t *perm,
                     const int8_t *active, int *err, cudaStream_t s)
 {
-    fill_csr_kernel<<<(n + 127) / 128, 128, 0, s>>>(d, n, rowptr, colind, aval, perm, active, err);
-    return 1;
+    return launch_fill_csr_t(d, n, rowptr, colind, aval, perm, active, err, s);
 }
-
 int launch_solve_diag(const DeviceLU &d, const int32_t *nodes, int count, bool upper, val_t *x, int n, int nrhs, cudaStream_t s)
 {
-    if (count <= 0) return 0;
-    if (upper) solve_diag_kernel<true><<<count, 256, 0, s>>>(d, nodes, x, n, nrhs);
-    else solve_diag_kernel<false><<<count, 256, 0, s>>>(d, nodes, x, n, nrhs);
-    return 1;
+    return launch_solve_diag_t(d, nodes, count, upper, x, n, nrhs, s);
 }
 int launch_solve_update(const DeviceLU &d, const Batch &b, int64_t ctas, bool upper, val_t *x, int n, int nrhs, cudaStream_t s)
 {
-    if (b.count <= 0 || ctas <= 0) return 0;
-    if (upper) solve_update_u_kernel<<<(unsigned)ctas, 256, 0, s>>>(d, b, x, n, nrhs);
-    else solve_update_l_kernel<<<(unsigned)ctas, SOLVE_ROWS, 0, s>>>(d, b, x, n, nrhs);
-    return 1;
+    return launch_solve_update_t(d, b, ctas, upper, x, n, nrhs, s);
 }
+#ifndef SLU_COMPLEX
+int launch_fill_csr(const BatchedLU &d, int n, const int32_t *rowptr, const int32_t *colind, const val_t *aval, const int32_t *perm,
+                    const int8_t *active, int *err, cudaStream_t s)
+{
+    return launch_fill_csr_t(d, n, rowptr, colind, aval, perm, active, err, s);
+}
+int launch_solve_diag(const BatchedLU &d, const int32_t *nodes, int count, bool upper, val_t *x, int n, int nrhs, cudaStream_t s)
+{
+    return launch_solve_diag_t(d, nodes, count, upper, x, n, nrhs, s);
+}
+int launch_solve_update(const BatchedLU &d, const Batch &b, int64_t ctas, bool upper, val_t *x, int n, int nrhs, cudaStream_t s)
+{
+    return launch_solve_update_t(d, b, ctas, upper, x, n, nrhs, s);
+}
+#endif
 int launch_solve_mask(const DeviceLU &d, const int32_t *nodes, int count, val_t *x, int n, int nrhs, const val_t *src, cudaStream_t s)
 {
     if (count <= 0) return 0;
