@@ -107,6 +107,11 @@ def lib():
     L.slu_b200_batch_factor.argtypes = [C.c_void_p, C.c_void_p]
     L.slu_b200_batch_solve.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
     L.slu_b200_batch_download.argtypes = [C.c_void_p, C.c_int]
+    L.slu_b200_z_batch_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(LUView), C.POINTER(Options), C.c_int]
+    L.slu_b200_z_batch_fill_csr.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.slu_b200_z_batch_factor.argtypes = [C.c_void_p, C.c_void_p]
+    L.slu_b200_z_batch_solve.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
+    L.slu_b200_z_batch_download.argtypes = [C.c_void_p, C.c_int]
     _lib = L
     return L
 
@@ -310,57 +315,60 @@ class Handle:
 
 
 class BatchHandle:
-    """A batched handle (slu_b200_batch_*): `batch` double-precision matrices with the sparsity pattern of `prob` (layer 0,
-    1 x 1 x 1 grid), factored and solved together.  The analysis is shared; each member has its own values."""
+    """A batched handle (slu_b200_batch_*): `batch` matrices with the sparsity pattern of `prob` (layer 0, 1 x 1 x 1
+    grid), factored and solved together.  The analysis is shared; each member has its own values.  A complex128 `prob`
+    takes the doublecomplex twins (slu_b200_z_batch_*): values, right-hand sides and solutions are then complex128."""
 
     def __init__(self, prob, batch, **opt):
         require_gpu()
-        if _is_complex(prob.dtype):
-            raise TypeError("batched handles are double precision")
         self.prob, self.batch = prob, int(batch)
+        self.z_ = _is_complex(prob.dtype)
         self.view, self._keep = make_view(prob, 0)
         self.opt = make_options(prob, **opt)
         self.h = C.c_void_p()
-        _check(lib().slu_b200_batch_create(C.byref(self.h), C.byref(self.view), C.byref(self.opt), self.batch))
+        _check(_fn("batch_create", self.z_)(C.byref(self.h), C.byref(self.view), C.byref(self.opt), self.batch))
+
+    def _dtype(self):
+        return np.complex128 if self.z_ else np.float64
 
     def fill_csr(self, rowptr, colind, vals, perm):
         """One CSR pattern and perm[old] = new for every member; vals: (batch, nnz), row j = member j's values."""
         rp = np.ascontiguousarray(rowptr, np.int32)
         ci = np.ascontiguousarray(colind, np.int32)
-        v = np.ascontiguousarray(vals, np.float64)
+        v = np.ascontiguousarray(vals, self._dtype())
         if v.shape != (self.batch, len(ci)):
             raise ValueError(f"vals must have shape ({self.batch}, {len(ci)}), not {v.shape}")
         pm = np.ascontiguousarray(perm, np.int32)
-        _check(lib().slu_b200_batch_fill_csr(self.h, len(rp) - 1, rp.ctypes.data_as(C.c_void_p), ci.ctypes.data_as(C.c_void_p),
-                                             v.ctypes.data_as(C.c_void_p), pm.ctypes.data_as(C.c_void_p)))
+        _check(_fn("batch_fill_csr", self.z_)(self.h, len(rp) - 1, rp.ctypes.data_as(C.c_void_p), ci.ctypes.data_as(C.c_void_p),
+                                              v.ctypes.data_as(C.c_void_p), pm.ctypes.data_as(C.c_void_p)))
 
     def factor(self):
         """-> int32 array (batch,): 0, or the 1-based column of the member's first exact zero pivot."""
         info = np.zeros(self.batch, np.int32)
-        _check(lib().slu_b200_batch_factor(self.h, info.ctypes.data_as(C.c_void_p)))
+        _check(_fn("batch_factor", self.z_)(self.h, info.ctypes.data_as(C.c_void_p)))
         return info
 
     def solve(self, b):
         """L_j U_j x_j = b_j for every member; b: (batch, n) or (batch, nrhs, n), ordering of the factored matrix."""
-        x = np.array(b, np.float64, order="C", copy=True)
+        x = np.array(b, self._dtype(), order="C", copy=True)
         if x.ndim not in (2, 3) or x.shape[0] != self.batch or x.shape[-1] != self.prob.n:
             raise ValueError(f"b must have shape ({self.batch}, n) or ({self.batch}, nrhs, n) with n = {self.prob.n}")
         nrhs = 1 if x.ndim == 2 else x.shape[1]
-        _check(lib().slu_b200_batch_solve(self.h, x.ctypes.data_as(C.c_void_p), self.prob.n, nrhs))
+        _check(_fn("batch_solve", self.z_)(self.h, x.ctypes.data_as(C.c_void_p), self.prob.n, nrhs))
         return x
 
     def download(self, member):
         """Member `member`'s L and U into prob.layers[0] (the reference layout)."""
-        _check(lib().slu_b200_batch_download(self.h, int(member)))
+        _check(_fn("batch_download", self.z_)(self.h, int(member)))
 
     def stats(self):
         s = Stats()
-        _check(lib().slu_b200_get_stats(self.h, C.byref(s)))
+        _check(_fn("get_stats", self.z_)(self.h, C.byref(s)))
         return s
 
     def close(self):
         if self.h:
-            lib().slu_b200_destroy(self.h)
+            _fn("destroy", self.z_)(self.h)
             self.h = C.c_void_p()
 
     def __del__(self):

@@ -168,10 +168,9 @@ int launch_solve_mask(const DeviceLU &d, const int32_t *nodes, int count, val_t 
 int launch_fill_csr(const DeviceLU &d, int n, const int32_t *rowptr, const int32_t *colind, const val_t *aval, const int32_t *perm,
                     const int8_t *active, int *err, cudaStream_t s);
 
-#ifndef SLU_COMPLEX
-// batched launches: the same kernels over d.members matrices of one pattern (gridDim.y = members).  dinv = member 0's
-// workspace; in the solve x holds the members' n x nrhs blocks back to back, in fill_csr aval their nnz values.
-// Always the FP64 DMMA path with the default tile shapes: the opt-in kernel variants are not batched.
+// batched launches (both precisions): the same kernels over d.members matrices of one pattern (gridDim.y = members).
+// dinv = member 0's workspace; in the solve x holds the members' n x nrhs blocks back to back, in fill_csr aval their
+// nnz values.  Always the FP64 DMMA path with the default tile shapes: the opt-in kernel variants are not batched.
 int launch_diag_lu(const BatchedLU &d, const Batch &b, int max_ns, int replace_tiny, double thresh, cudaStream_t s);
 int launch_diag_inv(const BatchedLU &d, const Batch &b, int64_t ctas, val_t *dinv, cudaStream_t s);
 int launch_trsm_l(const BatchedLU &d, const Batch &b, int64_t ctas, int max_ns, const val_t *dinv, cudaStream_t s);
@@ -181,7 +180,6 @@ int launch_solve_diag(const BatchedLU &d, const int32_t *nodes, int count, bool 
 int launch_solve_update(const BatchedLU &d, const Batch &b, int64_t ctas, bool upper, val_t *x, int n, int nrhs, cudaStream_t s);
 int launch_fill_csr(const BatchedLU &d, int n, const int32_t *rowptr, const int32_t *colind, const val_t *aval, const int32_t *perm,
                     const int8_t *active, int *err, cudaStream_t s);
-#endif
 
 #ifndef SLU_COMPLEX
 // slu_ozaki.cu: the Schur update of wide supernodes on wgmma (int8 slices, exact int32 accumulation in registers)

@@ -12,6 +12,8 @@
 //                    multiply-adds per complex one; the second factor is never built -- each lane reads the raw
 //                    (re, im) pair of U with a lane-constant swap and sign.  Subtract-scatter fused in the epilogue.
 //   u_convert / axpy as in the real build.
+// diag_lu, diag_inv, trsm and schur are templated on their DeviceLU type, as in slu_kernels.cu: the BatchedLU
+// instantiations serve the batched handles (slu_b200_z_batch_*, member = blockIdx.y).
 #define SLU_COMPLEX 1
 #include "slu_device.cuh"
 #include "slu_kernels_common.cuh"
@@ -31,9 +33,11 @@ __device__ __forceinline__ void cp_async16(void *smem, const void *gmem, bool pr
 // ------------------------------------------------------------------------------------------------
 // diagonal block LU (same schedule as the real kernel: 16-column panels in shared memory)
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(512) diag_lu_kernel(DeviceLU d, Batch b, int replace_tiny, double thresh)
+template <class LU>
+__global__ void __launch_bounds__(512) diag_lu_kernel(LU dd, Batch b, int replace_tiny, double thresh)
 {
     extern __shared__ double2 smz[];
+    const DeviceLU &d = member_view(dd);
     constexpr int NB = DIAG_NB;
     const int k = b.nodes[blockIdx.x];
     const NodeDesc nd = d.nodes[k];
@@ -141,23 +145,35 @@ __global__ void __launch_bounds__(512) diag_lu_kernel(DeviceLU d, Batch b, int r
     }
 }
 
-int launch_diag_lu(const DeviceLU &d, const Batch &b, int max_ns, int replace_tiny, double thresh, cudaStream_t s)
+template <class LU>
+static int launch_diag_lu_t(const LU &d, const Batch &b, int max_ns, int replace_tiny, double thresh, cudaStream_t s)
 {
     if (b.count <= 0) return 0;
     size_t smem = sizeof(zd) * 2 * DIAG_NB * (size_t)max_ns;
     static std::atomic<unsigned long long> attr_0{0};
-    ensure_dyn_smem(diag_lu_kernel, (int)(sizeof(zd) * 2 * DIAG_NB * MAX_NS_HELD), attr_0);
+    ensure_dyn_smem(diag_lu_kernel<LU>, (int)(sizeof(zd) * 2 * DIAG_NB * MAX_NS_HELD), attr_0);
     int threads = max_ns <= 32 ? 128 : (max_ns <= 128 ? 256 : 512);
-    diag_lu_kernel<<<b.count, threads, smem, s>>>(d, b, replace_tiny, thresh);
+    diag_lu_kernel<LU><<<member_grid(d, b.count), threads, smem, s>>>(d, b, replace_tiny, thresh);
     return 1;
+}
+int launch_diag_lu(const DeviceLU &d, const Batch &b, int max_ns, int replace_tiny, double thresh, cudaStream_t s)
+{
+    return launch_diag_lu_t(d, b, max_ns, replace_tiny, thresh, s);
+}
+int launch_diag_lu(const BatchedLU &d, const Batch &b, int max_ns, int replace_tiny, double thresh, cudaStream_t s)
+{
+    return launch_diag_lu_t(d, b, max_ns, replace_tiny, thresh, s);
 }
 
 // ------------------------------------------------------------------------------------------------
 // inverse of the 16x16 diagonal blocks: dinv[ws_inv + blk*512 + {0: inv U (column-major 16x16), 256: inv L}]
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(64) diag_inv_kernel(DeviceLU d, Batch b, zd *dinv)
+template <class LU>
+__global__ void __launch_bounds__(64) diag_inv_kernel(LU dd, Batch b, zd *dinv)
 {
     __shared__ zd M[16 * 17];
+    const DeviceLU &d = member_view(dd);
+    dinv = member_inv(dd, dinv);
     const int slot = find_slot(b.prefix, b.count, blockIdx.x);
     const int k = b.nodes[slot];
     const NodeDesc nd = d.nodes[k];
@@ -202,11 +218,20 @@ __global__ void __launch_bounds__(64) diag_inv_kernel(DeviceLU d, Batch b, zd *d
     }
 }
 
-int launch_diag_inv(const DeviceLU &d, const Batch &b, int64_t ctas, zd *dinv, cudaStream_t s)
+template <class LU>
+static int launch_diag_inv_t(const LU &d, const Batch &b, int64_t ctas, zd *dinv, cudaStream_t s)
 {
     if (b.count <= 0 || ctas <= 0) return 0;
-    diag_inv_kernel<<<(unsigned)ctas, 64, 0, s>>>(d, b, dinv);
+    diag_inv_kernel<LU><<<member_grid(d, (unsigned)ctas), 64, 0, s>>>(d, b, dinv);
     return 1;
+}
+int launch_diag_inv(const DeviceLU &d, const Batch &b, int64_t ctas, zd *dinv, cudaStream_t s)
+{
+    return launch_diag_inv_t(d, b, ctas, dinv, s);
+}
+int launch_diag_inv(const BatchedLU &d, const Batch &b, int64_t ctas, zd *dinv, cudaStream_t s)
+{
+    return launch_diag_inv_t(d, b, ctas, dinv, s);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -218,10 +243,12 @@ int launch_diag_inv(const DeviceLU &d, const Batch &b, int64_t ctas, zd *dinv, c
 // ------------------------------------------------------------------------------------------------
 constexpr int TZ_LD = TRSM_STRIP + 1;
 
-template <bool UCASE>
-__global__ void __launch_bounds__(256) trsm_kernel(DeviceLU d, Batch b, const zd *dinv)
+template <bool UCASE, class LU>
+__global__ void __launch_bounds__(256) trsm_kernel(LU dd, Batch b, const zd *dinv)
 {
     extern __shared__ double2 smz[];
+    const DeviceLU &d = member_view(dd);
+    dinv = member_inv(dd, dinv);
     const int slot = find_slot(b.prefix, b.count, blockIdx.x);
     const int k = b.nodes[slot];
     const NodeDesc nd = d.nodes[k];
@@ -305,14 +332,14 @@ __global__ void __launch_bounds__(256) trsm_kernel(DeviceLU d, Batch b, const zd
     }
 }
 
-template <bool UCASE>
-static int launch_trsm(const DeviceLU &d, const Batch &b, int64_t ctas, int max_ns, const zd *dinv, cudaStream_t s)
+template <bool UCASE, class LU>
+static int launch_trsm(const LU &d, const Batch &b, int64_t ctas, int max_ns, const zd *dinv, cudaStream_t s)
 {
     if (b.count <= 0 || ctas <= 0) return 0;
     static std::atomic<unsigned long long> attr_0{0};
-    ensure_dyn_smem(trsm_kernel<UCASE>, (int)(sizeof(zd) * (MAX_NS_HELD + 16) * TZ_LD), attr_0);
+    ensure_dyn_smem(trsm_kernel<UCASE, LU>, (int)(sizeof(zd) * (MAX_NS_HELD + 16) * TZ_LD), attr_0);
     const size_t smem = sizeof(zd) * ((size_t)max_ns + 16) * TZ_LD;
-    trsm_kernel<UCASE><<<(unsigned)ctas, 256, smem, s>>>(d, b, dinv);
+    trsm_kernel<UCASE, LU><<<member_grid(d, (unsigned)ctas), 256, smem, s>>>(d, b, dinv);
     return 1;
 }
 int launch_trsm_l(const DeviceLU &d, const Batch &b, int64_t ctas, int max_ns, const zd *dinv, cudaStream_t s)
@@ -320,6 +347,14 @@ int launch_trsm_l(const DeviceLU &d, const Batch &b, int64_t ctas, int max_ns, c
     return launch_trsm<false>(d, b, ctas, max_ns, dinv, s);
 }
 int launch_trsm_u(const DeviceLU &d, const Batch &b, int64_t ctas, int max_ns, const zd *dinv, cudaStream_t s)
+{
+    return launch_trsm<true>(d, b, ctas, max_ns, dinv, s);
+}
+int launch_trsm_l(const BatchedLU &d, const Batch &b, int64_t ctas, int max_ns, const zd *dinv, cudaStream_t s)
+{
+    return launch_trsm<false>(d, b, ctas, max_ns, dinv, s);
+}
+int launch_trsm_u(const BatchedLU &d, const Batch &b, int64_t ctas, int max_ns, const zd *dinv, cudaStream_t s)
 {
     return launch_trsm<true>(d, b, ctas, max_ns, dinv, s);
 }
@@ -411,12 +446,13 @@ __device__ __forceinline__ void zgemm_tile(const zd *__restrict__ A, int lda, co
 // ------------------------------------------------------------------------------------------------
 // Schur-complement update of a batch of supernodes: complex tile product + fused subtract-scatter
 // ------------------------------------------------------------------------------------------------
-template <int BM, int BNC, int WARPS_M, int WARPS_N>
+template <int BM, int BNC, int WARPS_M, int WARPS_N, class LU = DeviceLU>
 __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, 2)
-    schur_kernel(DeviceLU d, Batch b, int mode, int split_n, int split_i)
+    schur_kernel(LU dd, Batch b, int mode, int split_n, int split_i)
 {
     using C = ZCfg<BM, BNC, WARPS_M, WARPS_N>;
     extern __shared__ double smd[];
+    const DeviceLU &d = member_view(dd);
     const int64_t gt = (int64_t)blockIdx.x * split_n + split_i;
     if (gt >= b.prefix[b.count]) return;
     const int slot = find_slot(b.prefix, b.count, gt);
@@ -491,14 +527,14 @@ __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, 2)
     }
 }
 
-template <int BM, int BNC, int WARPS_M, int WARPS_N>
-static int launch_schur_t(const DeviceLU &d, const Batch &b, int64_t ctas, int mode, int split_n, int split_i, cudaStream_t s)
+template <int BM, int BNC, int WARPS_M, int WARPS_N, class LU = DeviceLU>
+static int launch_schur_t(const LU &d, const Batch &b, int64_t ctas, int mode, int split_n, int split_i, cudaStream_t s)
 {
     using C = ZCfg<BM, BNC, WARPS_M, WARPS_N>;
     static std::atomic<unsigned long long> attr_0{0};
-    ensure_dyn_smem(schur_kernel<BM, BNC, WARPS_M, WARPS_N>, (int)C::SMEM, attr_0);
+    ensure_dyn_smem(schur_kernel<BM, BNC, WARPS_M, WARPS_N, LU>, (int)C::SMEM, attr_0);
     const int64_t grid = (ctas + split_n - 1) / split_n;
-    schur_kernel<BM, BNC, WARPS_M, WARPS_N><<<(unsigned)grid, C::NT, C::SMEM, s>>>(d, b, mode, split_n, split_i);
+    schur_kernel<BM, BNC, WARPS_M, WARPS_N, LU><<<member_grid(d, (unsigned)grid), C::NT, C::SMEM, s>>>(d, b, mode, split_n, split_i);
     return 1;
 }
 
@@ -508,6 +544,14 @@ int launch_schur(const DeviceLU &d, const Batch &b, int64_t ctas, int big, int /
     if (b.count <= 0 || ctas <= 0) return 0;
     if (big) return launch_schur_t<SCHUR_BM_BIG, SCHUR_BN_TILE, 4, 2>(d, b, ctas, mode, split_n, split_i, s);
     return launch_schur_t<SCHUR_BM_SMALL, SCHUR_BN_SMALL, 2, 2>(d, b, ctas, mode, split_n, split_i, s);
+}
+
+// batched: the default tiles of the launcher above, no Z split
+int launch_schur(const BatchedLU &d, const Batch &b, int64_t ctas, int big, int mode, cudaStream_t s)
+{
+    if (b.count <= 0 || ctas <= 0) return 0;
+    if (big) return launch_schur_t<SCHUR_BM_BIG, SCHUR_BN_TILE, 4, 2>(d, b, ctas, mode, 1, 0, s);
+    return launch_schur_t<SCHUR_BM_SMALL, SCHUR_BN_SMALL, 2, 2>(d, b, ctas, mode, 1, 0, s);
 }
 
 // plain C -= A*B with the same main loop (kernel-level test)

@@ -25,11 +25,15 @@
 namespace SLU_NS {
 
 constexpr int SOLVE_ROWS = 256;   // rows of an L panel / columns of a U panel per CTA in the update kernels
+// __launch_bounds__ minimum of CTAs per SM for solve_diag / solve_update_u: 4 (64 registers) for the batched doublecomplex
+// instantiations, which ptxas otherwise compiles with a spill; 0 (no minimum) for every other one, which compile as before
+template <class LU>
+constexpr int SOLVE_MIN_CTAS = (VAL_DOUBLES == 2 && std::is_same<LU, BatchedLU>::value) ? 4 : 0;
 
 // x_k <- L_kk^-1 x_k (unit lower) or U_kk^-1 x_k (upper, non-unit): one CTA per supernode, column sweep in shared
 // memory.  16-column blocks: warp 0 finishes the block's 16 unknowns with shuffles, then all threads apply them.
 template <bool UPPER, class LU>
-__global__ void __launch_bounds__(256) solve_diag_kernel(LU dd, const int32_t *nodes, val_t *x, int n, int nrhs)
+__global__ void __launch_bounds__(256, SOLVE_MIN_CTAS<LU>) solve_diag_kernel(LU dd, const int32_t *nodes, val_t *x, int n, int nrhs)
 {
     __shared__ val_t xs[MAX_NS_HELD];
     const DeviceLU &d = member_view(dd);
@@ -116,7 +120,7 @@ __global__ void __launch_bounds__(SOLVE_ROWS) solve_update_l_kernel(LU dd, Batch
 
 // x_k -= U(k, cols) x[cols]: CTA = 256 packed columns of one U panel; warp w sweeps columns w, w+8, ..., lanes over rows
 template <class LU>
-__global__ void __launch_bounds__(256) solve_update_u_kernel(LU dd, Batch b, val_t *x, int n, int nrhs)
+__global__ void __launch_bounds__(256, SOLVE_MIN_CTAS<LU>) solve_update_u_kernel(LU dd, Batch b, val_t *x, int n, int nrhs)
 {
     __shared__ val_t part[8][MAX_NS_HELD];
     const DeviceLU &d = member_view(dd);
@@ -241,7 +245,6 @@ int launch_solve_update(const DeviceLU &d, const Batch &b, int64_t ctas, bool up
 {
     return launch_solve_update_t(d, b, ctas, upper, x, n, nrhs, s);
 }
-#ifndef SLU_COMPLEX
 int launch_fill_csr(const BatchedLU &d, int n, const int32_t *rowptr, const int32_t *colind, const val_t *aval, const int32_t *perm,
                     const int8_t *active, int *err, cudaStream_t s)
 {
@@ -255,7 +258,6 @@ int launch_solve_update(const BatchedLU &d, const Batch &b, int64_t ctas, bool u
 {
     return launch_solve_update_t(d, b, ctas, upper, x, n, nrhs, s);
 }
-#endif
 int launch_solve_mask(const DeviceLU &d, const int32_t *nodes, int count, val_t *x, int n, int nrhs, const val_t *src, cudaStream_t s)
 {
     if (count <= 0) return 0;
