@@ -238,6 +238,7 @@ struct slu_b200_handle_s {
     DevBuf<double> d_oz_scale;
     DevBuf<int> d_oz_rexp;
     int tc_slices = 0, tc_min_ns = 0;     // 0 slices: int8 tensor-core path off
+    int tc_max_m = 0;                     // > 0: only updates of fewer rows take the int8 path (its default); 0: no limit
     bool tc_force_off = false, tc_alloc_failed = false;   // slice workspace did not fit: analysed again without the int8 tensor-core path
     int tc_nonatomic = 0;                 // plain load/store scatter for destinations only one supernode of a level updates
     DevBuf<val_t> d_x, d_x2;              // triangular solve: right-hand sides / solution
@@ -597,6 +598,8 @@ int analyze(slu_b200_handle_s *H)
     // options.reserved[5] = narrowest supernode that takes it (0: default)
     H->tc_slices = H->opt.reserved[4] < 0 ? 0 : (H->opt.reserved[4] == 0 ? (OZ_DEFAULT_ON ? OZ_DEFAULT_SLICES : 0) : std::min(8, std::max(5, (int)H->opt.reserved[4])));
     H->tc_min_ns = H->opt.reserved[5] > 0 ? H->opt.reserved[5] : OZ_DEFAULT_MIN_NS;
+    H->tc_max_m = H->opt.reserved[4] == 0 ? OZ_DEFAULT_MAX_M : 0;
+    if (getenv("SLU_B200_TC_MAX_M")) H->tc_max_m = std::max(0, atoi(getenv("SLU_B200_TC_MAX_M")));
     if (getenv("SLU_B200_TC_SLICES")) { int v = atoi(getenv("SLU_B200_TC_SLICES")); H->tc_slices = v <= 0 ? 0 : std::min(8, std::max(5, v)); }
     if (getenv("SLU_B200_TC_MIN_NS")) H->tc_min_ns = std::max(1, atoi(getenv("SLU_B200_TC_MIN_NS")));
     if (H->tc_force_off) H->tc_slices = 0;
@@ -661,7 +664,7 @@ int analyze(slu_b200_handle_s *H)
                         bool use_tc = false;
                         int bn = H->opt.schur_variant != 1 ? SCHUR_BN_TILE : SCHUR_BN_BIG;
 #ifndef SLU_COMPLEX
-                        use_tc = H->tc_slices > 0 && nd.ns >= H->tc_min_ns && nd.ns <= 512;
+                        use_tc = H->tc_slices > 0 && nd.ns >= H->tc_min_ns && nd.ns <= 512 && (H->tc_max_m <= 0 || nd.m < H->tc_max_m);
                         if (use_tc) bn = OZ_NT_HOST;
 #endif
                         (use_tc ? tc : big).push_back(k);

@@ -141,7 +141,7 @@ int launch_diag_inv(const DeviceLU &d, const Batch &b, int64_t ctas, val_t *dinv
 int launch_trsm_l(const DeviceLU &d, const Batch &b, int64_t ctas, int max_ns, const val_t *dinv, cudaStream_t s);
 int launch_trsm_u(const DeviceLU &d, const Batch &b, int64_t ctas, int max_ns, const val_t *dinv, cudaStream_t s);
 int launch_schur_setup(const DeviceLU &d, const Batch &b, int64_t ctas, cudaStream_t s);
-// variant 0 (default): 128x64 tiles, 256 threads, 2 CTAs/SM; variant 1: 128x128 tiles, 512 threads, 1 CTA/SM
+// variant 0 (default): big tiles on schur_kernel_h (128x64, DMMA.16x8x8, 2 CTAs/SM); variant 1: 128x128 tiles, 512 threads
 // mode 0: every tile of each supernode; 1: only the urgent tiles (urg_rows/urg_cols); 2: only the others
 // split_n/split_i: this rank takes tiles t with t % split_n == split_i (cooperative ancestor forests)
 int launch_schur(const DeviceLU &d, const Batch &b, int64_t ctas, int big, int atomic, int variant, int mode, int split_n,
@@ -192,6 +192,11 @@ constexpr int OZ_DEFAULT_MIN_NS = 128;
 constexpr bool OZ_PERSIST_DEFAULT = false;     // persistent int8 Schur kernel (SLU_B200_TC_PERSIST=1|0)
 constexpr bool OZ_NONATOMIC_DEFAULT = false;   // SLU_B200_TC_NONATOMIC=1|0 overrides
 constexpr bool OZ_DEFAULT_ON = true;  // options.reserved[4] = -1 / SLU_B200_TC_SLICES=0: off
+// By default the int8 path takes only updates of fewer than OZ_DEFAULT_MAX_M rows (SLU_B200_TC_MAX_M overrides, 0: no
+// limit); larger ones go to the FP64 kernel on DMMA.16x8x8 (schur_kernel_h), which is faster there -- at S = 7 the int8
+// path's ceiling on the H100 is the FP64 tensor rate (DESIGN 4b).  An explicit slice count (options.reserved[4] = 5..8)
+// sets no row limit.
+constexpr int OZ_DEFAULT_MAX_M = 2048;
 inline int64_t oz_a_bytes(int m, int ns, int S) { return (int64_t)((m + 127) / 128) * ((ns + OZ_KSTEP - 1) / OZ_KSTEP) * S * 4096; }
 inline int64_t oz_b_bytes(int n, int ns, int S) { return (int64_t)((n + OZ_NT - 1) / OZ_NT) * ((ns + OZ_KSTEP - 1) / OZ_KSTEP) * S * OZ_NT * OZ_KSTEP; }
 inline int64_t oz_scale_elems(int m, int n) { return (int64_t)((m + 127) / 128) * 128 + (int64_t)((n + OZ_NT - 1) / OZ_NT) * OZ_NT; }

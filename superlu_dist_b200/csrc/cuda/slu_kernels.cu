@@ -5,7 +5,8 @@
 //   trsm_kernel<true>   U(k,:)     <- L_kk^-1 U(k,:)             (dUPanelTrSolve, dtrfCommWrapper.c:242-357)
 //   schur_setup_kernel  destination maps of one supernode       (index work of dscatter_l/dscatter_u,
 //                                                                 SRC/double/dscatter.c:138-174, 222-243)
-//   schur_kernel        V = L(below,k) U(k,:) on FP64 tensor cores (DMMA, mma.sync.m8n8k4.f64) with the
+//   schur_kernel_h      V = L(below,k) U(k,:) of the big tiles on FP64 tensor cores (mma.sync.m16n8k8.f64) with the
+//   schur_kernel        (small tiles and opt-in variants: mma.sync.m8n8k4.f64)
 //                       subtract-scatter fused into the epilogue: no bigV buffer
 //                                                                (dblock_gemm_scatter, SRC/double/dscatter3d.c:82-189)
 //   u_expand / u_pack   skyline <-> dense-packed U at the boundary (dRgather_U, SRC/double/dgather.c:256-398)
@@ -1078,6 +1079,26 @@ __device__ __forceinline__ void gemm_tile_v2(const double *__restrict__ A, int l
 // ------------------------------------------------------------------------------------------------
 // Schur-complement update of a batch of supernodes: GEMM tile + fused subtract-scatter epilogue
 // ------------------------------------------------------------------------------------------------
+// (tm, tn) of tile number `tile` of a supernode with BM x BN tiles.  mode 0: all tiles column by column; 1 (urgent): the
+// first tcu tile columns entirely, then the first tru tile rows of the rest; 2 (bulk): the others
+template <int BM, int BN>
+__device__ __forceinline__ void schur_tile_of(const NodeDesc &nd, int tile, int mode, int &tm, int &tn)
+{
+    const int tiles_m = (nd.m + BM - 1) / BM;
+    if (mode == 0) {
+        tm = tile % tiles_m; tn = tile / tiles_m;
+    } else {
+        const int tru = (nd.urg_rows + BM - 1) / BM, tcu = (nd.urg_cols + BN - 1) / BN;
+        if (mode == 1) {
+            if (tile < tiles_m * tcu) { tm = tile % tiles_m; tn = tile / tiles_m; }
+            else { const int t = tile - tiles_m * tcu; tm = t % tru; tn = tcu + t / tru; }
+        } else {
+            const int rm = tiles_m - tru;
+            tm = tru + tile % rm; tn = tcu + tile / rm;
+        }
+    }
+}
+
 template <int BM, int BN, int WARPS_M, int WARPS_N, bool ATOMIC, int BK = 16, int STAGES = 3, bool V2 = false, class LU = DeviceLU>
 __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, (32 * WARPS_M * WARPS_N <= 256) ? 2 : 1)
     schur_kernel(LU dd, Batch b, int mode, int split_n, int split_i)
@@ -1091,21 +1112,8 @@ __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, (32 * WARPS_M * WARPS_
     const int slot = find_slot(b.prefix, b.count, gt);
     const int k = b.nodes[slot];
     const NodeDesc nd = d.nodes[k];
-    const int tile = (int)(gt - b.prefix[slot]);
-    const int tiles_m = (nd.m + BM - 1) / BM;
     int tm, tn;
-    if (mode == 0) {
-        tm = tile % tiles_m; tn = tile / tiles_m;
-    } else {
-        const int tru = (nd.urg_rows + BM - 1) / BM, tcu = (nd.urg_cols + BN - 1) / BN;
-        if (mode == 1) {  // urgent: the first tcu tile columns entirely, then the first tru tile rows of the rest
-            if (tile < tiles_m * tcu) { tm = tile % tiles_m; tn = tile / tiles_m; }
-            else { const int t = tile - tiles_m * tcu; tm = t % tru; tn = tcu + t / tru; }
-        } else {
-            const int rm = tiles_m - tru;
-            tm = tru + tile % rm; tn = tcu + tile / rm;
-        }
-    }
+    schur_tile_of<BM, BN>(nd, (int)(gt - b.prefix[slot]), mode, tm, tn);
     const int m0 = tm * BM, n0 = tn * BN;
 
     double acc[C::MI][C::NI][2];
@@ -1181,6 +1189,207 @@ __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, (32 * WARPS_M * WARPS_
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// The Hopper main loop: mma.sync.m16n8k8.f64 (DMMA.16x8x8) on 64 x 32 warp tiles.  Per k8 step a warp issues 16 MMAs
+// fed by 12 16-byte shared loads (0.375 B of shared memory per FMA, against 0.5 with 32 x 32 tiles of DMMA.8x8x4).
+// The loader permutes the shared image so that every lane's fragment pairs are adjacent: rows g and g+8 of a 16-row
+// block of A (row r at prow(r)), k and k+4 of an 8-deep slice of B (at pk(k)).  A and B columns are only 8-byte
+// aligned in global memory (lda = nsupr, ldb = ns), so the copies stay 8-byte cp.async.
+// ------------------------------------------------------------------------------------------------
+template <int BM, int BN, int WARPS_M, int WARPS_N, int BK, int STAGES>
+struct HCfg {
+    static constexpr int NT = 32 * WARPS_M * WARPS_N;
+    static constexpr int WTM = BM / WARPS_M, WTN = BN / WARPS_N;
+    static constexpr int MT = WTM / 16, NT8 = WTN / 8;
+    static constexpr int LDA = BM + 4, LDB = BK + 8;  // == 4 and 8 (mod 16) doubles: conflict-free 16-byte fragment loads
+    static constexpr int A_STAGE = BK * LDA, B_STAGE = BN * LDB;
+    static constexpr size_t SMEM = sizeof(double) * STAGES * (A_STAGE + B_STAGE);
+    static_assert(WTM % 16 == 0 && WTN % 8 == 0 && BK % 8 == 0, "tile shape vs m16n8k8");
+};
+__device__ __forceinline__ int prow(int r) { return (r & ~15) | ((r & 7) << 1) | ((r >> 3) & 1); }
+__device__ __forceinline__ int pk(int k) { return (k & ~7) | ((k & 3) << 1) | ((k >> 2) & 1); }
+
+template <int BM, int BN, int WARPS_M, int WARPS_N, int BK, int STAGES>
+__device__ __forceinline__ void gemm_tile_h(const double *__restrict__ A, int lda, const double *__restrict__ B, int ldb,
+                                            int M, int N, int K, int m0, int n0, double *sm,
+                                            double (&acc)[BM / WARPS_M / 16][BN / WARPS_N / 8][4])
+{
+    using C = HCfg<BM, BN, WARPS_M, WARPS_N, BK, STAGES>;
+    constexpr int NW = C::NT / 32;
+    constexpr int CA = BK / NW, RA = BM / 32;       // A: columns per warp and 32-row slices per column
+    constexpr int CB = C::NT / BK, JB = BN / CB;    // B: columns per pass and passes
+    static_assert(BK % NW == 0 && BM % 32 == 0 && C::NT % BK == 0 && BN % CB == 0, "tile shape vs loader mapping");
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
+    const int wm0 = (warp % WARPS_M) * C::WTM, wn0 = (warp / WARPS_M) * C::WTN;
+    double *As = sm, *Bs = sm + STAGES * C::A_STAGE;
+    const int KT = (K + BK - 1) / BK;
+    const int KF = ((m0 + BM <= M) && (n0 + BN <= N)) ? K / BK : 0;  // k-steps the unpredicated loader serves
+
+    auto load = [&](int st, int kt) {  // edge tiles and the K tail: predicated, zero-filled
+        const int k0 = kt * BK;
+        double *as = As + st * C::A_STAGE, *bs = Bs + st * C::B_STAGE;
+#pragma unroll
+        for (int idx = tid; idx < BK * BM; idx += C::NT) {
+            const int kk = idx / BM, mm = idx - kk * BM;
+            const bool p = (m0 + mm < M) && (k0 + kk < K);
+            cp_async8(as + kk * C::LDA + prow(mm), p ? A + (size_t)(k0 + kk) * lda + m0 + mm : A, p);
+        }
+#pragma unroll
+        for (int idx = tid; idx < BK * BN; idx += C::NT) {
+            const int nn = idx / BK, kk = idx - nn * BK;
+            const bool p = (n0 + nn < N) && (k0 + kk < K);
+            cp_async8(bs + nn * C::LDB + pk(kk), p ? B + (size_t)(n0 + nn) * ldb + k0 + kk : B, p);
+        }
+    };
+    // running sources of the unpredicated loader (k-steps are issued in increasing order); each warp copies whole
+    // 32-row column slices of A, so the permuted destinations are a per-lane constant plus immediates
+    const double *pa = A + (size_t)warp * lda + m0 + lane;
+    const double *pb = B + (size_t)(n0 + tid / BK) * ldb + (tid % BK);
+    const size_t a_col = (size_t)NW * lda, a_step = (size_t)BK * lda, b_col = (size_t)CB * ldb;
+    double *const sa = As + warp * C::LDA + prow(lane), *const sb = Bs + (tid / BK) * C::LDB + pk(tid % BK);
+    auto load_fast = [&](int st) {
+        double *as = sa + st * C::A_STAGE, *bs = sb + st * C::B_STAGE;
+        const double *p = pa;
+#pragma unroll
+        for (int c = 0; c < CA; ++c) {
+#pragma unroll
+            for (int r = 0; r < RA; ++r) cp_async8_plain(as + c * NW * C::LDA + 32 * r, p + 32 * r);
+            p += a_col;
+        }
+        const double *q = pb;
+#pragma unroll
+        for (int j = 0; j < JB; ++j) {
+            cp_async8_plain(bs + j * CB * C::LDB, q);
+            q += b_col;
+        }
+        pa += a_step;
+        pb += BK;
+    };
+    auto issue = [&](int st, int kt) {
+        if (kt < KF) load_fast(st);
+        else load(st, kt);
+    };
+
+#pragma unroll
+    for (int s = 0; s < STAGES - 1; ++s) {
+        if (s < KT) issue(s, s);
+        cp_async_commit();
+    }
+    for (int kt = 0; kt < KT; ++kt) {
+        cp_async_wait<STAGES - 2>();
+        __syncthreads();
+        if (kt + STAGES - 1 < KT) issue((kt + STAGES - 1) % STAGES, kt + STAGES - 1);
+        cp_async_commit();
+        const double *as = As + (kt % STAGES) * C::A_STAGE + t * C::LDA + wm0 + 2 * g;
+        const double *bs = Bs + (kt % STAGES) * C::B_STAGE + (wn0 + g) * C::LDB + 2 * t;
+#pragma unroll
+        for (int k8 = 0; k8 < BK / 8; ++k8) {
+            double a[C::MT][4], bb[C::NT8][2];
+#pragma unroll
+            for (int mt = 0; mt < C::MT; ++mt) {
+                const double2 lo = *reinterpret_cast<const double2 *>(as + k8 * 8 * C::LDA + 16 * mt);
+                const double2 hi = *reinterpret_cast<const double2 *>(as + (k8 * 8 + 4) * C::LDA + 16 * mt);
+                a[mt][0] = lo.x; a[mt][1] = lo.y; a[mt][2] = hi.x; a[mt][3] = hi.y;
+            }
+#pragma unroll
+            for (int nt = 0; nt < C::NT8; ++nt) {
+                const double2 v = *reinterpret_cast<const double2 *>(bs + 8 * nt * C::LDB + 8 * k8);
+                bb[nt][0] = v.x; bb[nt][1] = v.y;
+            }
+#pragma unroll
+            for (int mt = 0; mt < C::MT; ++mt)
+#pragma unroll
+                for (int nt = 0; nt < C::NT8; ++nt) dmma1688(acc[mt][nt], a[mt], bb[nt]);
+        }
+    }
+    cp_async_wait<0>();
+}
+
+// Schur update on the Hopper main loop: the tile enumeration (modes, Z split) and destination maps of schur_kernel,
+// atomic scatter.  Thread (g, t) of a warp holds rows 16 mt + g + 8 h and columns 8 nt + 2 t + e of its warp tile.
+template <int BM, int BN, int WARPS_M, int WARPS_N, int BK, int STAGES, int MINB, class LU = DeviceLU>
+__global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, MINB)
+    schur_kernel_h(LU dd, Batch b, int mode, int split_n, int split_i)
+{
+    using C = HCfg<BM, BN, WARPS_M, WARPS_N, BK, STAGES>;
+    extern __shared__ __align__(16) double sm[];
+    const DeviceLU &d = member_view(dd);
+    const int64_t gt = (int64_t)blockIdx.x * split_n + split_i;
+    if (gt >= b.prefix[b.count]) return;
+    const int slot = find_slot(b.prefix, b.count, gt);
+    const int k = b.nodes[slot];
+    const NodeDesc nd = d.nodes[k];
+    int tm, tn;
+    schur_tile_of<BM, BN>(nd, (int)(gt - b.prefix[slot]), mode, tm, tn);
+    const int m0 = tm * BM, n0 = tn * BN;
+
+    double acc[C::MT][C::NT8][4];
+#pragma unroll
+    for (int mt = 0; mt < C::MT; ++mt)
+#pragma unroll
+        for (int nt = 0; nt < C::NT8; ++nt) acc[mt][nt][0] = acc[mt][nt][1] = acc[mt][nt][2] = acc[mt][nt][3] = 0.0;
+    gemm_tile_h<BM, BN, WARPS_M, WARPS_N, BK, STAGES>(d.val + nd.lval + nd.ns, nd.nsupr, d.val + nd.uval, nd.ns, nd.m,
+                                                      nd.ncols, nd.ns, m0, n0, sm, acc);
+
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int wm0 = m0 + (warp % WARPS_M) * C::WTM + (lane >> 2), wn0 = n0 + (warp / WARPS_M) * C::WTN + 2 * (lane & 3);
+    const RowInfo *rinfo = d.rowinfo + nd.ws_row;
+    const ColInfo *cinfo = d.colinfo + nd.ws_col;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        RowInfo ri[C::MT];
+        bool rok[C::MT];
+#pragma unroll
+        for (int mt = 0; mt < C::MT; ++mt) {
+            const int i = wm0 + 16 * mt + 8 * h;
+            rok[mt] = i < nd.m;
+            if (rok[mt]) ri[mt] = rinfo[i];
+        }
+#pragma unroll
+        for (int nt = 0; nt < C::NT8; ++nt) {
+            int64_t idx[2][C::MT];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int j = wn0 + 8 * nt + e;
+                const bool cok = j < nd.ncols;
+                ColInfo cj;
+                if (cok) cj = cinfo[j];
+#pragma unroll
+                for (int mt = 0; mt < C::MT; ++mt) {
+                    idx[e][mt] = -1;
+                    if (!cok || !rok[mt]) continue;
+                    const int i = wm0 + 16 * mt + 8 * h;
+                    if (ri[mt].ib >= cj.jb) {
+                        const int p = d.lrel[cj.lrel_off + i];
+                        if (p >= 0) idx[e][mt] = cj.lbase + p;
+                    } else {
+                        const int q = d.urel[ri[mt].urel_off + j];
+                        if (q >= 0) idx[e][mt] = ri[mt].ubase + (int64_t)q * ri[mt].ldu;
+                    }
+                }
+            }
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+#pragma unroll
+                for (int mt = 0; mt < C::MT; ++mt)
+                    if (idx[e][mt] >= 0) atomicAdd(d.val + idx[e][mt], flip_sign(acc[mt][nt][2 * h + e]));
+        }
+    }
+}
+
+// the tile of schur_kernel_h on the Schur path (SCHUR_BM_BIG x SCHUR_BN_TILE: the host plan enumerates these tiles)
+#define SCHUR_H_TILE SCHUR_BM_BIG, SCHUR_BN_TILE, 2, 2, 16, 3, 2
+template <int BM, int BN, int WARPS_M, int WARPS_N, int BK, int STAGES, int MINB, class LU>
+static int launch_schur_h(const LU &d, const Batch &b, int64_t ctas, int mode, int split_n, int split_i, cudaStream_t s)
+{
+    using C = HCfg<BM, BN, WARPS_M, WARPS_N, BK, STAGES>;
+    static std::atomic<unsigned long long> attr_0{0};
+    ensure_dyn_smem(schur_kernel_h<BM, BN, WARPS_M, WARPS_N, BK, STAGES, MINB, LU>, (int)C::SMEM, attr_0);
+    const int64_t grid = (ctas + split_n - 1) / split_n;
+    schur_kernel_h<BM, BN, WARPS_M, WARPS_N, BK, STAGES, MINB, LU><<<member_grid(d, (unsigned)grid), C::NT, C::SMEM, s>>>(d, b, mode, split_n, split_i);
+    return 1;
+}
+
 template <int BM, int BN, int WARPS_M, int WARPS_N, bool ATOMIC, int BK = 16, int STAGES = 3, bool V2 = false, class LU = DeviceLU>
 static int launch_schur_t(const LU &d, const Batch &b, int64_t ctas, int mode, int split_n, int split_i, cudaStream_t s)
 {
@@ -1196,8 +1405,9 @@ int launch_schur(const DeviceLU &d, const Batch &b, int64_t ctas, int big, int a
                  int split_i, int wide, cudaStream_t s)
 {
     if (b.count <= 0 || ctas <= 0) return 0;
-    // default: the running-pointer loader (gemm_tile_v2).
+    // default: the Hopper main loop for the big class, the running-pointer loader (gemm_tile_v2) for small tiles.
     // variant 6 = the round-1 general loader, kept for A/B runs.
+    if (variant == 0 && big) return launch_schur_h<SCHUR_H_TILE>(d, b, ctas, mode, split_n, split_i, s);
     if (variant == 0) variant = 4;
     if (variant == 6) variant = 0;
     if (variant == 4 || variant == 5) {  // strength-reduced loader + sign flip off the FP64 pipe (4), with BK = 32 (5)
@@ -1222,7 +1432,7 @@ int launch_schur(const BatchedLU &d, const Batch &b, int64_t ctas, int big, int 
 {
     if (b.count <= 0 || ctas <= 0) return 0;
     if (!big) return launch_schur_t<SCHUR_BM_SMALL, SCHUR_BN_SMALL, 2, 2, true, 16, 3, true>(d, b, ctas, mode, 1, 0, s);
-    return launch_schur_t<128, 64, 4, 2, true, 16, 3, true>(d, b, ctas, mode, 1, 0, s);
+    return launch_schur_h<SCHUR_H_TILE>(d, b, ctas, mode, 1, 0, s);
 }
 
 // plain C -= A*B with the same main loop (kernel-level test and micro-benchmark of tile configurations)
@@ -1270,11 +1480,62 @@ static int launch_gemm_sub_t(int m, int n, int k, const double *a, int lda, cons
     return 1;
 }
 
+// the same on the Hopper main loop (gemm_tile_h)
+template <int BM, int BN, int WARPS_M, int WARPS_N, int BK, int STAGES, int MINB>
+__global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, MINB)
+    gemm_sub_kernel_h(int M, int N, int K, const double *A, int lda, const double *B, int ldb, double *Cm, int ldc)
+{
+    using C = HCfg<BM, BN, WARPS_M, WARPS_N, BK, STAGES>;
+    extern __shared__ __align__(16) double sm[];
+    const int tiles_m = (M + BM - 1) / BM;
+    const int m0 = (blockIdx.x % tiles_m) * BM, n0 = (blockIdx.x / tiles_m) * BN;
+    double acc[C::MT][C::NT8][4];
+#pragma unroll
+    for (int mt = 0; mt < C::MT; ++mt)
+#pragma unroll
+        for (int nt = 0; nt < C::NT8; ++nt) acc[mt][nt][0] = acc[mt][nt][1] = acc[mt][nt][2] = acc[mt][nt][3] = 0.0;
+    gemm_tile_h<BM, BN, WARPS_M, WARPS_N, BK, STAGES>(A, lda, B, ldb, M, N, K, m0, n0, sm, acc);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int wm0 = m0 + (warp % WARPS_M) * C::WTM + (lane >> 2), wn0 = n0 + (warp / WARPS_M) * C::WTN + 2 * (lane & 3);
+#pragma unroll
+    for (int nt = 0; nt < C::NT8; ++nt)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int j = wn0 + 8 * nt + e;
+            if (j >= N) continue;
+#pragma unroll
+            for (int mt = 0; mt < C::MT; ++mt)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int i = wm0 + 16 * mt + 8 * h;
+                    if (i < M) atomicAdd(Cm + (size_t)j * ldc + i, flip_sign(acc[mt][nt][2 * h + e]));
+                }
+        }
+}
+
+template <int BM, int BN, int WARPS_M, int WARPS_N, int BK, int STAGES, int MINB>
+static int launch_gemm_sub_h(int m, int n, int k, const double *a, int lda, const double *b, int ldb, double *c, int ldc,
+                             cudaStream_t s)
+{
+    using C = HCfg<BM, BN, WARPS_M, WARPS_N, BK, STAGES>;
+    static std::atomic<unsigned long long> attr_0{0};
+    ensure_dyn_smem(gemm_sub_kernel_h<BM, BN, WARPS_M, WARPS_N, BK, STAGES, MINB>, (int)C::SMEM, attr_0);
+    const int64_t ctas = (int64_t)((m + BM - 1) / BM) * ((n + BN - 1) / BN);
+    gemm_sub_kernel_h<BM, BN, WARPS_M, WARPS_N, BK, STAGES, MINB><<<(unsigned)ctas, C::NT, C::SMEM, s>>>(m, n, k, a, lda, b, ldb, c, ldc);
+    return 1;
+}
+
 int launch_gemm_sub(int m, int n, int k, const double *a, int lda, const double *b, int ldb, double *c, int ldc,
                     int variant, cudaStream_t s)
 {
     if (m <= 0 || n <= 0) return 0;
     switch (variant) {
+    // 30..: the Hopper main loop (gemm_tile_h, DMMA.16x8x8, 64 x 32 warp tiles)
+    case 30: return launch_gemm_sub_h<128, 64, 2, 2, 16, 3, 2>(m, n, k, a, lda, b, ldb, c, ldc, s);
+    case 31: return launch_gemm_sub_h<128, 64, 2, 2, 32, 2, 2>(m, n, k, a, lda, b, ldb, c, ldc, s);
+    case 32: return launch_gemm_sub_h<128, 128, 2, 4, 16, 4, 1>(m, n, k, a, lda, b, ldb, c, ldc, s);
+    case 33: return launch_gemm_sub_h<128, 128, 2, 4, 32, 3, 1>(m, n, k, a, lda, b, ldb, c, ldc, s);
+    case 34: return launch_gemm_sub_h<64, 64, 1, 2, 16, 3, 3>(m, n, k, a, lda, b, ldb, c, ldc, s);    // 2 warps, 3 CTAs/SM
     case 20: return launch_gemm_sub_t<128, 64, 4, 2, 16, 3, 2>(m, n, k, a, lda, b, ldb, c, ldc, s);   // round-1 default loader
     case 21: return launch_gemm_sub_t<32, 32, 2, 2, 16, 3, 2>(m, n, k, a, lda, b, ldb, c, ldc, s);
     case 1: return launch_gemm_sub_t<128, 64, 4, 2, 16, 4, 2>(m, n, k, a, lda, b, ldb, c, ldc, s);
@@ -1299,7 +1560,7 @@ int launch_gemm_sub(int m, int n, int k, const double *a, int lda, const double 
     case 19: return launch_gemm_sub_t<128, 128, 4, 4, 16, 3, 1, true>(m, n, k, a, lda, b, ldb, c, ldc, s);
     default: break;
     }
-    if (m >= 96 && n >= 96) return launch_gemm_sub_t<128, 64, 4, 2, 16, 3, 2, true>(m, n, k, a, lda, b, ldb, c, ldc, s);
+    if (m >= 96 && n >= 96) return launch_gemm_sub_h<SCHUR_H_TILE>(m, n, k, a, lda, b, ldb, c, ldc, s);
     return launch_gemm_sub_t<32, 32, 2, 2, 16, 3, 2, true>(m, n, k, a, lda, b, ldb, c, ldc, s);
 }
 

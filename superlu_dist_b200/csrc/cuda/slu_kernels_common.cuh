@@ -81,6 +81,15 @@ __device__ __forceinline__ void dmma884(double &d0, double &d1, double a, double
                  : "+d"(d0), "+d"(d1)
                  : "d"(a), "d"(b));
 }
+// d(16x8) += a(16x8) b(8x8), sm_90 (SASS DMMA.16x8x8: 8x the work of DMMA.8x8x4 per instruction).  Lane l with
+// g = l/4, t = l%4 holds a = {A(g,t), A(g+8,t), A(g,t+4), A(g+8,t+4)}, b = {B(t,g), B(t+4,g)} and
+// d = {D(g,2t), D(g,2t+1), D(g+8,2t), D(g+8,2t+1)}.
+__device__ __forceinline__ void dmma1688(double (&d)[4], const double (&a)[4], const double (&b)[2])
+{
+    asm("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+        : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
+        : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
+}
 
 // ------------------------------------------------------------------------------------------------
 // destination maps of the Schur update of supernode k
