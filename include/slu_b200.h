@@ -119,7 +119,8 @@ typedef struct {
     int32_t my_supernodes;        /* supernodes this rank factored                           */
     double reserved[8];           /* [0] ms spent slicing (verbose >= 2), [1] Schur flops taken by the */
                                   /* tcgen05 path, [2] bytes of its int8 workspace, [3] slices in use,  */
-                                  /* [4] seconds of the last slu_b200_solve, [5] its kernel launches    */
+                                  /* [4] seconds of the last slu_b200_solve or _solve_trans, [5] its    */
+                                  /* kernel launches                                                    */
 } slu_b200_stats_t;
 
 typedef struct slu_b200_handle_s *slu_b200_handle_t;
@@ -161,6 +162,16 @@ int slu_b200_fill_csr(slu_b200_handle_t h, int n, const int32_t *rowptr, const i
  * 1 x 1 x Pz grids: collective, every rank passes the same b and receives the full x (NCCL all-reduces along Z
  * replace the ancestor reduce / dbroadcastAncestor3d, pd3dcomm.c:1145).  stats.reserved[4] = seconds of the call. */
 int slu_b200_solve(slu_b200_handle_t h, double *x, int ldx, int nrhs);
+/* Solve op(A) x = b on the same resident factors, as LAPACK getrs(trans) / SuperLU dgstrs(trans): trans takes the values
+ * of the reference's trans_t (SRC/include/superlu_enum_consts.h:34): 0 = NOTRANS (exactly slu_b200_solve), 1 = TRANS
+ * (A^T x = b), 2 = CONJ (A^H x = b; the same as 1 in double).  A^T = U^T L^T is solved as U^T y = b, then L^T x = y, over
+ * the level plan of the plain solve: no second analysis or factorization of A^T, no second copy of the factors.  Uses:
+ * adjoint solves for gradients and sensitivities, 1-norm condition estimation.  x, ldx, nrhs, the restrictions (a
+ * successful factorization, 1 x 1 x Pz, the cooperative schedule along Z) and stats.reserved[4] / [5] (the last solve of
+ * either kind) are those of slu_b200_solve.  x uses the ordering of the factored matrix F = P A P^T; since
+ * F^T = P A^T P^T, the caller permutes b and x exactly as for the plain solve.  trans outside {0, 1, 2} fails.
+ * The reference's pdgstrs3d has no transposed mode. */
+int slu_b200_solve_trans(slu_b200_handle_t h, double *x, int ldx, int nrhs, int trans);
 int slu_b200_get_stats(slu_b200_handle_t h, slu_b200_stats_t *out);
 void slu_b200_destroy(slu_b200_handle_t h);
 
@@ -215,7 +226,7 @@ int slu_b200_k_rerun_schur(slu_b200_handle_t h, int level, int reps, float *ms);
  * A batched handle takes only these calls plus slu_b200_get_stats and slu_b200_destroy; every other call on it fails,
  * and these fail on an unbatched handle.  Stats describe the whole handle: ops_fact, ops_schur, nnz_l, nnz_u and
  * lu_device_bytes are batch x the per-member values, tiny_pivots is summed over the members, t_factor_s is the device
- * time of the one batched call, stats.reserved[4] / [5] describe the last slu_b200_batch_solve.
+ * time of the one batched call, stats.reserved[4] / [5] describe the last slu_b200_batch_solve or _batch_solve_trans.
  * Measured on an NVIDIA H100 80GB HBM3 at a 400 W power limit, per member, against one unbatched handle looping over
  * the members: Poisson 16^3, B = 64: factor 0.081 vs 1.337 ms (16.5x), solve (nrhs 1) 0.039 vs 0.872 ms; Poisson 32^3,
  * B = 64: factor 1.41 vs 5.53 ms (3.9x); more in README.md. */
@@ -229,6 +240,8 @@ int slu_b200_batch_factor(slu_b200_handle_t h, int *info);
 /* x: batch blocks, block j at x + j*ldx*nrhs, each n x nrhs column-major (ldx >= n), ordering of the factored matrix;
  * b on entry, the solution on return.  Fails, naming the member, unless every member's last info was 0. */
 int slu_b200_batch_solve(slu_b200_handle_t h, double *x, int ldx, int nrhs);
+/* op(A_j) x_j = b_j for every member, trans as slu_b200_solve_trans; x and the restrictions as slu_b200_batch_solve */
+int slu_b200_batch_solve_trans(slu_b200_handle_t h, double *x, int ldx, int nrhs, int trans);
 /* write member j's L/U into the view's Lnzval / Unzval arrays, in the reference layout (as slu_b200_download) */
 int slu_b200_batch_download(slu_b200_handle_t h, int member);
 /* ---- doublecomplex twins (SRC/complex16/pzgstrf3d.c:120; the reference's z* handle API,
@@ -239,10 +252,11 @@ int slu_b200_batch_download(slu_b200_handle_t h, int member);
  * the precision-independent 2*m*n*k for the Schur update, sec_structs.c:692-693).
  * slu_b200_z_fill_csr and slu_b200_z_solve follow the same convention: val and x point at interleaved
  * doublecomplex, and n, ldx, nnz count complex elements.  The solve (the role of pzgstrs3d,
- * SRC/complex16/pzgstrs3d.c) has the restrictions of slu_b200_solve.
+ * SRC/complex16/pzgstrs3d.c) has the restrictions of slu_b200_solve.  slu_b200_z_solve_trans solves A^T x = b (trans 1)
+ * or A^H x = b (trans 2: every factor entry, the pivots included, is read conjugated), as slu_b200_solve_trans.
  * Checked on an H100 by tests/test_gpu_variants_complex.py: kernels vs NumPy, cg20 vs the reference's pzgstrf3d
- * factors, pzdrive3d drop-in; and by tests/test_gpu_solve_complex.py: solves on the resident factors, device-side
- * distribution. */
+ * factors, pzdrive3d drop-in; by tests/test_gpu_solve_complex.py: solves on the resident factors, device-side
+ * distribution; and by tests/test_gpu_solve_trans.py: transposed and conjugate-transposed solves against SciPy. */
 typedef struct slu_b200_zhandle_s *slu_b200_zhandle_t;
 int slu_b200_z_create(slu_b200_zhandle_t *h, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt);
 int slu_b200_z_upload(slu_b200_zhandle_t h);
@@ -252,6 +266,7 @@ int slu_b200_z_download(slu_b200_zhandle_t h);
 int slu_b200_z_fill_csr(slu_b200_zhandle_t h, int n, const int32_t *rowptr, const int32_t *colind, const double *val,
                         const int32_t *perm);
 int slu_b200_z_solve(slu_b200_zhandle_t h, double *x, int ldx, int nrhs);
+int slu_b200_z_solve_trans(slu_b200_zhandle_t h, double *x, int ldx, int nrhs, int trans);
 /* batched doublecomplex handles (the reference's pzgssvx3d_csc_batch, SRC/complex16/pzgssvx3d_csc_batch.c:80): the
  * slu_b200_batch_* calls above with the same semantics, restrictions and stats; val and x point at interleaved
  * doublecomplex, n, ldx and nnz count complex elements.  Stats through slu_b200_z_get_stats, slu_b200_z_destroy frees.
@@ -263,6 +278,7 @@ int slu_b200_z_batch_fill_csr(slu_b200_zhandle_t h, int n, const int32_t *rowptr
                               const double *val, const int32_t *perm);
 int slu_b200_z_batch_factor(slu_b200_zhandle_t h, int *info);
 int slu_b200_z_batch_solve(slu_b200_zhandle_t h, double *x, int ldx, int nrhs);
+int slu_b200_z_batch_solve_trans(slu_b200_zhandle_t h, double *x, int ldx, int nrhs, int trans);
 int slu_b200_z_batch_download(slu_b200_zhandle_t h, int member);
 int slu_b200_z_get_stats(slu_b200_zhandle_t h, slu_b200_stats_t *out);
 int slu_b200_z_plan(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, slu_b200_stats_t *stats);

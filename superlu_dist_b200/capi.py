@@ -112,6 +112,8 @@ def lib():
     L.slu_b200_z_batch_factor.argtypes = [C.c_void_p, C.c_void_p]
     L.slu_b200_z_batch_solve.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
     L.slu_b200_z_batch_download.argtypes = [C.c_void_p, C.c_int]
+    for f in ("slu_b200_solve_trans", "slu_b200_z_solve_trans", "slu_b200_batch_solve_trans", "slu_b200_z_batch_solve_trans"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
     _lib = L
     return L
 
@@ -128,6 +130,19 @@ def _fn(name, complex_):
 def _check(rc):
     if rc != 0:
         raise RuntimeError("libslu_b200: " + lib().slu_b200_last_error().decode())
+
+
+_TRANS = {"N": 0, "T": 1, "H": 2}   # the reference's trans_t: NOTRANS, TRANS, CONJ
+
+
+def _solve_call(name, complex_, trans):
+    """The solve entry point for trans 'N' | 'T' | 'H' (as SciPy's SuperLU.solve): (function, extra arguments).  'N' is
+    the plain call (slu_b200_<name>), the others the _trans twin; 'H' of a real problem is 'T'."""
+    if trans not in _TRANS:
+        raise ValueError(f"trans must be 'N', 'T' or 'H', not {trans!r}")
+    if trans == "N":
+        return _fn(name, complex_), ()
+    return _fn(name + "_trans", complex_), (_TRANS[trans],)
 
 
 def device_count():
@@ -286,12 +301,14 @@ class Handle:
         _check(_fn("fill_csr", self.z_)(self.h, len(rp) - 1, rp.ctypes.data_as(C.c_void_p), ci.ctypes.data_as(C.c_void_p),
                                         v.ctypes.data_as(C.c_void_p), pm.ctypes.data_as(C.c_void_p)))
 
-    def solve(self, b):
+    def solve(self, b, trans="N"):
         """L U x = b on the device-resident factors (slu_b200_solve / slu_b200_z_solve); b: (n,) or (nrhs, n), ordering
-        of the factored matrix, complex128 for a complex problem.  Returns x with the same shape and dtype."""
+        of the factored matrix, complex128 for a complex problem.  Returns x with the same shape and dtype.
+        trans = 'T' solves A^T x = b, 'H' A^H x = b (slu_b200_solve_trans / slu_b200_z_solve_trans) on the same factors."""
+        fn, extra = _solve_call("solve", self.z_, trans)
         x = np.array(b, self._dtype(), order="C", copy=True)
         nrhs = 1 if x.ndim == 1 else x.shape[0]
-        _check(_fn("solve", self.z_)(self.h, x.ctypes.data_as(C.c_void_p), self.prob.n, nrhs))
+        _check(fn(self.h, x.ctypes.data_as(C.c_void_p), self.prob.n, nrhs, *extra))
         return x
 
     def _dtype(self):
@@ -348,13 +365,15 @@ class BatchHandle:
         _check(_fn("batch_factor", self.z_)(self.h, info.ctypes.data_as(C.c_void_p)))
         return info
 
-    def solve(self, b):
-        """L_j U_j x_j = b_j for every member; b: (batch, n) or (batch, nrhs, n), ordering of the factored matrix."""
+    def solve(self, b, trans="N"):
+        """L_j U_j x_j = b_j for every member; b: (batch, n) or (batch, nrhs, n), ordering of the factored matrix.
+        trans = 'T' / 'H' solves A_j^T x_j = b_j / A_j^H x_j = b_j (slu_b200_batch_solve_trans)."""
+        fn, extra = _solve_call("batch_solve", self.z_, trans)
         x = np.array(b, self._dtype(), order="C", copy=True)
         if x.ndim not in (2, 3) or x.shape[0] != self.batch or x.shape[-1] != self.prob.n:
             raise ValueError(f"b must have shape ({self.batch}, n) or ({self.batch}, nrhs, n) with n = {self.prob.n}")
         nrhs = 1 if x.ndim == 2 else x.shape[1]
-        _check(_fn("batch_solve", self.z_)(self.h, x.ctypes.data_as(C.c_void_p), self.prob.n, nrhs))
+        _check(fn(self.h, x.ctypes.data_as(C.c_void_p), self.prob.n, nrhs, *extra))
         return x
 
     def download(self, member):

@@ -29,6 +29,7 @@
 #define slu_b200_download slu_b200_z_download
 #define slu_b200_fill_csr slu_b200_z_fill_csr
 #define slu_b200_solve slu_b200_z_solve
+#define slu_b200_solve_trans slu_b200_z_solve_trans
 #define slu_b200_get_stats slu_b200_z_get_stats
 #define slu_b200_destroy slu_b200_z_destroy
 #define slu_b200_plan slu_b200_z_plan
@@ -41,6 +42,7 @@
 #define slu_b200_batch_fill_csr slu_b200_z_batch_fill_csr
 #define slu_b200_batch_factor slu_b200_z_batch_factor
 #define slu_b200_batch_solve slu_b200_z_batch_solve
+#define slu_b200_batch_solve_trans slu_b200_z_batch_solve_trans
 #define slu_b200_batch_download slu_b200_z_batch_download
 #define SLU_API "slu_b200_z_"     // name prefix of the exported calls, for error messages
 #else
@@ -1697,14 +1699,40 @@ int slu_b200_fill_csr(slu_b200_handle_t H, int n, const int32_t *rowptr, const i
 // pd3dcomm.c:1145); a last all-reduce of the owned pieces gives every rank the full solution.  In doublecomplex xh holds
 // (re, im) pairs and n, ldx count complex elements; the all-reduces sum 2 * len doubles (a componentwise sum is the
 // complex sum).
-int slu_b200_solve(slu_b200_handle_t H, double *xh, int ldx, int nrhs)
+// trans = 1 / 2 solves A^T x = b / A^H x = b on the same factors: U^T forward, L^T backward, in the same level order and with
+// the same all-reduces along Z, because the forward scatter and the backward gather reach ancestors only, as in the plain
+// solve.
+
+// One level of one pass: the diagonal solve and the update, in the order of the pass (forward: diagonal first).  The update
+// streams the L panel (plain forward, transposed backward) or the U panel, tiled by sl_prefix / su_prefix.  A template for
+// both handle kinds, hence outside the extern "C" block.
+}  // extern "C"
+template <class LU>
+static int solve_level(const slu_b200_handle_s *H, const LU &d, const LevelPlan &L, bool backward, int trans, val_t *x, int n, int nrhs,
+                       cudaStream_t s)
+{
+    const int32_t *nodes = H->d_pool_i32.p + L.nodes_off;
+    const int64_t *p64 = H->d_pool_i64.p;
+    const bool upanel = backward == (trans == 0);
+    const Batch b{nodes, p64 + (upanel ? L.su_prefix : L.sl_prefix), L.count};
+    int launches = 0;
+    if (!backward) launches += launch_solve_diag(d, nodes, L.count, false, trans, x, n, nrhs, s);
+    launches += launch_solve_update(d, b, upanel ? L.su_ctas : L.sl_ctas, backward, trans, x, n, nrhs, s);
+    if (backward) launches += launch_solve_diag(d, nodes, L.count, true, trans, x, n, nrhs, s);
+    return launches;
+}
+extern "C" {
+
+// fn: "solve" or "solve_trans", for the messages
+static int solve_impl(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int trans, const char *fn)
 {
     if (!H || !xh) return fail("null argument");
-    if (refuse_batched(H, SLU_API "solve")) return -1;
-    if (!H->factored) return fail("slu_b200_solve needs a successful slu_b200_factor on this handle first");
+    if (refuse_batched(H, (std::string(SLU_API) + fn).c_str())) return -1;
+    if (trans < 0 || trans > 2) return fail(SLU_API "%s: trans = %d, must be 0 (A x = b), 1 (A^T x = b) or 2 (A^H x = b)", fn, trans);
+    if (!H->factored) return fail("slu_b200_%s needs a successful slu_b200_factor on this handle first", fn);
     if (nrhs < 1 || ldx < H->n) return fail("bad nrhs / ldx");
-    if (H->P2 > 1) return fail("slu_b200_solve: Pr x Pc > 1 is not supported yet (1 x 1 x Pz only)");
-    if (H->comm && !H->coop) return fail("slu_b200_solve: the Z-distributed solve needs the cooperative schedule (options.reserved[1] = 0)");
+    if (H->P2 > 1) return fail("slu_b200_%s: Pr x Pc > 1 is not supported yet (1 x 1 x Pz only)", fn);
+    if (H->comm && !H->coop) return fail("slu_b200_%s: the Z-distributed solve needs the cooperative schedule (options.reserved[1] = 0)", fn);
     const int n = H->n;
     const size_t len = (size_t)n * nrhs;
     if (H->d_x.n < len && (H->d_x.alloc(len) || H->d_x2.alloc(len))) return -1;
@@ -1724,8 +1752,7 @@ int slu_b200_solve(slu_b200_handle_t H, double *xh, int ldx, int nrhs)
     } else {
         CU(cudaMemcpyAsync(x, x2, len * sizeof(val_t), cudaMemcpyDeviceToDevice, s));
     }
-    const int64_t *p64 = H->d_pool_i64.p;
-    // forward: L y = b
+    // forward: L y = b (U^T y = b)
     size_t li = 0;
     for (int zl = 0; zl < H->max_lvl; ++zl) {
         if (multi && zl >= 1) {
@@ -1735,12 +1762,10 @@ int slu_b200_solve(slu_b200_handle_t H, double *xh, int ldx, int nrhs)
         for (; li < H->levels.size() && H->levels[li].zlvl <= zl; ++li) {
             const LevelPlan &L = H->levels[li];
             if (L.zlvl < zl || H->my_zero[zl]) continue;
-            const int32_t *nodes = H->d_pool_i32.p + L.nodes_off;
-            launches += launch_solve_diag(d, nodes, L.count, false, x, n, nrhs, s);
-            launches += launch_solve_update(d, Batch{nodes, p64 + L.sl_prefix, L.count}, L.sl_ctas, false, x, n, nrhs, s);
+            launches += solve_level(H, d, L, false, trans, x, n, nrhs, s);
         }
     }
-    // backward: U x = y
+    // backward: U x = y (L^T x = y)
     li = H->levels.size();
     for (int zl = H->max_lvl - 1; zl >= 0; --zl) {
         size_t lo = li;
@@ -1749,9 +1774,7 @@ int slu_b200_solve(slu_b200_handle_t H, double *xh, int ldx, int nrhs)
             for (size_t q = li; q-- > lo;) {
                 const LevelPlan &L = H->levels[q];
                 if (L.zlvl != zl) continue;
-                const int32_t *nodes = H->d_pool_i32.p + L.nodes_off;
-                launches += launch_solve_update(d, Batch{nodes, p64 + L.su_prefix, L.count}, L.su_ctas, true, x, n, nrhs, s);
-                launches += launch_solve_diag(d, nodes, L.count, true, x, n, nrhs, s);
+                launches += solve_level(H, d, L, true, trans, x, n, nrhs, s);
             }
         li = lo;
         if (multi && zl >= 1) {
@@ -1774,6 +1797,16 @@ int slu_b200_solve(slu_b200_handle_t H, double *xh, int ldx, int nrhs)
     H->st.reserved[4] = now_s() - t0;      // seconds of the last solve (H2D of b and D2H of x included)
     H->st.reserved[5] = (double)launches;
     return 0;
+}
+
+int slu_b200_solve(slu_b200_handle_t H, double *xh, int ldx, int nrhs)
+{
+    return solve_impl(H, xh, ldx, nrhs, 0, "solve");
+}
+
+int slu_b200_solve_trans(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int trans)
+{
+    return solve_impl(H, xh, ldx, nrhs, trans, "solve_trans");
 }
 
 #ifndef SLU_COMPLEX
@@ -1952,18 +1985,20 @@ int slu_b200_batch_factor(slu_b200_handle_t H, int *info)
     return 0;
 }
 
-// x: batch blocks, block j at x + j * ldx * nrhs, each n x nrhs column-major (ldx >= n): b on entry, the solution on return
-int slu_b200_batch_solve(slu_b200_handle_t H, double *xh, int ldx, int nrhs)
+// x: batch blocks, block j at x + j * ldx * nrhs, each n x nrhs column-major (ldx >= n): b on entry, the solution on return.
+// trans as solve_impl; fn: "batch_solve" or "batch_solve_trans", for the messages
+static int batch_solve_impl(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int trans, const char *fn)
 {
     if (!H || !xh) return fail("null argument");
-    if (refuse_unbatched(H, SLU_API "batch_solve")) return -1;
+    if (refuse_unbatched(H, (std::string(SLU_API) + fn).c_str())) return -1;
+    if (trans < 0 || trans > 2) return fail(SLU_API "%s: trans = %d, must be 0 (A x = b), 1 (A^T x = b) or 2 (A^H x = b)", fn, trans);
     const int B = H->batch, n = H->n;
     for (int j = 0; j < B; ++j) {
-        if (H->member_info[j] < 0) return fail(SLU_API "batch_solve needs a " SLU_API "batch_factor of the filled members first");
-        if (H->member_info[j] > 0) return fail(SLU_API "batch_solve: member %d has an exact zero pivot in column %d", j, H->member_info[j]);
+        if (H->member_info[j] < 0) return fail(SLU_API "%s needs a " SLU_API "batch_factor of the filled members first", fn);
+        if (H->member_info[j] > 0) return fail(SLU_API "%s: member %d has an exact zero pivot in column %d", fn, j, H->member_info[j]);
     }
     if (nrhs < 1 || ldx < n) return fail("bad nrhs / ldx");
-    if ((int64_t)n * nrhs > INT_MAX) return fail(SLU_API "batch_solve: n * nrhs must stay below 2^31 per member");
+    if ((int64_t)n * nrhs > INT_MAX) return fail(SLU_API "%s: n * nrhs must stay below 2^31 per member", fn);
     const size_t len = (size_t)n * nrhs * B;
     if (H->d_x.n < len && H->d_x.alloc(len)) return -1;
     cudaStream_t s = H->stream;
@@ -1973,20 +2008,11 @@ int slu_b200_batch_solve(slu_b200_handle_t H, double *xh, int ldx, int nrhs)
     // the B blocks are B * nrhs columns at pitch ldx: one 2D copy each way
     CU(cudaMemcpy2DAsync(x, (size_t)n * sizeof(val_t), xh, (size_t)ldx * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs * B,
                          cudaMemcpyHostToDevice, s));
-    const int64_t *p64 = H->d_pool_i64.p;
     int launches = 0;
-    for (size_t li = 0; li < H->levels.size(); ++li) {          // forward: L y = b
-        const LevelPlan &L = H->levels[li];
-        const int32_t *nodes = H->d_pool_i32.p + L.nodes_off;
-        launches += launch_solve_diag(d, nodes, L.count, false, x, n, nrhs, s);
-        launches += launch_solve_update(d, Batch{nodes, p64 + L.sl_prefix, L.count}, L.sl_ctas, false, x, n, nrhs, s);
-    }
-    for (size_t li = H->levels.size(); li-- > 0;) {             // backward: U x = y
-        const LevelPlan &L = H->levels[li];
-        const int32_t *nodes = H->d_pool_i32.p + L.nodes_off;
-        launches += launch_solve_update(d, Batch{nodes, p64 + L.su_prefix, L.count}, L.su_ctas, true, x, n, nrhs, s);
-        launches += launch_solve_diag(d, nodes, L.count, true, x, n, nrhs, s);
-    }
+    for (size_t li = 0; li < H->levels.size(); ++li)            // forward: L y = b (U^T y = b)
+        launches += solve_level(H, d, H->levels[li], false, trans, x, n, nrhs, s);
+    for (size_t li = H->levels.size(); li-- > 0;)               // backward: U x = y (L^T x = y)
+        launches += solve_level(H, d, H->levels[li], true, trans, x, n, nrhs, s);
     CU(cudaMemcpy2DAsync(xh, (size_t)ldx * sizeof(val_t), x, (size_t)n * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs * B,
                          cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
@@ -1994,6 +2020,16 @@ int slu_b200_batch_solve(slu_b200_handle_t H, double *xh, int ldx, int nrhs)
     H->st.reserved[4] = now_s() - t0;
     H->st.reserved[5] = (double)launches;
     return 0;
+}
+
+int slu_b200_batch_solve(slu_b200_handle_t H, double *xh, int ldx, int nrhs)
+{
+    return batch_solve_impl(H, xh, ldx, nrhs, 0, "batch_solve");
+}
+
+int slu_b200_batch_solve_trans(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int trans)
+{
+    return batch_solve_impl(H, xh, ldx, nrhs, trans, "batch_solve_trans");
 }
 
 // D2H of member `member`'s L and U into the view's Lnzval / Unzval, as slu_b200_download

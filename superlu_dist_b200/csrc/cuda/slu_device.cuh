@@ -158,10 +158,14 @@ int launch_gemm_sub(int m, int n, int k, const val_t *a, int lda, const val_t *b
                     int ldc, int variant, cudaStream_t s);
 
 // slu_solve.cu (double) / slu_solve_z.cu (doublecomplex): triangular solves on the resident factors.
-// x: device, n x nrhs elements of val_t, ordering of the factored matrix
+// x: device, n x nrhs elements of val_t, ordering of the factored matrix.  trans: 0 solves A x = b (forward pass with L,
+// backward with U; the update takes the L / U panel tiles), 1 A^T x = b and 2 A^H x = b (forward with U^T, backward with
+// L^T; the update takes the U / L panel tiles); 2 is 1 in double.
 constexpr int SOLVE_TILE = 256;
-int launch_solve_diag(const DeviceLU &d, const int32_t *nodes, int count, bool upper, val_t *x, int n, int nrhs, cudaStream_t s);
-int launch_solve_update(const DeviceLU &d, const Batch &b, int64_t ctas, bool upper, val_t *x, int n, int nrhs, cudaStream_t s);
+int launch_solve_diag(const DeviceLU &d, const int32_t *nodes, int count, bool backward, int trans, val_t *x, int n, int nrhs,
+                      cudaStream_t s);
+int launch_solve_update(const DeviceLU &d, const Batch &b, int64_t ctas, bool backward, int trans, val_t *x, int n, int nrhs,
+                        cudaStream_t s);
 // x[entries of the listed supernodes] = src[...] (src == nullptr: 0)
 int launch_solve_mask(const DeviceLU &d, const int32_t *nodes, int count, val_t *x, int n, int nrhs, const val_t *src, cudaStream_t s);
 // device-side distribution of a CSR matrix (device arrays) into the arena; *err counts entries without a slot
@@ -176,8 +180,10 @@ int launch_diag_inv(const BatchedLU &d, const Batch &b, int64_t ctas, val_t *din
 int launch_trsm_l(const BatchedLU &d, const Batch &b, int64_t ctas, int max_ns, const val_t *dinv, cudaStream_t s);
 int launch_trsm_u(const BatchedLU &d, const Batch &b, int64_t ctas, int max_ns, const val_t *dinv, cudaStream_t s);
 int launch_schur(const BatchedLU &d, const Batch &b, int64_t ctas, int big, int mode, cudaStream_t s);
-int launch_solve_diag(const BatchedLU &d, const int32_t *nodes, int count, bool upper, val_t *x, int n, int nrhs, cudaStream_t s);
-int launch_solve_update(const BatchedLU &d, const Batch &b, int64_t ctas, bool upper, val_t *x, int n, int nrhs, cudaStream_t s);
+int launch_solve_diag(const BatchedLU &d, const int32_t *nodes, int count, bool backward, int trans, val_t *x, int n, int nrhs,
+                      cudaStream_t s);
+int launch_solve_update(const BatchedLU &d, const Batch &b, int64_t ctas, bool backward, int trans, val_t *x, int n, int nrhs,
+                        cudaStream_t s);
 int launch_fill_csr(const BatchedLU &d, int n, const int32_t *rowptr, const int32_t *colind, const val_t *aval, const int32_t *perm,
                     const int8_t *active, int *err, cudaStream_t s);
 

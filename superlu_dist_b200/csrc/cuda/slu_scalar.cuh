@@ -50,6 +50,11 @@ __device__ __forceinline__ void vatomic_sub(val_t *p, val_t v)
     atomicAdd(&p->x, -v.x);
     atomicAdd(&p->y, -v.y);
 }
+__device__ __forceinline__ val_t vmul(val_t a, val_t b) { return zmul(a, b); }
+__device__ __forceinline__ val_t vrecip(val_t a) { return zrecip(a); }
+// conj(a) for CONJ = true (the conjugate-transposed solve reads every factor entry conjugated), a otherwise
+template <bool CONJ>
+__device__ __forceinline__ val_t vconj(val_t a) { return CONJ ? zmake(a.x, -a.y) : a; }
 #else
 __device__ __forceinline__ val_t vzero() { return 0.0; }
 __device__ __forceinline__ val_t vadd(val_t a, val_t b) { return a + b; }
@@ -59,6 +64,10 @@ __device__ __forceinline__ void vsubmul(val_t &acc, val_t a, val_t b) { acc -= a
 __device__ __forceinline__ val_t vdiv(val_t a, val_t piv) { return a / piv; }
 __device__ __forceinline__ val_t vshfl(unsigned mask, val_t v, int lane) { return __shfl_sync(mask, v, lane); }
 __device__ __forceinline__ void vatomic_sub(val_t *p, val_t v) { atomicAdd(p, -v); }
+__device__ __forceinline__ val_t vmul(val_t a, val_t b) { return a * b; }
+__device__ __forceinline__ val_t vrecip(val_t a) { return 1.0 / a; }
+template <bool CONJ>
+__device__ __forceinline__ val_t vconj(val_t a) { return a; }   // a real entry is its own conjugate
 #endif
 
 }  // namespace SLU_NS

@@ -9,7 +9,8 @@
 // with four small kernels per level; one right-hand side streams L and U once (HBM-bound: 8 bytes per stored entry,
 // 16 in doublecomplex).
 // x is a device vector in the ordering of the factored matrix (the caller applies the permutations, as pdgssvx3d does
-// around pdgstrs3d).
+// around pdgstrs3d).  The transposed and conjugate-transposed solves (A^T x = b, A^H x = b) run over the same levels with
+// U^T forward and L^T backward (below solve_update_u_kernel); pdgstrs3d itself has no such mode.
 //
 // Compiled twice, like slu_api.cu: as is for double, and through slu_solve_z.cu with SLU_COMPLEX for doublecomplex
 // (pzgstrs3d, SRC/complex16/pzgstrs3d.c).  The element arithmetic goes through the val_t helpers of slu_scalar.cuh;
@@ -160,6 +161,141 @@ __global__ void __launch_bounds__(256, SOLVE_MIN_CTAS<LU>) solve_update_u_kernel
     }
 }
 
+// ---- transposed solves: A^T x = b as U^T y = b, then L^T x = y, over the same level plan and in the same directions as
+// the plain solve, because both the targets of the forward scatter (the packed U columns) and the sources of the backward
+// gather (the L rows) are ancestor supernodes:
+//   forward   for every level, bottom-up:   y_k <- U_kk^-T x_k ;  x[ucols(k)] -= U(k,:)^T y_k       (atomic adds)
+//   backward  for every level, top-down:    x_k <- x_k - L(below,k)^T x[rows below] ;  x_k <- L_kk^-T x_k
+// CONJ (doublecomplex only) reads every factor entry conjugated, the pivots included: A^H = U^H L^H.  The zero padding
+// above the skyline segments of a packed U column adds nothing to its dot product.
+
+__device__ __forceinline__ val_t warp_sum(val_t v)
+{
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = vadd(v, vshfl(0xffffffffu, v, (threadIdx.x & 31) ^ o));
+    return v;
+}
+
+// y_k <- U_kk^-T x_k (forward: lower, non-unit) or x_k <- L_kk^-T x_k (backward: upper, unit): one CTA per supernode.
+// Row r of the transposed triangle is column r of the diagonal block, contiguous in memory.  Per 16-unknown block: one
+// warp per unknown gathers the unknowns solved before it along that column, and the 16 x 16 block is staged in shared
+// memory (blk[i][j] = block(c0 + i, c0 + j)) so that warp 0 solves it with shuffles, lane r owning unknown c0 + r.  The
+// forward pass multiplies by the pivots' reciprocals, taken in parallel while the block is staged.  In doublecomplex a
+// minimum of 4 CTAs per SM (64 registers): without it ptxas spills around the division of the unbatched forward kernel.
+template <bool BACKWARD, bool CONJ, class LU>
+__global__ void __launch_bounds__(256, VAL_DOUBLES == 2 ? 4 : 0) solve_diag_trans_kernel(LU dd, const int32_t *nodes, val_t *x, int n, int nrhs)
+{
+    __shared__ val_t xs[MAX_NS_HELD];
+    __shared__ val_t blk[16][17], rpiv[16];
+    const DeviceLU &d = member_view(dd);
+    x = member_ptr(dd, x, (uint32_t)(n * nrhs));   // the host keeps n * nrhs < 2^31
+    const NodeDesc nd = d.nodes[nodes[blockIdx.x]];
+    const int ns = nd.ns, lda = nd.nsupr, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const val_t *A = d.val + nd.lval;
+    for (int rhs = 0; rhs < nrhs; ++rhs) {
+        val_t *xk = x + (size_t)rhs * n + nd.fsupc;
+        for (int r = tid; r < ns; r += 256) xs[r] = xk[r];
+        __syncthreads();
+        for (int b = 0; b < ns; b += 16) {
+            const int c0 = BACKWARD ? max(0, ns - b - 16) : b, cb = BACKWARD ? ns - b - c0 : min(16, ns - b);
+            const int lo = BACKWARD ? c0 + cb : 0, hi = BACKWARD ? ns : c0;   // the unknowns solved so far
+            for (int rr = warp; rr < cb; rr += 8) {
+                const val_t *col = A + (size_t)(c0 + rr) * lda;
+                val_t acc = vzero();
+                for (int c = lo + lane; c < hi; c += 32) vaddmul(acc, vconj<CONJ>(col[c]), xs[c]);
+                acc = warp_sum(acc);
+                if (lane == 0) xs[c0 + rr] = vsub(xs[c0 + rr], acc);
+            }
+            {
+                const int i = tid & 15, j = tid >> 4;
+                blk[i][j] = (i < cb && j < cb) ? vconj<CONJ>(A[(size_t)(c0 + j) * lda + c0 + i]) : vzero();
+                if (!BACKWARD && tid < cb) rpiv[tid] = vrecip(vconj<CONJ>(A[(size_t)(c0 + tid) * lda + c0 + tid]));
+            }
+            __syncthreads();
+            if (tid < 32) {   // transposed triangle: entry (r, c) = blk[c][r]
+                val_t v = (tid < cb) ? xs[c0 + tid] : vzero();
+                if (!BACKWARD) {
+                    for (int c = 0; c < cb; ++c) {
+                        const val_t xc = vmul(vshfl(0xffffffffu, v, c), rpiv[c]);
+                        if (tid == c) v = xc;
+                        if (tid > c && tid < cb) vsubmul(v, blk[c][tid], xc);
+                    }
+                } else {
+                    for (int c = cb - 1; c > 0; --c) {
+                        const val_t xc = vshfl(0xffffffffu, v, c);
+                        if (tid < c) vsubmul(v, blk[c][tid], xc);
+                    }
+                }
+                if (tid < cb) xs[c0 + tid] = v;
+            }
+            __syncthreads();
+        }
+        for (int r = tid; r < ns; r += 256) xk[r] = xs[r];
+        __syncthreads();
+    }
+}
+
+// x[ucols(k)] -= U(k, :)^T y_k: CTA = 256 packed columns of one U panel; warp w takes columns w, w+8, ..., one dot
+// product per column with the lanes along its ns contiguous entries
+template <bool CONJ, class LU>
+__global__ void __launch_bounds__(256, SOLVE_MIN_CTAS<LU>) solve_scatter_ut_kernel(LU dd, Batch b, val_t *x, int n, int nrhs)
+{
+    __shared__ val_t ys[MAX_NS_HELD];
+    const DeviceLU &d = member_view(dd);
+    x = member_ptr(dd, x, (uint32_t)(n * nrhs));   // the host keeps n * nrhs < 2^31
+    const int slot = find_slot(b.prefix, b.count, blockIdx.x);
+    const NodeDesc nd = d.nodes[b.nodes[slot]];
+    const int j0 = (int)(blockIdx.x - b.prefix[slot]) * SOLVE_ROWS, j1 = min(nd.ncols, j0 + SOLVE_ROWS);
+    const int ns = nd.ns, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const val_t *U = d.val + nd.uval;
+    const int32_t *cols = d.ucols + nd.ucol;
+    for (int rhs = 0; rhs < nrhs; ++rhs) {
+        __syncthreads();
+        for (int r = threadIdx.x; r < ns; r += 256) ys[r] = x[(size_t)rhs * n + nd.fsupc + r];
+        __syncthreads();
+        for (int j = j0 + warp; j < j1; j += 8) {
+            const val_t *col = U + (size_t)j * ns;
+            val_t acc = vzero();
+            for (int r = lane; r < ns; r += 32) vaddmul(acc, vconj<CONJ>(col[r]), ys[r]);
+            acc = warp_sum(acc);
+            if (lane == 0) vatomic_sub(x + (size_t)rhs * n + cols[j], acc);
+        }
+    }
+}
+
+// x_k -= L(below, k)^T x[rows below]: CTA = 256 rows of one L panel, warp w = rows 32w ... 32w+31 of them, lane = row
+// (coalesced down each column); a warp sum per column into part[w][c], then the CTA's sums go to x_k with atomic adds
+template <bool CONJ, class LU>
+__global__ void __launch_bounds__(SOLVE_ROWS, SOLVE_MIN_CTAS<LU>) solve_gather_lt_kernel(LU dd, Batch b, val_t *x, int n, int nrhs)
+{
+    __shared__ val_t part[SOLVE_ROWS / 32][MAX_NS_HELD];
+    const DeviceLU &d = member_view(dd);
+    x = member_ptr(dd, x, (uint32_t)(n * nrhs));   // the host keeps n * nrhs < 2^31
+    const int slot = find_slot(b.prefix, b.count, blockIdx.x);
+    const NodeDesc nd = d.nodes[b.nodes[slot]];
+    const int i0 = (int)(blockIdx.x - b.prefix[slot]) * SOLVE_ROWS, i = i0 + threadIdx.x;
+    const int ns = nd.ns, lda = nd.nsupr, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int nwarps = min(SOLVE_ROWS / 32, (nd.m - i0 + 31) / 32);   // warps with at least one row of the panel
+    const val_t *L = d.val + nd.lval + ns;
+    const int row = i < nd.m ? d.lrows[nd.lrow + ns + i] : 0;
+    for (int rhs = 0; rhs < nrhs; ++rhs) {
+        if (warp < nwarps) {
+            const val_t xr = i < nd.m ? x[(size_t)rhs * n + row] : vzero();
+            for (int c = 0; c < ns; ++c) {
+                const val_t v = warp_sum(i < nd.m ? vmul(vconj<CONJ>(L[(size_t)c * lda + i]), xr) : vzero());
+                if (lane == 0) part[warp][c] = v;
+            }
+        }
+        __syncthreads();
+        for (int c = threadIdx.x; c < ns; c += SOLVE_ROWS) {
+            val_t sum = part[0][c];
+            for (int w = 1; w < nwarps; ++w) sum = vadd(sum, part[w][c]);
+            vatomic_sub(x + (size_t)rhs * n + nd.fsupc + c, sum);
+        }
+        __syncthreads();
+    }
+}
+
 // keep / zero the entries of the supernodes in a node list (multi-GPU ownership masks)
 __global__ void solve_mask_kernel(DeviceLU d, const int32_t *nodes, int count, val_t *x, int n, int nrhs, const val_t *src)
 {
@@ -216,19 +352,41 @@ static int launch_fill_csr_t(const LU &d, int n, const int32_t *rowptr, const in
     fill_csr_kernel<LU><<<member_grid(d, (n + 127) / 128), 128, 0, s>>>(d, n, rowptr, colind, aval, perm, active, err);
     return 1;
 }
+template <bool CONJ, class LU>
+static void launch_solve_trans_c(const LU &d, const int32_t *nodes, const Batch *b, unsigned ctas, bool backward, val_t *x, int n,
+                                 int nrhs, cudaStream_t s)
+{
+    if (!b && backward) solve_diag_trans_kernel<true, CONJ, LU><<<member_grid(d, ctas), 256, 0, s>>>(d, nodes, x, n, nrhs);
+    else if (!b) solve_diag_trans_kernel<false, CONJ, LU><<<member_grid(d, ctas), 256, 0, s>>>(d, nodes, x, n, nrhs);
+    else if (backward) solve_gather_lt_kernel<CONJ, LU><<<member_grid(d, ctas), SOLVE_ROWS, 0, s>>>(d, *b, x, n, nrhs);
+    else solve_scatter_ut_kernel<CONJ, LU><<<member_grid(d, ctas), 256, 0, s>>>(d, *b, x, n, nrhs);
+}
+// trans 1 / 2: the transposed kernels, conjugating in doublecomplex for 2 (in double 2 is 1)
 template <class LU>
-static int launch_solve_diag_t(const LU &d, const int32_t *nodes, int count, bool upper, val_t *x, int n, int nrhs, cudaStream_t s)
+static void launch_solve_trans(const LU &d, const int32_t *nodes, const Batch *b, unsigned ctas, bool backward, int trans, val_t *x,
+                               int n, int nrhs, cudaStream_t s)
+{
+    if constexpr (VAL_DOUBLES == 2)
+        if (trans == 2) return launch_solve_trans_c<true>(d, nodes, b, ctas, backward, x, n, nrhs, s);
+    launch_solve_trans_c<false>(d, nodes, b, ctas, backward, x, n, nrhs, s);
+}
+template <class LU>
+static int launch_solve_diag_t(const LU &d, const int32_t *nodes, int count, bool backward, int trans, val_t *x, int n, int nrhs,
+                               cudaStream_t s)
 {
     if (count <= 0) return 0;
-    if (upper) solve_diag_kernel<true, LU><<<member_grid(d, count), 256, 0, s>>>(d, nodes, x, n, nrhs);
+    if (trans) launch_solve_trans(d, nodes, nullptr, (unsigned)count, backward, trans, x, n, nrhs, s);
+    else if (backward) solve_diag_kernel<true, LU><<<member_grid(d, count), 256, 0, s>>>(d, nodes, x, n, nrhs);
     else solve_diag_kernel<false, LU><<<member_grid(d, count), 256, 0, s>>>(d, nodes, x, n, nrhs);
     return 1;
 }
 template <class LU>
-static int launch_solve_update_t(const LU &d, const Batch &b, int64_t ctas, bool upper, val_t *x, int n, int nrhs, cudaStream_t s)
+static int launch_solve_update_t(const LU &d, const Batch &b, int64_t ctas, bool backward, int trans, val_t *x, int n, int nrhs,
+                                 cudaStream_t s)
 {
     if (b.count <= 0 || ctas <= 0) return 0;
-    if (upper) solve_update_u_kernel<LU><<<member_grid(d, (unsigned)ctas), 256, 0, s>>>(d, b, x, n, nrhs);
+    if (trans) launch_solve_trans(d, b.nodes, &b, (unsigned)ctas, backward, trans, x, n, nrhs, s);
+    else if (backward) solve_update_u_kernel<LU><<<member_grid(d, (unsigned)ctas), 256, 0, s>>>(d, b, x, n, nrhs);
     else solve_update_l_kernel<LU><<<member_grid(d, (unsigned)ctas), SOLVE_ROWS, 0, s>>>(d, b, x, n, nrhs);
     return 1;
 }
@@ -237,26 +395,30 @@ int launch_fill_csr(const DeviceLU &d, int n, const int32_t *rowptr, const int32
 {
     return launch_fill_csr_t(d, n, rowptr, colind, aval, perm, active, err, s);
 }
-int launch_solve_diag(const DeviceLU &d, const int32_t *nodes, int count, bool upper, val_t *x, int n, int nrhs, cudaStream_t s)
+int launch_solve_diag(const DeviceLU &d, const int32_t *nodes, int count, bool backward, int trans, val_t *x, int n, int nrhs,
+                      cudaStream_t s)
 {
-    return launch_solve_diag_t(d, nodes, count, upper, x, n, nrhs, s);
+    return launch_solve_diag_t(d, nodes, count, backward, trans, x, n, nrhs, s);
 }
-int launch_solve_update(const DeviceLU &d, const Batch &b, int64_t ctas, bool upper, val_t *x, int n, int nrhs, cudaStream_t s)
+int launch_solve_update(const DeviceLU &d, const Batch &b, int64_t ctas, bool backward, int trans, val_t *x, int n, int nrhs,
+                        cudaStream_t s)
 {
-    return launch_solve_update_t(d, b, ctas, upper, x, n, nrhs, s);
+    return launch_solve_update_t(d, b, ctas, backward, trans, x, n, nrhs, s);
 }
 int launch_fill_csr(const BatchedLU &d, int n, const int32_t *rowptr, const int32_t *colind, const val_t *aval, const int32_t *perm,
                     const int8_t *active, int *err, cudaStream_t s)
 {
     return launch_fill_csr_t(d, n, rowptr, colind, aval, perm, active, err, s);
 }
-int launch_solve_diag(const BatchedLU &d, const int32_t *nodes, int count, bool upper, val_t *x, int n, int nrhs, cudaStream_t s)
+int launch_solve_diag(const BatchedLU &d, const int32_t *nodes, int count, bool backward, int trans, val_t *x, int n, int nrhs,
+                      cudaStream_t s)
 {
-    return launch_solve_diag_t(d, nodes, count, upper, x, n, nrhs, s);
+    return launch_solve_diag_t(d, nodes, count, backward, trans, x, n, nrhs, s);
 }
-int launch_solve_update(const BatchedLU &d, const Batch &b, int64_t ctas, bool upper, val_t *x, int n, int nrhs, cudaStream_t s)
+int launch_solve_update(const BatchedLU &d, const Batch &b, int64_t ctas, bool backward, int trans, val_t *x, int n, int nrhs,
+                        cudaStream_t s)
 {
-    return launch_solve_update_t(d, b, ctas, upper, x, n, nrhs, s);
+    return launch_solve_update_t(d, b, ctas, backward, trans, x, n, nrhs, s);
 }
 int launch_solve_mask(const DeviceLU &d, const int32_t *nodes, int count, val_t *x, int n, int nrhs, const val_t *src, cudaStream_t s)
 {
