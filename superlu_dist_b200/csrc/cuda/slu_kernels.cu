@@ -1079,22 +1079,33 @@ __device__ __forceinline__ void gemm_tile_v2(const double *__restrict__ A, int l
 // ------------------------------------------------------------------------------------------------
 // Schur-complement update of a batch of supernodes: GEMM tile + fused subtract-scatter epilogue
 // ------------------------------------------------------------------------------------------------
-// (tm, tn) of tile number `tile` of a supernode with BM x BN tiles.  mode 0: all tiles column by column; 1 (urgent): the
-// first tcu tile columns entirely, then the first tru tile rows of the rest; 2 (bulk): the others
+// Tile t of a rows x cols rectangle of tiles, in bands of SCHUR_BAND tile rows taken one after the other, column by
+// column within a band.  CTAs start in tile order, so the ~2 per SM in flight at once share a few row tiles of A (L panel)
+// and column tiles of B (U panel), a working set of about 6 MB.  Column by column over all rows of a tall update
+// (m ~ 10^4: 80 row tiles, 21 MB of A at k = 256), the tiles in flight touch the whole L panel for every column tile.
+constexpr int SCHUR_BAND = 16;
+__device__ __forceinline__ void band_order(int t, int rows, int cols, int &r, int &c)
+{
+    const int per = SCHUR_BAND * cols, b = t / per, r0 = b * SCHUR_BAND, h = min(SCHUR_BAND, rows - r0), u = t - b * per;
+    r = r0 + u % h; c = u / h;
+}
+
+// (tm, tn) of tile number `tile` of a supernode with BM x BN tiles.  mode 0: all tiles in bands; 1 (urgent): the
+// first tcu tile columns entirely, then the first tru tile rows of the rest; 2 (bulk): the others, in bands
 template <int BM, int BN>
 __device__ __forceinline__ void schur_tile_of(const NodeDesc &nd, int tile, int mode, int &tm, int &tn)
 {
-    const int tiles_m = (nd.m + BM - 1) / BM;
+    const int tiles_m = (nd.m + BM - 1) / BM, tiles_n = (nd.ncols + BN - 1) / BN;
     if (mode == 0) {
-        tm = tile % tiles_m; tn = tile / tiles_m;
+        band_order(tile, tiles_m, tiles_n, tm, tn);
     } else {
         const int tru = (nd.urg_rows + BM - 1) / BM, tcu = (nd.urg_cols + BN - 1) / BN;
         if (mode == 1) {
             if (tile < tiles_m * tcu) { tm = tile % tiles_m; tn = tile / tiles_m; }
             else { const int t = tile - tiles_m * tcu; tm = t % tru; tn = tcu + t / tru; }
         } else {
-            const int rm = tiles_m - tru;
-            tm = tru + tile % rm; tn = tcu + tile / rm;
+            band_order(tile, tiles_m - tru, tiles_n - tcu, tm, tn);
+            tm += tru; tn += tcu;
         }
     }
 }
