@@ -120,7 +120,8 @@ typedef struct {
     double reserved[8];           /* [0] ms spent slicing (verbose >= 2), [1] Schur flops taken by the */
                                   /* tcgen05 path, [2] bytes of its int8 workspace, [3] slices in use,  */
                                   /* [4] seconds of the last slu_b200_solve or _solve_trans, [5] its    */
-                                  /* kernel launches                                                    */
+                                  /* kernel launches, [6] seconds of the last slu_b200_gscon or         */
+                                  /* _batch_gscon, [7] the solve rounds it ran                          */
 } slu_b200_stats_t;
 
 typedef struct slu_b200_handle_s *slu_b200_handle_t;
@@ -172,6 +173,21 @@ int slu_b200_solve(slu_b200_handle_t h, double *x, int ldx, int nrhs);
  * F^T = P A^T P^T, the caller permutes b and x exactly as for the plain solve.  trans outside {0, 1, 2} fails.
  * The reference's pdgstrs3d has no transposed mode. */
 int slu_b200_solve_trans(slu_b200_handle_t h, double *x, int ldx, int nrhs, int trans);
+/* Reciprocal condition number estimate on the resident factors, as LAPACK dgecon and sequential SuperLU dgscon:
+ * *rcond = (1 / est) / anorm, where est estimates ||F^-1|| (= ||A^-1||) of the factored matrix F = P A P^T in the 1-norm
+ * (norm '1' or 'O') or the infinity-norm (norm 'I'; 'o' and 'i' are accepted too), and anorm = ||A|| in the same norm,
+ * computed by the caller (pdgssvx3d computes it with pdlangs).  est is LAPACK's dlacn2 (Hager / Higham) applied to F^-1
+ * exactly as dgecon drives it: "kase 1" solves with F and "kase 2" with F^T (swapped for norm 'I'), from the start vector
+ * (1/n, ..., 1/n), at most 5 iterations, the final alternating-sign vector; about 5 solves.  The whole iteration runs on
+ * device vectors: per solve the host reads back two counters, no n-vector crosses PCIe.  est is a lower bound of the
+ * norm and usually within a factor of 3 of it.
+ * anorm < 0 or NaN fails; anorm = 0 or +inf gives *rcond = 0 without a solve; a non-finite estimate gives *rcond = 0.
+ * The estimate describes L U as factored: where tiny pivots were replaced (options.replace_tiny_pivot), that is the
+ * perturbed matrix, not A.  Restrictions as slu_b200_solve (a successful factorization, 1 x 1 x Pz, collective along Z:
+ * every rank passes the same anorm and receives the same rcond).  stats.reserved[6] = seconds of the call,
+ * stats.reserved[7] = the solves it ran; stats.reserved[4] / [5] keep describing the last slu_b200_solve*.  The
+ * reference's pdgssvx3d has no condition estimator. */
+int slu_b200_gscon(slu_b200_handle_t h, char norm, double anorm, double *rcond);
 int slu_b200_get_stats(slu_b200_handle_t h, slu_b200_stats_t *out);
 void slu_b200_destroy(slu_b200_handle_t h);
 
@@ -242,6 +258,13 @@ int slu_b200_batch_factor(slu_b200_handle_t h, int *info);
 int slu_b200_batch_solve(slu_b200_handle_t h, double *x, int ldx, int nrhs);
 /* op(A_j) x_j = b_j for every member, trans as slu_b200_solve_trans; x and the restrictions as slu_b200_batch_solve */
 int slu_b200_batch_solve_trans(slu_b200_handle_t h, double *x, int ldx, int nrhs, int trans);
+/* rcond[j] for every member, as slu_b200_gscon with anorm[j] = ||A_j|| (both arrays hold batch entries).  The members
+ * run dlacn2 in lock-step: each round is one batched solve of one kase for all members; only the members waiting for
+ * that kase take its result, the others keep their pending vector.  The next round takes the other kase if any member
+ * waits for it, else the same one, so no member waits more than one round and a batch takes at most twice the solves
+ * of its slowest member.  stats.reserved[7] = the rounds.  Fails, naming the member, unless every member's last info
+ * was 0. */
+int slu_b200_batch_gscon(slu_b200_handle_t h, char norm, const double *anorm, double *rcond);
 /* write member j's L/U into the view's Lnzval / Unzval arrays, in the reference layout (as slu_b200_download) */
 int slu_b200_batch_download(slu_b200_handle_t h, int member);
 /* ---- doublecomplex twins (SRC/complex16/pzgstrf3d.c:120; the reference's z* handle API,
@@ -267,6 +290,9 @@ int slu_b200_z_fill_csr(slu_b200_zhandle_t h, int n, const int32_t *rowptr, cons
                         const int32_t *perm);
 int slu_b200_z_solve(slu_b200_zhandle_t h, double *x, int ldx, int nrhs);
 int slu_b200_z_solve_trans(slu_b200_zhandle_t h, double *x, int ldx, int nrhs, int trans);
+/* as slu_b200_gscon, with zgecon's zlacn2: "kase 2" solves with F^H, |x_i| is the modulus, the sign vector is x_i / |x_i|
+ * (1 where |x_i| is below the safe minimum) and there is no repeated-sign test */
+int slu_b200_z_gscon(slu_b200_zhandle_t h, char norm, double anorm, double *rcond);
 /* batched doublecomplex handles (the reference's pzgssvx3d_csc_batch, SRC/complex16/pzgssvx3d_csc_batch.c:80): the
  * slu_b200_batch_* calls above with the same semantics, restrictions and stats; val and x point at interleaved
  * doublecomplex, n, ldx and nnz count complex elements.  Stats through slu_b200_z_get_stats, slu_b200_z_destroy frees.
@@ -279,6 +305,7 @@ int slu_b200_z_batch_fill_csr(slu_b200_zhandle_t h, int n, const int32_t *rowptr
 int slu_b200_z_batch_factor(slu_b200_zhandle_t h, int *info);
 int slu_b200_z_batch_solve(slu_b200_zhandle_t h, double *x, int ldx, int nrhs);
 int slu_b200_z_batch_solve_trans(slu_b200_zhandle_t h, double *x, int ldx, int nrhs, int trans);
+int slu_b200_z_batch_gscon(slu_b200_zhandle_t h, char norm, const double *anorm, double *rcond);
 int slu_b200_z_batch_download(slu_b200_zhandle_t h, int member);
 int slu_b200_z_get_stats(slu_b200_zhandle_t h, slu_b200_stats_t *out);
 int slu_b200_z_plan(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, slu_b200_stats_t *stats);

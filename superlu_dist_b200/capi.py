@@ -114,6 +114,10 @@ def lib():
     L.slu_b200_z_batch_download.argtypes = [C.c_void_p, C.c_int]
     for f in ("slu_b200_solve_trans", "slu_b200_z_solve_trans", "slu_b200_batch_solve_trans", "slu_b200_z_batch_solve_trans"):
         getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
+    for f in ("slu_b200_gscon", "slu_b200_z_gscon"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_char, C.c_double, C.POINTER(C.c_double)]
+    for f in ("slu_b200_batch_gscon", "slu_b200_z_batch_gscon"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_char, C.c_void_p, C.c_void_p]
     _lib = L
     return L
 
@@ -143,6 +147,13 @@ def _solve_call(name, complex_, trans):
     if trans == "N":
         return _fn(name, complex_), ()
     return _fn(name + "_trans", complex_), (_TRANS[trans],)
+
+
+def _norm_byte(norm):
+    """'1' | 'O' | 'I' (as LAPACK's gecon; lower case too) -> the char argument of slu_b200_gscon, which checks the letter"""
+    if not (isinstance(norm, str) and len(norm) == 1 and norm.isascii()):
+        raise ValueError(f"norm must be '1', 'O' or 'I', not {norm!r}")
+    return norm.encode()
 
 
 def device_count():
@@ -311,6 +322,13 @@ class Handle:
         _check(fn(self.h, x.ctypes.data_as(C.c_void_p), self.prob.n, nrhs, *extra))
         return x
 
+    def rcond(self, anorm, norm="1"):
+        """Reciprocal condition number estimate on the resident factors (slu_b200_gscon / slu_b200_z_gscon), as LAPACK's
+        gecon: (1 / est ||F^-1||) / anorm with anorm = ||A|| in the same norm, '1' (or 'O') or 'I'."""
+        out = C.c_double(0.0)
+        _check(_fn("gscon", self.z_)(self.h, _norm_byte(norm), float(anorm), C.byref(out)))
+        return out.value
+
     def _dtype(self):
         return np.complex128 if self.z_ else np.float64
 
@@ -375,6 +393,14 @@ class BatchHandle:
         nrhs = 1 if x.ndim == 2 else x.shape[1]
         _check(fn(self.h, x.ctypes.data_as(C.c_void_p), self.prob.n, nrhs, *extra))
         return x
+
+    def rcond(self, anorm, norm="1"):
+        """Every member's reciprocal condition number estimate (slu_b200_batch_gscon), as Handle.rcond; anorm: (batch,)
+        norms of the members, or one value for all.  -> float64 array (batch,)"""
+        a = np.ascontiguousarray(np.broadcast_to(np.asarray(anorm, np.float64), (self.batch,)))
+        out = np.zeros(self.batch, np.float64)
+        _check(_fn("batch_gscon", self.z_)(self.h, _norm_byte(norm), a.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p)))
+        return out
 
     def download(self, member):
         """Member `member`'s L and U into prob.layers[0] (the reference layout)."""

@@ -44,6 +44,8 @@
 #define slu_b200_batch_solve slu_b200_z_batch_solve
 #define slu_b200_batch_solve_trans slu_b200_z_batch_solve_trans
 #define slu_b200_batch_download slu_b200_z_batch_download
+#define slu_b200_gscon slu_b200_z_gscon
+#define slu_b200_batch_gscon slu_b200_z_batch_gscon
 #define SLU_API "slu_b200_z_"     // name prefix of the exported calls, for error messages
 #else
 #define SLU_API "slu_b200_"
@@ -281,6 +283,12 @@ struct slu_b200_handle_s {
     int64_t member_len = 0, inv_len = 0;  // elements of one member's arena / diag-inverse workspace
     BatchedLU bdev{};
     std::vector<int> member_info;         // info of every member after the last slu_b200_batch_factor
+    // condition estimation (slu_b200_gscon): per member the pending vector (batched handles only), the last real sign
+    // vector, the state; the reduction partials and the two kase counters
+    DevBuf<val_t> d_cv, d_csgn;
+    DevBuf<CondState> d_cstate;
+    DevBuf<CondPart> d_cpart;
+    DevBuf<int> d_ccount;
 };
 
 namespace {
@@ -1344,6 +1352,7 @@ void slu_b200_destroy(slu_b200_handle_t H)
     H->d_useg.release(); H->d_pool_i32.release(); H->d_pool_i64.release(); H->d_lrel.release(); H->d_urel.release();
     H->d_lblk.release(); H->d_ublk.release(); H->d_rowinfo.release(); H->d_colinfo.release(); H->d_flags.release();
     H->d_x.release(); H->d_x2.release();
+    H->d_cv.release(); H->d_csgn.release(); H->d_cstate.release(); H->d_cpart.release(); H->d_ccount.release();
     H->d_tiny.release(); H->d_oz_i8.release(); H->d_oz_scale.release(); H->d_oz_rexp.release();
     delete H;
 }
@@ -1723,25 +1732,16 @@ static int solve_level(const slu_b200_handle_s *H, const LU &d, const LevelPlan 
 }
 extern "C" {
 
-// fn: "solve" or "solve_trans", for the messages
-static int solve_impl(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int trans, const char *fn)
+// The solve of an unbatched handle on device vectors: b in d_x2 (n x nrhs, both buffers hold n * nrhs elements), the
+// solution in *result (d_x, or d_x2 along Z) on every rank.  Enqueued on H->stream, not synchronised.  Returns the kernel
+// launches, < 0 on an error.
+static int solve_dev(slu_b200_handle_t H, int nrhs, int trans, val_t **result)
 {
-    if (!H || !xh) return fail("null argument");
-    if (refuse_batched(H, (std::string(SLU_API) + fn).c_str())) return -1;
-    if (trans < 0 || trans > 2) return fail(SLU_API "%s: trans = %d, must be 0 (A x = b), 1 (A^T x = b) or 2 (A^H x = b)", fn, trans);
-    if (!H->factored) return fail("slu_b200_%s needs a successful slu_b200_factor on this handle first", fn);
-    if (nrhs < 1 || ldx < H->n) return fail("bad nrhs / ldx");
-    if (H->P2 > 1) return fail("slu_b200_%s: Pr x Pc > 1 is not supported yet (1 x 1 x Pz only)", fn);
-    if (H->comm && !H->coop) return fail("slu_b200_%s: the Z-distributed solve needs the cooperative schedule (options.reserved[1] = 0)", fn);
     const int n = H->n;
     const size_t len = (size_t)n * nrhs;
-    if (H->d_x.n < len && (H->d_x.alloc(len) || H->d_x2.alloc(len))) return -1;
     cudaStream_t s = H->stream;
     const DeviceLU &d = H->dev;
     val_t *x = H->d_x.p, *x2 = H->d_x2.p;
-    double t0 = now_s();
-    CU(cudaMemcpy2DAsync(x2, (size_t)n * sizeof(val_t), xh, (size_t)ldx * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs,
-                         cudaMemcpyHostToDevice, s));
     const bool multi = H->comm != nullptr;
     int launches = 0;
     auto forest_nodes = [&](int zl) { return H->d_pool_i32.p + H->z_nodes_off[zl]; };
@@ -1782,14 +1782,37 @@ static int solve_impl(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int tr
             NC(g_nccl.AllReduce(x, x, len * VAL_DOUBLES, NCCL_FLOAT64, NCCL_SUM, H->gcomm[zl], s));
         }
     }
-    val_t *result = x;
+    *result = x;
     if (multi) {      // every rank contributes the entries it owns: the full solution everywhere
         CU(cudaMemsetAsync(x2, 0, len * sizeof(val_t), s));
         for (int zl = 0; zl < H->max_lvl; ++zl)
             if (!H->my_zero[zl]) launches += launch_solve_mask(d, forest_nodes(zl), (int)H->znodes[zl].size(), x2, n, nrhs, x, s);
         NC(g_nccl.AllReduce(x2, x2, len * VAL_DOUBLES, NCCL_FLOAT64, NCCL_SUM, H->comm, s));
-        result = x2;
+        *result = x2;
     }
+    return launches;
+}
+
+// fn: "solve" or "solve_trans", for the messages
+static int solve_impl(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int trans, const char *fn)
+{
+    if (!H || !xh) return fail("null argument");
+    if (refuse_batched(H, (std::string(SLU_API) + fn).c_str())) return -1;
+    if (trans < 0 || trans > 2) return fail(SLU_API "%s: trans = %d, must be 0 (A x = b), 1 (A^T x = b) or 2 (A^H x = b)", fn, trans);
+    if (!H->factored) return fail("slu_b200_%s needs a successful slu_b200_factor on this handle first", fn);
+    if (nrhs < 1 || ldx < H->n) return fail("bad nrhs / ldx");
+    if (H->P2 > 1) return fail("slu_b200_%s: Pr x Pc > 1 is not supported yet (1 x 1 x Pz only)", fn);
+    if (H->comm && !H->coop) return fail("slu_b200_%s: the Z-distributed solve needs the cooperative schedule (options.reserved[1] = 0)", fn);
+    const int n = H->n;
+    const size_t len = (size_t)n * nrhs;
+    if (H->d_x.n < len && (H->d_x.alloc(len) || H->d_x2.alloc(len))) return -1;
+    cudaStream_t s = H->stream;
+    double t0 = now_s();
+    CU(cudaMemcpy2DAsync(H->d_x2.p, (size_t)n * sizeof(val_t), xh, (size_t)ldx * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs,
+                         cudaMemcpyHostToDevice, s));
+    val_t *result = nullptr;
+    const int launches = solve_dev(H, nrhs, trans, &result);
+    if (launches < 0) return -1;
     CU(cudaMemcpy2DAsync(xh, (size_t)ldx * sizeof(val_t), result, (size_t)n * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs,
                          cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
@@ -1985,6 +2008,20 @@ int slu_b200_batch_factor(slu_b200_handle_t H, int *info)
     return 0;
 }
 
+// The solve of a batched handle on device vectors, in place in d_x (batch blocks of n x nrhs).  Enqueued on H->stream, not
+// synchronised.  Returns the kernel launches.
+static int batch_solve_dev(slu_b200_handle_t H, int nrhs, int trans)
+{
+    const BatchedLU &d = H->bdev;
+    val_t *x = H->d_x.p;
+    int launches = 0;
+    for (size_t li = 0; li < H->levels.size(); ++li)            // forward: L y = b (U^T y = b)
+        launches += solve_level(H, d, H->levels[li], false, trans, x, H->n, nrhs, H->stream);
+    for (size_t li = H->levels.size(); li-- > 0;)               // backward: U x = y (L^T x = y)
+        launches += solve_level(H, d, H->levels[li], true, trans, x, H->n, nrhs, H->stream);
+    return launches;
+}
+
 // x: batch blocks, block j at x + j * ldx * nrhs, each n x nrhs column-major (ldx >= n): b on entry, the solution on return.
 // trans as solve_impl; fn: "batch_solve" or "batch_solve_trans", for the messages
 static int batch_solve_impl(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int trans, const char *fn)
@@ -2002,17 +2039,12 @@ static int batch_solve_impl(slu_b200_handle_t H, double *xh, int ldx, int nrhs, 
     const size_t len = (size_t)n * nrhs * B;
     if (H->d_x.n < len && H->d_x.alloc(len)) return -1;
     cudaStream_t s = H->stream;
-    const BatchedLU &d = H->bdev;
     val_t *x = H->d_x.p;
     double t0 = now_s();
     // the B blocks are B * nrhs columns at pitch ldx: one 2D copy each way
     CU(cudaMemcpy2DAsync(x, (size_t)n * sizeof(val_t), xh, (size_t)ldx * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs * B,
                          cudaMemcpyHostToDevice, s));
-    int launches = 0;
-    for (size_t li = 0; li < H->levels.size(); ++li)            // forward: L y = b (U^T y = b)
-        launches += solve_level(H, d, H->levels[li], false, trans, x, n, nrhs, s);
-    for (size_t li = H->levels.size(); li-- > 0;)               // backward: U x = y (L^T x = y)
-        launches += solve_level(H, d, H->levels[li], true, trans, x, n, nrhs, s);
+    const int launches = batch_solve_dev(H, nrhs, trans);
     CU(cudaMemcpy2DAsync(xh, (size_t)ldx * sizeof(val_t), x, (size_t)n * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs * B,
                          cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
@@ -2030,6 +2062,101 @@ int slu_b200_batch_solve(slu_b200_handle_t H, double *xh, int ldx, int nrhs)
 int slu_b200_batch_solve_trans(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int trans)
 {
     return batch_solve_impl(H, xh, ldx, nrhs, trans, "batch_solve_trans");
+}
+
+// ---- condition estimation on the resident factors (LAPACK dgecon / zgecon, sequential SuperLU dgscon / zgscon) --------
+// dlacn2 / zlacn2 estimate ||B||_1 for B = F^-1 (norm '1') or B = F^-T / F^-H (norm 'I'), F = P A P^T, by reverse
+// communication: "kase 1" asks for B x, "kase 2" for B^T x (B^H x).  Each round here is one solve of every member on
+// device vectors (solve_dev / batch_solve_dev, exactly the launches of a solve) and the step kernels of slu_cond.cu; the
+// host only reads back how many members wait for kase 1 and for kase 2.  The next round takes the kase other than the
+// last one if any member waits for it, else the same one: with one member these are exactly dlacn2's solves, and in a
+// batch no member waits more than one round.
+// Where the next vectors live: a batched handle keeps every member's pending vector in d_cv, because a member whose kase
+// is not the round's must keep it; each round copies d_cv into d_x, where the batched solve runs in place.  An unbatched
+// handle's one member takes every round, so its step kernels write the next vector straight into d_x2, where solve_dev
+// takes its right-hand side (in place over the solution along Z, where the solve ends in d_x2).
+constexpr int COND_MAX_ROUNDS = 64;     // dlacn2 makes at most 11 solves; lock-step at most doubles that
+
+// the preconditions of the matching solve are checked by the caller; B = 1 member on an unbatched handle
+static int gscon_impl(slu_b200_handle_t H, char norm, const double *anorm, double *rcond, const char *fn)
+{
+    const bool batched = H->batch > 0;
+    const int B = batched ? H->batch : 1, n = H->n;
+    const bool one = norm == '1' || norm == 'O' || norm == 'o';
+    if (!one && norm != 'I' && norm != 'i')
+        return fail("%s: norm must be '1', 'O' or 'I' (got character code %d)", fn, (int)(unsigned char)norm);
+    for (int j = 0; j < B; ++j) {
+        if (anorm[j] >= 0.0) continue;
+        if (batched) return fail("%s: anorm[%d] = %g, must be >= 0", fn, j, anorm[j]);
+        return fail("%s: anorm = %g, must be >= 0", fn, anorm[j]);
+    }
+    const double t0 = now_s();
+    int rounds = 0;
+    bool any = false;
+    for (int j = 0; j < B; ++j) {
+        rcond[j] = 0.0;                                   // anorm 0 or +inf: rcond 0 without a solve
+        any = any || (anorm[j] > 0.0 && std::isfinite(anorm[j]));
+    }
+    if (any) {
+        const size_t len = (size_t)n * B;
+        const size_t parts = (size_t)((n + COND_CHUNK - 1) / COND_CHUNK) * B;
+        if (batched && H->d_cv.n < len && H->d_cv.alloc(len)) return -1;
+        if (VAL_DOUBLES == 1 && H->d_csgn.n < len && H->d_csgn.alloc(len)) return -1;     // the real repeated-sign test
+        if (H->d_cstate.n < (size_t)B && (H->d_cstate.alloc(B) || H->d_cpart.alloc(parts) || H->d_ccount.alloc(2))) return -1;
+        if (batched ? (H->d_x.n < len && H->d_x.alloc(len)) : (H->d_x.n < len && (H->d_x.alloc(len) || H->d_x2.alloc(len)))) return -1;
+        cudaStream_t s = H->stream;
+        val_t *v = batched ? H->d_cv.p : H->d_x2.p;       // the pending vectors
+        launch_cond_init(H->d_cstate.p, v, n, B, s);
+        for (int kase = 1;;) {
+            if (rounds == COND_MAX_ROUNDS) return fail("%s: the estimator did not finish in %d solves", fn, rounds);
+            const int trans = (kase == 1) == one ? 0 : (VAL_DOUBLES == 2 ? 2 : 1);
+            val_t *x = H->d_x.p;
+            if (batched) {
+                CU(cudaMemcpyAsync(x, v, len * sizeof(val_t), cudaMemcpyDeviceToDevice, s));
+                batch_solve_dev(H, 1, trans);
+            } else if (solve_dev(H, 1, trans, &x) < 0) {
+                return -1;
+            }
+            CU(cudaMemsetAsync(H->d_ccount.p, 0, 2 * sizeof(int), s));
+            launch_cond_step(H->d_cstate.p, kase, x, v, H->d_csgn.p, H->d_cpart.p, H->d_ccount.p, n, B, s);
+            int waiting[2] = {0, 0};                      // members waiting for kase 1 / kase 2
+            CU(cudaMemcpyAsync(waiting, H->d_ccount.p, sizeof waiting, cudaMemcpyDeviceToHost, s));
+            CU(cudaStreamSynchronize(s));
+            ++rounds;
+            if (waiting[2 - kase] > 0) kase = 3 - kase;
+            else if (waiting[kase - 1] == 0) break;
+        }
+        CU(cudaGetLastError());
+        std::vector<CondState> st(B);
+        CU(cudaMemcpy(st.data(), H->d_cstate.p, B * sizeof(CondState), cudaMemcpyDeviceToHost));
+        for (int j = 0; j < B; ++j)
+            if (anorm[j] > 0.0 && std::isfinite(anorm[j]) && std::isfinite(st[j].est) && st[j].est != 0.0)
+                rcond[j] = (1.0 / st[j].est) / anorm[j];
+    }
+    H->st.reserved[6] = now_s() - t0;
+    H->st.reserved[7] = (double)rounds;
+    return 0;
+}
+
+int slu_b200_gscon(slu_b200_handle_t H, char norm, double anorm, double *rcond)
+{
+    if (!H || !rcond) return fail("null argument");
+    if (refuse_batched(H, SLU_API "gscon")) return -1;
+    if (!H->factored) return fail(SLU_API "gscon needs a successful " SLU_API "factor on this handle first");
+    if (H->P2 > 1) return fail(SLU_API "gscon: Pr x Pc > 1 is not supported yet (1 x 1 x Pz only)");
+    if (H->comm && !H->coop) return fail(SLU_API "gscon: the Z-distributed solve needs the cooperative schedule (options.reserved[1] = 0)");
+    return gscon_impl(H, norm, &anorm, rcond, SLU_API "gscon");
+}
+
+int slu_b200_batch_gscon(slu_b200_handle_t H, char norm, const double *anorm, double *rcond)
+{
+    if (!H || !anorm || !rcond) return fail("null argument");
+    if (refuse_unbatched(H, SLU_API "batch_gscon")) return -1;
+    for (int j = 0; j < H->batch; ++j) {
+        if (H->member_info[j] < 0) return fail(SLU_API "batch_gscon needs a " SLU_API "batch_factor of the filled members first");
+        if (H->member_info[j] > 0) return fail(SLU_API "batch_gscon: member %d has an exact zero pivot in column %d", j, H->member_info[j]);
+    }
+    return gscon_impl(H, norm, anorm, rcond, SLU_API "batch_gscon");
 }
 
 // D2H of member `member`'s L and U into the view's Lnzval / Unzval, as slu_b200_download

@@ -187,6 +187,25 @@ int launch_solve_update(const BatchedLU &d, const Batch &b, int64_t ctas, bool b
 int launch_fill_csr(const BatchedLU &d, int n, const int32_t *rowptr, const int32_t *colind, const val_t *aval, const int32_t *perm,
                     const int8_t *active, int *err, cudaStream_t s);
 
+// slu_cond.cu (double) / slu_cond_z.cu (doublecomplex): the step kernels of the dlacn2 / zlacn2 1-norm estimator
+// (slu_b200_gscon).  One CondState per member: dlacn2's EST, ESTOLD and ISAVE(1..3) as phase, j, iter; kase = the solve
+// the member waits for (1: with B, 2: with B^T / B^H, 0: done); act = the next vector its last step wrote.
+// Vectors: `members` blocks of n elements back to back.
+constexpr int COND_CHUNK = 2048;      // elements per CTA of the per-member reductions
+enum { COND_NONE = 0, COND_EJ = 1, COND_SIGN = 2, COND_ALT = 3 };
+struct CondState {
+    double est, estold;
+    int32_t phase, kase, j, iter, act, pad;
+};
+struct CondPart { double sum, maxv; int32_t maxi, diff; };   // one chunk: sum |x_i|, max |x_i| at the lowest index, sign changes
+// v = 1/n for every member, state reset (kase 1)
+int launch_cond_init(CondState *st, val_t *v, int n, int members, cudaStream_t s);
+// after a solve of kase `kase` whose results are x: the members waiting for it take one dlacn2 step and write their next
+// vector into v; counts[0] / [1] (zeroed by the caller) receive how many members then wait for kase 1 / 2.  3 launches.
+// part: members * ceil(n / COND_CHUNK) entries
+int launch_cond_step(CondState *st, int kase, const val_t *x, val_t *v, val_t *sgn, CondPart *part, int *counts, int n, int members,
+                     cudaStream_t s);
+
 #ifndef SLU_COMPLEX
 // slu_ozaki.cu: the Schur update of wide supernodes on wgmma (int8 slices, exact int32 accumulation in registers)
 constexpr int OZ_NT = 32;             // columns of one CTA's int8 Schur tile (rows: 128)
