@@ -94,7 +94,8 @@ typedef struct {
                                   /* uses slu_b200_factor_host (overlapped transfers), [3] level-by-  */
                                   /* level arena so that factor_host also overlaps the upload,        */
                                   /* [4] tcgen05 path for wide supernodes: int8 slices per operand    */
-                                  /* (0 = default 7, 5..8, < 0 = off: FP64 DMMA only), [5] narrowest   */
+                                  /* (0 = default: off, 5..8 opt in, < 0 = off: FP64 DMMA only; needs  */
+                                  /* balanced pivot-row scales, e.g. an equilibrated A), [5] narrowest */
                                   /* supernode that takes the tcgen05 path (0 = default 128)          */
 } slu_b200_options_t;
 

@@ -249,7 +249,7 @@ def make_options(prob, device=-1, verbose=0, world_size=1, world_rank=0, nccl_id
     o.reserved[2] = pipeline       # 1: pdgstrf3d_b200 overlaps H2D / factor / D2H (slu_b200_factor_host)
     o.reserved[1] = no_coop        # 1: reference-style ancestors (owner layer factors alone after a pairwise reduce)
     o.reserved[3] = overlap_h2d    # 1: level-by-level arena; factor_host also overlaps the upload (opt-in, DESIGN 9)
-    o.reserved[4] = tc_slices      # int8 tensor-core path: int8 slices per operand (0 default, < 0 off, 5..8)
+    o.reserved[4] = tc_slices      # int8 tensor-core path: int8 slices per operand (0 default: off, < 0 off, 5..8)
     o.reserved[5] = tc_min_ns      # narrowest supernode on the int8 tensor-core path (0: default)
     o.world_size, o.world_rank = world_size, world_rank
     if nccl_id is not None:

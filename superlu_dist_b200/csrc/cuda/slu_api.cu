@@ -242,7 +242,7 @@ struct slu_b200_handle_s {
     DevBuf<double> d_oz_scale;
     DevBuf<int> d_oz_rexp;
     int tc_slices = 0, tc_min_ns = 0;     // 0 slices: int8 tensor-core path off
-    int tc_max_m = 0;                     // > 0: only updates of fewer rows take the int8 path (its default); 0: no limit
+    int tc_max_m = 0;                     // > 0: only updates of fewer rows take the int8 path (SLU_B200_TC_MAX_M); 0: no limit
     bool tc_force_off = false, tc_alloc_failed = false;   // slice workspace did not fit: analysed again without the int8 tensor-core path
     int tc_nonatomic = 0;                 // plain load/store scatter for destinations only one supernode of a level updates
     DevBuf<val_t> d_x, d_x2;              // triangular solve: right-hand sides / solution
@@ -604,11 +604,10 @@ int analyze(slu_b200_handle_s *H)
     int64_t ws_oz_i8_max = 0, ws_oz_s_max = 0;
     double ops_tc = 0;
 #ifndef SLU_COMPLEX
-    // int8 tensor-core path (slu_ozaki.cu): options.reserved[4] = int8 slices per operand (0: default, < 0: off),
+    // int8 tensor-core path (slu_ozaki.cu): options.reserved[4] = int8 slices per operand (0: default = off, < 0: off),
     // options.reserved[5] = narrowest supernode that takes it (0: default)
     H->tc_slices = H->opt.reserved[4] < 0 ? 0 : (H->opt.reserved[4] == 0 ? (OZ_DEFAULT_ON ? OZ_DEFAULT_SLICES : 0) : std::min(8, std::max(5, (int)H->opt.reserved[4])));
     H->tc_min_ns = H->opt.reserved[5] > 0 ? H->opt.reserved[5] : OZ_DEFAULT_MIN_NS;
-    H->tc_max_m = H->opt.reserved[4] == 0 ? OZ_DEFAULT_MAX_M : 0;
     if (getenv("SLU_B200_TC_MAX_M")) H->tc_max_m = std::max(0, atoi(getenv("SLU_B200_TC_MAX_M")));
     if (getenv("SLU_B200_TC_SLICES")) { int v = atoi(getenv("SLU_B200_TC_SLICES")); H->tc_slices = v <= 0 ? 0 : std::min(8, std::max(5, v)); }
     if (getenv("SLU_B200_TC_MIN_NS")) H->tc_min_ns = std::max(1, atoi(getenv("SLU_B200_TC_MIN_NS")));

@@ -216,12 +216,11 @@ constexpr int OZ_DEFAULT_SLICES = 7;  // 48 bits per operand: error ~1e-15 * k *
 constexpr int OZ_DEFAULT_MIN_NS = 128;
 constexpr bool OZ_PERSIST_DEFAULT = false;     // persistent int8 Schur kernel (SLU_B200_TC_PERSIST=1|0)
 constexpr bool OZ_NONATOMIC_DEFAULT = false;   // SLU_B200_TC_NONATOMIC=1|0 overrides
-constexpr bool OZ_DEFAULT_ON = true;  // options.reserved[4] = -1 / SLU_B200_TC_SLICES=0: off
-// By default the int8 path takes only updates of fewer than OZ_DEFAULT_MAX_M rows (SLU_B200_TC_MAX_M overrides, 0: no
-// limit); larger ones go to the FP64 kernel on DMMA.16x8x8 (schur_kernel_h), which is faster there -- at S = 7 the int8
-// path's ceiling on the H100 is the FP64 tensor rate (DESIGN 4b).  An explicit slice count (options.reserved[4] = 5..8)
-// sets no row limit.
-constexpr int OZ_DEFAULT_MAX_M = 2048;
+// Off by default: the slices are scaled per L row and per U column, not per k, so the error is relative to rowmax * colmax
+// of each update and grows as (max / min pivot-row scale)^2 on a matrix that is not equilibrated (DESIGN 4b).  An
+// explicit slice count (options.reserved[4] = 5..8, or SLU_B200_TC_SLICES) opts in; SLU_B200_TC_MAX_M limits it to
+// updates of fewer rows (0: no limit).
+constexpr bool OZ_DEFAULT_ON = false;
 inline int64_t oz_a_bytes(int m, int ns, int S) { return (int64_t)((m + 127) / 128) * ((ns + OZ_KSTEP - 1) / OZ_KSTEP) * S * 4096; }
 inline int64_t oz_b_bytes(int n, int ns, int S) { return (int64_t)((n + OZ_NT - 1) / OZ_NT) * ((ns + OZ_KSTEP - 1) / OZ_KSTEP) * S * OZ_NT * OZ_KSTEP; }
 inline int64_t oz_scale_elems(int m, int n) { return (int64_t)((m + 127) / 128) * 128 + (int64_t)((n + OZ_NT - 1) / OZ_NT) * OZ_NT; }

@@ -3,7 +3,7 @@
 Tolerances.  With S slices an operand row is known to 2^-(7S-1) of ITS power-of-two scale 2^e (max|row| <= 2^e < 2 max|row|),
 and the S cross terms of weight 2^-(7S+5) per (s, t) pair with s + t = S are dropped, so for every element
     |(C - A B)_ij - exact| <= k * (S + 2) * 2^(4-7S) * rowmax_i * colmax_j        (worst case, any data)
-= k * 2.9e-11 (S = 6), 2.6e-13 (S = 7, the default), 2.2e-15 (S = 8) in units of rowmax * colmax.  Typical data sit one to two
+= k * 2.9e-11 (S = 6), 2.6e-13 (S = 7), 2.2e-15 (S = 8) in units of rowmax * colmax.  The path is opt-in (tc_slices).  Typical data sit one to two
 orders below; the worst case is approached
 only for k of a few (no averaging).  Inside the factorization the parity bar of the other tests applies unchanged: entry-wise
 1e-10 relative to max|factor| against the oracle, residual probe <= 1e-12."""
@@ -80,23 +80,26 @@ def test_factorization_through_tcgen05(kw, slices):
     assert rel_err(a.lval, b.lval) < 1e-10 and rel_err(a.uval, b.uval) < 1e-10
 
 
-def test_tcgen05_off_switch_and_residual():
-    """options.reserved[4] = -1 turns the path off (FP64 DMMA only); with it on (default) the size-independent residual
-    probe stays at the 1e-15 level."""
-    prob, _ = poisson_problem(32, leaf=64, relax=32, maxsup=256)
-    pre = prob.layers[0].copy()
-    info, st = capi.pdgstrf3d(prob, 0, tc_slices=-1)
-    assert info == 0 and st.reserved[1] == 0 and int(st.reserved[3]) == 0
-    every = np.ones(prob.nsupers, bool)
-    assert residual_probe(prob, [(pre, every)], [(prob.layers[0], every)]) < 1e-12
+def test_tcgen05_default_off_and_opt_in_residual():
+    """The path is off by default (its error is relative to rowmax * colmax of each update, so it needs balanced pivot
+    scales: tests/test_scaled_parity.py) and with options.reserved[4] = -1 (FP64 DMMA only); opted in with 7 slices it
+    carries most of the Schur flops and the size-independent residual probe stays at the 1e-15 level."""
+    for tc in (0, -1):
+        prob, _ = poisson_problem(32, leaf=64, relax=32, maxsup=256)
+        pre = prob.layers[0].copy()
+        every = np.ones(prob.nsupers, bool)
+        info, st = capi.pdgstrf3d(prob, 0, tc_slices=tc)
+        assert info == 0 and st.reserved[1] == 0 and int(st.reserved[3]) == 0, tc
+        assert residual_probe(prob, [(pre, every)], [(prob.layers[0], every)]) < 1e-12
     prob2, _ = poisson_problem(32, leaf=64, relax=32, maxsup=256)
-    info, st = capi.pdgstrf3d(prob2, 0)
-    assert info == 0 and st.reserved[1] > 0.5 * st.ops_schur               # default: on, and it carries most of the flops
+    info, st = capi.pdgstrf3d(prob2, 0, tc_slices=7)
+    assert info == 0 and st.reserved[1] > 0.5 * st.ops_schur and int(st.reserved[3]) == 7   # on: most of the flops
     assert residual_probe(prob2, [(pre, every)], [(prob2.layers[0], every)]) < 1e-12
 
 
-def test_persistent_kernel_matches():
-    """The persistent warp-specialised form of the kernel (SLU_B200_TC_PERSIST=1, read once per process: child)."""
+def test_persistent_kernel_matches_opt_in():
+    """The persistent warp-specialised form of the kernel (SLU_B200_TC_PERSIST=1, read once per process: child), with
+    the int8 path opted in (7 slices)."""
     code = f'''
 import os, sys
 os.environ["SLU_B200_TC_PERSIST"] = "1"
@@ -106,7 +109,7 @@ from superlu_dist_b200 import capi
 from util import poisson_problem, rel_err
 for kw in (dict(N=14, leaf=8, relax=16, maxsup=256), dict(N=18, leaf=16, relax=32, maxsup=256)):
     prob, _ = poisson_problem(**kw); chk, _ = poisson_problem(**kw)
-    info, st = capi.pdgstrf3d(prob, 0, tc_min_ns=64)
+    info, st = capi.pdgstrf3d(prob, 0, tc_slices=7, tc_min_ns=64)
     oracle.factor(chk)
     assert info == 0 and st.reserved[1] > 0
     assert rel_err(prob.layers[0].lval, chk.layers[0].lval) < 1e-10 and rel_err(prob.layers[0].uval, chk.layers[0].uval) < 1e-10

@@ -1,7 +1,7 @@
 """The FP64 Schur kernel of the big tiles on mma.sync.m16n8k8.f64 (schur_kernel_h, gemm_tile_h): the GEMM main loop
 against NumPy at edge shapes, and whole factorizations with 256- and 512-column supernodes against the oracle, with and
-without look-ahead and batched.  tc_slices = -1 keeps the int8 path off, so that every big tile takes the new kernel
-(by default the int8 path takes the wide updates of fewer than OZ_DEFAULT_MAX_M rows, which is all of them here)."""
+without look-ahead and batched.  The int8 path is off by default; tc_slices = -1 turns it off explicitly, so that every
+big tile takes this kernel whatever the default."""
 import os
 
 import numpy as np
@@ -36,13 +36,13 @@ def test_gemm_sub_m16n8k8(variant, m, n, k):
 @pytest.mark.parametrize("tc", [0, -1])
 @pytest.mark.parametrize("kw", [_W256, _W512])
 def test_factorization_matches_oracle(kw, tc):
-    """tc = 0: the default routing; -1: the new kernel for every big tile."""
+    """tc = 0: the default routing (FP64: the int8 path is opt-in); -1: this kernel for every big tile, explicitly."""
     prob, _ = poisson_problem(**kw)
     chk, _ = poisson_problem(**kw)
     assert np.diff(np.asarray(prob.xsup)).max() == kw["maxsup"]
     info, st = capi.pdgstrf3d(prob, 0, tc_slices=tc)
     oinfo, oops, _ = oracle.factor(chk)
-    assert info == oinfo == 0 and (tc == 0 or st.reserved[1] == 0)
+    assert info == oinfo == 0 and st.reserved[1] == 0
     assert abs(st.ops_fact - oops) <= 1e-9 * oops
     a, b = prob.layers[0], chk.layers[0]
     assert rel_err(a.lval, b.lval) < TOL and rel_err(a.uval, b.uval) < TOL
