@@ -189,6 +189,24 @@ int slu_b200_solve_trans(slu_b200_handle_t h, double *x, int ldx, int nrhs, int 
  * stats.reserved[7] = the solves it ran; stats.reserved[4] / [5] keep describing the last slu_b200_solve*.  The
  * reference's pdgssvx3d has no condition estimator. */
 int slu_b200_gscon(slu_b200_handle_t h, char norm, double anorm, double *rcond);
+/* Selected inversion on the resident factors (SelInv / PSelInv): H = F^-T on the stored pattern of L+U, F = P A P^T = L U,
+ * into a second HBM arena of the factors' layout (allocated on first use, freed by destroy).  One sweep over the level plan,
+ * top-down, about twice the Schur-update flops; deterministic (every entry written once with plain stores: two calls on the
+ * same factors give bit-identical H); the factors are only read.  A^-1(i, j) = H(perm[j], perm[i]): the entries of A^-1 on
+ * the pattern of A^T, and of A where A is structurally symmetric.  Where tiny pivots were replaced the result describes
+ * L U as factored, as for slu_b200_gscon.  If the second arena does not fit, the call fails and the handle stays usable for
+ * solves.  Restrictions (all fail with a message): a successful factorization (info = 0), an unbatched handle, a 1 x 1 x 1
+ * grid (world_size 1).  Double only; the reference's pdgssvx3d has no selected inversion.
+ * out (may be NULL): [0] seconds, [1] flops (accounting in DESIGN.md), [2] kernel launches, [3] HBM bytes it holds. */
+int slu_b200_selinv(slu_b200_handle_t h, double out[4]);
+/* out[p] = (A^-1)(i, colind[p]) for every entry p of row i of the CSR pattern; A = P^T F P, perm[old] = new as in
+ * slu_b200_fill_csr.  Fails, with the count, if any (perm[colind[p]], perm[i]) has no slot in L+U.  Needs slu_b200_selinv
+ * on the current factors: a later upload, fill_csr or factor invalidates the inverse; n must match the handle. */
+int slu_b200_selinv_get(slu_b200_handle_t h, int n, const int32_t *rowptr, const int32_t *colind,
+                        const int32_t *perm, double *out);
+/* log|det A| and its sign (+1 / -1) from the resident factors: sum of log |U_kk(i,i)| in a fixed order (deterministic),
+ * sign from the count of negative pivots; the symmetric permutation does not change det.  Restrictions of selinv. */
+int slu_b200_logdet(slu_b200_handle_t h, double *logabs, double *sign);
 int slu_b200_get_stats(slu_b200_handle_t h, slu_b200_stats_t *out);
 void slu_b200_destroy(slu_b200_handle_t h);
 

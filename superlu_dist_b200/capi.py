@@ -118,6 +118,9 @@ def lib():
         getattr(L, f).argtypes = [C.c_void_p, C.c_char, C.c_double, C.POINTER(C.c_double)]
     for f in ("slu_b200_batch_gscon", "slu_b200_z_batch_gscon"):
         getattr(L, f).argtypes = [C.c_void_p, C.c_char, C.c_void_p, C.c_void_p]
+    L.slu_b200_selinv.argtypes = [C.c_void_p, C.c_void_p]
+    L.slu_b200_selinv_get.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.slu_b200_logdet.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double)]
     _lib = L
     return L
 
@@ -328,6 +331,43 @@ class Handle:
         out = C.c_double(0.0)
         _check(_fn("gscon", self.z_)(self.h, _norm_byte(norm), float(anorm), C.byref(out)))
         return out.value
+
+    def _real_only(self, what):
+        if self.z_:
+            raise TypeError(f"{what} is implemented for double problems only")
+
+    def selinv(self):
+        """Selected inversion on the resident factors (slu_b200_selinv): H = F^-T on the pattern of L + U, kept in HBM for
+        inv_entries / inv_diag.  -> (seconds, flops, kernel launches, HBM bytes held)"""
+        self._real_only("selinv")
+        out = (C.c_double * 4)()
+        _check(lib().slu_b200_selinv(self.h, out))
+        return tuple(out)
+
+    def inv_entries(self, rowptr, colind, perm):
+        """(A^-1)(i, colind[p]) for every entry p of row i of a CSR pattern (slu_b200_selinv_get), perm[old] = new as in
+        fill_csr; every entry must have a slot in L + U.  -> float64 array (nnz,)"""
+        self._real_only("inv_entries")
+        rp = np.ascontiguousarray(rowptr, np.int32)
+        ci = np.ascontiguousarray(colind, np.int32)
+        pm = np.ascontiguousarray(perm, np.int32)
+        out = np.empty(len(ci), np.float64)
+        _check(lib().slu_b200_selinv_get(self.h, len(rp) - 1, rp.ctypes.data_as(C.c_void_p), ci.ctypes.data_as(C.c_void_p),
+                                         pm.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p)))
+        return out
+
+    def inv_diag(self, perm=None):
+        """The diagonal of A^-1 (perm[old] = new; None: the identity, i.e. the diagonal of F^-1)."""
+        n = self.prob.n
+        pm = np.arange(n, dtype=np.int32) if perm is None else perm
+        return self.inv_entries(np.arange(n + 1, dtype=np.int32), np.arange(n, dtype=np.int32), pm)
+
+    def logdet(self):
+        """(sign, log |det A|) from the resident factors (slu_b200_logdet), as numpy.linalg.slogdet"""
+        self._real_only("logdet")
+        la, sg = C.c_double(0.0), C.c_double(0.0)
+        _check(lib().slu_b200_logdet(self.h, C.byref(la), C.byref(sg)))
+        return sg.value, la.value
 
     def _dtype(self):
         return np.complex128 if self.z_ else np.float64

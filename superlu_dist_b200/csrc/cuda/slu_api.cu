@@ -216,6 +216,13 @@ struct LevelPlan {
     int64_t sl_prefix = 0, sl_ctas = 0, su_prefix = 0, su_ctas = 0;   // triangular solve: 256-row / 256-column tiles
 };
 
+// selected inversion (slu_b200_selinv): per level, offsets into d_si_pool of the CTA prefixes of the three products
+// (gemm[0..2], slu_selinv.cu modes) and the two triangular solves (trsm[0]: rows, [1]: columns), and their CTA counts
+struct SelinvLevel {
+    int64_t gemm_prefix[3] = {0, 0, 0}, gemm_ctas[3] = {0, 0, 0};
+    int64_t trsm_prefix[2] = {0, 0}, trsm_ctas[2] = {0, 0};
+};
+
 }  // namespace
 
 struct slu_b200_handle_s {
@@ -289,6 +296,12 @@ struct slu_b200_handle_s {
     DevBuf<CondState> d_cstate;
     DevBuf<CondPart> d_cpart;
     DevBuf<int> d_ccount;
+    // selected inversion (slu_b200_selinv, double only): H = F^-T in a second arena of the factors' layout, its level plan,
+    // and whether it describes the current factors (a later upload, fill_csr or factor clears it)
+    DevBuf<val_t> d_hinv;
+    DevBuf<int64_t> d_si_pool;
+    std::vector<SelinvLevel> si_levels;
+    bool si_ready = false;
 };
 
 namespace {
@@ -1353,6 +1366,7 @@ void slu_b200_destroy(slu_b200_handle_t H)
     H->d_x.release(); H->d_x2.release();
     H->d_cv.release(); H->d_csgn.release(); H->d_cstate.release(); H->d_cpart.release(); H->d_ccount.release();
     H->d_tiny.release(); H->d_oz_i8.release(); H->d_oz_scale.release(); H->d_oz_rexp.release();
+    H->d_hinv.release(); H->d_si_pool.release();
     delete H;
 }
 
@@ -1467,6 +1481,7 @@ int slu_b200_upload(slu_b200_handle_t H)
     if (refuse_batched(H, SLU_API "upload")) return -1;
     double t0 = now_s();
     H->factored = false;
+    H->si_ready = false;
     if (transfer(H, true)) return -1;
     H->st.t_upload_s = now_s() - t0;
     H->uploaded = true;
@@ -1488,6 +1503,7 @@ static int factor_impl(slu_b200_handle_t H, int *info, bool pipelined, bool up_p
     if (!H || !info) return fail("null argument");
     if (refuse_batched(H, SLU_API "factor")) return -1;
     if (!H->uploaded) return fail("slu_b200_factor before slu_b200_upload");
+    H->si_ready = false;
     if (pipelined && pipe_prepare(H)) return -1;
     cudaStream_t s = H->stream;
     const DeviceLU &d = H->dev;
@@ -1671,6 +1687,7 @@ int slu_b200_fill_csr(slu_b200_handle_t H, int n, const int32_t *rowptr, const i
     if (refuse_batched(H, SLU_API "fill_csr")) return -1;
     if (n != H->n) return fail("matrix order %d does not match the handle's %d", n, H->n);
     if (H->P2 > 1) return fail("slu_b200_fill_csr handles 1 x 1 x Pz grids");
+    H->si_ready = false;
     double t0 = now_s();
     const int64_t nnz = rowptr[n];
     DevBuf<int32_t> drp, dci, dperm;
@@ -1881,6 +1898,148 @@ int slu_b200_k_rerun_schur(slu_b200_handle_t H, int level, int reps, float *ms)
     float t = 0;
     CU(cudaEventElapsedTime(&t, ev[0], ev[1]));
     *ms = t / reps;
+    return 0;
+}
+
+// ---- selected inversion and log-determinant on the resident factors (double only) ----------------------------------
+// slu_selinv.cu holds the kernels and the recurrences.  The sweep walks the level plan top-down (the backward solve's
+// order): every Schur destination of a supernode lies in a supernode of a later level, so its gathered block M = H(R, C)
+// is final.  Per level 7 launches: the destination maps and the 16x16 diagonal-block inverses are rebuilt in the
+// factorization's per-level workspaces, then three products and two triangular solves; a level with no Schur update (the
+// root) has no maps to build and makes 6.
+static int selinv_refuse(const slu_b200_handle_s *H, const char *fn)
+{
+    if (refuse_batched(H, fn)) return -1;
+    if (H->opt.world_size > 1 || H->max_lvl > 1 || H->P2 > 1) return fail("%s handles 1 x 1 x 1 grids (world_size 1)", fn);
+    if (!H->factored) return fail("%s needs a successful slu_b200_factor (info = 0) on this handle first", fn);
+    return 0;
+}
+
+// CTA prefixes of the selinv kernels, from the level plan: built once per handle
+static int selinv_plan(slu_b200_handle_s *H)
+{
+    std::vector<int64_t> pool;
+    H->si_levels.assign(H->levels.size(), SelinvLevel{});
+    auto tiles = [](int64_t a) { return (a + SELINV_TILE - 1) / SELINV_TILE; };
+    for (size_t li = 0; li < H->levels.size(); ++li) {
+        const LevelPlan &L = H->levels[li];
+        SelinvLevel &S = H->si_levels[li];
+        std::vector<int64_t> p[5];
+        for (auto &v : p) v.assign(1, 0);
+        for (int t = 0; t < L.count; ++t) {
+            const NodeDesc &nd = H->nodes[H->h_pool_i32[L.nodes_off + t]];
+            p[0].push_back(p[0].back() + tiles(nd.m) * tiles(nd.ns));
+            p[1].push_back(p[1].back() + tiles(nd.ns) * tiles(nd.ncols));
+            p[2].push_back(p[2].back() + tiles(nd.ns) * tiles(nd.ns));
+            p[3].push_back(p[3].back() + (nd.nsupr + SELINV_VECS - 1) / SELINV_VECS);
+            p[4].push_back(p[4].back() + (nd.ns + nd.ncols + SELINV_VECS - 1) / SELINV_VECS);
+        }
+        for (int q = 0; q < 5; ++q) {
+            if (p[q].back() > 2147483647LL) return fail("slu_b200_selinv: a level needs more than 2^31 CTAs in one launch");
+            int64_t &off = q < 3 ? S.gemm_prefix[q] : S.trsm_prefix[q - 3];
+            int64_t &ctas = q < 3 ? S.gemm_ctas[q] : S.trsm_ctas[q - 3];
+            off = (int64_t)pool.size();
+            ctas = p[q].back();
+            pool.insert(pool.end(), p[q].begin(), p[q].end());
+        }
+    }
+    return H->d_si_pool.upload(pool);
+}
+
+int slu_b200_selinv(slu_b200_handle_t H, double out[4])
+{
+    if (!H) return fail("null handle");
+    if (selinv_refuse(H, "slu_b200_selinv")) return -1;
+    H->si_ready = false;
+    if (H->si_levels.empty() && selinv_plan(H)) return -1;
+    if (!H->d_hinv.p && H->d_hinv.alloc((size_t)H->member_len)) {
+        cudaGetLastError();
+        std::string why = g_err;
+        H->d_hinv.release();
+        return fail("slu_b200_selinv: the inverse needs a second arena of %.2f GB beside the factors, which does not fit (%s); "
+                    "the factors are unchanged", 8e-9 * H->member_len, why.c_str());
+    }
+    cudaStream_t s = H->stream;
+    const DeviceLU &d = H->dev;
+    const int64_t *p64 = H->d_pool_i64.p, *sp = H->d_si_pool.p;
+    double *hv = H->d_hinv.p;
+    double flops = 0;
+    int launches = 0;
+    const double t0 = now_s();
+    CU(cudaMemsetAsync(H->d_flags.p + 1, 0, sizeof(int), s));
+    for (size_t li = H->levels.size(); li-- > 0;) {
+        const LevelPlan &L = H->levels[li];
+        const SelinvLevel &S = H->si_levels[li];
+        const int32_t *nodes = H->d_pool_i32.p + L.nodes_off;
+        launches += launch_schur_setup(d, Batch{nodes, p64 + L.setup_prefix, L.count}, L.setup_ctas, s);
+        launches += launch_diag_inv(d, Batch{nodes, p64 + L.inv_prefix, L.count}, L.inv_ctas, H->d_inv.p, s);
+        for (int q = 0; q < 3; ++q) launches += launch_selinv_gemm(d, Batch{nodes, sp + S.gemm_prefix[q], L.count}, S.gemm_ctas[q], q, hv, s);
+        for (int q = 0; q < 2; ++q)
+            launches += launch_selinv_trsm(d, Batch{nodes, sp + S.trsm_prefix[q], L.count}, S.trsm_ctas[q], q, H->d_inv.p, hv, s);
+        for (int t = 0; t < L.count; ++t) {
+            const NodeDesc &nd = H->nodes[H->h_pool_i32[L.nodes_off + t]];
+            const double m = nd.m, n = nd.ncols, ns = nd.ns;
+            flops += 4.0 * m * n * ns + 2.0 * m * ns * ns + (nd.nsupr + ns + n) * ns * ns;
+        }
+    }
+    int bad = 0;
+    CU(cudaMemcpyAsync(&bad, H->d_flags.p + 1, sizeof(int), cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    if (bad) return fail("slu_b200_selinv: %d Schur-update destinations were not found in the L/U structure", bad);
+    H->si_ready = true;
+    if (out) {
+        out[0] = now_s() - t0;
+        out[1] = flops;
+        out[2] = (double)launches;
+        out[3] = (double)(H->d_hinv.bytes() + H->d_si_pool.bytes());
+    }
+    return 0;
+}
+
+int slu_b200_selinv_get(slu_b200_handle_t H, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm, double *out)
+{
+    if (!H || !rowptr || !colind || !perm || !out) return fail("null argument");
+    if (selinv_refuse(H, "slu_b200_selinv_get")) return -1;
+    if (!H->si_ready) return fail("slu_b200_selinv_get needs slu_b200_selinv on the current factors first (a later upload, fill_csr or factor invalidates it)");
+    if (n != H->n) return fail("slu_b200_selinv_get: matrix order %d does not match the handle's %d", n, H->n);
+    const int64_t nnz = rowptr[n];
+    if (rowptr[0] != 0 || nnz < 0) return fail("slu_b200_selinv_get: bad rowptr");
+    DevBuf<int32_t> drp, dci, dperm;
+    DevBuf<double> dout;
+    if (drp.alloc((size_t)n + 1) || dci.alloc((size_t)nnz) || dperm.alloc((size_t)n) || dout.alloc((size_t)nnz)) return -1;
+    cudaStream_t s = H->stream;
+    CU(cudaMemcpyAsync(drp.p, rowptr, ((size_t)n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(dci.p, colind, (size_t)nnz * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(dperm.p, perm, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemsetAsync(H->d_flags.p + 1, 0, sizeof(int), s));
+    launch_selinv_get(H->dev, H->d_hinv.p, n, drp.p, dci.p, dperm.p, dout.p, H->d_flags.p + 1, s);
+    int bad = 0;
+    CU(cudaMemcpyAsync(out, dout.p, (size_t)nnz * sizeof(double), cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&bad, H->d_flags.p + 1, sizeof(int), cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    if (bad) return fail("slu_b200_selinv_get: %d entries have no slot in the L/U structure (A^-1 is known on the pattern of L+U only)", bad);
+    return 0;
+}
+
+int slu_b200_logdet(slu_b200_handle_t H, double *logabs, double *sign)
+{
+    if (!H || !logabs || !sign) return fail("null argument");
+    if (selinv_refuse(H, "slu_b200_logdet")) return -1;
+    const int count = (int)H->znodes[0].size();
+    const int nparts = (count + SELINV_VECS - 1) / SELINV_VECS;
+    DevBuf<double> part, res;
+    DevBuf<int> neg;
+    if (part.alloc((size_t)nparts) || neg.alloc((size_t)nparts) || res.alloc(2)) return -1;
+    cudaStream_t s = H->stream;
+    launch_selinv_logdet(H->dev, H->d_pool_i32.p + H->z_nodes_off[0], count, part.p, neg.p, res.p, s);
+    double r[2] = {0.0, 1.0};
+    CU(cudaMemcpyAsync(r, res.p, sizeof r, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    *logabs = r[0];
+    *sign = r[1];
     return 0;
 }
 #endif  // !SLU_COMPLEX
