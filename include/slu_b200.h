@@ -196,7 +196,7 @@ int slu_b200_gscon(slu_b200_handle_t h, char norm, double anorm, double *rcond);
  * the pattern of A^T, and of A where A is structurally symmetric.  Where tiny pivots were replaced the result describes
  * L U as factored, as for slu_b200_gscon.  If the second arena does not fit, the call fails and the handle stays usable for
  * solves.  Restrictions (all fail with a message): a successful factorization (info = 0), an unbatched handle, a 1 x 1 x 1
- * grid (world_size 1).  Double only; the reference's pdgssvx3d has no selected inversion.
+ * grid (world_size 1).  Doublecomplex through slu_b200_z_selinv below; the reference's pdgssvx3d has no selected inversion.
  * out (may be NULL): [0] seconds, [1] flops (accounting in DESIGN.md), [2] kernel launches, [3] HBM bytes it holds. */
 int slu_b200_selinv(slu_b200_handle_t h, double out[4]);
 /* out[p] = (A^-1)(i, colind[p]) for every entry p of row i of the CSR pattern; A = P^T F P, perm[old] = new as in
@@ -312,6 +312,16 @@ int slu_b200_z_solve_trans(slu_b200_zhandle_t h, double *x, int ldx, int nrhs, i
 /* as slu_b200_gscon, with zgecon's zlacn2: "kase 2" solves with F^H, |x_i| is the modulus, the sign vector is x_i / |x_i|
  * (1 where |x_i| is below the safe minimum) and there is no repeated-sign test */
 int slu_b200_z_gscon(slu_b200_zhandle_t h, char norm, double anorm, double *rcond);
+/* as slu_b200_selinv / _selinv_get / _logdet, with the same restrictions, messages and invalidation.  H = F^-T with a
+ * plain transpose, not the conjugate, so A^-1(i, j) = H(perm[j], perm[i]) holds unchanged (for a Hermitian A,
+ * A^-1(j, i) = conj(A^-1(i, j))).  out[1] counts 2 flops per complex multiply-add, as ops_fact does: 4x that in real
+ * flops.  selinv_get's out holds nnz interleaved doublecomplex (a complex NaN where a failed entry has no slot).
+ * z_logdet: *logabs = log |det A| = sum of log |u_ii|; sign[0..1] = exp(i theta), theta = sum of arg u_ii reduced
+ * modulo 2 pi (|sign| = 1), as complex numpy.linalg.slogdet returns it; fixed-order sums, deterministic. */
+int slu_b200_z_selinv(slu_b200_zhandle_t h, double out[4]);
+int slu_b200_z_selinv_get(slu_b200_zhandle_t h, int n, const int32_t *rowptr, const int32_t *colind,
+                          const int32_t *perm, double *out);
+int slu_b200_z_logdet(slu_b200_zhandle_t h, double *logabs, double *sign);
 /* batched doublecomplex handles (the reference's pzgssvx3d_csc_batch, SRC/complex16/pzgssvx3d_csc_batch.c:80): the
  * slu_b200_batch_* calls above with the same semantics, restrictions and stats; val and x point at interleaved
  * doublecomplex, n, ldx and nnz count complex elements.  Stats through slu_b200_z_get_stats, slu_b200_z_destroy frees.

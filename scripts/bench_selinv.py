@@ -1,6 +1,8 @@
-"""Selected inversion on the resident factors (slu_b200_selinv) against the factorization and against solves.
+"""Selected inversion on the resident factors (slu_b200_selinv, or slu_b200_z_selinv with --dtype c128) against the
+factorization and against solves.
 
-    python scripts/bench_selinv.py [--workloads poisson fem3] [--poisson-grid 48] [--fem-grid 0] [--steps K] [--warmup W]
+    python scripts/bench_selinv.py [--dtype f64|c128] [--workloads poisson fem3] [--poisson-grid 48] [--fem-grid 0]
+                                   [--steps K] [--warmup W]
 
 Workloads: Poisson 48^3 with the non-symmetric seeded values of scripts/bench_solve_trans.py, and the FEM workload of
 bench.py (27-point, 3 dof per node) at the largest grid whose factors fit twice beside their workspace in 80 GB
@@ -12,6 +14,9 @@ for inv_diag / inv_entries (H2D of the pattern and D2H of the values included); 
 the library's flop count (out[1]) over the selinv time.  diag(A^-1) by solves: timed batches of 8 unit-vector solves,
 extrapolated to n / 8 batches.  Sampled entries of inv_diag are checked against those solves.  Prints one JSON line per
 workload with the card's name and power limit read in the same run.  One GPU; writes nothing to disk.
+--dtype c128 runs the same on doublecomplex values (bench_solve_trans.values(..., True)); the FEM grid is sized by
+slu_b200_z_plan (16 bytes per entry), and the JSON line adds real_tflops = 4 x the library's rate, which counts a complex
+multiply-add as 2 flops.
 """
 import argparse
 import os
@@ -33,6 +38,7 @@ FEM_GRIDS = (68, 64, 60, 56, 52, 48, 44, 40, 36)
 
 def parse():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--dtype", default="f64", choices=["f64", "c128"])
     ap.add_argument("--workloads", nargs="+", default=["poisson", "fem3"], choices=["poisson", "fem3"])
     ap.add_argument("--poisson-grid", type=int, default=48)
     ap.add_argument("--fem-grid", type=int, default=0, help="0: the largest grid of FEM_GRIDS whose factors fit twice")
@@ -49,18 +55,25 @@ def symbolic(kind, g):
     return rp, ci, v, sym
 
 
-def fits_twice(sym):
+def new_problem(sym, cplx):
     prob = LUProblem.from_symbolic(sym, npdep=1)
+    if cplx:
+        prob.dtype = np.dtype(np.complex128)
     prob.add_layer(0)
+    return prob
+
+
+def fits_twice(sym, cplx):
+    prob = new_problem(sym, cplx)
     st = capi.plan(prob, 0)
     return 2 * st.lu_device_bytes + st.index_device_bytes <= 0.9 * HBM_BYTES, st
 
 
 def run_one(kind, g, rp, ci, v, sym, args, gpu):
     n = len(rp) - 1
-    prob = LUProblem.from_symbolic(sym, npdep=1)
-    prob.add_layer(0)
-    val = values(rp, ci, v, False)
+    cplx = args.dtype == "c128"
+    prob = new_problem(sym, cplx)
+    val = values(rp, ci, v, cplx)
     pm = np.asarray(prob.perm, np.int32)
     h = capi.Handle(prob, 0, device=0)
     t_fac, t_si, t_diag, t_ent, out = [], [], [], [], None
@@ -84,7 +97,7 @@ def run_one(kind, g, rp, ci, v, sym, args, gpu):
     ts, worst = [], 0.0
     for b in range(args.solve_batches + 1):
         cols = rng.choice(n, 8, replace=False)
-        rhs = np.zeros((8, n))
+        rhs = np.zeros((8, n), prob.dtype)
         rhs[np.arange(8), pm[cols]] = 1.0
         x = h.solve(rhs)
         if b:
@@ -96,6 +109,11 @@ def run_one(kind, g, rp, ci, v, sym, args, gpu):
     h.close()
     med = lambda xs: float(np.median(xs))  # noqa: E731
     name = bench.workload_name(g, kind)
+    extra = {}
+    if cplx:
+        name = name.replace("fp64", "c128")
+        extra = {"dtype": "c128", "real_tflops": round(4 * out[1] / med(t_si) / 1e12, 2),
+                 "flop_count": "library count: a complex multiply-add counts 2, real_tflops = 4 x selinv_tflops"}
     print(bench.json_line({
         "metric": "selinv_ms", "value": round(med(t_si) * 1e3, 2), "unit": "ms", "higher_is_better": False,
         "workload": name, "values": "non-symmetric, diagonally dominant (scripts/bench_solve_trans.py)", "n": n,
@@ -107,7 +125,7 @@ def run_one(kind, g, rp, ci, v, sym, args, gpu):
         "diag_by_solves_s": round(med(ts) * n / 8, 1), "solve_8rhs_ms": round(med(ts) * 1e3, 2),
         "diag_check_max_rel_err": worst, "gpu": gpu,
         "how": "factor: stats.t_factor_s; selinv: out[0] (host clock around the call); inv_diag / inv_entries: host clock "
-               "around the call; diag by solves: n / 8 x the median of timed 8-right-hand-side unit-vector solves"}))
+               "around the call; diag by solves: n / 8 x the median of timed 8-right-hand-side unit-vector solves", **extra}))
 
 
 def main():
@@ -121,7 +139,7 @@ def main():
         else:
             for g in ((args.fem_grid,) if args.fem_grid > 0 else FEM_GRIDS):
                 rp, ci, v, sym = symbolic(kind, g)
-                if args.fem_grid > 0 or fits_twice(sym)[0]:
+                if args.fem_grid > 0 or fits_twice(sym, args.dtype == "c128")[0]:
                     break
         run_one(kind, g, rp, ci, v, sym, args, gpu)
 

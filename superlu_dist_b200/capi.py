@@ -118,9 +118,12 @@ def lib():
         getattr(L, f).argtypes = [C.c_void_p, C.c_char, C.c_double, C.POINTER(C.c_double)]
     for f in ("slu_b200_batch_gscon", "slu_b200_z_batch_gscon"):
         getattr(L, f).argtypes = [C.c_void_p, C.c_char, C.c_void_p, C.c_void_p]
-    L.slu_b200_selinv.argtypes = [C.c_void_p, C.c_void_p]
-    L.slu_b200_selinv_get.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.slu_b200_logdet.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double)]
+    for f in ("slu_b200_selinv", "slu_b200_z_selinv"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_void_p]
+    for f in ("slu_b200_selinv_get", "slu_b200_z_selinv_get"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    for f in ("slu_b200_logdet", "slu_b200_z_logdet"):
+        getattr(L, f).argtypes = [C.c_void_p, C.POINTER(C.c_double), C.c_void_p]
     _lib = L
     return L
 
@@ -332,28 +335,23 @@ class Handle:
         _check(_fn("gscon", self.z_)(self.h, _norm_byte(norm), float(anorm), C.byref(out)))
         return out.value
 
-    def _real_only(self, what):
-        if self.z_:
-            raise TypeError(f"{what} is implemented for double problems only")
-
     def selinv(self):
-        """Selected inversion on the resident factors (slu_b200_selinv): H = F^-T on the pattern of L + U, kept in HBM for
-        inv_entries / inv_diag.  -> (seconds, flops, kernel launches, HBM bytes held)"""
-        self._real_only("selinv")
+        """Selected inversion on the resident factors (slu_b200_selinv / slu_b200_z_selinv): H = F^-T on the pattern of
+        L + U (a plain transpose in complex too), kept in HBM for inv_entries / inv_diag.  -> (seconds, flops, kernel
+        launches, HBM bytes held); in complex the flops count a complex multiply-add as 2, as ops_fact does."""
         out = (C.c_double * 4)()
-        _check(lib().slu_b200_selinv(self.h, out))
+        _check(_fn("selinv", self.z_)(self.h, out))
         return tuple(out)
 
     def inv_entries(self, rowptr, colind, perm):
         """(A^-1)(i, colind[p]) for every entry p of row i of a CSR pattern (slu_b200_selinv_get), perm[old] = new as in
-        fill_csr; every entry must have a slot in L + U.  -> float64 array (nnz,)"""
-        self._real_only("inv_entries")
+        fill_csr; every entry must have a slot in L + U.  -> float64 (complex128 for a complex problem) array (nnz,)"""
         rp = np.ascontiguousarray(rowptr, np.int32)
         ci = np.ascontiguousarray(colind, np.int32)
         pm = np.ascontiguousarray(perm, np.int32)
-        out = np.empty(len(ci), np.float64)
-        _check(lib().slu_b200_selinv_get(self.h, len(rp) - 1, rp.ctypes.data_as(C.c_void_p), ci.ctypes.data_as(C.c_void_p),
-                                         pm.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p)))
+        out = np.empty(len(ci), self._dtype())
+        _check(_fn("selinv_get", self.z_)(self.h, len(rp) - 1, rp.ctypes.data_as(C.c_void_p), ci.ctypes.data_as(C.c_void_p),
+                                          pm.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p)))
         return out
 
     def inv_diag(self, perm=None):
@@ -363,11 +361,11 @@ class Handle:
         return self.inv_entries(np.arange(n + 1, dtype=np.int32), np.arange(n, dtype=np.int32), pm)
 
     def logdet(self):
-        """(sign, log |det A|) from the resident factors (slu_b200_logdet), as numpy.linalg.slogdet"""
-        self._real_only("logdet")
-        la, sg = C.c_double(0.0), C.c_double(0.0)
-        _check(lib().slu_b200_logdet(self.h, C.byref(la), C.byref(sg)))
-        return sg.value, la.value
+        """(sign, log |det A|) from the resident factors (slu_b200_logdet / slu_b200_z_logdet), as numpy.linalg.slogdet:
+        the sign is a float +-1, or for a complex problem a complex128 of modulus 1"""
+        la, sg = C.c_double(0.0), np.zeros(2 if self.z_ else 1, np.float64)
+        _check(_fn("logdet", self.z_)(self.h, C.byref(la), sg.ctypes.data_as(C.c_void_p)))
+        return (complex(sg[0], sg[1]) if self.z_ else float(sg[0])), la.value
 
     def _dtype(self):
         return np.complex128 if self.z_ else np.float64

@@ -46,6 +46,9 @@
 #define slu_b200_batch_download slu_b200_z_batch_download
 #define slu_b200_gscon slu_b200_z_gscon
 #define slu_b200_batch_gscon slu_b200_z_batch_gscon
+#define slu_b200_selinv slu_b200_z_selinv
+#define slu_b200_selinv_get slu_b200_z_selinv_get
+#define slu_b200_logdet slu_b200_z_logdet
 #define SLU_API "slu_b200_z_"     // name prefix of the exported calls, for error messages
 #else
 #define SLU_API "slu_b200_"
@@ -296,7 +299,7 @@ struct slu_b200_handle_s {
     DevBuf<CondState> d_cstate;
     DevBuf<CondPart> d_cpart;
     DevBuf<int> d_ccount;
-    // selected inversion (slu_b200_selinv, double only): H = F^-T in a second arena of the factors' layout, its level plan,
+    // selected inversion (slu_b200_selinv / slu_b200_z_selinv): H = F^-T in a second arena of the factors' layout, its level plan,
     // and whether it describes the current factors (a later upload, fill_csr or factor clears it)
     DevBuf<val_t> d_hinv;
     DevBuf<int64_t> d_si_pool;
@@ -1900,27 +1903,30 @@ int slu_b200_k_rerun_schur(slu_b200_handle_t H, int level, int reps, float *ms)
     *ms = t / reps;
     return 0;
 }
+#endif  // !SLU_COMPLEX
 
-// ---- selected inversion and log-determinant on the resident factors (double only) ----------------------------------
-// slu_selinv.cu holds the kernels and the recurrences.  The sweep walks the level plan top-down (the backward solve's
-// order): every Schur destination of a supernode lies in a supernode of a later level, so its gathered block M = H(R, C)
-// is final.  Per level 7 launches: the destination maps and the 16x16 diagonal-block inverses are rebuilt in the
-// factorization's per-level workspaces, then three products and two triangular solves; a level with no Schur update (the
-// root) has no maps to build and makes 6.
+// ---- selected inversion and log-determinant on the resident factors ------------------------------------------------
+// slu_selinv.cu holds the kernels and the recurrences (slu_selinv_z.cu the doublecomplex build).  The sweep walks the
+// level plan top-down (the backward solve's order): every Schur destination of a supernode lies in a supernode of a later
+// level, so its gathered block M = H(R, C) is final.  Per level 7 launches: the destination maps and the 16x16
+// diagonal-block inverses are rebuilt in the factorization's per-level workspaces, then three products and two
+// triangular solves; a level with no Schur update (the root) has no maps to build and makes 6.
 static int selinv_refuse(const slu_b200_handle_s *H, const char *fn)
 {
     if (refuse_batched(H, fn)) return -1;
     if (H->opt.world_size > 1 || H->max_lvl > 1 || H->P2 > 1) return fail("%s handles 1 x 1 x 1 grids (world_size 1)", fn);
-    if (!H->factored) return fail("%s needs a successful slu_b200_factor (info = 0) on this handle first", fn);
+    if (!H->factored) return fail("%s needs a successful " SLU_API "factor (info = 0) on this handle first", fn);
     return 0;
 }
 
-// CTA prefixes of the selinv kernels, from the level plan: built once per handle
+// CTA prefixes of the selinv kernels, from the level plan: built once per handle.  Product tiles are SELINV_TILE_M rows
+// by SELINV_TILE_N val_t columns (64 x 64 real outputs: 32 complex columns in doublecomplex).
 static int selinv_plan(slu_b200_handle_s *H)
 {
     std::vector<int64_t> pool;
     H->si_levels.assign(H->levels.size(), SelinvLevel{});
-    auto tiles = [](int64_t a) { return (a + SELINV_TILE - 1) / SELINV_TILE; };
+    auto tr = [](int64_t a) { return (a + SELINV_TILE_M - 1) / SELINV_TILE_M; };
+    auto tc = [](int64_t a) { return (a + SELINV_TILE_N - 1) / SELINV_TILE_N; };
     for (size_t li = 0; li < H->levels.size(); ++li) {
         const LevelPlan &L = H->levels[li];
         SelinvLevel &S = H->si_levels[li];
@@ -1928,14 +1934,14 @@ static int selinv_plan(slu_b200_handle_s *H)
         for (auto &v : p) v.assign(1, 0);
         for (int t = 0; t < L.count; ++t) {
             const NodeDesc &nd = H->nodes[H->h_pool_i32[L.nodes_off + t]];
-            p[0].push_back(p[0].back() + tiles(nd.m) * tiles(nd.ns));
-            p[1].push_back(p[1].back() + tiles(nd.ns) * tiles(nd.ncols));
-            p[2].push_back(p[2].back() + tiles(nd.ns) * tiles(nd.ns));
+            p[0].push_back(p[0].back() + tr(nd.m) * tc(nd.ns));
+            p[1].push_back(p[1].back() + tr(nd.ns) * tc(nd.ncols));
+            p[2].push_back(p[2].back() + tr(nd.ns) * tc(nd.ns));
             p[3].push_back(p[3].back() + (nd.nsupr + SELINV_VECS - 1) / SELINV_VECS);
             p[4].push_back(p[4].back() + (nd.ns + nd.ncols + SELINV_VECS - 1) / SELINV_VECS);
         }
         for (int q = 0; q < 5; ++q) {
-            if (p[q].back() > 2147483647LL) return fail("slu_b200_selinv: a level needs more than 2^31 CTAs in one launch");
+            if (p[q].back() > 2147483647LL) return fail(SLU_API "selinv: a level needs more than 2^31 CTAs in one launch");
             int64_t &off = q < 3 ? S.gemm_prefix[q] : S.trsm_prefix[q - 3];
             int64_t &ctas = q < 3 ? S.gemm_ctas[q] : S.trsm_ctas[q - 3];
             off = (int64_t)pool.size();
@@ -1949,20 +1955,20 @@ static int selinv_plan(slu_b200_handle_s *H)
 int slu_b200_selinv(slu_b200_handle_t H, double out[4])
 {
     if (!H) return fail("null handle");
-    if (selinv_refuse(H, "slu_b200_selinv")) return -1;
+    if (selinv_refuse(H, SLU_API "selinv")) return -1;
     H->si_ready = false;
     if (H->si_levels.empty() && selinv_plan(H)) return -1;
     if (!H->d_hinv.p && H->d_hinv.alloc((size_t)H->member_len)) {
         cudaGetLastError();
         std::string why = g_err;
         H->d_hinv.release();
-        return fail("slu_b200_selinv: the inverse needs a second arena of %.2f GB beside the factors, which does not fit (%s); "
-                    "the factors are unchanged", 8e-9 * H->member_len, why.c_str());
+        return fail(SLU_API "selinv: the inverse needs a second arena of %.2f GB beside the factors, which does not fit (%s); "
+                    "the factors are unchanged", 1e-9 * sizeof(val_t) * H->member_len, why.c_str());
     }
     cudaStream_t s = H->stream;
     const DeviceLU &d = H->dev;
     const int64_t *p64 = H->d_pool_i64.p, *sp = H->d_si_pool.p;
-    double *hv = H->d_hinv.p;
+    val_t *hv = H->d_hinv.p;
     double flops = 0;
     int launches = 0;
     const double t0 = now_s();
@@ -1976,6 +1982,8 @@ int slu_b200_selinv(slu_b200_handle_t H, double out[4])
         for (int q = 0; q < 3; ++q) launches += launch_selinv_gemm(d, Batch{nodes, sp + S.gemm_prefix[q], L.count}, S.gemm_ctas[q], q, hv, s);
         for (int q = 0; q < 2; ++q)
             launches += launch_selinv_trsm(d, Batch{nodes, sp + S.trsm_prefix[q], L.count}, S.trsm_ctas[q], q, H->d_inv.p, hv, s);
+        // 2 flops per multiply-add in both precisions (a complex multiply-add counts once, as ops_fact counts the complex
+        // Schur update): 4x this in real flops in doublecomplex
         for (int t = 0; t < L.count; ++t) {
             const NodeDesc &nd = H->nodes[H->h_pool_i32[L.nodes_off + t]];
             const double m = nd.m, n = nd.ncols, ns = nd.ns;
@@ -1986,7 +1994,7 @@ int slu_b200_selinv(slu_b200_handle_t H, double out[4])
     CU(cudaMemcpyAsync(&bad, H->d_flags.p + 1, sizeof(int), cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     CU(cudaGetLastError());
-    if (bad) return fail("slu_b200_selinv: %d Schur-update destinations were not found in the L/U structure", bad);
+    if (bad) return fail(SLU_API "selinv: %d Schur-update destinations were not found in the L/U structure", bad);
     H->si_ready = true;
     if (out) {
         out[0] = now_s() - t0;
@@ -2000,13 +2008,13 @@ int slu_b200_selinv(slu_b200_handle_t H, double out[4])
 int slu_b200_selinv_get(slu_b200_handle_t H, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm, double *out)
 {
     if (!H || !rowptr || !colind || !perm || !out) return fail("null argument");
-    if (selinv_refuse(H, "slu_b200_selinv_get")) return -1;
-    if (!H->si_ready) return fail("slu_b200_selinv_get needs slu_b200_selinv on the current factors first (a later upload, fill_csr or factor invalidates it)");
-    if (n != H->n) return fail("slu_b200_selinv_get: matrix order %d does not match the handle's %d", n, H->n);
+    if (selinv_refuse(H, SLU_API "selinv_get")) return -1;
+    if (!H->si_ready) return fail(SLU_API "selinv_get needs " SLU_API "selinv on the current factors first (a later upload, fill_csr or factor invalidates it)");
+    if (n != H->n) return fail(SLU_API "selinv_get: matrix order %d does not match the handle's %d", n, H->n);
     const int64_t nnz = rowptr[n];
-    if (rowptr[0] != 0 || nnz < 0) return fail("slu_b200_selinv_get: bad rowptr");
+    if (rowptr[0] != 0 || nnz < 0) return fail(SLU_API "selinv_get: bad rowptr");
     DevBuf<int32_t> drp, dci, dperm;
-    DevBuf<double> dout;
+    DevBuf<val_t> dout;
     if (drp.alloc((size_t)n + 1) || dci.alloc((size_t)nnz) || dperm.alloc((size_t)n) || dout.alloc((size_t)nnz)) return -1;
     cudaStream_t s = H->stream;
     CU(cudaMemcpyAsync(drp.p, rowptr, ((size_t)n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, s));
@@ -2015,34 +2023,33 @@ int slu_b200_selinv_get(slu_b200_handle_t H, int n, const int32_t *rowptr, const
     CU(cudaMemsetAsync(H->d_flags.p + 1, 0, sizeof(int), s));
     launch_selinv_get(H->dev, H->d_hinv.p, n, drp.p, dci.p, dperm.p, dout.p, H->d_flags.p + 1, s);
     int bad = 0;
-    CU(cudaMemcpyAsync(out, dout.p, (size_t)nnz * sizeof(double), cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(out, dout.p, (size_t)nnz * sizeof(val_t), cudaMemcpyDeviceToHost, s));
     CU(cudaMemcpyAsync(&bad, H->d_flags.p + 1, sizeof(int), cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     CU(cudaGetLastError());
-    if (bad) return fail("slu_b200_selinv_get: %d entries have no slot in the L/U structure (A^-1 is known on the pattern of L+U only)", bad);
+    if (bad) return fail(SLU_API "selinv_get: %d entries have no slot in the L/U structure (A^-1 is known on the pattern of L+U only)", bad);
     return 0;
 }
 
 int slu_b200_logdet(slu_b200_handle_t H, double *logabs, double *sign)
 {
     if (!H || !logabs || !sign) return fail("null argument");
-    if (selinv_refuse(H, "slu_b200_logdet")) return -1;
+    if (selinv_refuse(H, SLU_API "logdet")) return -1;
     const int count = (int)H->znodes[0].size();
     const int nparts = (count + SELINV_VECS - 1) / SELINV_VECS;
     DevBuf<double> part, res;
-    DevBuf<int> neg;
-    if (part.alloc((size_t)nparts) || neg.alloc((size_t)nparts) || res.alloc(2)) return -1;
+    DevBuf<phase_t> ph;
+    if (part.alloc((size_t)nparts) || ph.alloc((size_t)nparts) || res.alloc(1 + VAL_DOUBLES)) return -1;
     cudaStream_t s = H->stream;
-    launch_selinv_logdet(H->dev, H->d_pool_i32.p + H->z_nodes_off[0], count, part.p, neg.p, res.p, s);
-    double r[2] = {0.0, 1.0};
+    launch_selinv_logdet(H->dev, H->d_pool_i32.p + H->z_nodes_off[0], count, part.p, ph.p, res.p, s);
+    double r[1 + VAL_DOUBLES] = {0.0, 1.0};   // log |det|, then the sign: +-1, or exp(i theta) as (re, im)
     CU(cudaMemcpyAsync(r, res.p, sizeof r, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     CU(cudaGetLastError());
     *logabs = r[0];
-    *sign = r[1];
+    for (int c = 0; c < VAL_DOUBLES; ++c) sign[c] = r[1 + c];
     return 0;
 }
-#endif  // !SLU_COMPLEX
 
 // ---- batched handles: many matrices of one sparsity pattern (pdgssvx3d_csc_batch, SRC/double/pdgssvx3d_csc_batch.c:81,
 // and its doublecomplex twin pzgssvx3d_csc_batch, SRC/complex16/pzgssvx3d_csc_batch.c:80; dsparseTreeFactorBatchGPU,

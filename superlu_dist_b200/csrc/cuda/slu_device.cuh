@@ -235,24 +235,33 @@ int launch_oz_schur(const DeviceLU &d, const Batch &b, int64_t ctas, int mode, i
 // slu_ozaki.cu: C -= A*B through int8 slices on wgmma (variants 110..149: slices, stages, cluster)
 int launch_gemm_sub_ozaki(int m, int n, int k, const double *a, int lda, const double *b, int ldb, double *c, int ldc,
                           int variant, cudaStream_t s);
+#endif
 
-// slu_selinv.cu: selected inversion H = F^-T on the stored pattern of L + U into a second arena hv of the factors' layout
-// (slu_b200_selinv).  Per level, top-down, after launch_schur_setup and launch_diag_inv of the level: the three products
-// (mode 0: H(R,K) = -M U_KC^T, tiles of m x ns; 1: H(K,C) = -L_RK^T M, ns x ncols; 2: H(K,K) = I - L_RK^T H(R,K), ns x ns;
-// SELINV_TILE x SELINV_TILE tiles), then the triangular solves (cols 0: every row of L panel K of hv times U_KK^-T;
+// slu_selinv.cu (double) / slu_selinv_z.cu (doublecomplex): selected inversion H = F^-T on the stored pattern of L + U into
+// a second arena hv of the factors' layout (slu_b200_selinv).  Per level, top-down, after launch_schur_setup and
+// launch_diag_inv of the level: the three products (mode 0: H(R,K) = -M U_KC^T, tiles of m x ns; 1: H(K,C) = -L_RK^T M,
+// ns x ncols; 2: H(K,K) = I - L_RK^T H(R,K), ns x ns; SELINV_TILE_M rows x SELINV_TILE_N val_t columns per tile, 64 x 64
+// real outputs in both precisions), then the triangular solves (cols 0: every row of L panel K of hv times U_KK^-T;
 // 1: L_KK^-T times the ns + ncols columns of H(K,K) and H(K,C); SELINV_VECS vectors per CTA).  Each launcher makes one
 // launch per call, even for an empty batch.
-constexpr int SELINV_TILE = 64;
-constexpr int SELINV_VECS = 128;
-int launch_selinv_gemm(const DeviceLU &d, const Batch &b, int64_t ctas, int mode, double *hv, cudaStream_t s);
-int launch_selinv_trsm(const DeviceLU &d, const Batch &b, int64_t ctas, int cols, const double *dinv, double *hv, cudaStream_t s);
-// log |det| into out[0] and the sign into out[1], over the listed supernodes' pivots; part / pneg: ceil(count / SELINV_VECS)
-// entries.  2 launches.
-int launch_selinv_logdet(const DeviceLU &d, const int32_t *nodes, int count, double *part, int *pneg, double *out, cudaStream_t s);
-// out[p] = H(perm[colind[p]], perm[i]) for the entries p of row i; *err counts entries without a slot (out = NaN there)
-int launch_selinv_get(const DeviceLU &d, const double *hv, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm,
-                      double *out, int *err, cudaStream_t s);
+constexpr int SELINV_TILE_M = 64;
+#ifdef SLU_COMPLEX
+constexpr int SELINV_TILE_N = 32;   // complex columns: 64 real ones
+typedef double phase_t;             // log-determinant phase: the sum of the pivots' arguments
+#else
+constexpr int SELINV_TILE_N = 64;
+typedef int phase_t;                // log-determinant phase: the number of negative pivots
 #endif
+constexpr int SELINV_VECS = 128;
+int launch_selinv_gemm(const DeviceLU &d, const Batch &b, int64_t ctas, int mode, val_t *hv, cudaStream_t s);
+int launch_selinv_trsm(const DeviceLU &d, const Batch &b, int64_t ctas, int cols, const val_t *dinv, val_t *hv, cudaStream_t s);
+// log |det| into out[0] and the phase after it, over the listed supernodes' pivots: double out[1] = the sign (+1 / -1),
+// doublecomplex out[1], out[2] = exp(i theta), theta = sum of arg u_ii reduced modulo 2 pi; part / pph:
+// ceil(count / SELINV_VECS) entries.  2 launches.
+int launch_selinv_logdet(const DeviceLU &d, const int32_t *nodes, int count, double *part, phase_t *pph, double *out, cudaStream_t s);
+// out[p] = H(perm[colind[p]], perm[i]) for the entries p of row i; *err counts entries without a slot (out = NaN there)
+int launch_selinv_get(const DeviceLU &d, const val_t *hv, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm,
+                      val_t *out, int *err, cudaStream_t s);
 
 #ifdef SLU_COMPLEX
 constexpr int SCHUR_BM_BIG = 128, SCHUR_BN_BIG = 32, SCHUR_BM_SMALL = 32, SCHUR_BN_SMALL = 16;

@@ -55,6 +55,10 @@ __device__ __forceinline__ val_t vrecip(val_t a) { return zrecip(a); }
 // conj(a) for CONJ = true (the conjugate-transposed solve reads every factor entry conjugated), a otherwise
 template <bool CONJ>
 __device__ __forceinline__ val_t vconj(val_t a) { return CONJ ? zmake(a.x, -a.y) : a; }
+__device__ __forceinline__ val_t vnan() { return zmake(NAN, NAN); }
+// acc + a * b and acc - a * b as values (one fused multiply-add each in double)
+__device__ __forceinline__ val_t vfma(val_t a, val_t b, val_t acc) { zaddmul(acc, a, b); return acc; }
+__device__ __forceinline__ val_t vfnma(val_t a, val_t b, val_t acc) { zsubmul(acc, a, b); return acc; }
 #else
 __device__ __forceinline__ val_t vzero() { return 0.0; }
 __device__ __forceinline__ val_t vadd(val_t a, val_t b) { return a + b; }
@@ -68,6 +72,9 @@ __device__ __forceinline__ val_t vmul(val_t a, val_t b) { return a * b; }
 __device__ __forceinline__ val_t vrecip(val_t a) { return 1.0 / a; }
 template <bool CONJ>
 __device__ __forceinline__ val_t vconj(val_t a) { return a; }   // a real entry is its own conjugate
+__device__ __forceinline__ val_t vnan() { return NAN; }
+__device__ __forceinline__ val_t vfma(val_t a, val_t b, val_t acc) { return fma(a, b, acc); }
+__device__ __forceinline__ val_t vfnma(val_t a, val_t b, val_t acc) { return fma(-a, b, acc); }
 #endif
 
 }  // namespace SLU_NS
