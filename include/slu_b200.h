@@ -154,7 +154,9 @@ int slu_b200_download(slu_b200_handle_t h);
  * slu_b200_upload of the caller's Lnzval/Unzval arrays, scatter the matrix itself into the panels.  A: n x n host CSR
  * (int32 indices, no duplicate entries); perm[old] = new is the final permutation of the factored matrix
  * (P (A) P^T, rows and columns alike).  12 bytes per nonzero cross PCIe instead of 8 bytes per factor entry; the value
- * arrays of the view may then be NULL-backed (never read) if the caller also skips slu_b200_download.  1 x 1 x Pz. */
+ * arrays of the view may then be NULL-backed (never read) if the caller also skips slu_b200_download.  1 x 1 x Pz.
+ * An entry of a U column above that column's skyline start (Ufstnz) has no slot, as an entry outside the structure:
+ * the call fails with the count of such entries rather than writing it into the zero padding above the segment. */
 int slu_b200_fill_csr(slu_b200_handle_t h, int n, const int32_t *rowptr, const int32_t *colind, const double *val,
                       const int32_t *perm);
 /* Solve L U x = b with the factors still resident in HBM (after a successful slu_b200_factor / _factor_host on this

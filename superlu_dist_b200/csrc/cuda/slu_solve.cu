@@ -340,7 +340,8 @@ __global__ void fill_csr_kernel(LU dd, int n, const int32_t *__restrict__ rowptr
             const NodeDesc *nd = d.nodes + kr;
             const int32_t *uc = d.ucols + nd->ucol;
             const int q = lower_bound_i32(uc, nd->ncols, pj);
-            if (q >= nd->ncols || uc[q] != pj) { atomicAdd(err, 1); continue; }
+            // above the column's skyline start is dense-packed padding, not a slot
+            if (q >= nd->ncols || uc[q] != pj || pi < d.ufst[nd->ucol + q]) { atomicAdd(err, 1); continue; }
             d.val[nd->uval + (int64_t)q * nd->ns + (pi - nd->fsupc)] = aval[p];
         }
     }

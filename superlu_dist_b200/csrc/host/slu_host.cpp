@@ -534,18 +534,26 @@ extern "C" void sluh_fill_values(int n, const int32_t *rowptr, const int32_t *co
 #pragma omp parallel for schedule(dynamic, 256)
     for (int s = 0; s < nsupers; ++s)
         for (int c = xsup[s]; c < xsup[s + 1]; ++c) supno[c] = s;
-    // flat row lists of L panels, flat (column, segment offset) lists of U panels
+    // flat row lists of L panels, flat (column, first row, segment offset) lists of U panels; a U panel lists only the
+    // columns with a non-empty skyline segment (fstnz < klst), as the device analysis does
     std::vector<int64_t> lro((size_t)nsupers + 1, 0), uco((size_t)nsupers + 1, 0);
     for (int s = 0; s < nsupers; ++s) {
         lro[s + 1] = lro[s] + lidx[lidx_off[s] + 1];
         int64_t nc = 0;
         if (uidx_off[s + 1] > uidx_off[s]) {
-            int ns = xsup[s + 1] - xsup[s];
-            nc = uidx[uidx_off[s] + 1] / ns;  // full segments in our own export
+            const int32_t *ui = uidx + uidx_off[s];
+            int klst = xsup[s + 1];
+            int64_t u = BR_HEADER;
+            for (int b = 0; b < ui[0]; ++b) {
+                int jb = ui[u], jns = xsup[jb + 1] - xsup[jb];
+                for (int c = 0; c < jns; ++c) nc += ui[u + UB_DESCRIPTOR + c] < klst;
+                u += UB_DESCRIPTOR + jns;
+            }
         }
         uco[s + 1] = uco[s] + nc;
     }
-    std::vector<int32_t> lrows((size_t)lro[nsupers]), ucols((size_t)uco[nsupers]), useg((size_t)uco[nsupers]);
+    std::vector<int32_t> lrows((size_t)lro[nsupers]), ucols((size_t)uco[nsupers]), ufst((size_t)uco[nsupers]),
+        useg((size_t)uco[nsupers]);
 #pragma omp parallel for schedule(dynamic, 64)
     for (int s = 0; s < nsupers; ++s) {
         const int32_t *li = lidx + lidx_off[s];
@@ -564,7 +572,7 @@ extern "C" void sluh_fill_values(int n, const int32_t *rowptr, const int32_t *co
             int jb = ui[u], jf = xsup[jb], jns = xsup[jb + 1] - jf;
             for (int c = 0; c < jns; ++c) {
                 int fst = ui[u + UB_DESCRIPTOR + c];
-                if (fst < klst) { ucols[(size_t)oc] = jf + c; useg[(size_t)oc] = seg - (fst - xsup[s]); ++oc; seg += klst - fst; }
+                if (fst < klst) { ucols[(size_t)oc] = jf + c; ufst[(size_t)oc] = fst; useg[(size_t)oc] = seg - (fst - xsup[s]); ++oc; seg += klst - fst; }
             }
             u += UB_DESCRIPTOR + jns;
         }
@@ -589,7 +597,11 @@ extern "C" void sluh_fill_values(int n, const int32_t *rowptr, const int32_t *co
             } else {
                 const int32_t *b = ucols.data() + uco[ib], *e = ucols.data() + uco[ib + 1];
                 const int32_t *it = std::lower_bound(b, e, c);
-                if (it == e || *it != c) { fprintf(stderr, "sluh_fill_values: (%d,%d) not in U structure\n", r, c); abort(); }
+                // an entry above its column's skyline start has no slot either
+                if (it == e || *it != c || r < ufst[(size_t)(uco[ib] + (it - b))]) {
+                    fprintf(stderr, "sluh_fill_values: (%d,%d) not in U structure\n", r, c);
+                    abort();
+                }
                 uval[uval_off[ib] + useg[(size_t)(uco[ib] + (it - b))] + (r - xsup[ib])] = val[q];
             }
         }

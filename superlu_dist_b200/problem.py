@@ -133,6 +133,102 @@ class LUProblem:
         p.load_values(lay, pre)
         return p
 
+    def prune_u(self, rowptr, colind):
+        """Cut every U block row down to the exact skyline of the unsymmetric F = P A P^T (A: the CSR pattern of the
+        matrix this problem was built from, perm[old] = new), as the reference stores unsymmetric patterns: per column j
+        of U panel k only the segment [fstnz, klst), columns with an empty segment and blocks without columns dropped.
+        L keeps the structure of P (A + A^T) P^T, a valid superset.  Call before any layer exists.
+
+        fstnz_k(j) is the first row of k with F(i, j) != 0, or the first row of k that an earlier supernode s updates
+        in column j: s's pruned U panel has column j and s's L panel lists rows of k.  The diagonal block of k is dense,
+        so below fstnz every row of the column may be non-zero.  The analytic operation counts no longer apply."""
+        if self.layers:
+            raise ValueError("prune_u changes the U layout: call it before add_layer")
+        n, ns_all = self.n, self.nsupers
+        xsup = np.asarray(self.xsup, np.int64)
+        supno = np.repeat(np.arange(ns_all), np.diff(xsup))
+        # the U column list of every panel (keys k * n + j, ascending) and each block's extent in it
+        keys, first = [], np.zeros(ns_all + 1, np.int64)
+        blocks = [None] * ns_all
+        for k in range(ns_all):
+            cols = []
+            if self.uidx_off[k + 1] > self.uidx_off[k]:
+                idx = self.uidx[self.uidx_off[k]:self.uidx_off[k + 1]]
+                klst, u, blk = int(xsup[k + 1]), BR_HEADER, []
+                for _ in range(int(idx[0])):
+                    jb = int(idx[u])
+                    jf, jns = int(xsup[jb]), int(xsup[jb + 1] - xsup[jb])
+                    c = np.nonzero(idx[u + UB_DESCRIPTOR:u + UB_DESCRIPTOR + jns] < klst)[0] + jf
+                    blk.append(jb)
+                    cols.append(c)
+                    u += UB_DESCRIPTOR + jns
+                blocks[k] = blk
+            cols = np.concatenate(cols) if cols else np.zeros(0, np.int64)
+            keys.append(k * n + cols)
+            first[k + 1] = first[k] + len(cols)
+        keys = np.concatenate(keys) if keys else np.zeros(0, np.int64)
+        fst = np.repeat(xsup[1:], np.diff(first))              # klst: empty
+
+        def lookup(k, cols):
+            q = np.searchsorted(keys, k * n + cols)
+            if np.any(q >= len(keys)) or np.any(keys[np.minimum(q, len(keys) - 1)] != k * n + cols):
+                raise ValueError("F has an entry outside the U structure of P (A + A^T) P^T")
+            return q
+        # entries of F above the diagonal blocks
+        rowptr, colind = np.asarray(rowptr), np.asarray(colind)
+        perm = np.asarray(self.perm, np.int64)
+        fi = perm[np.repeat(np.arange(n), np.diff(rowptr))]
+        fj = perm[colind]
+        up = supno[fi] < supno[fj]
+        fi, fj = fi[up], fj[up]
+        np.minimum.at(fst, lookup(supno[fi], fj), fi)
+        # updates of earlier supernodes, in ascending order (fstnz of s is final once every s' < s has been applied)
+        for s in range(ns_all):
+            if first[s + 1] == first[s]:
+                continue
+            live = fst[first[s]:first[s + 1]] < xsup[s + 1]
+            cols_s = keys[first[s]:first[s + 1]][live] - s * n
+            if not len(cols_s):
+                continue
+            idx = self.lidx[self.lidx_off[s]:self.lidx_off[s + 1]]
+            w = BC_HEADER
+            for b in range(int(idx[0])):
+                ib, nb = int(idx[w]), int(idx[w + 1])
+                if b:
+                    tgt = cols_s[cols_s >= xsup[ib + 1]]
+                    if len(tgt):
+                        q = lookup(ib, tgt)
+                        fst[q] = np.minimum(fst[q], int(idx[w + LB_DESCRIPTOR]))
+                w += LB_DESCRIPTOR + nb
+        # the new U index arrays
+        out, off, vlen = [], [0], np.zeros(ns_all, np.int64)
+        for k in range(ns_all):
+            if blocks[k] is None:
+                off.append(off[-1])
+                continue
+            klst = int(xsup[k + 1])
+            colfst = dict(zip((keys[first[k]:first[k + 1]] - k * n).tolist(), fst[first[k]:first[k + 1]].tolist()))
+            body, nblk, nnz = [], 0, 0
+            for jb in blocks[k]:
+                jf, jns = int(xsup[jb]), int(xsup[jb + 1] - xsup[jb])
+                f = [colfst.get(jf + c, klst) for c in range(jns)]
+                bnnz = sum(klst - x for x in f)
+                if bnnz:
+                    body += [jb, bnnz] + f
+                    nblk += 1
+                    nnz += bnnz
+            if nblk:
+                out.append(np.array([nblk, nnz, BR_HEADER + len(body)] + body, np.int32))
+                off.append(off[-1] + BR_HEADER + len(body))
+                vlen[k] = nnz
+            else:
+                off.append(off[-1])
+        self.uidx = np.concatenate(out) if out else np.zeros(1, np.int32)
+        self.uidx_off = np.array(off, np.int64)
+        self.uval_len = vlen
+        self.ops_fact = self.ops_schur = None
+        return self
+
     def load_values(self, layer, rec):
         for k in range(self.nsupers):
             a = rec.get(f"Lval:{k}")
