@@ -87,9 +87,7 @@ typedef struct {
     int32_t world_size;           /* ranks in the 3D grid (1: no communication)              */
     int32_t world_rank;           /* my rank: mydep*(nprow*npcol) + myrow*npcol + mycol      */
     unsigned char nccl_id[128];   /* ncclUniqueId from slu_b200_nccl_unique_id on rank 0     */
-    int32_t schur_variant;        /* 0 (default) = 4: 128x64 DMMA tiles, 2 CTAs/SM, running-pointer loader;
-                                     5: the same with BK=32; 6: the round-1 general loader; 1: 128x128 tiles,
-                                     1 CTA/SM; 3: general loader, BK=32 for wide supernodes */
+    int32_t schur_variant;        /* retired, must be 0: create and plan refuse any other value     */
     int32_t reserved[7];          /* [0] no look-ahead, [1] reference-style ancestors, [2] pdgstrf3d_b200 */
                                   /* uses slu_b200_factor_host (overlapped transfers), [3] level-by-  */
                                   /* level arena so that factor_host also overlaps the upload,        */
@@ -258,8 +256,7 @@ int slu_b200_k_rerun_schur(slu_b200_handle_t h, int level, int reps, float *ms);
  * (stats.lu_device_bytes = batch x one member), diag-inverse workspace and info flag.  A batched factorization makes
  * exactly as many kernel launches as one unbatched factorization, each over batch x the CTAs (gridDim.y = member).
  * Double precision here and doublecomplex through the slu_b200_z_batch_* twins below; 1 x 1 x 1 grid, FP64 DMMA
- * kernels only (the int8 path, schur_variant != 0 and the opt-in SLU_B200_DIAG_V3 / SLU_B200_TRSM_RL kernels are not
- * used; stats.reserved[1] = 0).
+ * kernels only (the int8 path is not used; stats.reserved[1] = 0).
  * A batched handle takes only these calls plus slu_b200_get_stats and slu_b200_destroy; every other call on it fails,
  * and these fail on an unbatched handle.  Stats describe the whole handle: ops_fact, ops_schur, nnz_l, nnz_u and
  * lu_device_bytes are batch x the per-member values, tiny_pivots is summed over the members, t_factor_s is the device

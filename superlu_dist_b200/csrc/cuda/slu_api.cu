@@ -204,7 +204,7 @@ struct EventSet {            // timing events with the same guarantee
 };
 
 struct LevelPlan {
-    int zlvl = 0, count = 0, max_ns = 0, atomic = 1;
+    int zlvl = 0, count = 0, max_ns = 0;
     int64_t nodes_off = 0;
     int64_t trsml_prefix = 0, trsml_ctas = 0, trsmu_prefix = 0, trsmu_ctas = 0, setup_prefix = 0, setup_ctas = 0;
     int64_t inv_prefix = 0, inv_ctas = 0;
@@ -254,7 +254,6 @@ struct slu_b200_handle_s {
     int tc_slices = 0, tc_min_ns = 0;     // 0 slices: int8 tensor-core path off
     int tc_max_m = 0;                     // > 0: only updates of fewer rows take the int8 path (SLU_B200_TC_MAX_M); 0: no limit
     bool tc_force_off = false, tc_alloc_failed = false;   // slice workspace did not fit: analysed again without the int8 tensor-core path
-    int tc_nonatomic = 0;                 // plain load/store scatter for destinations only one supernode of a level updates
     DevBuf<val_t> d_x, d_x2;              // triangular solve: right-hand sides / solution
     std::vector<int64_t> z_nodes_off;     // [zl] offset into d_pool_i32 of the forest's node list (solve masks)
     bool factored = false;
@@ -628,7 +627,6 @@ int analyze(slu_b200_handle_s *H)
     if (getenv("SLU_B200_TC_SLICES")) { int v = atoi(getenv("SLU_B200_TC_SLICES")); H->tc_slices = v <= 0 ? 0 : std::min(8, std::max(5, v)); }
     if (getenv("SLU_B200_TC_MIN_NS")) H->tc_min_ns = std::max(1, atoi(getenv("SLU_B200_TC_MIN_NS")));
     if (H->tc_force_off) H->tc_slices = 0;
-    H->tc_nonatomic = getenv("SLU_B200_TC_NONATOMIC") ? atoi(getenv("SLU_B200_TC_NONATOMIC")) : (OZ_NONATOMIC_DEFAULT ? 1 : 0);
 #endif
     H->levels.clear();
     for (int zl = 0; zl < max_lvl; ++zl) {
@@ -639,11 +637,11 @@ int analyze(slu_b200_handle_s *H)
         for (auto &nodes : by) {
             if (nodes.empty()) continue;
             LevelPlan L;
-            L.zlvl = zl; L.count = (int)nodes.size(); L.atomic = 1;  // RED.ADD.F64 beats a load/store read-modify-write here
+            L.zlvl = zl; L.count = (int)nodes.size();
             L.nodes_off = (int64_t)pool_i32.size();
             pool_i32.insert(pool_i32.end(), nodes.begin(), nodes.end());
-            // which destination panels are updated by MORE than one supernode of this level?  Only those need atomic
-            // scatters; an exclusive destination is updated tile-disjointly by its single source (slu_ozaki.cu).
+            // which destination panels are updated by MORE than one supernode of this level?  (LBlk / UBlk.shared; an
+            // exclusive destination is updated tile-disjointly by its single source.  Every scatter is a RED today.)
             for (int k : nodes) {
                 const NodeDesc &nd = H->nodes[k];
                 if (nd.m <= 0 || nd.ncols <= 0) continue;
@@ -687,7 +685,7 @@ int analyze(slu_b200_handle_s *H)
                     wr += nd.m; wc += nd.ncols; wl += nd.lrel_total; wu += nd.urel_total;
                     if (nd.m >= 96 && nd.ncols >= 96) {
                         bool use_tc = false;
-                        int bn = H->opt.schur_variant != 1 ? SCHUR_BN_TILE : SCHUR_BN_BIG;
+                        int bn = SCHUR_BN_TILE;
 #ifndef SLU_COMPLEX
                         use_tc = H->tc_slices > 0 && nd.ns >= H->tc_min_ns && nd.ns <= 512 && (H->tc_max_m <= 0 || nd.m < H->tc_max_m);
                         if (use_tc) bn = OZ_NT_HOST;
@@ -1378,14 +1376,14 @@ static int create_impl(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, con
 {
     if (!out || !lu || !opt) return fail("null argument");
     *out = nullptr;
+    if (opt->schur_variant != 0) return fail("options.schur_variant is retired and must be 0 (got %d)", opt->schur_variant);
     if (slu_b200_device_count() < 1) return fail("no CUDA device: libslu_b200 has no CPU fallback");
     if (device_setup(opt)) return -1;
     slu_b200_handle_s *H = new slu_b200_handle_s;
     H->view = *lu;
     H->opt = *opt;
     H->batch = batch;
-    if (batch) {             // the int8 path and the opt-in Schur variants are not batched
-        H->opt.schur_variant = 0;
+    if (batch) {             // the int8 path and the overlapped upload are not batched
         H->opt.reserved[3] = 0;
         H->opt.reserved[4] = -1;
         H->tc_force_off = true;
@@ -1575,29 +1573,24 @@ static int factor_impl(slu_b200_handle_t H, int *info, bool pipelined, bool up_p
             const int32_t *bign = H->d_pool_i32.p + L.big_nodes;
             if (lookahead || pipelined) CU(cudaEventRecord(H->ev_panel[li], s));
             if (pipelined && pipe_download_level(H, li)) return -1;
-            // non-atomic scatter of exclusive destinations (int8 tensor-core path): this level's updates must not overlap the bulk
-            // update of the level before (it targets the same ancestors); the panel work above still did
-            const int tc_na = (H->tc_nonatomic && !up_pipe) ? 1 : 0;
-            if (tc_na && lookahead && li >= first + 1 && (L.tc_count > 0 || H->levels[li - 1].tc_count > 0))
-                CU(cudaStreamWaitEvent(s, H->ev_bulk[li - 1], 0));
             if (lookahead) {
-                H->st.gpu_launches += launch_schur(d, Batch{bign, p64 + L.urg_prefix, L.big_count}, L.urg_ctas, 1, L.atomic, H->opt.schur_variant, 1, split_n, split_i, H->opt.schur_variant == 3 && L.max_ns >= 128, s);
-                H->st.gpu_launches += launch_schur(d, Batch{H->d_pool_i32.p + L.small_nodes, p64 + L.small_prefix, L.small_count}, L.small_ctas, 0, L.atomic, H->opt.schur_variant, 0, split_n, split_i, H->opt.schur_variant == 3 && L.max_ns >= 128, s);
+                H->st.gpu_launches += launch_schur(d, Batch{bign, p64 + L.urg_prefix, L.big_count}, L.urg_ctas, 1, 1, split_n, split_i, s);
+                H->st.gpu_launches += launch_schur(d, Batch{H->d_pool_i32.p + L.small_nodes, p64 + L.small_prefix, L.small_count}, L.small_ctas, 0, 0, split_n, split_i, s);
 #ifndef SLU_COMPLEX
-                H->st.gpu_launches += launch_oz_schur(d, Batch{tcn, p64 + L.tc_urg_prefix, L.tc_count}, L.tc_urg_ctas, 1, split_n, split_i, H->tc_slices, tc_na, s);
+                H->st.gpu_launches += launch_oz_schur(d, Batch{tcn, p64 + L.tc_urg_prefix, L.tc_count}, L.tc_urg_ctas, 1, split_n, split_i, H->tc_slices, s);
 #endif
                 CU(cudaStreamWaitEvent(s2, H->ev_panel[li], 0));
 #ifndef SLU_COMPLEX
-                H->st.gpu_launches += launch_oz_schur(d, Batch{tcn, p64 + L.tc_bulk_prefix, L.tc_count}, L.tc_bulk_ctas, 2, split_n, split_i, H->tc_slices, tc_na, s2);
+                H->st.gpu_launches += launch_oz_schur(d, Batch{tcn, p64 + L.tc_bulk_prefix, L.tc_count}, L.tc_bulk_ctas, 2, split_n, split_i, H->tc_slices, s2);
 #endif
-                H->st.gpu_launches += launch_schur(d, Batch{bign, p64 + L.bulk_prefix, L.big_count}, L.bulk_ctas, 1, L.atomic, H->opt.schur_variant, 2, split_n, split_i, H->opt.schur_variant == 3 && L.max_ns >= 128, s2);
+                H->st.gpu_launches += launch_schur(d, Batch{bign, p64 + L.bulk_prefix, L.big_count}, L.bulk_ctas, 1, 2, split_n, split_i, s2);
                 CU(cudaEventRecord(H->ev_bulk[li], s2));
             } else {
 #ifndef SLU_COMPLEX
-                H->st.gpu_launches += launch_oz_schur(d, Batch{tcn, p64 + L.tc_prefix, L.tc_count}, L.tc_ctas, 0, split_n, split_i, H->tc_slices, tc_na, s);
+                H->st.gpu_launches += launch_oz_schur(d, Batch{tcn, p64 + L.tc_prefix, L.tc_count}, L.tc_ctas, 0, split_n, split_i, H->tc_slices, s);
 #endif
-                H->st.gpu_launches += launch_schur(d, Batch{bign, p64 + L.big_prefix, L.big_count}, L.big_ctas, 1, L.atomic, H->opt.schur_variant, 0, split_n, split_i, H->opt.schur_variant == 3 && L.max_ns >= 128, s);
-                H->st.gpu_launches += launch_schur(d, Batch{H->d_pool_i32.p + L.small_nodes, p64 + L.small_prefix, L.small_count}, L.small_ctas, 0, L.atomic, H->opt.schur_variant, 0, split_n, split_i, H->opt.schur_variant == 3 && L.max_ns >= 128, s);
+                H->st.gpu_launches += launch_schur(d, Batch{bign, p64 + L.big_prefix, L.big_count}, L.big_ctas, 1, 0, split_n, split_i, s);
+                H->st.gpu_launches += launch_schur(d, Batch{H->d_pool_i32.p + L.small_nodes, p64 + L.small_prefix, L.small_count}, L.small_ctas, 0, 0, split_n, split_i, s);
             }
             if (prof) {
                 cudaEventRecord(pe[4], s);
@@ -1892,8 +1885,8 @@ int slu_b200_k_rerun_schur(slu_b200_handle_t H, int level, int reps, float *ms)
         launch_oz_slice(d, tcn, L.tc_count, p64 + L.tc_p_rt, L.tc_n_rt, p64 + L.tc_p_ak, L.tc_n_ak, p64 + L.tc_p_b, L.tc_n_b, H->tc_slices, s);
     for (int r = -1; r < reps; ++r) {
         if (r == 0) CU(cudaEventRecord(ev[0], s));
-        launch_oz_schur(d, Batch{tcn, p64 + L.tc_prefix, L.tc_count}, L.tc_ctas, 0, 1, 0, H->tc_slices, 0, s);
-        launch_schur(d, Batch{H->d_pool_i32.p + L.big_nodes, p64 + L.big_prefix, L.big_count}, L.big_ctas, 1, L.atomic, H->opt.schur_variant, 0, 1, 0, 0, s);
+        launch_oz_schur(d, Batch{tcn, p64 + L.tc_prefix, L.tc_count}, L.tc_ctas, 0, 1, 0, H->tc_slices, s);
+        launch_schur(d, Batch{H->d_pool_i32.p + L.big_nodes, p64 + L.big_prefix, L.big_count}, L.big_ctas, 1, 0, 1, 0, s);
     }
     CU(cudaEventRecord(ev[1], s));
     CU(cudaStreamSynchronize(s));
@@ -2366,6 +2359,7 @@ int pdgstrf3d_b200(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, 
 int slu_b200_plan(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, slu_b200_stats_t *stats)
 {
     if (!lu || !opt || !stats) return fail("null argument");
+    if (opt->schur_variant != 0) return fail("options.schur_variant is retired and must be 0 (got %d)", opt->schur_variant);
     if (lu->nprow * lu->npcol != 1) return fail("slu_b200_plan handles 1 x 1 x Pz grids (a Pr x Pc layer needs its peers' index pieces)");
     struct Guard { Guard() { g_plan_only = true; } ~Guard() { g_plan_only = false; } } guard;
     slu_b200_handle_s *H = new slu_b200_handle_s;

@@ -113,9 +113,7 @@ struct Batch {               // one kernel launch over several supernodes
 };
 
 constexpr int DIAG_NB = 16;
-constexpr bool DIAG_CLUSTER_DEFAULT = true;   // 8-CTA cluster LU of 65..256-column diagonal blocks (SLU_B200_DIAG_CLUSTER=1|0 overrides)
 constexpr int TRSM_NB = 16;
-constexpr bool TRSM_RL_DEFAULT = false;      // right-looking register-blocked panel solve (SLU_B200_TRSM_RL=1|0 overrides)
 constexpr int MAX_NS = 512;  // MAX_SUPER_SIZE, SRC/include/superlu_defs.h:154
 #ifdef SLU_COMPLEX
 constexpr int TRSM_STRIP = 32;      // vectors a TRSM CTA keeps in shared memory (16-byte elements)
@@ -141,11 +139,10 @@ int launch_diag_inv(const DeviceLU &d, const Batch &b, int64_t ctas, val_t *dinv
 int launch_trsm_l(const DeviceLU &d, const Batch &b, int64_t ctas, int max_ns, const val_t *dinv, cudaStream_t s);
 int launch_trsm_u(const DeviceLU &d, const Batch &b, int64_t ctas, int max_ns, const val_t *dinv, cudaStream_t s);
 int launch_schur_setup(const DeviceLU &d, const Batch &b, int64_t ctas, cudaStream_t s);
-// variant 0 (default): big tiles on schur_kernel_h (128x64, DMMA.16x8x8, 2 CTAs/SM); variant 1: 128x128 tiles, 512 threads
+// big: SCHUR_BM_BIG x SCHUR_BN_TILE tiles (double: schur_kernel_h, DMMA.16x8x8, 2 CTAs/SM), else SCHUR_BM_SMALL x SCHUR_BN_SMALL
 // mode 0: every tile of each supernode; 1: only the urgent tiles (urg_rows/urg_cols); 2: only the others
 // split_n/split_i: this rank takes tiles t with t % split_n == split_i (cooperative ancestor forests)
-int launch_schur(const DeviceLU &d, const Batch &b, int64_t ctas, int big, int atomic, int variant, int mode, int split_n,
-                 int split_i, int wide, cudaStream_t s);
+int launch_schur(const DeviceLU &d, const Batch &b, int64_t ctas, int big, int mode, int split_n, int split_i, cudaStream_t s);
 // skyline (sky + sky_off[slot]) <-> dense-packed U panel of each node of the batch; 32 columns per CTA
 int launch_u_convert(const DeviceLU &d, const Batch &b, int64_t ctas, int pack, val_t *sky,
                      const int64_t *sky_off, cudaStream_t s);
@@ -174,7 +171,7 @@ int launch_fill_csr(const DeviceLU &d, int n, const int32_t *rowptr, const int32
 
 // batched launches (both precisions): the same kernels over d.members matrices of one pattern (gridDim.y = members).
 // dinv = member 0's workspace; in the solve x holds the members' n x nrhs blocks back to back, in fill_csr aval their
-// nnz values.  Always the FP64 DMMA path with the default tile shapes: the opt-in kernel variants are not batched.
+// nnz values.  Always the FP64 DMMA path: the int8 path is not batched.
 int launch_diag_lu(const BatchedLU &d, const Batch &b, int max_ns, int replace_tiny, double thresh, cudaStream_t s);
 int launch_diag_inv(const BatchedLU &d, const Batch &b, int64_t ctas, val_t *dinv, cudaStream_t s);
 int launch_trsm_l(const BatchedLU &d, const Batch &b, int64_t ctas, int max_ns, const val_t *dinv, cudaStream_t s);
@@ -214,8 +211,6 @@ constexpr int OZ_NT_HOST = OZ_NT * OZ_CL;  // columns of the tile unit the host 
 constexpr int OZ_KSTEP = 32;          // int8 k per wgmma instruction and per pipeline stage
 constexpr int OZ_DEFAULT_SLICES = 7;  // 48 bits per operand: error ~1e-15 * k * rowmax * colmax (scripts/ozaki_emulate.py)
 constexpr int OZ_DEFAULT_MIN_NS = 128;
-constexpr bool OZ_PERSIST_DEFAULT = false;     // persistent int8 Schur kernel (SLU_B200_TC_PERSIST=1|0)
-constexpr bool OZ_NONATOMIC_DEFAULT = false;   // SLU_B200_TC_NONATOMIC=1|0 overrides
 // Off by default: the slices are scaled per L row and per U column, not per k, so the error is relative to rowmax * colmax
 // of each update and grows as (max / min pivot-row scale)^2 on a matrix that is not equilibrated (DESIGN 4b).  An
 // explicit slice count (options.reserved[4] = 5..8, or SLU_B200_TC_SLICES) opts in; SLU_B200_TC_MAX_M limits it to
@@ -228,10 +223,7 @@ inline int64_t oz_scale_elems(int m, int n) { return (int64_t)((m + 127) / 128) 
 int launch_oz_slice(const DeviceLU &d, const int32_t *nodes, int count, const int64_t *p_rt, int64_t n_rt, const int64_t *p_ak,
                     int64_t n_ak, const int64_t *p_b, int64_t n_b, int S, cudaStream_t s);
 // fused GEMM + scatter of the batch's 128 x OZ_NT tiles; mode / split as launch_schur
-// nonatomic: destinations flagged exclusive (LBlk/UBlk.shared == 0) are updated with plain load/store instead of RED --
-// the caller must then order this level's updates after ALL earlier levels' (no bulk update of level l-1 in flight)
-int launch_oz_schur(const DeviceLU &d, const Batch &b, int64_t ctas, int mode, int split_n, int split_i, int S, int nonatomic,
-                    cudaStream_t s);
+int launch_oz_schur(const DeviceLU &d, const Batch &b, int64_t ctas, int mode, int split_n, int split_i, int S, cudaStream_t s);
 // slu_ozaki.cu: C -= A*B through int8 slices on wgmma (variants 110..149: slices, stages, cluster)
 int launch_gemm_sub_ozaki(int m, int n, int k, const double *a, int lda, const double *b, int ldb, double *c, int ldc,
                           int variant, cudaStream_t s);
@@ -264,9 +256,9 @@ int launch_selinv_get(const DeviceLU &d, const val_t *hv, int n, const int32_t *
                       val_t *out, int *err, cudaStream_t s);
 
 #ifdef SLU_COMPLEX
-constexpr int SCHUR_BM_BIG = 128, SCHUR_BN_BIG = 32, SCHUR_BM_SMALL = 32, SCHUR_BN_SMALL = 16;
+constexpr int SCHUR_BM_BIG = 128, SCHUR_BM_SMALL = 32, SCHUR_BN_SMALL = 16;
 #else
-constexpr int SCHUR_BM_BIG = 128, SCHUR_BN_BIG = 128, SCHUR_BM_SMALL = 32, SCHUR_BN_SMALL = 32;
+constexpr int SCHUR_BM_BIG = 128, SCHUR_BM_SMALL = 32, SCHUR_BN_SMALL = 32;
 #endif
 constexpr int SETUP_THREADS = 256;
 

@@ -6,7 +6,7 @@
 //   schur_setup_kernel  destination maps of one supernode       (index work of dscatter_l/dscatter_u,
 //                                                                 SRC/double/dscatter.c:138-174, 222-243)
 //   schur_kernel_h      V = L(below,k) U(k,:) of the big tiles on FP64 tensor cores (mma.sync.m16n8k8.f64) with the
-//   schur_kernel        (small tiles and opt-in variants: mma.sync.m8n8k4.f64)
+//   schur_kernel        (small tiles: mma.sync.m8n8k4.f64)
 //                       subtract-scatter fused into the epilogue: no bigV buffer
 //                                                                (dblock_gemm_scatter, SRC/double/dscatter3d.c:82-189)
 //   u_expand / u_pack   skyline <-> dense-packed U at the boundary (dRgather_U, SRC/double/dgather.c:256-398)
@@ -18,8 +18,6 @@
 #include "slu_kernels_common.cuh"
 
 #include <climits>
-#include <cstdlib>
-#include <type_traits>
 
 namespace slu {
 
@@ -133,204 +131,7 @@ __global__ void __launch_bounds__(512) diag_lu_kernel(LU dd, Batch b, int replac
 }
 
 // ------------------------------------------------------------------------------------------------
-// diagonal block LU, Crout form on the FP64 tensor cores (opt-in: SLU_B200_DIAG_V3=1, supernodes <= 256 columns).
-// The right-looking kernel above streams the whole trailing block through L2 at every 16-column step and factors
-// the 16x16 pivot block through shared memory; on a 252-column block it takes 0.54 ms -- at every level of the
-// elimination tree, replicated on every rank of a cooperative group.  Here step j forms only
-//   panel  P = A(j0:, j0:j0+16)     - L(j0:, 0:j0)      U(0:j0, j0:j0+16)      (rem x 16, K = j0)
-//   rows   R = A(j0:j0+16, j0+16:)  - L(j0:j0+16, 0:j0) U(0:j0, j0+16:)        (16 x ncr, K = j0)
-// as DMMA products (16 warps: two 8-row tiles each for P, two 8-column tiles each for R; the operand every warp
-// shares is staged in shared memory, the other is read straight from L2), warp 0 factors the 16x16 pivot block in
-// registers with shuffles, and the rows below / columns to the right are solved one per thread as before.
-// Same arithmetic rules as the reference (reciprocal pivot, tiny-pivot replacement, zero pivot -> info).
-// ------------------------------------------------------------------------------------------------
-constexpr int D3_LD = 260;   // column stride of the staged panels: >= 256 + 4 and == 4 (mod 16) doubles
-constexpr int D3_MAX_NS = 256;
-constexpr size_t D3_SMEM = sizeof(double) * (16 * D3_LD + 17 * D3_LD + 16 * D3_LD + 20 * D3_LD);
-
-// one elimination step of the 16x16 pivot block held one row per lane; C is a template constant so that every
-// index into x[] is static (the rows stay in registers)
-template <int C>
-__device__ __forceinline__ void lu16_steps(double (&x)[16], int lane, int r, int jb, int replace_tiny, double thresh,
-                                           const DeviceLU &d, int col0)
-{
-    if constexpr (C < 16) {
-        double p = __shfl_sync(0xffffffffu, x[C], C);
-        if (C < jb) {
-            if (replace_tiny && fabs(p) < thresh) {  // pdgstrf2.c:544-560
-                p = (p < 0) ? -thresh : thresh;
-                if (lane == C) { x[C] = p; if (replace_tiny == 1) atomicAdd(d.tiny, 1ULL); }
-            }
-            if (p == 0.0 && lane == 0) atomicMin(d.info, col0 + C + 1);  // pdgstrf2.c:568-571
-        }
-        const double rp = (p != 0.0) ? 1.0 / p : 1.0;
-        const bool below = r > C;
-        if (below && p != 0.0) x[C] *= rp;
-        const double l = x[C];
-#pragma unroll
-        for (int cc = C + 1; cc < 16; ++cc) {
-            const double u = __shfl_sync(0xffffffffu, x[cc], C);
-            if (below) x[cc] -= l * u;
-        }
-        lu16_steps<C + 1>(x, lane, r, jb, replace_tiny, thresh, d, col0);
-    }
-}
-
-__global__ void __launch_bounds__(512) diag_lu_kernel_v3(DeviceLU d, Batch b, int replace_tiny, double thresh, int skip_lo, int skip_hi)
-{
-    extern __shared__ double sm[];
-    double *Pl = sm;                  // L panel         Pl[c * D3_LD + i],  i < rem, c < 16
-    double *Pu = Pl + 16 * D3_LD;     // U row block     Pu[col * 17 + r],   col < ncr, r < 16
-    double *Ub = Pu + 17 * D3_LD;     // U(p, j0 + c)    Ub[c * D3_LD + p],  p < j0
-    double *Lb = Ub + 16 * D3_LD;     // L(j0 + r, p)    Lb[p * 20 + r],     p < j0
-    const int k = b.nodes[blockIdx.x];
-    const NodeDesc nd = d.nodes[k];
-    if (nd.ns >= skip_lo && nd.ns <= skip_hi) return;   // taken by the cluster kernel
-    const int ns = nd.ns, lda = nd.nsupr, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int lr = lane >> 2, lk = lane & 3;
-    double *A = d.val + nd.lval;
-
-    for (int j0 = 0; j0 < ns; j0 += 16) {
-        const int jb = min(16, ns - j0), rem = ns - j0, ncr = rem - jb;  // ncr > 0 implies jb == 16
-        // ---- stage the shared operands ---------------------------------------------------------------------
-        for (int idx = tid; idx < 16 * j0; idx += 512) {
-            const int c = idx / j0, p = idx - c * j0;
-            Ub[c * D3_LD + p] = (c < jb) ? A[(size_t)(j0 + c) * lda + p] : 0.0;
-        }
-        for (int idx = tid; idx < 16 * j0; idx += 512) {
-            const int p = idx >> 4, r = idx & 15;
-            Lb[p * 20 + r] = (r < jb) ? A[(size_t)p * lda + j0 + r] : 0.0;
-        }
-        __syncthreads();
-        // ---- P = A(panel) - L(j0:, 0:j0) U(0:j0, panel): warp w owns the 8-row tiles w and w + 16 -------------
-        {
-            double acc[2][2][2];
-#pragma unroll
-            for (int t = 0; t < 2; ++t)
-#pragma unroll
-                for (int ni = 0; ni < 2; ++ni) acc[t][ni][0] = acc[t][ni][1] = 0.0;
-            const int i0 = warp * 8 + lr, i1 = (warp + 16) * 8 + lr;   // rows relative to j0
-            const bool ok0 = i0 < rem, ok1 = i1 < rem;
-            if (warp * 8 < rem) {
-#pragma unroll 4
-                for (int p0 = 0; p0 < j0; p0 += 4) {
-                    const double *col = A + (size_t)(p0 + lk) * lda + j0;
-                    const double a0 = ok0 ? col[i0] : 0.0, a1 = ok1 ? col[i1] : 0.0;
-#pragma unroll
-                    for (int ni = 0; ni < 2; ++ni) {
-                        const double bv = Ub[(ni * 8 + lr) * D3_LD + p0 + lk];
-                        dmma884(acc[0][ni][0], acc[0][ni][1], a0, bv);
-                        dmma884(acc[1][ni][0], acc[1][ni][1], a1, bv);
-                    }
-                }
-            }
-#pragma unroll
-            for (int t = 0; t < 2; ++t) {
-                const int i = t ? i1 : i0;
-                if (i >= rem) continue;
-#pragma unroll
-                for (int ni = 0; ni < 2; ++ni)
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const int c = ni * 8 + 2 * lk + e;
-                        // columns past the block are padded with the identity so that the 16x16 LU below is harmless
-                        Pl[c * D3_LD + i] = (c < jb) ? A[(size_t)(j0 + c) * lda + j0 + i] - acc[t][ni][e] : ((i == c) ? 1.0 : 0.0);
-                    }
-            }
-        }
-        // ---- R = A(rows) - L(rows, 0:j0) U(0:j0, j0+16:): warp w owns the 8-column tiles w and w + 16 -----------
-        if (ncr > 0 && warp * 8 < ncr) {
-            double acc[2][2][2];
-#pragma unroll
-            for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-                for (int t = 0; t < 2; ++t) acc[mi][t][0] = acc[mi][t][1] = 0.0;
-            const int c0 = warp * 8 + lr, c1 = (warp + 16) * 8 + lr;   // columns relative to j0 + 16 (B fragment)
-            const bool ok0 = c0 < ncr, ok1 = c1 < ncr;
-            const double *b0p = A + (size_t)(j0 + 16 + (ok0 ? c0 : 0)) * lda, *b1p = A + (size_t)(j0 + 16 + (ok1 ? c1 : 0)) * lda;
-#pragma unroll 4
-            for (int p0 = 0; p0 < j0; p0 += 4) {
-                const double bv0 = ok0 ? b0p[p0 + lk] : 0.0, bv1 = ok1 ? b1p[p0 + lk] : 0.0;
-#pragma unroll
-                for (int mi = 0; mi < 2; ++mi) {
-                    const double av = Lb[(p0 + lk) * 20 + mi * 8 + lr];
-                    dmma884(acc[mi][0][0], acc[mi][0][1], av, bv0);
-                    dmma884(acc[mi][1][0], acc[mi][1][1], av, bv1);
-                }
-            }
-#pragma unroll
-            for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-                for (int t = 0; t < 2; ++t)
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const int col = (t ? warp + 16 : warp) * 8 + 2 * lk + e, r = mi * 8 + lr;  // C fragment
-                        if (col < ncr) Pu[col * 17 + r] = A[(size_t)(j0 + 16 + col) * lda + j0 + r] - acc[mi][t][e];
-                    }
-        }
-        __syncthreads();
-        // ---- warp 0: LU of the 16x16 pivot block in registers (lane r holds row r) ------------------------------
-        if (warp == 0) {
-            const int r = lane & 15;
-            double x[16];
-#pragma unroll
-            for (int c = 0; c < 16; ++c) x[c] = Pl[c * D3_LD + r];
-            lu16_steps<0>(x, lane, r, jb, replace_tiny, thresh, d, nd.fsupc + j0);
-            if (lane < 16) {
-#pragma unroll
-                for (int c = 0; c < 16; ++c) Pl[c * D3_LD + r] = x[c];
-            }
-        }
-        __syncthreads();
-        // ---- rows below: x U11 = p (one row per thread); columns to the right: L11 y = r (one column per thread) ----
-        if (tid < 256) {
-            const int i = 16 + tid;
-            if (i < rem) {
-                double x[16];
-#pragma unroll
-                for (int c = 0; c < 16; ++c) x[c] = Pl[c * D3_LD + i];
-#pragma unroll
-                for (int c = 0; c < 16; ++c) {
-                    double v = x[c];
-#pragma unroll
-                    for (int p = 0; p < 16; ++p)
-                        if (p < c) v -= x[p] * Pl[c * D3_LD + p];
-                    const double pv = Pl[c * D3_LD + c];
-                    x[c] = (pv != 0.0) ? v * (1.0 / pv) : v;
-                }
-#pragma unroll
-                for (int c = 0; c < 16; ++c) Pl[c * D3_LD + i] = x[c];
-            }
-        } else {
-            const int col = tid - 256;
-            if (col < ncr) {
-                double x[16];
-#pragma unroll
-                for (int p = 0; p < 16; ++p) x[p] = Pu[col * 17 + p];
-#pragma unroll
-                for (int p = 0; p < 16; ++p)
-#pragma unroll
-                    for (int q = p + 1; q < 16; ++q) x[q] -= Pl[p * D3_LD + q] * x[p];
-#pragma unroll
-                for (int p = 0; p < 16; ++p) Pu[col * 17 + p] = x[p];
-            }
-        }
-        __syncthreads();
-        // ---- write the finished panel and row block back -----------------------------------------------------
-        for (int idx = tid; idx < jb * rem; idx += 512) {
-            const int c = idx / rem, i = idx - c * rem;
-            A[(size_t)(j0 + c) * lda + j0 + i] = Pl[c * D3_LD + i];
-        }
-        for (int idx = tid; idx < 16 * ncr; idx += 512) {
-            const int col = idx >> 4, r = idx & 15;
-            A[(size_t)(j0 + 16 + col) * lda + j0 + r] = Pu[col * 17 + r];
-        }
-        __syncthreads();
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// diagonal block LU on a thread-block cluster (supernodes of 65..256 columns).  The one-CTA kernels above stream the
+// diagonal block LU on a thread-block cluster (supernodes of 65..256 columns).  The one-CTA kernel above streams the
 // block through L2 from ONE SM at every 16-column step: 0.54 ms for a 252-column block, at every level of the
 // elimination tree and on every rank of a cooperative group -- the Amdahl term of the 8-GPU run (VERDICT r1).
 // Here a cluster of 8 CTAs (8 SMs of one GPC) holds the whole block in shared memory, one 32-column slab per CTA:
@@ -483,39 +284,18 @@ __global__ void __cluster_dims__(DC_CL, 1, 1) __launch_bounds__(256) diag_lu_clu
     }
 }
 
-static bool diag_cluster_enabled()
-{
-    static const int on = (getenv("SLU_B200_DIAG_CLUSTER") ? atoi(getenv("SLU_B200_DIAG_CLUSTER")) : (DIAG_CLUSTER_DEFAULT ? 1 : 0));
-    return on != 0;
-}
-
-static bool diag_v3_enabled()
-{
-    static const int on = (getenv("SLU_B200_DIAG_V3") && atoi(getenv("SLU_B200_DIAG_V3")) != 0) ? 1 : 0;
-    return on != 0;
-}
-
 template <class LU>
 static int launch_diag_lu_t(const LU &d, const Batch &b, int max_ns, int replace_tiny, double thresh, cudaStream_t s)
 {
     if (b.count <= 0) return 0;
-    constexpr bool batched = std::is_same<LU, BatchedLU>::value;   // the opt-in v3 kernel is not batched
     int launched = 0, skip_lo = 1, skip_hi = 0;    // empty range: the one-CTA kernel takes every supernode
-    if (max_ns >= DC_MIN_NS && diag_cluster_enabled()) {
+    if (max_ns >= DC_MIN_NS) {
         static std::atomic<unsigned long long> attrc{0};
         ensure_dyn_smem(diag_lu_cluster_kernel<LU>, (int)DC_SMEM, attrc);
         diag_lu_cluster_kernel<LU><<<member_grid(d, b.count * DC_CL), 256, DC_SMEM, s>>>(d, b, replace_tiny, thresh);
         skip_lo = DC_MIN_NS; skip_hi = DC_MAX_NS;
         ++launched;
         if (b.count == 1 && max_ns <= DC_MAX_NS) return launched;   // the single supernode of a chain level went to the cluster
-    }
-    if constexpr (!batched) {
-        if (max_ns <= D3_MAX_NS && diag_v3_enabled()) {
-            static std::atomic<unsigned long long> attr3_0{0};
-            ensure_dyn_smem(diag_lu_kernel_v3, (int)D3_SMEM, attr3_0);
-            diag_lu_kernel_v3<<<b.count, 512, D3_SMEM, s>>>(d, b, replace_tiny, thresh, skip_lo, skip_hi);
-            return launched + 1;
-        }
     }
     size_t smem = sizeof(double) * 2 * DIAG_NB * (size_t)max_ns;
     static std::atomic<unsigned long long> attr_0{0};
@@ -740,146 +520,10 @@ __global__ void __launch_bounds__(256) trsm_kernel(LU dd, Batch b, const double 
     else trsm_body<UCASE, false, TRSM_STRIP / 2>(d, nd, strip, dinv, Ys);
 }
 
-// ------------------------------------------------------------------------------------------------
-// Right-looking panel solve with the strip held in REGISTERS (supernodes <= 256 columns).  The left-looking kernel above
-// does 1.5 shared-memory fragment loads per DMMA (one 8-row tile x two 8-column tiles per warp) and reaches 8 TF/s.
-// Here warp w owns columns [32w, 32w+32) of the 64-vector strip as DMMA accumulators (8 x 4 tiles) for the whole sweep;
-// step j (16 columns): the owning warp multiplies its 64 x 16 block by inv(T_jj) (through shared memory, C- to
-// A-fragment), publishes X_j, and every warp holding later columns subtracts X_j T(j, its columns): 32 A-fragment
-// loads for 128 DMMAs, the T fragments straight from L2.  One block barrier per step (X_j double-buffered).
-// Same arithmetic as above (16 x 16 inverted diagonal blocks from diag_inv_kernel, substitution elsewhere).
-// ------------------------------------------------------------------------------------------------
-constexpr int TRL_XLD = TRSM_STRIP + 4;
-template <bool UCASE>
-__global__ void __launch_bounds__(256, 1) trsm_rl_kernel(DeviceLU d, Batch b, const double *dinv)
-{
-    __shared__ double Xs[2][16 * TRL_XLD];
-    const int slot = find_slot(b.prefix, b.count, blockIdx.x);
-    const int k = b.nodes[slot];
-    const int strip = (int)(blockIdx.x - b.prefix[slot]);
-    const NodeDesc nd = d.nodes[k];
-    const int ns = nd.ns, lda = nd.nsupr, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, lr = lane >> 2, lk = lane & 3;
-    const double *T = d.val + nd.lval;
-    const double *inv = dinv + nd.ws_inv;
-    const int nvec = UCASE ? nd.ncols : nd.m;
-    const int v0 = strip * TRSM_STRIP, nv = min(TRSM_STRIP, nvec - v0);
-    double *X = UCASE ? d.val + nd.uval + (size_t)v0 * ns : d.val + nd.lval + ns + v0;
-    const int cw = warp * 32;                       // my first column
-    const bool active = cw < ns;
-
-    double acc[8][4][2];
-#pragma unroll
-    for (int mi = 0; mi < 8; ++mi)
-#pragma unroll
-        for (int ni = 0; ni < 4; ++ni)
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                const int sv = mi * 8 + lr, c = cw + ni * 8 + 2 * lk + e;
-                double v = 0.0;
-                if (active && sv < nv && c < ns) v = UCASE ? X[(size_t)sv * ns + c] : X[(size_t)c * lda + sv];
-                acc[mi][ni][e] = v;
-            }
-
-    const int nblk = (ns + 15) >> 4;
-    for (int j = 0; j < nblk; ++j) {
-        const int j0 = j * 16, buf = j & 1;
-        double *xs = Xs[buf];
-        if (warp == (j0 >> 5)) {
-            // ---- X_j = (my 64 x 16 block) * inv(T_jj) ------------------------------------------------------------
-            const int h = (j0 >> 4) & 1;
-#pragma unroll
-            for (int mi = 0; mi < 8; ++mi)
-#pragma unroll
-                for (int n2 = 0; n2 < 2; ++n2)
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) xs[(n2 * 8 + 2 * lk + e) * TRL_XLD + mi * 8 + lr] = h ? acc[mi][2 + n2][e] : acc[mi][n2][e];
-            __syncwarp();
-            const double *ib = inv + (size_t)j * 512;
-            double out[8][2][2];
-#pragma unroll
-            for (int mi = 0; mi < 8; ++mi)
-#pragma unroll
-                for (int n2 = 0; n2 < 2; ++n2) out[mi][n2][0] = out[mi][n2][1] = 0.0;
-#pragma unroll
-            for (int k4 = 0; k4 < 4; ++k4) {
-                double bb[2];
-#pragma unroll
-                for (int n2 = 0; n2 < 2; ++n2) {
-                    const int pp = 4 * k4 + lk, c = n2 * 8 + lr;
-                    bb[n2] = UCASE ? ib[256 + pp * 16 + c] : ib[c * 16 + pp];
-                }
-#pragma unroll
-                for (int mi = 0; mi < 8; ++mi) {
-                    const double a = xs[(4 * k4 + lk) * TRL_XLD + mi * 8 + lr];
-#pragma unroll
-                    for (int n2 = 0; n2 < 2; ++n2) dmma884(out[mi][n2][0], out[mi][n2][1], a, bb[n2]);
-                }
-            }
-            __syncwarp();
-#pragma unroll
-            for (int mi = 0; mi < 8; ++mi)
-#pragma unroll
-                for (int n2 = 0; n2 < 2; ++n2)
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        xs[(n2 * 8 + 2 * lk + e) * TRL_XLD + mi * 8 + lr] = out[mi][n2][e];
-                        if (h) acc[mi][2 + n2][e] = out[mi][n2][e]; else acc[mi][n2][e] = out[mi][n2][e];
-                    }
-        }
-        __syncthreads();
-        // ---- columns to the right of block j: acc -= X_j * T(j-block, my columns) --------------------------------------
-        if (active && cw + 32 > j0 + 16) {
-            const int ni0 = (cw > j0) ? 0 : ((j0 + 16 - cw) >> 3);   // my first 8-column tile past the block
-#pragma unroll
-            for (int k4 = 0; k4 < 4; ++k4) {
-                const int pr = j0 + 4 * k4 + lk;                     // row of T
-                double bb[4];
-#pragma unroll
-                for (int ni = 0; ni < 4; ++ni) {
-                    const int c = cw + ni * 8 + lr;
-                    bb[ni] = (ni >= ni0 && c < ns && pr < ns) ? (UCASE ? T[(size_t)pr * lda + c] : T[(size_t)c * lda + pr]) : 0.0;
-                }
-#pragma unroll
-                for (int mi = 0; mi < 8; ++mi) {
-                    const double a = -xs[(4 * k4 + lk) * TRL_XLD + mi * 8 + lr];
-#pragma unroll
-                    for (int ni = 0; ni < 4; ++ni)
-                        if (ni >= ni0) dmma884(acc[mi][ni][0], acc[mi][ni][1], a, bb[ni]);
-                }
-            }
-        }
-    }
-    if (active)
-#pragma unroll
-        for (int mi = 0; mi < 8; ++mi)
-#pragma unroll
-            for (int ni = 0; ni < 4; ++ni)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int sv = mi * 8 + lr, c = cw + ni * 8 + 2 * lk + e;
-                    if (sv < nv && c < ns) {
-                        if (UCASE) X[(size_t)sv * ns + c] = acc[mi][ni][e];
-                        else X[(size_t)c * lda + sv] = acc[mi][ni][e];
-                    }
-                }
-}
-
-static bool trsm_rl_enabled()
-{
-    static const int on = getenv("SLU_B200_TRSM_RL") ? atoi(getenv("SLU_B200_TRSM_RL")) : (TRSM_RL_DEFAULT ? 1 : 0);
-    return on != 0;
-}
-
 template <bool UCASE, class LU>
 static int launch_trsm(const LU &d, const Batch &b, int64_t ctas, int max_ns, const double *dinv, cudaStream_t s)
 {
     if (b.count <= 0 || ctas <= 0) return 0;
-    if constexpr (!std::is_same<LU, BatchedLU>::value) {   // the opt-in register-blocked kernel is not batched
-        if (max_ns <= 256 && trsm_rl_enabled()) {
-            trsm_rl_kernel<UCASE><<<(unsigned)ctas, 256, 0, s>>>(d, b, dinv);
-            return 1;
-        }
-    }
     static std::atomic<unsigned long long> attr_0{0};
     ensure_dyn_smem(trsm_kernel<UCASE, false, LU>, 227 * 1024, attr_0);
     static std::atomic<unsigned long long> attr_1{0};
@@ -913,8 +557,9 @@ int launch_trsm_u(const BatchedLU &d, const Batch &b, int64_t ctas, int max_ns, 
 // ------------------------------------------------------------------------------------------------
 // FP64 tensor-core GEMM tile (DMMA m8n8k4), cp.async multi-stage pipeline
 // ------------------------------------------------------------------------------------------------
-template <int BM, int BN, int WARPS_M, int WARPS_N, int BK = 16, int STAGES = 3>
+template <int BM, int BN, int WARPS_M, int WARPS_N>
 struct GemmCfg {
+    static constexpr int BK = 16, STAGES = 3;
     static constexpr int NT = 32 * WARPS_M * WARPS_N;
     static constexpr int WTM = BM / WARPS_M, WTN = BN / WARPS_N;
     static constexpr int MI = WTM / 8, NI = WTN / 8;
@@ -923,76 +568,18 @@ struct GemmCfg {
     static constexpr size_t SMEM = sizeof(double) * STAGES * (A_STAGE + B_STAGE);
 };
 
-// acc[mi][ni][2] += A(m0.., :) * B(:, n0..) for the CTA tile; A is M x K (lda), B is K x N (ldb)
-template <int BM, int BN, int WARPS_M, int WARPS_N, int BK = 16, int STAGES = 3>
+// acc[mi][ni][2] += A(m0.., :) * B(:, n0..) for the CTA tile; A is M x K (lda), B is K x N (ldb).
+// Interior tiles (no M/N edge) and full k-steps use running pointers: every warp copies whole 32-row column
+// slices of A (row offsets become immediates) and the B slices advance by constant strides.  Edge tiles and the
+// K tail take the general predicated loader, which spends ~300 instructions per k-step on 64-bit address arithmetic
+// and predicates.
+template <int BM, int BN, int WARPS_M, int WARPS_N>
 __device__ __forceinline__ void gemm_tile(const double *__restrict__ A, int lda, const double *__restrict__ B,
                                           int ldb, int M, int N, int K, int m0, int n0, double *sm,
                                           double (&acc)[BM / WARPS_M / 8][BN / WARPS_N / 8][2])
 {
-    using C = GemmCfg<BM, BN, WARPS_M, WARPS_N, BK, STAGES>;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int wm0 = (warp % WARPS_M) * C::WTM, wn0 = (warp / WARPS_M) * C::WTN;
-    double *As = sm, *Bs = sm + STAGES * C::A_STAGE;
-    const int KT = (K + BK - 1) / BK;
-
-    auto load = [&](int st, int kt) {
-        const int k0 = kt * BK;
-        double *as = As + st * C::A_STAGE, *bs = Bs + st * C::B_STAGE;
-#pragma unroll
-        for (int idx = tid; idx < BK * BM; idx += C::NT) {
-            int kk = idx / BM, mm = idx - kk * BM;
-            bool p = (m0 + mm < M) && (k0 + kk < K);
-            const double *src = p ? A + (size_t)(k0 + kk) * lda + m0 + mm : A;
-            cp_async8(as + kk * C::LDA + mm, src, p);
-        }
-#pragma unroll
-        for (int idx = tid; idx < BK * BN; idx += C::NT) {
-            int nn = idx / BK, kk = idx - nn * BK;
-            bool p = (n0 + nn < N) && (k0 + kk < K);
-            const double *src = p ? B + (size_t)(n0 + nn) * ldb + k0 + kk : B;
-            cp_async8(bs + nn * C::LDB + kk, src, p);
-        }
-    };
-
-#pragma unroll
-    for (int s = 0; s < STAGES - 1; ++s) {
-        if (s < KT) load(s, s);
-        cp_async_commit();
-    }
-    for (int kt = 0; kt < KT; ++kt) {
-        cp_async_wait<STAGES - 2>();
-        __syncthreads();
-        if (kt + STAGES - 1 < KT) load((kt + STAGES - 1) % STAGES, kt + STAGES - 1);
-        cp_async_commit();
-        const double *as = As + (kt % STAGES) * C::A_STAGE, *bs = Bs + (kt % STAGES) * C::B_STAGE;
-#pragma unroll
-        for (int k4 = 0; k4 < BK / 4; ++k4) {
-            double a[C::MI], bb[C::NI];
-#pragma unroll
-            for (int mi = 0; mi < C::MI; ++mi) a[mi] = as[(k4 * 4 + (lane & 3)) * C::LDA + wm0 + mi * 8 + (lane >> 2)];
-#pragma unroll
-            for (int ni = 0; ni < C::NI; ++ni) bb[ni] = bs[(wn0 + ni * 8 + (lane >> 2)) * C::LDB + k4 * 4 + (lane & 3)];
-#pragma unroll
-            for (int mi = 0; mi < C::MI; ++mi)
-#pragma unroll
-                for (int ni = 0; ni < C::NI; ++ni) dmma884(acc[mi][ni][0], acc[mi][ni][1], a[mi], bb[ni]);
-        }
-    }
-    cp_async_wait<0>();
-}
-
-// Same tile product with a strength-reduced loader ("where the Schur kernel's time goes": the
-// general loader above spends ~300 instructions per k-step on 64-bit address arithmetic and predicates, 30 % of a
-// warp's main-loop time, and a warp alone cannot keep the DMMA pipe busy while its sibling CTA is in its epilogue).
-// Interior tiles (no M/N edge) and full k-steps use running pointers: every warp copies whole 32-row column
-// slices of A (row offsets become immediates) and the B slices advance by constant strides; edge tiles and the
-// K tail fall back to the general predicated loader.
-template <int BM, int BN, int WARPS_M, int WARPS_N, int BK = 16, int STAGES = 3>
-__device__ __forceinline__ void gemm_tile_v2(const double *__restrict__ A, int lda, const double *__restrict__ B,
-                                             int ldb, int M, int N, int K, int m0, int n0, double *sm,
-                                             double (&acc)[BM / WARPS_M / 8][BN / WARPS_N / 8][2])
-{
-    using C = GemmCfg<BM, BN, WARPS_M, WARPS_N, BK, STAGES>;
+    using C = GemmCfg<BM, BN, WARPS_M, WARPS_N>;
+    constexpr int BK = C::BK, STAGES = C::STAGES;
     constexpr int NW = C::NT / 32;                  // warps
     constexpr int CA = BK / NW, RA = BM / 32;       // A: columns per warp and 32-row slices per column
     constexpr int CB = C::NT / BK, JB = BN / CB;    // B: columns per pass and passes
@@ -1110,11 +697,11 @@ __device__ __forceinline__ void schur_tile_of(const NodeDesc &nd, int tile, int 
     }
 }
 
-template <int BM, int BN, int WARPS_M, int WARPS_N, bool ATOMIC, int BK = 16, int STAGES = 3, bool V2 = false, class LU = DeviceLU>
+template <int BM, int BN, int WARPS_M, int WARPS_N, class LU>
 __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, (32 * WARPS_M * WARPS_N <= 256) ? 2 : 1)
     schur_kernel(LU dd, Batch b, int mode, int split_n, int split_i)
 {
-    using C = GemmCfg<BM, BN, WARPS_M, WARPS_N, BK, STAGES>;
+    using C = GemmCfg<BM, BN, WARPS_M, WARPS_N>;
     extern __shared__ double sm[];
     const DeviceLU &d = member_view(dd);
     // cooperative ancestors: the ranks of a Z group deal the tiles of the batch round-robin
@@ -1133,12 +720,8 @@ __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, (32 * WARPS_M * WARPS_
 #pragma unroll
         for (int ni = 0; ni < C::NI; ++ni) acc[mi][ni][0] = acc[mi][ni][1] = 0.0;
 
-    if constexpr (V2)
-        gemm_tile_v2<BM, BN, WARPS_M, WARPS_N, BK, STAGES>(d.val + nd.lval + nd.ns, nd.nsupr, d.val + nd.uval, nd.ns,
-                                                           nd.m, nd.ncols, nd.ns, m0, n0, sm, acc);
-    else
-    gemm_tile<BM, BN, WARPS_M, WARPS_N, BK, STAGES>(d.val + nd.lval + nd.ns, nd.nsupr, d.val + nd.uval, nd.ns, nd.m,
-                                                    nd.ncols, nd.ns, m0, n0, sm, acc);
+    gemm_tile<BM, BN, WARPS_M, WARPS_N>(d.val + nd.lval + nd.ns, nd.nsupr, d.val + nd.uval, nd.ns, nd.m, nd.ncols, nd.ns,
+                                        m0, n0, sm, acc);
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int wm0 = m0 + (warp % WARPS_M) * C::WTM, wn0 = n0 + (warp / WARPS_M) * C::WTN;
@@ -1155,8 +738,7 @@ __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, (32 * WARPS_M * WARPS_
     }
 #pragma unroll
     for (int ni = 0; ni < C::NI; ++ni) {
-        // destination offsets of the 2 x MI elements of this 8-column slab, then one batch of
-        // independent read-modify-writes (the loads are issued together: one DRAM latency per slab)
+        // destination offsets of the 2 x MI elements of this 8-column slab, then one batch of independent REDs
         int64_t idx[2][C::MI];
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
@@ -1178,25 +760,11 @@ __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, (32 * WARPS_M * WARPS_
                 }
             }
         }
-        if (ATOMIC) {
 #pragma unroll
-            for (int e = 0; e < 2; ++e)
+        for (int e = 0; e < 2; ++e)
 #pragma unroll
-                for (int mi = 0; mi < C::MI; ++mi)
-                    if (idx[e][mi] >= 0) atomicAdd(d.val + idx[e][mi], V2 ? flip_sign(acc[mi][ni][e]) : -acc[mi][ni][e]);
-        } else {
-            double old[2][C::MI];
-#pragma unroll
-            for (int e = 0; e < 2; ++e)
-#pragma unroll
-                for (int mi = 0; mi < C::MI; ++mi)
-                    if (idx[e][mi] >= 0) old[e][mi] = __ldcg(d.val + idx[e][mi]);
-#pragma unroll
-            for (int e = 0; e < 2; ++e)
-#pragma unroll
-                for (int mi = 0; mi < C::MI; ++mi)
-                    if (idx[e][mi] >= 0) __stcg(d.val + idx[e][mi], old[e][mi] - acc[mi][ni][e]);
-        }
+            for (int mi = 0; mi < C::MI; ++mi)
+                if (idx[e][mi] >= 0) atomicAdd(d.val + idx[e][mi], flip_sign(acc[mi][ni][e]));
     }
 }
 
@@ -1401,57 +969,39 @@ static int launch_schur_h(const LU &d, const Batch &b, int64_t ctas, int mode, i
     return 1;
 }
 
-template <int BM, int BN, int WARPS_M, int WARPS_N, bool ATOMIC, int BK = 16, int STAGES = 3, bool V2 = false, class LU = DeviceLU>
-static int launch_schur_t(const LU &d, const Batch &b, int64_t ctas, int mode, int split_n, int split_i, cudaStream_t s)
+// the small tiles (updates of fewer than 96 rows or columns): schur_kernel on mma.sync.m8n8k4.f64
+template <class LU>
+static int launch_schur_small(const LU &d, const Batch &b, int64_t ctas, int mode, int split_n, int split_i, cudaStream_t s)
 {
-    using C = GemmCfg<BM, BN, WARPS_M, WARPS_N, BK, STAGES>;
+    using C = GemmCfg<SCHUR_BM_SMALL, SCHUR_BN_SMALL, 2, 2>;
     static std::atomic<unsigned long long> attr_0{0};
-    ensure_dyn_smem(schur_kernel<BM, BN, WARPS_M, WARPS_N, ATOMIC, BK, STAGES, V2, LU>, (int)C::SMEM, attr_0);
+    ensure_dyn_smem(schur_kernel<SCHUR_BM_SMALL, SCHUR_BN_SMALL, 2, 2, LU>, (int)C::SMEM, attr_0);
     const int64_t grid = (ctas + split_n - 1) / split_n;
-    schur_kernel<BM, BN, WARPS_M, WARPS_N, ATOMIC, BK, STAGES, V2, LU><<<member_grid(d, (unsigned)grid), C::NT, C::SMEM, s>>>(d, b, mode, split_n, split_i);
+    schur_kernel<SCHUR_BM_SMALL, SCHUR_BN_SMALL, 2, 2, LU><<<member_grid(d, (unsigned)grid), C::NT, C::SMEM, s>>>(d, b, mode, split_n, split_i);
     return 1;
 }
 
-int launch_schur(const DeviceLU &d, const Batch &b, int64_t ctas, int big, int atomic, int variant, int mode, int split_n,
-                 int split_i, int wide, cudaStream_t s)
+int launch_schur(const DeviceLU &d, const Batch &b, int64_t ctas, int big, int mode, int split_n, int split_i, cudaStream_t s)
 {
     if (b.count <= 0 || ctas <= 0) return 0;
-    // default: the Hopper main loop for the big class, the running-pointer loader (gemm_tile_v2) for small tiles.
-    // variant 6 = the round-1 general loader, kept for A/B runs.
-    if (variant == 0 && big) return launch_schur_h<SCHUR_H_TILE>(d, b, ctas, mode, split_n, split_i, s);
-    if (variant == 0) variant = 4;
-    if (variant == 6) variant = 0;
-    if (variant == 4 || variant == 5) {  // strength-reduced loader + sign flip off the FP64 pipe (4), with BK = 32 (5)
-        if (!big) return launch_schur_t<SCHUR_BM_SMALL, SCHUR_BN_SMALL, 2, 2, true, 16, 3, true>(d, b, ctas, mode, split_n, split_i, s);
-        if (variant == 5) return launch_schur_t<128, 64, 4, 2, true, 32, 2, true>(d, b, ctas, mode, split_n, split_i, s);
-        return launch_schur_t<128, 64, 4, 2, true, 16, 3, true>(d, b, ctas, mode, split_n, split_i, s);
-    }
-    if (big) {
-        // wide supernodes (k >= 128): BK = 32 with 2 stages halves the block barriers per tile (27.7 vs 25.9 TF/s
-        // at k = 256 in scripts/gemm_variants.py); narrow ones keep BK = 16 x 3 stages (better at k = 64)
-        if (variant != 1 && wide) return launch_schur_t<128, 64, 4, 2, true, 32, 2>(d, b, ctas, mode, split_n, split_i, s);
-        if (variant != 1) return launch_schur_t<128, 64, 4, 2, true>(d, b, ctas, mode, split_n, split_i, s);
-        return atomic ? launch_schur_t<SCHUR_BM_BIG, SCHUR_BN_BIG, 4, 4, true>(d, b, ctas, mode, split_n, split_i, s)
-                      : launch_schur_t<SCHUR_BM_BIG, SCHUR_BN_BIG, 4, 4, false>(d, b, ctas, mode, split_n, split_i, s);
-    }
-    return atomic ? launch_schur_t<SCHUR_BM_SMALL, SCHUR_BN_SMALL, 2, 2, true>(d, b, ctas, mode, split_n, split_i, s)
-                  : launch_schur_t<SCHUR_BM_SMALL, SCHUR_BN_SMALL, 2, 2, false>(d, b, ctas, mode, split_n, split_i, s);
+    if (big) return launch_schur_h<SCHUR_H_TILE>(d, b, ctas, mode, split_n, split_i, s);
+    return launch_schur_small(d, b, ctas, mode, split_n, split_i, s);
 }
 
-// batched: the default tiles of the launcher above (schur_variant 0, atomic scatter, no Z split)
+// batched: the same two kernels, no Z split
 int launch_schur(const BatchedLU &d, const Batch &b, int64_t ctas, int big, int mode, cudaStream_t s)
 {
     if (b.count <= 0 || ctas <= 0) return 0;
-    if (!big) return launch_schur_t<SCHUR_BM_SMALL, SCHUR_BN_SMALL, 2, 2, true, 16, 3, true>(d, b, ctas, mode, 1, 0, s);
-    return launch_schur_h<SCHUR_H_TILE>(d, b, ctas, mode, 1, 0, s);
+    if (big) return launch_schur_h<SCHUR_H_TILE>(d, b, ctas, mode, 1, 0, s);
+    return launch_schur_small(d, b, ctas, mode, 1, 0, s);
 }
 
 // plain C -= A*B with the same main loop (kernel-level test and micro-benchmark of tile configurations)
-template <int BM, int BN, int WARPS_M, int WARPS_N, int BK, int STAGES, int MINB, bool V2 = false>
-__global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, MINB)
+template <int BM, int BN, int WARPS_M, int WARPS_N>
+__global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, 2)
     gemm_sub_kernel(int M, int N, int K, const double *A, int lda, const double *B, int ldb, double *Cm, int ldc)
 {
-    using C = GemmCfg<BM, BN, WARPS_M, WARPS_N, BK, STAGES>;
+    using C = GemmCfg<BM, BN, WARPS_M, WARPS_N>;
     extern __shared__ double sm[];
     const int tiles_m = (M + BM - 1) / BM;
     const int m0 = (blockIdx.x % tiles_m) * BM, n0 = (blockIdx.x / tiles_m) * BN;
@@ -1460,9 +1010,7 @@ __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, MINB)
     for (int mi = 0; mi < C::MI; ++mi)
 #pragma unroll
         for (int ni = 0; ni < C::NI; ++ni) acc[mi][ni][0] = acc[mi][ni][1] = 0.0;
-    if constexpr (V2) gemm_tile_v2<BM, BN, WARPS_M, WARPS_N, BK, STAGES>(A, lda, B, ldb, M, N, K, m0, n0, sm, acc);
-    else
-    gemm_tile<BM, BN, WARPS_M, WARPS_N, BK, STAGES>(A, lda, B, ldb, M, N, K, m0, n0, sm, acc);
+    gemm_tile<BM, BN, WARPS_M, WARPS_N>(A, lda, B, ldb, M, N, K, m0, n0, sm, acc);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int wm0 = m0 + (warp % WARPS_M) * C::WTM, wn0 = n0 + (warp / WARPS_M) * C::WTN;
 #pragma unroll
@@ -1474,20 +1022,20 @@ __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, MINB)
 #pragma unroll
             for (int mi = 0; mi < C::MI; ++mi) {
                 const int i = wm0 + mi * 8 + (lane >> 2);
-                if (i < M) atomicAdd(Cm + (size_t)j * ldc + i, V2 ? flip_sign(acc[mi][ni][e]) : -acc[mi][ni][e]);
+                if (i < M) atomicAdd(Cm + (size_t)j * ldc + i, flip_sign(acc[mi][ni][e]));
             }
         }
 }
 
-template <int BM, int BN, int WARPS_M, int WARPS_N, int BK, int STAGES, int MINB, bool V2 = false>
+template <int BM, int BN, int WARPS_M, int WARPS_N>
 static int launch_gemm_sub_t(int m, int n, int k, const double *a, int lda, const double *b, int ldb, double *c, int ldc,
                              cudaStream_t s)
 {
-    using C = GemmCfg<BM, BN, WARPS_M, WARPS_N, BK, STAGES>;
+    using C = GemmCfg<BM, BN, WARPS_M, WARPS_N>;
     static std::atomic<unsigned long long> attr_0{0};
-    ensure_dyn_smem(gemm_sub_kernel<BM, BN, WARPS_M, WARPS_N, BK, STAGES, MINB, V2>, (int)C::SMEM, attr_0);
+    ensure_dyn_smem(gemm_sub_kernel<BM, BN, WARPS_M, WARPS_N>, (int)C::SMEM, attr_0);
     int64_t ctas = (int64_t)((m + BM - 1) / BM) * ((n + BN - 1) / BN);
-    gemm_sub_kernel<BM, BN, WARPS_M, WARPS_N, BK, STAGES, MINB, V2><<<(unsigned)ctas, C::NT, C::SMEM, s>>>(m, n, k, a, lda, b, ldb, c, ldc);
+    gemm_sub_kernel<BM, BN, WARPS_M, WARPS_N><<<(unsigned)ctas, C::NT, C::SMEM, s>>>(m, n, k, a, lda, b, ldb, c, ldc);
     return 1;
 }
 
@@ -1547,32 +1095,10 @@ int launch_gemm_sub(int m, int n, int k, const double *a, int lda, const double 
     case 32: return launch_gemm_sub_h<128, 128, 2, 4, 16, 4, 1>(m, n, k, a, lda, b, ldb, c, ldc, s);
     case 33: return launch_gemm_sub_h<128, 128, 2, 4, 32, 3, 1>(m, n, k, a, lda, b, ldb, c, ldc, s);
     case 34: return launch_gemm_sub_h<64, 64, 1, 2, 16, 3, 3>(m, n, k, a, lda, b, ldb, c, ldc, s);    // 2 warps, 3 CTAs/SM
-    case 20: return launch_gemm_sub_t<128, 64, 4, 2, 16, 3, 2>(m, n, k, a, lda, b, ldb, c, ldc, s);   // round-1 default loader
-    case 21: return launch_gemm_sub_t<32, 32, 2, 2, 16, 3, 2>(m, n, k, a, lda, b, ldb, c, ldc, s);
-    case 1: return launch_gemm_sub_t<128, 64, 4, 2, 16, 4, 2>(m, n, k, a, lda, b, ldb, c, ldc, s);
-    case 2: return launch_gemm_sub_t<128, 64, 4, 2, 32, 2, 2>(m, n, k, a, lda, b, ldb, c, ldc, s);
-    case 3: return launch_gemm_sub_t<128, 128, 4, 4, 16, 3, 1>(m, n, k, a, lda, b, ldb, c, ldc, s);
-    case 4: return launch_gemm_sub_t<128, 64, 2, 4, 16, 3, 2>(m, n, k, a, lda, b, ldb, c, ldc, s);
-    case 5: return launch_gemm_sub_t<64, 64, 2, 2, 16, 4, 4>(m, n, k, a, lda, b, ldb, c, ldc, s);
-    case 6: return launch_gemm_sub_t<128, 64, 4, 2, 8, 4, 2>(m, n, k, a, lda, b, ldb, c, ldc, s);
-    case 7: return launch_gemm_sub_t<32, 32, 2, 2, 16, 3, 2>(m, n, k, a, lda, b, ldb, c, ldc, s);
-    case 8: return launch_gemm_sub_t<128, 128, 2, 4, 16, 3, 1>(m, n, k, a, lda, b, ldb, c, ldc, s);   // warp tile 64x32
-    case 9: return launch_gemm_sub_t<128, 64, 2, 2, 16, 3, 2>(m, n, k, a, lda, b, ldb, c, ldc, s);    // warp tile 64x32, 4 warps
-    case 10: return launch_gemm_sub_t<256, 64, 4, 2, 16, 3, 1>(m, n, k, a, lda, b, ldb, c, ldc, s);   // warp tile 64x32
-    case 11: return launch_gemm_sub_t<128, 128, 4, 2, 16, 3, 1>(m, n, k, a, lda, b, ldb, c, ldc, s);  // warp tile 32x64
-    case 12: return launch_gemm_sub_t<128, 128, 4, 4, 16, 4, 1>(m, n, k, a, lda, b, ldb, c, ldc, s);  // 16 warps, 4 stages
-    case 13: return launch_gemm_sub_t<128, 128, 2, 4, 32, 2, 1>(m, n, k, a, lda, b, ldb, c, ldc, s);  // 64x32, BK32
-    // 14..: the strength-reduced loader (gemm_tile_v2) on the shapes above -- opt-in until validated on the GPU
-    case 14: return launch_gemm_sub_t<128, 64, 4, 2, 16, 3, 2, true>(m, n, k, a, lda, b, ldb, c, ldc, s);
-    case 15: return launch_gemm_sub_t<128, 64, 4, 2, 32, 2, 2, true>(m, n, k, a, lda, b, ldb, c, ldc, s);
-    case 16: return launch_gemm_sub_t<128, 64, 4, 2, 16, 4, 2, true>(m, n, k, a, lda, b, ldb, c, ldc, s);
-    case 17: return launch_gemm_sub_t<32, 32, 2, 2, 16, 3, 2, true>(m, n, k, a, lda, b, ldb, c, ldc, s);
-    case 18: return launch_gemm_sub_t<128, 128, 4, 2, 16, 3, 1, true>(m, n, k, a, lda, b, ldb, c, ldc, s);  // warp tile 32x64
-    case 19: return launch_gemm_sub_t<128, 128, 4, 4, 16, 3, 1, true>(m, n, k, a, lda, b, ldb, c, ldc, s);
     default: break;
     }
     if (m >= 96 && n >= 96) return launch_gemm_sub_h<SCHUR_H_TILE>(m, n, k, a, lda, b, ldb, c, ldc, s);
-    return launch_gemm_sub_t<32, 32, 2, 2, 16, 3, 2, true>(m, n, k, a, lda, b, ldb, c, ldc, s);
+    return launch_gemm_sub_t<SCHUR_BM_SMALL, SCHUR_BN_SMALL, 2, 2>(m, n, k, a, lda, b, ldb, c, ldc, s);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -538,8 +538,7 @@ static int launch_schur_t(const LU &d, const Batch &b, int64_t ctas, int mode, i
     return 1;
 }
 
-int launch_schur(const DeviceLU &d, const Batch &b, int64_t ctas, int big, int /*atomic*/, int /*variant*/, int mode,
-                 int split_n, int split_i, int /*wide*/, cudaStream_t s)
+int launch_schur(const DeviceLU &d, const Batch &b, int64_t ctas, int big, int mode, int split_n, int split_i, cudaStream_t s)
 {
     if (b.count <= 0 || ctas <= 0) return 0;
     if (big) return launch_schur_t<SCHUR_BM_BIG, SCHUR_BN_TILE, 4, 2>(d, b, ctas, mode, split_n, split_i, s);

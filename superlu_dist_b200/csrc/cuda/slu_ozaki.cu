@@ -34,7 +34,6 @@
 #include "slu_wgmma.cuh"
 
 #include <cstdio>
-#include <cstdlib>
 
 namespace slu {
 namespace oz {
@@ -114,10 +113,6 @@ __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sy
 // register budget of the 384-thread CTA: the producer warpgroup gives back what the accumulators of the consumers need
 __device__ __forceinline__ void producer_regs() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory"); }
 __device__ __forceinline__ void consumer_regs() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory"); }
-__device__ __forceinline__ void consumer_bar_sync()   // the 256 consumer threads only (named barrier 1)
-{
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-}
 
 // shared-memory matrix descriptor, K-major, no swizzle: start >> 4 at [0,14), LBO >> 4 at [16,30) (128 B between the two
 // 16-byte K chunks), SBO >> 4 at [32,46) (256 B between 8-row groups), base offset 0, layout type 0 at [62,64)
@@ -526,19 +521,16 @@ __global__ void __launch_bounds__(128) schur_slice_b_kernel(DeviceLU d, const in
 }
 
 // Destinations of a consumer thread's 2 x NT/4 elements of tile (tm, tn) of supernode nd (column descriptors of the
-// tile in shared memory: sc_*); off = -1: no destination.  excl bit q: exclusive destination, plain load/store.
+// tile in shared memory: sc_*); off = -1: no destination.
 struct Dest {
     long long off[2][OZ_NT / 4];
     double rs[2];
-    unsigned excl;
 };
 template <int NT>
-__device__ __forceinline__ void dest_offsets(const DeviceLU &d, const NodeDesc &nd, int tm, int tn, bool tile_ok, int nonatomic,
-                                             const int *sc_jb, const int *sc_pad, const long long *sc_lbase,
-                                             const long long *sc_lrel, Dest &D)
+__device__ __forceinline__ void dest_offsets(const DeviceLU &d, const NodeDesc &nd, int tm, int tn, bool tile_ok,
+                                             const int *sc_jb, const long long *sc_lbase, const long long *sc_lrel, Dest &D)
 {
     static_assert(NT == OZ_NT, "Dest holds OZ_NT / 4 columns per row");
-    D.excl = 0;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         const int i = tm * TM + tile_row(h);
@@ -556,10 +548,10 @@ __device__ __forceinline__ void dest_offsets(const DeviceLU &d, const NodeDesc &
             if (jb < 0) continue;
             if (ri.ib >= jb) {   // destination in L panel jb: row position of my row there
                 if (sc_lrel[c] != last_off) { last_off = sc_lrel[c]; lpos = d.lrel[last_off + i]; }
-                if (lpos >= 0) { D.off[h][q] = sc_lbase[c] + lpos; if (nonatomic && !sc_pad[c]) D.excl |= 1u << (h * 16 + q); }
+                if (lpos >= 0) D.off[h][q] = sc_lbase[c] + lpos;
             } else {             // destination in U panel ib: packed column position of column j there
                 const int p = d.urel[ri.urel_off + tn * NT + c];
-                if (p >= 0) { D.off[h][q] = ri.ubase + (long long)p * ri.ldu; if (nonatomic && !ri.shared) D.excl |= 1u << (h * 16 + q); }
+                if (p >= 0) D.off[h][q] = ri.ubase + (long long)p * ri.ldu;
             }
         }
     }
@@ -576,21 +568,20 @@ __device__ __forceinline__ void scatter(const DeviceLU &d, const uint32_t *acc, 
             if (o < 0) continue;
             const int c = tile_col(q >> 1, q & 1);
             const double val = flip_sign(combine<S, NT>(acc, 2 * (q >> 1) * 2 + 2 * h + (q & 1), ks) * D.rs[h] * sc_scale[c]);
-            if (D.excl >> (h * 16 + q) & 1) __stcg(d.val + o, __ldcg(d.val + o) + val);
-            else atomicAdd(d.val + o, val);
+            atomicAdd(d.val + o, val);
         }
 }
 template <int NT>
 __device__ __forceinline__ void load_col_desc(const DeviceLU &d, const NodeDesc &nd, int tn, bool tile_ok, int c, int *sc_jb,
-                                              int *sc_pad, long long *sc_lbase, long long *sc_lrel, double *sc_scale)
+                                              long long *sc_lbase, long long *sc_lrel, double *sc_scale)
 {
     const int j = tn * NT + c, mpad = (nd.m + TM - 1) / TM * TM;
     if (tile_ok && j < nd.ncols) {
         const ColInfo cj = d.colinfo[nd.ws_col + j];
-        sc_jb[c] = cj.jb; sc_pad[c] = cj.pad; sc_lbase[c] = cj.lbase; sc_lrel[c] = cj.lrel_off;
+        sc_jb[c] = cj.jb; sc_lbase[c] = cj.lbase; sc_lrel[c] = cj.lrel_off;
         sc_scale[c] = d.oz_scale[nd.ws_ozs + mpad + j];
     } else {
-        sc_jb[c] = -1; sc_pad[c] = 0; sc_lbase[c] = 0; sc_lrel[c] = -1; sc_scale[c] = 0.0;
+        sc_jb[c] = -1; sc_lbase[c] = 0; sc_lrel[c] = -1; sc_scale[c] = 0.0;
     }
 }
 
@@ -599,11 +590,11 @@ __device__ __forceinline__ void load_col_desc(const DeviceLU &d, const NodeDesc 
 // The destination offsets are worked out after the MMAs: held across the k-loop beside the S * NT / 2 accumulators
 // they would spill.  Two consumer warpgroups per SM and the producer's prefetch cover part of that index chase.
 template <int S, int NT, int STAGES, int CL>
-__global__ void __launch_bounds__(THREADS, 1) schur_kernel_tc(DeviceLU d, Batch b, int mode, int split_n, int split_i, int nonatomic)
+__global__ void __launch_bounds__(THREADS, 1) schur_kernel_tc(DeviceLU d, Batch b, int mode, int split_n, int split_i)
 {
     using C = TileCfg<S, NT, STAGES>;
     extern __shared__ uint8_t oz_smem[];
-    __shared__ int sc_jb[NT], sc_pad[NT];
+    __shared__ int sc_jb[NT];
     __shared__ long long sc_lbase[NT], sc_lrel[NT];
     __shared__ double sc_scale[NT];
     constexpr int NTC = NT * CL;
@@ -633,7 +624,7 @@ __global__ void __launch_bounds__(THREADS, 1) schur_kernel_tc(DeviceLU d, Batch 
     const int tn = tnc * CL + cr, tnb = min(tn, tiles_n - 1);   // a column tile past the edge still runs the protocol
     const int KS = (nd.ns + KSTEP - 1) / KSTEP;
     if (threadIdx.x == 0) pipe.init();
-    if (threadIdx.x < NT) load_col_desc<NT>(d, nd, tn, tn < tiles_n, threadIdx.x, sc_jb, sc_pad, sc_lbase, sc_lrel, sc_scale);
+    if (threadIdx.x < NT) load_col_desc<NT>(d, nd, tn, tn < tiles_n, threadIdx.x, sc_jb, sc_lbase, sc_lrel, sc_scale);
     if (CL > 1) cluster_sync_all(); else __syncthreads();   // CL > 1: nobody multicasts before every barrier exists
     if (threadIdx.x >= CONSUMERS) {
         producer_regs();
@@ -644,126 +635,10 @@ __global__ void __launch_bounds__(THREADS, 1) schur_kernel_tc(DeviceLU d, Batch 
         uint32_t acc[C::ACC];
         pipe.mma(KS, 0, acc);
         Dest D;
-        dest_offsets<NT>(d, nd, tm, tn, tn < tiles_n, nonatomic, sc_jb, sc_pad, sc_lbase, sc_lrel, D);
+        dest_offsets<NT>(d, nd, tm, tn, tn < tiles_n, sc_jb, sc_lbase, sc_lrel, D);
         scatter<S, NT>(d, acc, KS, D, sc_scale);
     }
     if (CL > 1) cluster_sync_all();   // peers may still signal my barriers until they are done
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Persistent form of the same tile product: a CTA lives for many tiles (tile t -> CTA t / tiles_per_cta) so that CTA
-// launch and barrier set-up are paid once and the producer warp keeps the bulk-copy ring full ACROSS tiles (the next
-// tile's operands arrive during the current tile's epilogue).  Column descriptors in shared memory are
-// double-buffered by tile parity.
-// ---------------------------------------------------------------------------------------------------------------
-struct TileDesc {     // what the roles need to know about tile gt
-    const int8_t *ga, *gb;
-    int ks, k, tm, tn;
-};
-
-// decode global tile index -> supernode, tile coordinates, operand pointers (same enumeration as schur_kernel_tc, CL = 1)
-template <int S, int NT>
-__device__ __forceinline__ bool decode_tile(const DeviceLU &d, const Batch &b, int mode, int64_t gt, int &slot_cache, TileDesc &t)
-{
-    using C = TileCfg<S, NT, 1>;
-    if (gt >= b.prefix[b.count]) return false;
-    int slot = slot_cache;
-    if (!(slot >= 0 && slot < b.count && b.prefix[slot] <= gt && gt < b.prefix[slot + 1])) slot = find_slot(b.prefix, b.count, gt);
-    slot_cache = slot;
-    const int k = b.nodes[slot];
-    const NodeDesc *nd = d.nodes + k;
-    const int m = nd->m, ns = nd->ns;
-    const int tile = (int)(gt - b.prefix[slot]);
-    const int tiles_m = (m + TM - 1) / TM;
-    int tm, tn;
-    if (mode == 0) {
-        tm = tile % tiles_m; tn = tile / tiles_m;
-    } else {
-        const int tru = (nd->urg_rows + TM - 1) / TM, tcu = (nd->urg_cols + NT - 1) / NT;
-        if (mode == 1) {
-            if (tile < tiles_m * tcu) { tm = tile % tiles_m; tn = tile / tiles_m; }
-            else { const int q = tile - tiles_m * tcu; tm = q % tru; tn = tcu + q / tru; }
-        } else {
-            const int rm = tiles_m - tru;
-            tm = tru + tile % rm; tn = tcu + tile / rm;
-        }
-    }
-    t.k = k; t.tm = tm; t.tn = tn;
-    t.ks = (ns + KSTEP - 1) / KSTEP;
-    t.ga = d.oz_i8 + nd->ws_oza + (size_t)tm * t.ks * C::A_STAGE;
-    t.gb = d.oz_i8 + nd->ws_ozb + (size_t)tn * t.ks * C::B_STAGE;
-    return true;
-}
-
-template <int S, int NT, int STAGES>
-__global__ void __launch_bounds__(THREADS, 1) schur_kernel_tc_persist(DeviceLU d, Batch b, int mode, int split_n, int split_i, int nonatomic,
-                                                                      int tiles_per_cta, long long mine)
-{
-    using C = TileCfg<S, NT, STAGES>;
-    extern __shared__ uint8_t oz_smem[];
-    __shared__ int sc_jb[2][NT], sc_pad[2][NT];
-    __shared__ long long sc_lbase[2][NT], sc_lrel[2][NT];
-    __shared__ double sc_scale[2][NT];
-    const Pipe<S, NT, STAGES, 1> pipe(oz_smem);
-    if (threadIdx.x == 0) pipe.init();
-    __syncthreads();
-    // this rank's tiles are gt = q * split_n + split_i, q < mine (cooperative ancestors); CTA c takes the tiles_per_cta
-    // consecutive q from c * tiles_per_cta.  A CTA lives for a bounded number of tiles so that the kernels of the
-    // high-priority stream (the next level's panel work) still find free SMs quickly -- CTAs are not preempted.
-    const long long q0 = (long long)blockIdx.x * tiles_per_cta, q1 = min(q0 + tiles_per_cta, mine);
-    int slot_cache = -1;
-    uint32_t g = 0;
-    if (threadIdx.x >= CONSUMERS) {
-        producer_regs();
-        if (threadIdx.x == CONSUMERS) {   // ---- producer ----
-            for (long long q = q0; q < q1; ++q) {
-                TileDesc t;
-                if (!decode_tile<S, NT>(d, b, mode, q * split_n + split_i, slot_cache, t)) break;
-                g = pipe.load(t.ga, t.gb, t.ks, g);
-            }
-        }
-        return;
-    }
-    consumer_regs();
-    uint32_t it = 0;
-    for (long long q = q0; q < q1; ++q, ++it) {   // ---- consumers: MMA and epilogue of each tile ----
-        TileDesc t;
-        if (!decode_tile<S, NT>(d, b, mode, q * split_n + split_i, slot_cache, t)) break;
-        const NodeDesc nd = d.nodes[t.k];
-        const int par = it & 1;
-        if (threadIdx.x < NT)
-            load_col_desc<NT>(d, nd, t.tn, true, threadIdx.x, sc_jb[par], sc_pad[par], sc_lbase[par], sc_lrel[par], sc_scale[par]);
-        consumer_bar_sync();
-        uint32_t acc[C::ACC];
-        g = pipe.mma(t.ks, g, acc);
-        Dest D;
-        dest_offsets<NT>(d, nd, t.tm, t.tn, true, nonatomic, sc_jb[par], sc_pad[par], sc_lbase[par], sc_lrel[par], D);
-        scatter<S, NT>(d, acc, t.ks, D, sc_scale[par]);
-    }
-}
-
-template <int S>
-static int launch_schur_tc_persist_t(const DeviceLU &d, const Batch &b, int64_t ctas, int mode, int split_n, int split_i, int nonatomic,
-                                     cudaStream_t s)
-{
-    constexpr int STAGES = 4;
-    using C = TileCfg<S, OZ_NT, STAGES>;
-    static std::atomic<unsigned long long> attr{0};
-    ensure_dyn_smem(schur_kernel_tc_persist<S, OZ_NT, STAGES>, (int)C::SMEM, attr);
-    static int nsm = 0, tmax = 0;
-    if (!nsm) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
-        if (nsm <= 0) nsm = 132;
-        tmax = getenv("SLU_B200_TC_TILES_PER_CTA") ? std::max(1, atoi(getenv("SLU_B200_TC_TILES_PER_CTA"))) : 16;
-    }
-    const long long mine = (ctas + split_n - 1) / split_n;
-    // enough CTAs for ~8 waves over #SMs slots, at most tmax tiles each
-    const int per = (int)std::max<long long>(1, std::min<long long>(tmax, mine / (8LL * nsm)));
-    const long long grid = (mine + per - 1) / per;
-    schur_kernel_tc_persist<S, OZ_NT, STAGES><<<(unsigned)grid, THREADS, C::SMEM, s>>>(d, b, mode, split_n, split_i, nonatomic, per, mine);
-    return 1;
 }
 
 template <int S>
@@ -776,7 +651,7 @@ static int launch_slice_t(const DeviceLU &d, const int32_t *nodes, int count, co
     return 3;
 }
 template <int S>
-static int launch_schur_tc_t(const DeviceLU &d, const Batch &b, int64_t ctas, int mode, int split_n, int split_i, int nonatomic, cudaStream_t s)
+static int launch_schur_tc_t(const DeviceLU &d, const Batch &b, int64_t ctas, int mode, int split_n, int split_i, cudaStream_t s)
 {
     // one CTA per SM (the S * NT / 2 accumulator registers per consumer thread rule out two): a four-deep ring
     constexpr int CL = OZ_CL, STAGES = 4;
@@ -785,11 +660,11 @@ static int launch_schur_tc_t(const DeviceLU &d, const Batch &b, int64_t ctas, in
     ensure_dyn_smem(schur_kernel_tc<S, OZ_NT, STAGES, CL>, (int)C::SMEM, attr);
     const int64_t grid = (ctas + split_n - 1) / split_n * CL;
     if (CL == 1) {
-        schur_kernel_tc<S, OZ_NT, STAGES, CL><<<(unsigned)grid, THREADS, C::SMEM, s>>>(d, b, mode, split_n, split_i, nonatomic);
+        schur_kernel_tc<S, OZ_NT, STAGES, CL><<<(unsigned)grid, THREADS, C::SMEM, s>>>(d, b, mode, split_n, split_i);
     } else {
         DeviceLU dd = d;
         Batch bb = b;
-        void *args[] = {&dd, &bb, &mode, &split_n, &split_i, &nonatomic};
+        void *args[] = {&dd, &bb, &mode, &split_n, &split_i};
         launch_clustered(schur_kernel_tc<S, OZ_NT, STAGES, CL>, dim3((unsigned)grid), THREADS, C::SMEM, CL, s, args);
     }
     return 1;
@@ -808,24 +683,14 @@ int launch_oz_slice(const DeviceLU &d, const int32_t *nodes, int count, const in
     default: return oz::launch_slice_t<7>(d, nodes, count, p_rt, n_rt, p_ak, n_ak, p_b, n_b, s);
     }
 }
-int launch_oz_schur(const DeviceLU &d, const Batch &b, int64_t ctas, int mode, int split_n, int split_i, int S, int nonatomic,
-                    cudaStream_t s)
+int launch_oz_schur(const DeviceLU &d, const Batch &b, int64_t ctas, int mode, int split_n, int split_i, int S, cudaStream_t s)
 {
     if (b.count <= 0 || ctas <= 0) return 0;
-    static const int persist = getenv("SLU_B200_TC_PERSIST") ? atoi(getenv("SLU_B200_TC_PERSIST")) : (OZ_PERSIST_DEFAULT ? 1 : 0);
-    if (persist && OZ_CL == 1) {
-        switch (S) {
-        case 6: return oz::launch_schur_tc_persist_t<6>(d, b, ctas, mode, split_n, split_i, nonatomic, s);
-        case 8: return oz::launch_schur_tc_persist_t<8>(d, b, ctas, mode, split_n, split_i, nonatomic, s);
-        case 7: return oz::launch_schur_tc_persist_t<7>(d, b, ctas, mode, split_n, split_i, nonatomic, s);
-        default: break;
-        }
-    }
     switch (S) {
-    case 5: return oz::launch_schur_tc_t<5>(d, b, ctas, mode, split_n, split_i, nonatomic, s);
-    case 6: return oz::launch_schur_tc_t<6>(d, b, ctas, mode, split_n, split_i, nonatomic, s);
-    case 8: return oz::launch_schur_tc_t<8>(d, b, ctas, mode, split_n, split_i, nonatomic, s);
-    default: return oz::launch_schur_tc_t<7>(d, b, ctas, mode, split_n, split_i, nonatomic, s);
+    case 5: return oz::launch_schur_tc_t<5>(d, b, ctas, mode, split_n, split_i, s);
+    case 6: return oz::launch_schur_tc_t<6>(d, b, ctas, mode, split_n, split_i, s);
+    case 8: return oz::launch_schur_tc_t<8>(d, b, ctas, mode, split_n, split_i, s);
+    default: return oz::launch_schur_tc_t<7>(d, b, ctas, mode, split_n, split_i, s);
     }
 }
 

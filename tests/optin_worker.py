@@ -1,6 +1,6 @@
-"""Child process of tests/test_gpu_variants_complex.py: exercises the opt-in Schur main loop (gemm_tile_v2: running-pointer
-loader + sign flip off the FP64 pipe; schur_variant 4/5, SLU_B200_GEMM_VARIANT 14..19) against NumPy and the oracle.
-Runs in its own process so that a fault in a not-yet-validated kernel cannot poison the CUDA context of the suite."""
+"""Child process of tests/test_gpu_variants_complex.py: the doublecomplex kernels and pzgstrf3d_b200 against NumPy, the
+oracle and the reference's own factors, the pzdrive3d drop-in, and the overlapped upload.  Runs in its own process so
+that a fault in a kernel cannot poison the CUDA context of the suite."""
 import os
 import sys
 
@@ -8,41 +8,6 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-
-
-def gemm_cases():
-    from superlu_dist_b200 import capi
-    shapes = [(1, 1, 1), (7, 5, 3), (33, 31, 17), (128, 64, 16), (128, 64, 48), (256, 128, 33), (130, 257, 100),
-              (384, 192, 256), (95, 400, 30), (513, 129, 37), (640, 320, 15), (512, 512, 416)]
-    for variant in (14, 15, 16, 17, 18, 19):
-        os.environ["SLU_B200_GEMM_VARIANT"] = str(variant)
-        for (m, n, k) in shapes:
-            rng = np.random.default_rng(m * 7 + n * 3 + k)
-            a, b, c = rng.standard_normal((m, k)), rng.standard_normal((k, n)), rng.standard_normal((m, n))
-            out, _ = capi.k_gemm_sub(a, b, c)
-            ref = c - a @ b
-            err = np.abs(out - ref).max()
-            assert err <= 1e-13 * k * max(np.abs(ref).max(), 1), (variant, m, n, k, err)
-    os.environ.pop("SLU_B200_GEMM_VARIANT", None)
-    print("gemm_sub v2 variants ok")
-
-
-def factor_cases():
-    from oracle import oracle
-    from superlu_dist_b200 import capi
-    from util import poisson_problem, rel_err
-    for variant in (4, 5):
-        for kw in (dict(N=12, leaf=8, relax=8, maxsup=32), dict(N=14, leaf=8, relax=16, maxsup=256),
-                   dict(N=6, leaf=4, relax=8, maxsup=200, fem=3)):
-            prob, _ = poisson_problem(**kw)
-            chk, _ = poisson_problem(**kw)
-            info, st = capi.pdgstrf3d(prob, 0, schur_variant=variant)
-            oinfo, oops, _ = oracle.factor(chk)
-            a, b = prob.layers[0], chk.layers[0]
-            err = max(rel_err(a.lval, b.lval), rel_err(a.uval, b.uval))
-            assert info == oinfo == 0 and err < 1e-10, (variant, kw, info, oinfo, err)
-            assert abs(st.ops_fact - oops) <= 1e-9 * oops
-    print("factorization with schur_variant 4/5 ok")
 
 
 def z_kernel_cases():
@@ -140,102 +105,6 @@ def z_dropin_case():
     print("pzdrive3d drop-in ok")
 
 
-def diag_v3_cases(env="SLU_B200_DIAG_V3"):
-    """The Crout/DMMA diagonal-block LU (SLU_B200_DIAG_V3=1) or the 8-CTA cluster LU (SLU_B200_DIAG_CLUSTER=1):
-    kernel-level cases of tests/test_gpu_kernels.py plus whole factorizations against the oracle."""
-    os.environ[env] = "1"      # read once per process by launch_diag_lu
-    from oracle import oracle
-    from superlu_dist_b200 import capi
-    from util import poisson_problem, rel_err
-
-    def lu_nopivot(a):
-        a = a.copy()
-        n = a.shape[1]
-        for j in range(n - 1):
-            if a[j, j] != 0:
-                a[j + 1:n, j] /= a[j, j]
-            a[j + 1:n, j + 1:] -= np.outer(a[j + 1:n, j], a[j, j + 1:])
-        return a
-
-    for ns, extra in [(1, 0), (5, 3), (16, 0), (17, 40), (33, 7), (48, 0), (65, 2), (96, 0), (100, 1), (129, 30), (200, 0),
-                      (240, 5), (255, 1), (256, 19)]:
-        rng = np.random.default_rng(ns)
-        a = rng.standard_normal((ns + extra, ns))
-        a[:ns] += ns * np.eye(ns)
-        ref = a.copy()
-        ref[:ns] = lu_nopivot(a[:ns])
-        out, info, tiny = capi.k_diag_lu(a)
-        assert info == 0 and tiny == 0
-        assert np.abs(out - ref).max() <= 1e-12 * ns * np.abs(ref).max(), (env, ns, extra, np.abs(out - ref).max())
-    # tiny / zero pivots inside a wide block (cluster path: ns >= 65)
-    a = rng.standard_normal((100, 100)) + 100 * np.eye(100)
-    a[70, 70] = 1e-30
-    a[:70, 70] = 0.0
-    a[70, :70] = 0.0
-    out, info, tiny = capi.k_diag_lu(a.copy(), replace_tiny=1, thresh=1e-3)
-    bb = a.copy()
-    bb[70, 70] = 1e-3
-    assert tiny >= 1 and info == 0 and np.abs(out - lu_nopivot(bb)).max() <= 1e-9 * np.abs(lu_nopivot(bb)).max()
-    a = rng.standard_normal((90, 90)) + 90 * np.eye(90)
-    a[:, 40] = 0.0
-    a[40, :] = 0.0
-    out, info, tiny = capi.k_diag_lu(a.copy(), col0=1000)
-    assert info == 1041, info
-    rng = np.random.default_rng(3)
-    a = rng.standard_normal((40, 40)) + 40 * np.eye(40)
-    a[0, 0] = 1e-30
-    out, info, tiny = capi.k_diag_lu(a.copy(), replace_tiny=1, thresh=1e-3)
-    b = a.copy()
-    b[0, 0] = 1e-3
-    assert tiny >= 1 and info == 0 and np.abs(out - lu_nopivot(b)).max() <= 1e-9 * np.abs(lu_nopivot(b)).max()
-    a = rng.standard_normal((8, 8)) + 8 * np.eye(8)
-    a[:, 0] = 0.0
-    out, info, tiny = capi.k_diag_lu(a.copy(), col0=100)
-    assert info == 101
-    for kw in (dict(N=12, leaf=8, relax=8, maxsup=32), dict(N=14, leaf=8, relax=16, maxsup=256),
-               dict(N=6, leaf=4, relax=8, maxsup=200, fem=3)):
-        prob, _ = poisson_problem(**kw)
-        chk, _ = poisson_problem(**kw)
-        info, st = capi.pdgstrf3d(prob, 0)
-        oinfo, oops, _ = oracle.factor(chk)
-        a, b = prob.layers[0], chk.layers[0]
-        err = max(rel_err(a.lval, b.lval), rel_err(a.uval, b.uval))
-        assert info == oinfo == 0 and err < 1e-10, (kw, info, oinfo, err)
-    print("diag LU v3 ok")
-
-
-def trsm_rl_cases():
-    """The right-looking register-blocked panel solve (SLU_B200_TRSM_RL=1): kernel-level cases against SciPy plus whole
-    factorizations against the oracle."""
-    os.environ["SLU_B200_TRSM_RL"] = "1"
-    import scipy.linalg as sl
-    from oracle import oracle
-    from superlu_dist_b200 import capi
-    from util import poisson_problem, rel_err
-    for ns, m in [(1, 1), (7, 3), (16, 64), (31, 65), (33, 64), (64, 200), (100, 63), (129, 130), (200, 70), (255, 129), (256, 130)]:
-        rng = np.random.default_rng(ns * 1000 + m)
-        lu = rng.standard_normal((ns, ns)) + ns * np.eye(ns)
-        x = rng.standard_normal((m, ns))
-        ref = sl.solve_triangular(np.triu(lu), x.T, trans="T", lower=False).T
-        out = capi.k_trsm(lu, x, ucase=False)
-        assert np.abs(out - ref).max() <= 1e-12 * ns * max(np.abs(ref).max(), 1), ("trsm_l rl", ns, m, np.abs(out - ref).max())
-        lu = rng.standard_normal((ns, ns)) / ns + np.eye(ns)
-        x = rng.standard_normal((ns, m))
-        ref = sl.solve_triangular(np.tril(lu, -1) + np.eye(ns), x, lower=True, unit_diagonal=True)
-        out = capi.k_trsm(lu, x, ucase=True)
-        assert np.abs(out - ref).max() <= 1e-12 * ns * max(np.abs(ref).max(), 1), ("trsm_u rl", ns, m, np.abs(out - ref).max())
-    for kw in (dict(N=12, leaf=8, relax=8, maxsup=32), dict(N=14, leaf=8, relax=16, maxsup=256),
-               dict(N=6, leaf=4, relax=8, maxsup=200, fem=3)):
-        prob, _ = poisson_problem(**kw)
-        chk, _ = poisson_problem(**kw)
-        info, st = capi.pdgstrf3d(prob, 0)
-        oinfo, oops, _ = oracle.factor(chk)
-        a, b = prob.layers[0], chk.layers[0]
-        err = max(rel_err(a.lval, b.lval), rel_err(a.uval, b.uval))
-        assert info == oinfo == 0 and err < 1e-10, (kw, info, oinfo, err)
-    print("right-looking TRSM ok")
-
-
 def overlap_h2d_cases():
     """slu_b200_factor_host with options.reserved[3]: zeroed arena, staged atomic-add upload per level, factorization
     and download all overlapped -- against the oracle, and against the plain path on the same matrix."""
@@ -265,20 +134,10 @@ def overlap_h2d_cases():
 
 if __name__ == "__main__":
     what = sys.argv[1] if len(sys.argv) > 1 else "all"
-    if what in ("gemm", "all"):
-        gemm_cases()
-    if what in ("factor", "all"):
-        factor_cases()
     if what in ("zkernels", "all"):
         z_kernel_cases()
     if what in ("zfactor", "all"):
         z_factor_cases()
-    if what == "diagv3":           # its own process: the switch is an environment variable read once
-        diag_v3_cases()
-    if what == "trsmrl":
-        trsm_rl_cases()
-    if what == "diagcluster":
-        diag_v3_cases("SLU_B200_DIAG_CLUSTER")
     if what in ("zdropin", "all"):
         z_dropin_case()
     if what in ("h2d", "all"):

@@ -60,6 +60,8 @@ def test_plan_matches_oracle_accounting(kw, cplx):
         assert abs(st.ops_fact - oops) <= 1e-12 * oops
         assert st.lu_device_bytes == (st.nnz_l + st.nnz_u) * (16 if cplx else 8)
         assert st.nnz_l == int(prob.lval_len.sum()) and st.my_supernodes == prob.nsupers and st.nlevels >= 1
+    with pytest.raises(RuntimeError, match="schur_variant is retired and must be 0"):
+        capi.plan(prob, 0, schur_variant=4)
 
 
 def test_plan_supernode_width_limits():

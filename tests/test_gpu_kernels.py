@@ -21,8 +21,10 @@ def lu_nopivot(a):
     return a
 
 
-@pytest.mark.parametrize("ns,extra", [(1, 0), (5, 3), (16, 0), (17, 40), (33, 7), (100, 1), (256, 19), (300, 0)])
+@pytest.mark.parametrize("ns,extra", [(1, 0), (5, 3), (16, 0), (17, 40), (33, 7), (48, 0), (65, 2), (96, 0), (100, 1),
+                                      (129, 30), (200, 0), (240, 5), (255, 1), (256, 19), (300, 0)])
 def test_diag_lu(ns, extra):
+    """Blocks of 65..256 columns take the 8-CTA cluster kernel, the others the one-CTA kernel."""
     rng = np.random.default_rng(ns)
     a = rng.standard_normal((ns + extra, ns))
     a[:ns] += ns * np.eye(ns)
@@ -46,6 +48,21 @@ def test_diag_lu_tiny_and_zero_pivot():
     a[:, 0] = 0.0   # exact zero pivot at column 0 (and it stays zero)
     out, info, tiny = capi.k_diag_lu(a.copy(), col0=100)
     assert info == 101  # 1-based global column, pdgstrf2.c:568-571
+    # the same inside a block wide enough for the cluster kernel (ns >= 65), past its first 32-column slab
+    a = rng.standard_normal((100, 100)) + 100 * np.eye(100)
+    a[70, 70] = 1e-30
+    a[:70, 70] = 0.0
+    a[70, :70] = 0.0
+    out, info, tiny = capi.k_diag_lu(a.copy(), replace_tiny=1, thresh=1e-3)
+    b = a.copy()
+    b[70, 70] = 1e-3
+    assert tiny >= 1 and info == 0
+    assert np.abs(out - lu_nopivot(b)).max() <= 1e-9 * np.abs(lu_nopivot(b)).max()
+    a = rng.standard_normal((90, 90)) + 90 * np.eye(90)
+    a[:, 40] = 0.0
+    a[40, :] = 0.0
+    out, info, tiny = capi.k_diag_lu(a.copy(), col0=1000)
+    assert info == 1041
 
 
 @pytest.mark.parametrize("ns,m", [(1, 1), (7, 3), (16, 64), (31, 65), (64, 200), (256, 130), (300, 70)])

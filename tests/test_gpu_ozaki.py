@@ -95,25 +95,3 @@ def test_tcgen05_default_off_and_opt_in_residual():
     info, st = capi.pdgstrf3d(prob2, 0, tc_slices=7)
     assert info == 0 and st.reserved[1] > 0.5 * st.ops_schur and int(st.reserved[3]) == 7   # on: most of the flops
     assert residual_probe(prob2, [(pre, every)], [(prob2.layers[0], every)]) < 1e-12
-
-
-def test_persistent_kernel_matches_opt_in():
-    """The persistent warp-specialised form of the kernel (SLU_B200_TC_PERSIST=1, read once per process: child), with
-    the int8 path opted in (7 slices)."""
-    code = f'''
-import os, sys
-os.environ["SLU_B200_TC_PERSIST"] = "1"
-sys.path.insert(0, {os.path.dirname(HERE)!r}); sys.path.insert(0, {HERE!r})
-from oracle import oracle
-from superlu_dist_b200 import capi
-from util import poisson_problem, rel_err
-for kw in (dict(N=14, leaf=8, relax=16, maxsup=256), dict(N=18, leaf=16, relax=32, maxsup=256)):
-    prob, _ = poisson_problem(**kw); chk, _ = poisson_problem(**kw)
-    info, st = capi.pdgstrf3d(prob, 0, tc_slices=7, tc_min_ns=64)
-    oracle.factor(chk)
-    assert info == 0 and st.reserved[1] > 0
-    assert rel_err(prob.layers[0].lval, chk.layers[0].lval) < 1e-10 and rel_err(prob.layers[0].uval, chk.layers[0].uval) < 1e-10
-print("ok")
-'''
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0 and "ok" in r.stdout, (r.stdout[-1500:], r.stderr[-3000:])

@@ -28,7 +28,8 @@ def test_matches_reference_factors(name):
 
 
 @pytest.mark.parametrize("N,leaf,relax,maxsup,fem", [(6, 4, 4, 8, None), (10, 8, 8, 32, None), (16, 32, 16, 64, None),
-                                                      (18, 16, 32, 256, None), (6, 8, 12, 48, 3), (12, 64, 1, 4, None)])
+                                                      (18, 16, 32, 256, None), (6, 8, 12, 48, 3), (12, 64, 1, 4, None),
+                                                      (12, 8, 8, 32, None), (14, 8, 16, 256, None), (6, 4, 8, 200, 3)])
 def test_matches_oracle_on_generated(N, leaf, relax, maxsup, fem):
     prob, _ = poisson_problem(N, leaf, relax, maxsup, fem=fem)
     chk, _ = poisson_problem(N, leaf, relax, maxsup, fem=fem)
@@ -91,6 +92,13 @@ def test_factor_host_on_unsymmetric_pattern(name):
     info, st = capi.pdgstrf3d(prob, 0, pipeline=1, overlap_h2d=1)
     assert info == int(post["info"][0])
     assert rel_err(prob.layers[0].lval, ref.lval) < TOL and rel_err(prob.layers[0].uval, ref.uval) < TOL
+
+
+def test_retired_schur_variant_is_refused():
+    """options.schur_variant once selected other Schur tile kernels; the field keeps its place in the struct and must be 0."""
+    prob, _ = poisson_problem(N=6, leaf=4, relax=8, maxsup=32)
+    with pytest.raises(RuntimeError, match="schur_variant is retired and must be 0"):
+        capi.Handle(prob, 0, schur_variant=4)
 
 
 @pytest.mark.parametrize("kw", [dict(N=10, leaf=8, relax=8, maxsup=32), dict(N=16, leaf=16, relax=32, maxsup=256),
