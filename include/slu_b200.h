@@ -195,8 +195,8 @@ int slu_b200_gscon(slu_b200_handle_t h, char norm, double anorm, double *rcond);
  * same factors give bit-identical H); the factors are only read.  A^-1(i, j) = H(perm[j], perm[i]): the entries of A^-1 on
  * the pattern of A^T, and of A where A is structurally symmetric.  Where tiny pivots were replaced the result describes
  * L U as factored, as for slu_b200_gscon.  If the second arena does not fit, the call fails and the handle stays usable for
- * solves.  Restrictions (all fail with a message): a successful factorization (info = 0), an unbatched handle, a 1 x 1 x 1
- * grid (world_size 1).  Doublecomplex through slu_b200_z_selinv below; the reference's pdgssvx3d has no selected inversion.
+ * solves.  Restrictions (all fail with a message): a successful factorization (info = 0), an unbatched handle (batched
+ * handles: slu_b200_batch_selinv below), a 1 x 1 x 1 grid (world_size 1).  Doublecomplex through slu_b200_z_selinv below; the reference's pdgssvx3d has no selected inversion.
  * out (may be NULL): [0] seconds, [1] flops (accounting in DESIGN.md), [2] kernel launches, [3] HBM bytes it holds. */
 int slu_b200_selinv(slu_b200_handle_t h, double out[4]);
 /* out[p] = (A^-1)(i, colind[p]) for every entry p of row i of the CSR pattern; A = P^T F P, perm[old] = new as in
@@ -257,8 +257,9 @@ int slu_b200_k_rerun_schur(slu_b200_handle_t h, int level, int reps, float *ms);
  * exactly as many kernel launches as one unbatched factorization, each over batch x the CTAs (gridDim.y = member).
  * Double precision here and doublecomplex through the slu_b200_z_batch_* twins below; 1 x 1 x 1 grid, FP64 DMMA
  * kernels only (the int8 path is not used; stats.reserved[1] = 0).
- * A batched handle takes only these calls plus slu_b200_get_stats and slu_b200_destroy; every other call on it fails,
- * and these fail on an unbatched handle.  Stats describe the whole handle: ops_fact, ops_schur, nnz_l, nnz_u and
+ * A batched handle takes only these calls (create, fill_csr, factor, solve, solve_trans, gscon, selinv, selinv_get,
+ * logdet and download, each with the batch_ prefix) plus slu_b200_get_stats and slu_b200_destroy; every other call on it
+ * fails, and these fail on an unbatched handle.  Stats describe the whole handle: ops_fact, ops_schur, nnz_l, nnz_u and
  * lu_device_bytes are batch x the per-member values, tiny_pivots is summed over the members, t_factor_s is the device
  * time of the one batched call, stats.reserved[4] / [5] describe the last slu_b200_batch_solve or _batch_solve_trans.
  * Measured on an NVIDIA H100 80GB HBM3 at a 400 W power limit, per member, against one unbatched handle looping over
@@ -285,6 +286,21 @@ int slu_b200_batch_solve_trans(slu_b200_handle_t h, double *x, int ldx, int nrhs
 int slu_b200_batch_gscon(slu_b200_handle_t h, char norm, const double *anorm, double *rcond);
 /* write member j's L/U into the view's Lnzval / Unzval arrays, in the reference layout (as slu_b200_download) */
 int slu_b200_batch_download(slu_b200_handle_t h, int member);
+/* Selected inversion of every member, as slu_b200_selinv: H_j = F_j^-T on the stored pattern of L+U, into a second HBM
+ * arena of batch x one member's factors (allocated on first use, freed by destroy).  One sweep over the level plan for all
+ * members: out[2] (kernel launches) equals an unbatched sweep's whatever the batch (7 per level, 6 at the root), each
+ * launch over batch x the CTAs.  out[1] = batch x the per-member flops; out[0] and out[3] as slu_b200_selinv.
+ * Deterministic, factors only read.  If the second arena does not fit, the call fails with its size and the handle stays
+ * usable for batch_solve / batch_gscon.  Fails, naming the member, unless every member's last info was 0. */
+int slu_b200_batch_selinv(slu_b200_handle_t h, double out[4]);
+/* as slu_b200_selinv_get for every member, one CSR pattern and perm shared: out holds batch x nnz values, member-major
+ * (member j's at out + j*nnz).  Needs slu_b200_batch_selinv on the current factors (a later batch_fill_csr or batch_factor
+ * invalidates it); an entry with no slot fails with the count of one member, as the unbatched call. */
+int slu_b200_batch_selinv_get(slu_b200_handle_t h, int n, const int32_t *rowptr, const int32_t *colind,
+                              const int32_t *perm, double *out);
+/* logabs[batch], sign[batch]: every member's log|det A_j| and sign, as slu_b200_logdet (needs no batch_selinv).  Fails,
+ * naming the member, unless every member's last info was 0. */
+int slu_b200_batch_logdet(slu_b200_handle_t h, double *logabs, double *sign);
 /* ---- doublecomplex twins (SRC/complex16/pzgstrf3d.c:120; the reference's z* handle API,
  * SRC/include/superlu_upacked.h:84-97).  Same view/options/stats structs: the Lnzval_bc_ptr / Unzval_br_ptr
  * entries point at arrays of doublecomplex {double r, i} (SRC/include/dcomplex.h:30) and are declared double*
@@ -335,6 +351,13 @@ int slu_b200_z_batch_solve(slu_b200_zhandle_t h, double *x, int ldx, int nrhs);
 int slu_b200_z_batch_solve_trans(slu_b200_zhandle_t h, double *x, int ldx, int nrhs, int trans);
 int slu_b200_z_batch_gscon(slu_b200_zhandle_t h, char norm, const double *anorm, double *rcond);
 int slu_b200_z_batch_download(slu_b200_zhandle_t h, int member);
+/* as slu_b200_batch_selinv / _batch_selinv_get / _batch_logdet, with the z conventions of slu_b200_z_selinv: out of
+ * z_batch_selinv_get holds batch x nnz interleaved doublecomplex, member-major; z_batch_logdet's sign holds 2 x batch
+ * doubles, exp(i theta_j) as (re, im) pairs. */
+int slu_b200_z_batch_selinv(slu_b200_zhandle_t h, double out[4]);
+int slu_b200_z_batch_selinv_get(slu_b200_zhandle_t h, int n, const int32_t *rowptr, const int32_t *colind,
+                                const int32_t *perm, double *out);
+int slu_b200_z_batch_logdet(slu_b200_zhandle_t h, double *logabs, double *sign);
 int slu_b200_z_get_stats(slu_b200_zhandle_t h, slu_b200_stats_t *out);
 int slu_b200_z_plan(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, slu_b200_stats_t *stats);
 void slu_b200_z_destroy(slu_b200_zhandle_t h);

@@ -124,6 +124,12 @@ def lib():
         getattr(L, f).argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     for f in ("slu_b200_logdet", "slu_b200_z_logdet"):
         getattr(L, f).argtypes = [C.c_void_p, C.POINTER(C.c_double), C.c_void_p]
+    for f in ("slu_b200_batch_selinv", "slu_b200_z_batch_selinv"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_void_p]
+    for f in ("slu_b200_batch_selinv_get", "slu_b200_z_batch_selinv_get"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    for f in ("slu_b200_batch_logdet", "slu_b200_z_batch_logdet"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     _lib = L
     return L
 
@@ -439,6 +445,39 @@ class BatchHandle:
         out = np.zeros(self.batch, np.float64)
         _check(_fn("batch_gscon", self.z_)(self.h, _norm_byte(norm), a.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p)))
         return out
+
+    def selinv(self):
+        """Selected inversion of every member (slu_b200_batch_selinv / slu_b200_z_batch_selinv), as Handle.selinv, kept in
+        HBM for inv_entries / inv_diag.  -> (seconds, flops of all members, kernel launches, HBM bytes held); the launches
+        are those of one unbatched sweep whatever the batch."""
+        out = (C.c_double * 4)()
+        _check(_fn("batch_selinv", self.z_)(self.h, out))
+        return tuple(out)
+
+    def inv_entries(self, rowptr, colind, perm):
+        """(A_j^-1)(i, colind[p]) for every member j and every entry p of row i of one CSR pattern
+        (slu_b200_batch_selinv_get), perm[old] = new as in fill_csr.  -> float64 (complex128) array (batch, nnz)"""
+        rp = np.ascontiguousarray(rowptr, np.int32)
+        ci = np.ascontiguousarray(colind, np.int32)
+        pm = np.ascontiguousarray(perm, np.int32)
+        out = np.empty((self.batch, len(ci)), self._dtype())
+        _check(_fn("batch_selinv_get", self.z_)(self.h, len(rp) - 1, rp.ctypes.data_as(C.c_void_p), ci.ctypes.data_as(C.c_void_p),
+                                                pm.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p)))
+        return out
+
+    def inv_diag(self, perm=None):
+        """The diagonal of every member's A_j^-1 (perm as Handle.inv_diag).  -> (batch, n)"""
+        n = self.prob.n
+        pm = np.arange(n, dtype=np.int32) if perm is None else perm
+        return self.inv_entries(np.arange(n + 1, dtype=np.int32), np.arange(n, dtype=np.int32), pm)
+
+    def logdet(self):
+        """(sign, log |det A_j|) of every member (slu_b200_batch_logdet), as numpy.linalg.slogdet of a stack: sign (batch,)
+        float64 of +-1, or complex128 of modulus 1 for a complex problem; logabs (batch,) float64"""
+        la = np.zeros(self.batch, np.float64)
+        sg = np.zeros(self.batch, np.complex128 if self.z_ else np.float64)
+        _check(_fn("batch_logdet", self.z_)(self.h, la.ctypes.data_as(C.c_void_p), sg.ctypes.data_as(C.c_void_p)))
+        return sg, la
 
     def download(self, member):
         """Member `member`'s L and U into prob.layers[0] (the reference layout)."""

@@ -49,6 +49,9 @@
 #define slu_b200_selinv slu_b200_z_selinv
 #define slu_b200_selinv_get slu_b200_z_selinv_get
 #define slu_b200_logdet slu_b200_z_logdet
+#define slu_b200_batch_selinv slu_b200_z_batch_selinv
+#define slu_b200_batch_selinv_get slu_b200_z_batch_selinv_get
+#define slu_b200_batch_logdet slu_b200_z_batch_logdet
 #define SLU_API "slu_b200_z_"     // name prefix of the exported calls, for error messages
 #else
 #define SLU_API "slu_b200_"
@@ -1945,32 +1948,34 @@ static int selinv_plan(slu_b200_handle_s *H)
     return H->d_si_pool.upload(pool);
 }
 
-int slu_b200_selinv(slu_b200_handle_t H, double out[4])
+// The sweep on device LU d (H->dev, or H->bdev for every member of a batched handle: the same launches with gridDim.y =
+// members).  The destination maps are value-independent and built on H->dev for all members, as in slu_b200_batch_factor.
+// fn names the call in the messages.
+}  // extern "C"
+template <class LU>
+static int selinv_sweep(slu_b200_handle_t H, const LU &d, int members, const char *fn, double out[4])
 {
-    if (!H) return fail("null handle");
-    if (selinv_refuse(H, SLU_API "selinv")) return -1;
     H->si_ready = false;
     if (H->si_levels.empty() && selinv_plan(H)) return -1;
-    if (!H->d_hinv.p && H->d_hinv.alloc((size_t)H->member_len)) {
+    if (!H->d_hinv.p && H->d_hinv.alloc((size_t)H->member_len * members)) {
         cudaGetLastError();
         std::string why = g_err;
         H->d_hinv.release();
-        return fail(SLU_API "selinv: the inverse needs a second arena of %.2f GB beside the factors, which does not fit (%s); "
-                    "the factors are unchanged", 1e-9 * sizeof(val_t) * H->member_len, why.c_str());
+        return fail("%s: the inverse needs a second arena of %.2f GB beside the factors, which does not fit (%s); "
+                    "the factors are unchanged", fn, 1e-9 * sizeof(val_t) * H->member_len * members, why.c_str());
     }
     cudaStream_t s = H->stream;
-    const DeviceLU &d = H->dev;
     const int64_t *p64 = H->d_pool_i64.p, *sp = H->d_si_pool.p;
     val_t *hv = H->d_hinv.p;
     double flops = 0;
     int launches = 0;
     const double t0 = now_s();
-    CU(cudaMemsetAsync(H->d_flags.p + 1, 0, sizeof(int), s));
+    CU(cudaMemsetAsync(H->dev.err, 0, sizeof(int), s));
     for (size_t li = H->levels.size(); li-- > 0;) {
         const LevelPlan &L = H->levels[li];
         const SelinvLevel &S = H->si_levels[li];
         const int32_t *nodes = H->d_pool_i32.p + L.nodes_off;
-        launches += launch_schur_setup(d, Batch{nodes, p64 + L.setup_prefix, L.count}, L.setup_ctas, s);
+        launches += launch_schur_setup(H->dev, Batch{nodes, p64 + L.setup_prefix, L.count}, L.setup_ctas, s);
         launches += launch_diag_inv(d, Batch{nodes, p64 + L.inv_prefix, L.count}, L.inv_ctas, H->d_inv.p, s);
         for (int q = 0; q < 3; ++q) launches += launch_selinv_gemm(d, Batch{nodes, sp + S.gemm_prefix[q], L.count}, S.gemm_ctas[q], q, hv, s);
         for (int q = 0; q < 2; ++q)
@@ -1984,18 +1989,26 @@ int slu_b200_selinv(slu_b200_handle_t H, double out[4])
         }
     }
     int bad = 0;
-    CU(cudaMemcpyAsync(&bad, H->d_flags.p + 1, sizeof(int), cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&bad, H->dev.err, sizeof(int), cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     CU(cudaGetLastError());
-    if (bad) return fail(SLU_API "selinv: %d Schur-update destinations were not found in the L/U structure", bad);
+    if (bad) return fail("%s: %d Schur-update destinations were not found in the L/U structure", fn, bad);
     H->si_ready = true;
     if (out) {
         out[0] = now_s() - t0;
-        out[1] = flops;
+        out[1] = flops * members;
         out[2] = (double)launches;
         out[3] = (double)(H->d_hinv.bytes() + H->d_si_pool.bytes());
     }
     return 0;
+}
+extern "C" {
+
+int slu_b200_selinv(slu_b200_handle_t H, double out[4])
+{
+    if (!H) return fail("null handle");
+    if (selinv_refuse(H, SLU_API "selinv")) return -1;
+    return selinv_sweep(H, H->dev, 1, SLU_API "selinv", out);
 }
 
 int slu_b200_selinv_get(slu_b200_handle_t H, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm, double *out)
@@ -2089,6 +2102,7 @@ int slu_b200_batch_fill_csr(slu_b200_handle_t H, int n, const int32_t *rowptr, c
     CU(cudaMemcpyAsync(dci.p, colind, (size_t)nnz * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(dv.p, val, (size_t)nnz * B * sizeof(val_t), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(dperm.p, perm, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    H->si_ready = false;
     CU(cudaMemsetAsync(H->val.p, 0, H->val.bytes(), s));
     CU(cudaMemsetAsync(err, 0, sizeof(int), s));
     launch_fill_csr(H->bdev, n, drp.p, dci.p, dv.p, dperm.p, dact.p, err, s);
@@ -2110,6 +2124,7 @@ int slu_b200_batch_factor(slu_b200_handle_t H, int *info)
     if (!H || !info) return fail("null argument");
     if (refuse_unbatched(H, SLU_API "batch_factor")) return -1;
     if (!H->uploaded) return fail(SLU_API "batch_factor before " SLU_API "batch_fill_csr");
+    H->si_ready = false;
     const int B = H->batch;
     cudaStream_t s = H->stream, s2 = H->stream2;
     const BatchedLU &d = H->bdev;
@@ -2326,6 +2341,82 @@ int slu_b200_batch_download(slu_b200_handle_t H, int member)
     double t0 = now_s();
     if (transfer(H, false, member)) return -1;
     H->st.t_download_s = now_s() - t0;
+    return 0;
+}
+
+// ---- selected inversion and log-determinants on batched handles: selinv_sweep over H->bdev, so the sweep makes exactly the
+// launches of one unbatched sweep, each over every member (gridDim.y = member).  The H arena holds `batch` member arenas,
+// member_len elements apart as the members' factors are.
+static int batch_selinv_refuse(const slu_b200_handle_s *H, const char *fn)
+{
+    if (refuse_unbatched(H, fn)) return -1;
+    for (int j = 0; j < H->batch; ++j) {
+        if (H->member_info[j] < 0) return fail("%s needs a " SLU_API "batch_factor of the filled members first", fn);
+        if (H->member_info[j] > 0) return fail("%s: member %d has an exact zero pivot in column %d", fn, j, H->member_info[j]);
+    }
+    return 0;
+}
+
+int slu_b200_batch_selinv(slu_b200_handle_t H, double out[4])
+{
+    if (!H) return fail("null handle");
+    if (batch_selinv_refuse(H, SLU_API "batch_selinv")) return -1;
+    return selinv_sweep(H, H->bdev, H->batch, SLU_API "batch_selinv", out);
+}
+
+// out: batch x nnz values, member j's at out + j * nnz
+int slu_b200_batch_selinv_get(slu_b200_handle_t H, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm,
+                              double *out)
+{
+    if (!H || !rowptr || !colind || !perm || !out) return fail("null argument");
+    if (batch_selinv_refuse(H, SLU_API "batch_selinv_get")) return -1;
+    if (!H->si_ready)
+        return fail(SLU_API "batch_selinv_get needs " SLU_API "batch_selinv on the current factors first (a later batch_fill_csr or "
+                    "batch_factor invalidates it)");
+    if (n != H->n) return fail(SLU_API "batch_selinv_get: matrix order %d does not match the handle's %d", n, H->n);
+    const int64_t nnz = rowptr[n];
+    if (rowptr[0] != 0 || nnz < 0) return fail(SLU_API "batch_selinv_get: bad rowptr");
+    const int B = H->batch;
+    DevBuf<int32_t> drp, dci, dperm;
+    DevBuf<val_t> dout;
+    if (drp.alloc((size_t)n + 1) || dci.alloc((size_t)nnz) || dperm.alloc((size_t)n) || dout.alloc((size_t)nnz * B)) return -1;
+    cudaStream_t s = H->stream;
+    CU(cudaMemcpyAsync(drp.p, rowptr, ((size_t)n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(dci.p, colind, (size_t)nnz * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(dperm.p, perm, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemsetAsync(H->dev.err, 0, sizeof(int), s));
+    launch_selinv_get(H->bdev, H->d_hinv.p, n, drp.p, dci.p, dperm.p, dout.p, H->dev.err, s);
+    int bad = 0;
+    CU(cudaMemcpyAsync(out, dout.p, (size_t)nnz * B * sizeof(val_t), cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&bad, H->dev.err, sizeof(int), cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    if (bad) return fail(SLU_API "batch_selinv_get: %d entries have no slot in the L/U structure (A^-1 is known on the pattern of L+U only)", bad);
+    return 0;
+}
+
+// logabs[batch]; sign[batch] (double) or sign[2 * batch] = exp(i theta_j) as (re, im) pairs (doublecomplex)
+int slu_b200_batch_logdet(slu_b200_handle_t H, double *logabs, double *sign)
+{
+    if (!H || !logabs || !sign) return fail("null argument");
+    if (batch_selinv_refuse(H, SLU_API "batch_logdet")) return -1;
+    const int B = H->batch;
+    const int count = (int)H->znodes[0].size();
+    const int nparts = (count + SELINV_VECS - 1) / SELINV_VECS;
+    DevBuf<double> part, res;
+    DevBuf<phase_t> ph;
+    if (part.alloc((size_t)nparts * B) || ph.alloc((size_t)nparts * B) || res.alloc((size_t)(1 + VAL_DOUBLES) * B)) return -1;
+    cudaStream_t s = H->stream;
+    launch_selinv_logdet(H->bdev, H->d_pool_i32.p + H->z_nodes_off[0], count, part.p, ph.p, res.p, s);
+    std::vector<double> r((size_t)(1 + VAL_DOUBLES) * B, 0.0);
+    for (int j = 0; j < B; ++j) r[(size_t)j * (1 + VAL_DOUBLES) + 1] = 1.0;   // no supernode: log |det| 0, sign 1
+    if (nparts > 0) CU(cudaMemcpyAsync(r.data(), res.p, r.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    for (int j = 0; j < B; ++j) {
+        logabs[j] = r[(size_t)j * (1 + VAL_DOUBLES)];
+        for (int c = 0; c < VAL_DOUBLES; ++c) sign[(size_t)j * VAL_DOUBLES + c] = r[(size_t)j * (1 + VAL_DOUBLES) + 1 + c];
+    }
     return 0;
 }
 

@@ -254,6 +254,15 @@ int launch_selinv_logdet(const DeviceLU &d, const int32_t *nodes, int count, dou
 // out[p] = H(perm[colind[p]], perm[i]) for the entries p of row i; *err counts entries without a slot (out = NaN there)
 int launch_selinv_get(const DeviceLU &d, const val_t *hv, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm,
                       val_t *out, int *err, cudaStream_t s);
+// batched (slu_b200_batch_selinv ...): the same launches over d.members matrices of one pattern (gridDim.y = members).  hv =
+// member 0's H arena, the members' arenas d.val_stride elements apart; dinv as launch_diag_inv.  logdet: part / pph hold
+// members x ceil(count / SELINV_VECS) entries, out members x (1 + VAL_DOUBLES).  get: out holds members x nnz values,
+// member-major; *err counts member 0's entries without a slot only (the count of the unbatched call).
+int launch_selinv_gemm(const BatchedLU &d, const Batch &b, int64_t ctas, int mode, val_t *hv, cudaStream_t s);
+int launch_selinv_trsm(const BatchedLU &d, const Batch &b, int64_t ctas, int cols, const val_t *dinv, val_t *hv, cudaStream_t s);
+int launch_selinv_logdet(const BatchedLU &d, const int32_t *nodes, int count, double *part, phase_t *pph, double *out, cudaStream_t s);
+int launch_selinv_get(const BatchedLU &d, const val_t *hv, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm,
+                      val_t *out, int *err, cudaStream_t s);
 
 #ifdef SLU_COMPLEX
 constexpr int SCHUR_BM_BIG = 128, SCHUR_BM_SMALL = 32, SCHUR_BN_SMALL = 16;

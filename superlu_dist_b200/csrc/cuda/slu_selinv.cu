@@ -18,14 +18,24 @@
 // unchanged.  Element arithmetic goes through the val_t helpers of slu_scalar.cuh; the complex products stay on the FP64
 // DMMA pipe through the real embedding of zgemm_tile (slu_kernels_z.cu): [Ar Ai] times [[Br Bi] [-Bi Br]], the second
 // factor read from the raw interleaved tile with a lane-constant swap and sign.
+//
+// Every kernel is templated on its DeviceLU type, as the factorization and the solve are: the BatchedLU instantiations
+// (slu_b200_batch_selinv ...) run the same body over every member of a batched handle, the member in blockIdx.y.  A
+// member's H arena has exactly its factors' layout, so the members' H arenas are val_stride elements apart as their
+// factors are.
 #include "slu_device.cuh"
 #define SLU_COMMON_HELPERS_ONLY
 #include "slu_kernels_common.cuh"
 #include "slu_scalar.cuh"
 
 #include <cmath>
+#include <type_traits>
 
 namespace SLU_NS {
+
+// the member's H arena (the identity for a plain DeviceLU)
+template <class T> __device__ __forceinline__ T *member_h(const DeviceLU &, T *hv) { return hv; }
+template <class T> __device__ __forceinline__ T *member_h(const BatchedLU &d, T *hv) { return hv + (int64_t)blockIdx.y * d.val_stride; }
 
 // ------------------------------------------------------------------------------------------------
 // GEMM tiles on DMMA m16n8k8: 64 x 64 real output tiles (SELINV_TILE_M rows x SELINV_TILE_N val_t columns: 64 complex
@@ -75,15 +85,23 @@ __device__ __forceinline__ void si_put_b(double *Bs, int k, int c, val_t v)
 #endif
 }
 
+// __launch_bounds__ minimum of CTAs per SM: 2 for the batched instantiations, 0 (no minimum) for the unbatched ones, which
+// compile as before.  Two 128-thread CTAs leave the 255-register cap as it is; without the hint ptxas compiles the batched
+// doublecomplex mode 1 at 168 registers with a 12-byte spill in the k-loop, and with it no batched product spills.
+template <class LU>
+constexpr int SELINV_MIN_CTAS = std::is_same<LU, BatchedLU>::value ? 2 : 0;
+
 // MODE 0: out(i, p) = H(R,K), A(i, j) = M, B(j, p) = U_KC(p, j), inner ncols
 // MODE 1: out(p, j) = H(K,C), A(p, i) = L_RK(i, p), B(i, j) = M, inner m
 // MODE 2: out(p, q) = H(K,K), A(p, i) = L_RK(i, p), B(i, q) = H(R,K)(i, q), inner m
-template <int MODE>
-__global__ void __launch_bounds__(SI_NT) selinv_gemm_kernel(DeviceLU d, Batch b, val_t *__restrict__ hv)
+template <int MODE, class LU>
+__global__ void __launch_bounds__(SI_NT, SELINV_MIN_CTAS<LU>) selinv_gemm_kernel(LU dd, Batch b, val_t *__restrict__ hv)
 {
     __shared__ __align__(16) double As[SI_RK * SI_LDA];
     __shared__ __align__(16) double Bs[SI_BN * SI_LDB];
     if (blockIdx.x >= b.prefix[b.count]) return;
+    const DeviceLU &d = member_view(dd);
+    hv = member_h(dd, hv);
     const int slot = find_slot(b.prefix, b.count, blockIdx.x);
     const NodeDesc nd = d.nodes[b.nodes[slot]];
     const int ns = nd.ns, m = nd.m, nc = nd.ncols, lda = nd.nsupr;
@@ -212,11 +230,14 @@ __global__ void __launch_bounds__(SI_NT) selinv_gemm_kernel(DeviceLU d, Batch b,
 // columns of H(K,K) and the ncols columns of H(K,C), T = L_KK^T (unit; its block inverse is inv(L_bb) read transposed).
 // In doublecomplex the block inverses are read transposed exactly as in double, never conjugated.
 // ------------------------------------------------------------------------------------------------
-template <int COLS>
-__global__ void __launch_bounds__(SELINV_VECS) selinv_trsm_kernel(DeviceLU d, Batch b, const val_t *__restrict__ dinv,
+template <int COLS, class LU>
+__global__ void __launch_bounds__(SELINV_VECS) selinv_trsm_kernel(LU dd, Batch b, const val_t *__restrict__ dinv,
                                                                    val_t *__restrict__ hv)
 {
     if (blockIdx.x >= b.prefix[b.count]) return;
+    const DeviceLU &d = member_view(dd);
+    dinv = member_inv(dd, dinv);
+    hv = member_h(dd, hv);
     const int slot = find_slot(b.prefix, b.count, blockIdx.x);
     const NodeDesc nd = d.nodes[b.nodes[slot]];
     const int ns = nd.ns, lda = nd.nsupr;
@@ -281,9 +302,14 @@ __device__ __forceinline__ void si_block_reduce(double &s, phase_t &ph)
     }
 }
 
-__global__ void __launch_bounds__(SELINV_VECS) selinv_logdet_partial_kernel(DeviceLU d, const int32_t *nodes, int count, double *part,
+// batched: grid (nparts, members), member j's partials at j * nparts
+template <class LU>
+__global__ void __launch_bounds__(SELINV_VECS) selinv_logdet_partial_kernel(LU dd, const int32_t *nodes, int count, double *part,
                                                                             phase_t *pph)
 {
+    const DeviceLU &d = member_view(dd);
+    part = member_ptr(dd, part, gridDim.x);
+    pph = member_ptr(dd, pph, gridDim.x);
     const int t = blockIdx.x * SELINV_VECS + threadIdx.x;
     double s = 0.0;
     phase_t ph = 0;
@@ -311,9 +337,16 @@ __global__ void __launch_bounds__(SELINV_VECS) selinv_logdet_partial_kernel(Devi
     if (threadIdx.x == 0) { part[blockIdx.x] = s; pph[blockIdx.x] = ph; }
 }
 
-// out[0] = log |det|; double: out[1] = the sign; doublecomplex: out[1], out[2] = exp(i theta)
+// out[0] = log |det|; double: out[1] = the sign; doublecomplex: out[1], out[2] = exp(i theta).  MEMBERS: grid (1, members),
+// member j's partials at j * nparts and its result at out + j * (1 + VAL_DOUBLES)
+template <bool MEMBERS>
 __global__ void __launch_bounds__(SELINV_VECS) selinv_logdet_final_kernel(const double *part, const phase_t *pph, int nparts, double *out)
 {
+    if (MEMBERS) {
+        part += (size_t)blockIdx.y * nparts;
+        pph += (size_t)blockIdx.y * nparts;
+        out += (size_t)blockIdx.y * (1 + VAL_DOUBLES);
+    }
     double s = 0.0;
     phase_t ph = 0;
     for (int i = threadIdx.x; i < nparts; i += SELINV_VECS) { s += part[i]; ph += pph[i]; }
@@ -330,14 +363,21 @@ __global__ void __launch_bounds__(SELINV_VECS) selinv_logdet_final_kernel(const 
 
 // ------------------------------------------------------------------------------------------------
 // out[p] = A^-1(i, colind[p]) = H(perm[colind[p]], perm[i]): the slot search of fill_csr_kernel with the roles of row and
-// column swapped, reading instead of writing.  One thread per row of the pattern.
+// column swapped, reading instead of writing.  One thread per row of the pattern.  Batched: member j's values at
+// out + j * nnz; a missing slot depends on the structure only, so only member 0 counts it.
 // ------------------------------------------------------------------------------------------------
-__global__ void selinv_get_kernel(DeviceLU d, const val_t *__restrict__ hv, int n, const int32_t *__restrict__ rowptr,
+template <class LU>
+__global__ void selinv_get_kernel(LU dd, const val_t *__restrict__ hv, int n, const int32_t *__restrict__ rowptr,
                                   const int32_t *__restrict__ colind, const int32_t *__restrict__ perm, val_t *__restrict__ out,
                                   int *err)
 {
+    constexpr bool BATCHED = std::is_same<LU, BatchedLU>::value;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    const DeviceLU &d = member_view(dd);
+    hv = member_h(dd, hv);
+    if (BATCHED) out += (int64_t)blockIdx.y * rowptr[n];
+    const bool count = !BATCHED || blockIdx.y == 0;
     const int pj = perm[i];                       // column of H
     const int ks = d.supno[pj];
     for (int p = rowptr[i]; p < rowptr[i + 1]; ++p) {
@@ -348,53 +388,93 @@ __global__ void selinv_get_kernel(DeviceLU d, const val_t *__restrict__ hv, int 
             const int32_t *srow = d.lsrow + nd->lrow;
             const int q = lower_bound_i32(srow, nd->nsupr, pi);
             if (q < nd->nsupr && srow[q] == pi) v = hv[nd->lval + (int64_t)(pj - nd->fsupc) * nd->nsupr + d.lspos[nd->lrow + q]];
-            else atomicAdd(err, 1);
+            else if (count) atomicAdd(err, 1);
         } else {                                  // U panel of block row supno(pi)
             const NodeDesc *nd = d.nodes + d.supno[pi];
             const int32_t *uc = d.ucols + nd->ucol;
             const int q = lower_bound_i32(uc, nd->ncols, pj);
             if (q < nd->ncols && uc[q] == pj) v = hv[nd->uval + (int64_t)q * nd->ns + (pi - nd->fsupc)];
-            else atomicAdd(err, 1);
+            else if (count) atomicAdd(err, 1);
         }
         out[p] = v;
     }
 }
 
 // ------------------------------------------------------------------------------------------------
-int launch_selinv_gemm(const DeviceLU &d, const Batch &b, int64_t ctas, int mode, val_t *hv, cudaStream_t s)
+// The batched launchers make exactly the launches of the unbatched ones, with gridDim.y = members.
+template <class LU>
+static int launch_selinv_gemm_t(const LU &d, const Batch &b, int64_t ctas, int mode, val_t *hv, cudaStream_t s)
 {
     if (b.count <= 0) return 0;
-    const unsigned grid = (unsigned)(ctas > 0 ? ctas : 1);   // an empty batch still makes its launch: the count stays fixed
-    if (mode == 0) selinv_gemm_kernel<0><<<grid, SI_NT, 0, s>>>(d, b, hv);
-    else if (mode == 1) selinv_gemm_kernel<1><<<grid, SI_NT, 0, s>>>(d, b, hv);
-    else selinv_gemm_kernel<2><<<grid, SI_NT, 0, s>>>(d, b, hv);
+    const dim3 grid = member_grid(d, (unsigned)(ctas > 0 ? ctas : 1));   // an empty batch still makes its launch: the count stays fixed
+    if (mode == 0) selinv_gemm_kernel<0, LU><<<grid, SI_NT, 0, s>>>(d, b, hv);
+    else if (mode == 1) selinv_gemm_kernel<1, LU><<<grid, SI_NT, 0, s>>>(d, b, hv);
+    else selinv_gemm_kernel<2, LU><<<grid, SI_NT, 0, s>>>(d, b, hv);
     return 1;
 }
 
-int launch_selinv_trsm(const DeviceLU &d, const Batch &b, int64_t ctas, int cols, const val_t *dinv, val_t *hv, cudaStream_t s)
+template <class LU>
+static int launch_selinv_trsm_t(const LU &d, const Batch &b, int64_t ctas, int cols, const val_t *dinv, val_t *hv, cudaStream_t s)
 {
     if (b.count <= 0) return 0;
-    const unsigned grid = (unsigned)(ctas > 0 ? ctas : 1);
-    if (cols) selinv_trsm_kernel<1><<<grid, SELINV_VECS, 0, s>>>(d, b, dinv, hv);
-    else selinv_trsm_kernel<0><<<grid, SELINV_VECS, 0, s>>>(d, b, dinv, hv);
+    const dim3 grid = member_grid(d, (unsigned)(ctas > 0 ? ctas : 1));
+    if (cols) selinv_trsm_kernel<1, LU><<<grid, SELINV_VECS, 0, s>>>(d, b, dinv, hv);
+    else selinv_trsm_kernel<0, LU><<<grid, SELINV_VECS, 0, s>>>(d, b, dinv, hv);
     return 1;
 }
 
-int launch_selinv_logdet(const DeviceLU &d, const int32_t *nodes, int count, double *part, phase_t *pph, double *out, cudaStream_t s)
+template <class LU>
+static int launch_selinv_logdet_t(const LU &d, const int32_t *nodes, int count, double *part, phase_t *pph, double *out, cudaStream_t s)
 {
     const int nparts = (count + SELINV_VECS - 1) / SELINV_VECS;
     if (nparts <= 0) return 0;
-    selinv_logdet_partial_kernel<<<nparts, SELINV_VECS, 0, s>>>(d, nodes, count, part, pph);
-    selinv_logdet_final_kernel<<<1, SELINV_VECS, 0, s>>>(part, pph, nparts, out);
+    selinv_logdet_partial_kernel<LU><<<member_grid(d, nparts), SELINV_VECS, 0, s>>>(d, nodes, count, part, pph);
+    selinv_logdet_final_kernel<std::is_same<LU, BatchedLU>::value><<<member_grid(d, 1), SELINV_VECS, 0, s>>>(part, pph, nparts, out);
     return 2;
 }
 
+template <class LU>
+static int launch_selinv_get_t(const LU &d, const val_t *hv, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm,
+                               val_t *out, int *err, cudaStream_t s)
+{
+    if (n <= 0) return 0;
+    selinv_get_kernel<LU><<<member_grid(d, (n + 127) / 128), 128, 0, s>>>(d, hv, n, rowptr, colind, perm, out, err);
+    return 1;
+}
+
+int launch_selinv_gemm(const DeviceLU &d, const Batch &b, int64_t ctas, int mode, val_t *hv, cudaStream_t s)
+{
+    return launch_selinv_gemm_t(d, b, ctas, mode, hv, s);
+}
+int launch_selinv_trsm(const DeviceLU &d, const Batch &b, int64_t ctas, int cols, const val_t *dinv, val_t *hv, cudaStream_t s)
+{
+    return launch_selinv_trsm_t(d, b, ctas, cols, dinv, hv, s);
+}
+int launch_selinv_logdet(const DeviceLU &d, const int32_t *nodes, int count, double *part, phase_t *pph, double *out, cudaStream_t s)
+{
+    return launch_selinv_logdet_t(d, nodes, count, part, pph, out, s);
+}
 int launch_selinv_get(const DeviceLU &d, const val_t *hv, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm,
                       val_t *out, int *err, cudaStream_t s)
 {
-    if (n <= 0) return 0;
-    selinv_get_kernel<<<(n + 127) / 128, 128, 0, s>>>(d, hv, n, rowptr, colind, perm, out, err);
-    return 1;
+    return launch_selinv_get_t(d, hv, n, rowptr, colind, perm, out, err, s);
+}
+int launch_selinv_gemm(const BatchedLU &d, const Batch &b, int64_t ctas, int mode, val_t *hv, cudaStream_t s)
+{
+    return launch_selinv_gemm_t(d, b, ctas, mode, hv, s);
+}
+int launch_selinv_trsm(const BatchedLU &d, const Batch &b, int64_t ctas, int cols, const val_t *dinv, val_t *hv, cudaStream_t s)
+{
+    return launch_selinv_trsm_t(d, b, ctas, cols, dinv, hv, s);
+}
+int launch_selinv_logdet(const BatchedLU &d, const int32_t *nodes, int count, double *part, phase_t *pph, double *out, cudaStream_t s)
+{
+    return launch_selinv_logdet_t(d, nodes, count, part, pph, out, s);
+}
+int launch_selinv_get(const BatchedLU &d, const val_t *hv, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm,
+                      val_t *out, int *err, cudaStream_t s)
+{
+    return launch_selinv_get_t(d, hv, n, rowptr, colind, perm, out, err, s);
 }
 
 }  // namespace SLU_NS
