@@ -207,6 +207,35 @@ int slu_b200_selinv_get(slu_b200_handle_t h, int n, const int32_t *rowptr, const
 /* log|det A| and its sign (+1 / -1) from the resident factors: sum of log |U_kk(i,i)| in a fixed order (deterministic),
  * sign from the count of negative pivots; the symmetric permutation does not change det.  Restrictions of selinv. */
 int slu_b200_logdet(slu_b200_handle_t h, double *logabs, double *sign);
+/* Partial factorization with a Schur complement (MUMPS ICNTL(19), PARDISO iparm(36)): with F = P A P^T = [A11 A12; A21 A22]
+ * and the s = nschur "Schur" unknowns last, eliminate A11 only and keep S = A22 - A21 A11^-1 A12.  Uses: domain
+ * decomposition (S is the interface operator), sparse-dense block coupling, Kron reduction, static condensation, marginal
+ * precision matrices.  The view must come from a symbolic factorization that keeps the Schur columns last in whole
+ * supernodes (sluh_symbolic_schur; hostlib.schur_order orders a pattern so).
+ * schur_create: as slu_b200_create, but the supernodes with xsup[k] >= n - nschur are left out of the level plan; their
+ * panels keep their place in HBM and receive every Schur update of the eliminated part.  Fails with a message unless
+ * 1 <= nschur < n, n - nschur is a supernode boundary (the message names the supernode across it), the grid is 1 x 1 x 1
+ * with world_size 1 and the int8 tensor-core path is off (options.reserved[4] <= 0; FP64 DMMA only, as on batched handles).
+ * A Schur handle takes slu_b200_upload, _fill_csr, _factor, _download, _get_stats, _destroy and the schur_* calls below;
+ * factor_host, solve, solve_trans, gscon, selinv, selinv_get, logdet, the batch_* and kernel-export calls fail on it with
+ * a message and leave it usable, and the schur_* calls fail on ordinary and batched handles.  factor eliminates the
+ * non-Schur supernodes only: info = 0 or the 1-based column of the first exact zero pivot among them; ops_fact, ops_schur,
+ * nlevels and my_supernodes count the eliminated work.  download writes L11, U11, L21 and U12, and S in the Schur panels,
+ * in the reference layout.
+ * schur_get: S into the host array S, s x s column-major (lds >= s); row and column t are F's index n - s + t.  Every
+ * stored entry of the Schur panels is written once by one gather kernel into a zeroed device buffer (kept by the handle
+ * until destroy), then copied back: entries outside the stored pattern are exactly 0 and two calls on the same factors are
+ * bit-identical.  If the s x s buffer does not fit, the call fails with its size.  Needs a successful factor (info = 0).
+ * stats.reserved[6] = seconds of the call, stats.reserved[7] = device milliseconds of the gather kernel.
+ * schur_condense: the forward pass of the solve over the eliminated supernodes: x holds b on entry, and y1 = L11^-1 b1 in
+ * the eliminated positions and g = b2 - A21 A11^-1 b1 in the Schur positions on return.
+ * schur_expand: the backward pass: x holds y1 (as condense left it) and x2 in the Schur positions on entry,
+ * x1 = A11^-1 (b1 - A12 x2) and x2 on return.  So condense, x2 = S^-1 g (by the caller), expand solves A x = b.
+ * Both: x, ldx and nrhs as slu_b200_solve (ordering of F), need a successful factor, set stats.reserved[4] / [5]. */
+int slu_b200_schur_create(slu_b200_handle_t *h, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, int nschur);
+int slu_b200_schur_get(slu_b200_handle_t h, double *S, int lds);
+int slu_b200_schur_condense(slu_b200_handle_t h, double *x, int ldx, int nrhs);
+int slu_b200_schur_expand(slu_b200_handle_t h, double *x, int ldx, int nrhs);
 int slu_b200_get_stats(slu_b200_handle_t h, slu_b200_stats_t *out);
 void slu_b200_destroy(slu_b200_handle_t h);
 
@@ -337,6 +366,12 @@ int slu_b200_z_selinv(slu_b200_zhandle_t h, double out[4]);
 int slu_b200_z_selinv_get(slu_b200_zhandle_t h, int n, const int32_t *rowptr, const int32_t *colind,
                           const int32_t *perm, double *out);
 int slu_b200_z_logdet(slu_b200_zhandle_t h, double *logabs, double *sign);
+/* as slu_b200_schur_create / _schur_get / _schur_condense / _schur_expand, with the same restrictions and messages; S and
+ * x hold interleaved doublecomplex (S: s x s complex), lds and ldx count complex elements. */
+int slu_b200_z_schur_create(slu_b200_zhandle_t *h, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, int nschur);
+int slu_b200_z_schur_get(slu_b200_zhandle_t h, double *S, int lds);
+int slu_b200_z_schur_condense(slu_b200_zhandle_t h, double *x, int ldx, int nrhs);
+int slu_b200_z_schur_expand(slu_b200_zhandle_t h, double *x, int ldx, int nrhs);
 /* batched doublecomplex handles (the reference's pzgssvx3d_csc_batch, SRC/complex16/pzgssvx3d_csc_batch.c:80): the
  * slu_b200_batch_* calls above with the same semantics, restrictions and stats; val and x point at interleaved
  * doublecomplex, n, ldx and nnz count complex elements.  Stats through slu_b200_z_get_stats, slu_b200_z_destroy frees.

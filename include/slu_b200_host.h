@@ -47,6 +47,12 @@ typedef struct sluh_symb sluh_symb;
  * (0: exact fundamental supernodes). */
 sluh_symb *sluh_symbolic(int n, const int32_t *rowptr, const int32_t *colind,
                          const int32_t *perm_in, int relax, int maxsup, double amalg);
+/* Partial factorization (slu_b200_schur_create): as sluh_symbolic, but the nschur columns that perm_in sends to
+ * n - nschur .. n - 1 (the Schur set) stay there in their relative order.  The other columns are postordered on their own
+ * elimination forest and partitioned as by sluh_symbolic; the Schur block is cut into supernodes of maxsup columns, so
+ * n - nschur is a supernode boundary.  nschur = 0 is sluh_symbolic.  NULL if nschur is outside [0, n]. */
+sluh_symb *sluh_symbolic_schur(int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm_in,
+                               int relax, int maxsup, double amalg, int nschur);
 void sluh_symb_free(sluh_symb *s);
 int32_t sluh_symb_nsupers(const sluh_symb *s);
 /* sizes[0..3] = total lengths of the L index, L value, U index, U value arenas;

@@ -130,6 +130,12 @@ def lib():
         getattr(L, f).argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     for f in ("slu_b200_batch_logdet", "slu_b200_z_batch_logdet"):
         getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    for f in ("slu_b200_schur_create", "slu_b200_z_schur_create"):
+        getattr(L, f).argtypes = [C.POINTER(C.c_void_p), C.POINTER(LUView), C.POINTER(Options), C.c_int]
+    for f in ("slu_b200_schur_get", "slu_b200_z_schur_get"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+    for f in ("slu_b200_schur_condense", "slu_b200_z_schur_condense", "slu_b200_schur_expand", "slu_b200_z_schur_expand"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
     _lib = L
     return L
 
@@ -391,6 +397,45 @@ class Handle:
             self.close()
         except Exception:
             pass
+
+
+class SchurHandle(Handle):
+    """A partial factorization (slu_b200_schur_create / slu_b200_z_schur_create): eliminate all unknowns of `prob` (layer 0,
+    1 x 1 x 1 grid) but the last `nschur`, which must form whole supernodes (LUProblem.from_matrix(..., nschur=...)).
+    upload / fill_csr / factor / download as Handle; schur() returns S = A22 - A21 A11^-1 A12, condense / expand the two
+    partial solves.  Every other call of Handle fails on it.  A complex128 `prob` takes the doublecomplex twins."""
+
+    def __init__(self, prob, nschur, **opt):
+        require_gpu()
+        self.prob, self.nschur = prob, int(nschur)
+        self.z_ = _is_complex(prob.dtype)
+        self.view, self._keep = make_view(prob, 0)
+        self.opt = make_options(prob, **opt)
+        self.h = C.c_void_p()
+        _check(_fn("schur_create", self.z_)(C.byref(self.h), C.byref(self.view), C.byref(self.opt), self.nschur))
+
+    def schur(self):
+        """S (s, s), float64 or complex128: row / column t is unknown n - s + t of the factored ordering; exactly 0 off
+        the stored pattern."""
+        s = self.nschur
+        out = np.empty((s, s), self._dtype(), order="F")
+        _check(_fn("schur_get", self.z_)(self.h, out.ctypes.data_as(C.c_void_p), s))
+        return out
+
+    def _pass(self, name, b):
+        x = np.array(b, self._dtype(), order="C", copy=True)
+        nrhs = 1 if x.ndim == 1 else x.shape[0]
+        _check(_fn(name, self.z_)(self.h, x.ctypes.data_as(C.c_void_p), self.prob.n, nrhs))
+        return x
+
+    def condense(self, b):
+        """b: (n,) or (nrhs, n) in the factored ordering -> y1 = L11^-1 b1 in the eliminated positions, g = b2 - A21 A11^-1 b1
+        in the last s"""
+        return self._pass("schur_condense", b)
+
+    def expand(self, y):
+        """y: condense's result with x2 in the last s positions -> x1 = A11^-1 (b1 - A12 x2) there, x2 kept"""
+        return self._pass("schur_expand", y)
 
 
 class BatchHandle:

@@ -52,6 +52,10 @@
 #define slu_b200_batch_selinv slu_b200_z_batch_selinv
 #define slu_b200_batch_selinv_get slu_b200_z_batch_selinv_get
 #define slu_b200_batch_logdet slu_b200_z_batch_logdet
+#define slu_b200_schur_create slu_b200_z_schur_create
+#define slu_b200_schur_get slu_b200_z_schur_get
+#define slu_b200_schur_condense slu_b200_z_schur_condense
+#define slu_b200_schur_expand slu_b200_z_schur_expand
 #define SLU_API "slu_b200_z_"     // name prefix of the exported calls, for error messages
 #else
 #define SLU_API "slu_b200_"
@@ -307,6 +311,13 @@ struct slu_b200_handle_s {
     DevBuf<int64_t> d_si_pool;
     std::vector<SelinvLevel> si_levels;
     bool si_ready = false;
+    // partial factorization (slu_b200_schur_create): the supernodes from column schur_first = n - nschur on are in no level
+    // of the plan, so factor, condense and expand stop at them; d_sunits lists the gather's (supernode, column) units and
+    // d_S is the s x s buffer of slu_b200_schur_get (allocated on first use, freed by destroy).  nschur = 0: not a Schur
+    // handle.
+    int nschur = 0, schur_first = INT_MAX;
+    DevBuf<int2> d_sunits;
+    DevBuf<val_t> d_S;
 };
 
 namespace {
@@ -593,6 +604,7 @@ int analyze(slu_b200_handle_s *H)
 #endif
             double sch = 2.0 * nd.m * (double)ldu * nd.ncols;
             if (H->my_zero[zl]) continue;  // replicated ancestor copy: counted by its owner layer only
+            if (nd.fsupc >= H->schur_first) continue;  // a Schur supernode of a partial factorization: not eliminated
             if (H->P2 > 1 && (k % v.nprow != v.myrow || k % v.npcol != v.mycol)) continue;  // ... and by the diagonal owner
             ops += diag + utrsm + sch;
             ops_schur += sch;
@@ -636,7 +648,8 @@ int analyze(slu_b200_handle_s *H)
         int maxlev = -1;
         for (int k : H->znodes[zl]) maxlev = std::max(maxlev, lev[k]);
         std::vector<std::vector<int32_t>> by(maxlev + 1);
-        for (int k : H->znodes[zl]) by[lev[k]].push_back(k);
+        for (int k : H->znodes[zl])
+            if (xsup[k] < H->schur_first) by[lev[k]].push_back(k);   // a partial factorization leaves its Schur supernodes out
         for (auto &nodes : by) {
             if (nodes.empty()) continue;
             LevelPlan L;
@@ -834,7 +847,8 @@ int analyze(slu_b200_handle_s *H)
                                       H->d_urel.bytes() + H->d_oz_i8.bytes() + H->d_oz_scale.bytes() + H->d_oz_rexp.bytes());
     int mine = 0;
     for (int zl = 0; zl < max_lvl; ++zl)
-        if (!H->my_zero[zl]) mine += (int)H->znodes[zl].size();
+        if (!H->my_zero[zl])
+            for (int k : H->znodes[zl]) mine += xsup[k] < H->schur_first;
     st.my_supernodes = mine;
     return 0;
 }
@@ -1288,6 +1302,13 @@ int refuse_batched(const slu_b200_handle_s *H, const char *fn)
     return H->batch ? fail("%s on a batched handle (%d members): use the " SLU_API "batch_* calls", fn, H->batch) : 0;
 }
 
+// a Schur handle (slu_b200_schur_create) takes upload, fill_csr, factor, download, get_stats, destroy and the schur_* calls
+int refuse_schur(const slu_b200_handle_s *H, const char *fn)
+{
+    return H->nschur ? fail("%s on a Schur handle (partial factorization, nschur = %d): its factors are incomplete; use the "
+                            SLU_API "schur_* calls", fn, H->nschur) : 0;
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -1370,23 +1391,38 @@ void slu_b200_destroy(slu_b200_handle_t H)
     H->d_x.release(); H->d_x2.release();
     H->d_cv.release(); H->d_csgn.release(); H->d_cstate.release(); H->d_cpart.release(); H->d_ccount.release();
     H->d_tiny.release(); H->d_oz_i8.release(); H->d_oz_scale.release(); H->d_oz_rexp.release();
-    H->d_hinv.release(); H->d_si_pool.release();
+    H->d_hinv.release(); H->d_si_pool.release(); H->d_sunits.release(); H->d_S.release();
     delete H;
 }
 
 // batch > 0: a batched handle (slu_b200_batch_create), 1 x 1 x 1 grid, FP64 DMMA kernels only
-static int create_impl(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, int batch)
+// nschur > 0: a Schur handle (slu_b200_schur_create), 1 x 1 x 1 grid, FP64 DMMA kernels only
+static int create_impl(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, int batch, int nschur = 0)
 {
     if (!out || !lu || !opt) return fail("null argument");
     *out = nullptr;
     if (opt->schur_variant != 0) return fail("options.schur_variant is retired and must be 0 (got %d)", opt->schur_variant);
+    if (nschur) {
+        const char *fn = SLU_API "schur_create";
+        if (nschur < 1 || nschur >= lu->n) return fail("%s: nschur = %d, must satisfy 1 <= nschur < n = %d", fn, nschur, lu->n);
+        if (lu->nprow != 1 || lu->npcol != 1 || lu->npdep != 1 || opt->world_size > 1)
+            return fail("%s handles 1 x 1 x 1 grids (world_size 1)", fn);
+        if (opt->reserved[4] > 0) return fail("%s: the int8 tensor-core path (options.reserved[4] = %d) is not available on a Schur handle", fn, opt->reserved[4]);
+        const int n0 = lu->n - nschur;
+        for (int k = 0; k < lu->nsupers; ++k)
+            if (lu->xsup[k] < n0 && lu->xsup[k + 1] > n0)
+                return fail("%s: column n - nschur = %d is not a supernode boundary: supernode %d spans columns %d..%d", fn, n0, k,
+                            lu->xsup[k], lu->xsup[k + 1] - 1);
+    }
     if (slu_b200_device_count() < 1) return fail("no CUDA device: libslu_b200 has no CPU fallback");
     if (device_setup(opt)) return -1;
     slu_b200_handle_s *H = new slu_b200_handle_s;
     H->view = *lu;
     H->opt = *opt;
     H->batch = batch;
-    if (batch) {             // the int8 path and the overlapped upload are not batched
+    H->nschur = nschur;
+    if (nschur) H->schur_first = lu->n - nschur;
+    if (batch || nschur) {   // the int8 path and the overlapped upload are not batched, nor used by a partial factorization
         H->opt.reserved[3] = 0;
         H->opt.reserved[4] = -1;
         H->tc_force_off = true;
@@ -1442,6 +1478,15 @@ static int create_impl(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, con
         if (analyze(H)) { slu_b200_destroy(H); return -1; }
     }
     if (build_pieces(H)) { slu_b200_destroy(H); return -1; }
+    if (nschur) {            // the gather units: every L column and every packed U column of the Schur supernodes
+        std::vector<int2> units;
+        for (int k = 0; k < H->nsupers; ++k) {
+            if (H->xsup[k] < H->schur_first) continue;
+            const NodeDesc &nd = H->nodes[k];
+            for (int c = 0; c < nd.ns + nd.ncols; ++c) units.push_back(make_int2(k, c));
+        }
+        if (H->d_sunits.upload(units)) { slu_b200_destroy(H); return -1; }
+    }
     if (batch) {             // the stats describe the whole handle: every member's work
         slu_b200_stats_t &st = H->st;
         st.ops_fact *= batch; st.ops_schur *= batch; st.schur_bytes *= batch;
@@ -1646,7 +1691,7 @@ int slu_b200_factor(slu_b200_handle_t H, int *info) { return factor_impl(H, info
 int slu_b200_factor_host(slu_b200_handle_t H, int *info)
 {
     if (!H || !info) return fail("null argument");
-    if (refuse_batched(H, SLU_API "factor_host")) return -1;
+    if (refuse_batched(H, SLU_API "factor_host") || refuse_schur(H, SLU_API "factor_host")) return -1;
     // The overlapped transfers move whole panels between the caller's arrays and the arena, which needs the U
     // skylines to equal their dense-packed form (symmetric patterns) and 1 x 1 x Pz pieces.  Anything else -- the
     // unsymmetric patterns SuperLU exists for, Pr x Pc pieces -- takes the plain path: upload (with the skyline
@@ -1812,7 +1857,7 @@ static int solve_dev(slu_b200_handle_t H, int nrhs, int trans, val_t **result)
 static int solve_impl(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int trans, const char *fn)
 {
     if (!H || !xh) return fail("null argument");
-    if (refuse_batched(H, (std::string(SLU_API) + fn).c_str())) return -1;
+    if (refuse_batched(H, (std::string(SLU_API) + fn).c_str()) || refuse_schur(H, (std::string(SLU_API) + fn).c_str())) return -1;
     if (trans < 0 || trans > 2) return fail(SLU_API "%s: trans = %d, must be 0 (A x = b), 1 (A^T x = b) or 2 (A^H x = b)", fn, trans);
     if (!H->factored) return fail("slu_b200_%s needs a successful slu_b200_factor on this handle first", fn);
     if (nrhs < 1 || ldx < H->n) return fail("bad nrhs / ldx");
@@ -1856,7 +1901,7 @@ int slu_b200_solve_trans(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int
 int slu_b200_k_level_export(slu_b200_handle_t H, int level, void *device_lu, int device_lu_bytes, int32_t *nodes, int max_nodes)
 {
     if (!H || level < 0 || level >= (int)H->levels.size()) return fail("bad handle / level");
-    if (refuse_batched(H, "slu_b200_k_level_export")) return -1;
+    if (refuse_batched(H, "slu_b200_k_level_export") || refuse_schur(H, "slu_b200_k_level_export")) return -1;
     if (device_lu && device_lu_bytes == (int)sizeof(DeviceLU)) memcpy(device_lu, &H->dev, sizeof(DeviceLU));
     else if (device_lu) return fail("DeviceLU is %d bytes", (int)sizeof(DeviceLU));
     const LevelPlan &L = H->levels[level];
@@ -1874,7 +1919,7 @@ int slu_b200_k_level_export(slu_b200_handle_t H, int level, void *device_lu, int
 int slu_b200_k_rerun_schur(slu_b200_handle_t H, int level, int reps, float *ms)
 {
     if (!H || level < 0 || level >= (int)H->levels.size() || reps < 1 || !ms) return fail("bad argument");
-    if (refuse_batched(H, "slu_b200_k_rerun_schur")) return -1;
+    if (refuse_batched(H, "slu_b200_k_rerun_schur") || refuse_schur(H, "slu_b200_k_rerun_schur")) return -1;
     const LevelPlan &L = H->levels[level];
     cudaStream_t s = H->stream;
     const DeviceLU &d = H->dev;
@@ -1909,7 +1954,7 @@ int slu_b200_k_rerun_schur(slu_b200_handle_t H, int level, int reps, float *ms)
 // triangular solves; a level with no Schur update (the root) has no maps to build and makes 6.
 static int selinv_refuse(const slu_b200_handle_s *H, const char *fn)
 {
-    if (refuse_batched(H, fn)) return -1;
+    if (refuse_batched(H, fn) || refuse_schur(H, fn)) return -1;
     if (H->opt.world_size > 1 || H->max_lvl > 1 || H->P2 > 1) return fail("%s handles 1 x 1 x 1 grids (world_size 1)", fn);
     if (!H->factored) return fail("%s needs a successful " SLU_API "factor (info = 0) on this handle first", fn);
     return 0;
@@ -2055,6 +2100,102 @@ int slu_b200_logdet(slu_b200_handle_t H, double *logabs, double *sign)
     *logabs = r[0];
     for (int c = 0; c < VAL_DOUBLES; ++c) sign[c] = r[1 + c];
     return 0;
+}
+
+// ---- partial factorization: the Schur complement and the two partial solves ------------------------------------------
+// A Schur handle is an ordinary one whose level plan leaves out the supernodes of the last nschur columns (analyze).  The
+// factorization then eliminates A11 only; every Schur update of the eliminated part still lands in the Schur panels, which
+// start as A22 and end as S = A22 - A21 A11^-1 A12 on the symbolic pattern.  The forward pass of the solve over the same
+// plan is condense (its update scatter subtracts L21 y1 from the Schur rows), the backward pass with x2 in the Schur
+// positions is expand.
+static int schur_refuse(const slu_b200_handle_s *H, const char *fn)
+{
+    if (!H->nschur) return fail("%s needs a Schur handle (" SLU_API "schur_create)", fn);
+    if (!H->factored) return fail("%s needs a successful " SLU_API "factor (info = 0) on this handle first", fn);
+    return 0;
+}
+
+int slu_b200_schur_create(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, int nschur)
+{
+    if (!out || !lu || !opt) return fail("null argument");
+    *out = nullptr;
+    if (nschur < 1 || nschur >= lu->n)
+        return fail(SLU_API "schur_create: nschur = %d, must satisfy 1 <= nschur < n = %d", nschur, lu->n);
+    return create_impl(out, lu, opt, 0, nschur);
+}
+
+int slu_b200_schur_get(slu_b200_handle_t H, double *S, int lds)
+{
+    if (!H || !S) return fail("null argument");
+    const char *fn = SLU_API "schur_get";
+    if (schur_refuse(H, fn)) return -1;
+    const int s = H->nschur;
+    if (lds < s) return fail("%s: lds = %d, must be >= nschur = %d", fn, lds, s);
+    const double t0 = now_s();
+    const size_t elems = (size_t)s * s;
+    if (!H->d_S.p && H->d_S.alloc(elems)) {
+        const std::string why = g_err;
+        H->d_S.release();
+        cudaGetLastError();
+        return fail("%s: the %d x %d Schur complement needs %.2f GB of HBM: %s", fn, s, s, 1e-9 * (double)(elems * sizeof(val_t)),
+                    why.c_str());
+    }
+    EventSet ev;
+    if (ev.create()) return fail("cannot create events");
+    cudaStream_t st = H->stream;
+    CU(cudaMemsetAsync(H->d_S.p, 0, elems * sizeof(val_t), st));
+    CU(cudaEventRecord(ev[0], st));
+    launch_schur_gather(H->dev, H->d_sunits.p, (int64_t)H->d_sunits.n, H->schur_first, s, H->d_S.p, st);
+    CU(cudaEventRecord(ev[1], st));
+    if (lds == s)   // one contiguous copy
+        CU(cudaMemcpyAsync(S, H->d_S.p, elems * sizeof(val_t), cudaMemcpyDeviceToHost, st));
+    else
+        CU(cudaMemcpy2DAsync(S, (size_t)lds * sizeof(val_t), H->d_S.p, (size_t)s * sizeof(val_t), (size_t)s * sizeof(val_t), (size_t)s,
+                             cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    float ms = 0;
+    CU(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+    H->st.reserved[6] = now_s() - t0;      // seconds of the call
+    H->st.reserved[7] = ms;                // device milliseconds of the gather kernel
+    return 0;
+}
+
+// condense: the forward pass over the plan; expand: the backward pass.  x: host, n x nrhs (ldx >= n), ordering of F.
+static int schur_pass(slu_b200_handle_t H, double *xh, int ldx, int nrhs, bool backward, const char *fn)
+{
+    if (!H || !xh) return fail("null argument");
+    if (schur_refuse(H, fn)) return -1;
+    if (nrhs < 1 || ldx < H->n) return fail("%s: bad nrhs / ldx", fn);
+    const int n = H->n;
+    const size_t len = (size_t)n * nrhs;
+    if (H->d_x.n < len && (H->d_x.alloc(len) || H->d_x2.alloc(len))) return -1;
+    cudaStream_t s = H->stream;
+    const double t0 = now_s();
+    CU(cudaMemcpy2DAsync(H->d_x.p, (size_t)n * sizeof(val_t), xh, (size_t)ldx * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs,
+                         cudaMemcpyHostToDevice, s));
+    int launches = 0;
+    if (!backward)
+        for (size_t li = 0; li < H->levels.size(); ++li) launches += solve_level(H, H->dev, H->levels[li], false, 0, H->d_x.p, n, nrhs, s);
+    else
+        for (size_t li = H->levels.size(); li-- > 0;) launches += solve_level(H, H->dev, H->levels[li], true, 0, H->d_x.p, n, nrhs, s);
+    CU(cudaMemcpy2DAsync(xh, (size_t)ldx * sizeof(val_t), H->d_x.p, (size_t)n * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs,
+                         cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    H->st.reserved[4] = now_s() - t0;
+    H->st.reserved[5] = (double)launches;
+    return 0;
+}
+
+int slu_b200_schur_condense(slu_b200_handle_t H, double *x, int ldx, int nrhs)
+{
+    return schur_pass(H, x, ldx, nrhs, false, SLU_API "schur_condense");
+}
+
+int slu_b200_schur_expand(slu_b200_handle_t H, double *x, int ldx, int nrhs)
+{
+    return schur_pass(H, x, ldx, nrhs, true, SLU_API "schur_expand");
 }
 
 // ---- batched handles: many matrices of one sparsity pattern (pdgssvx3d_csc_batch, SRC/double/pdgssvx3d_csc_batch.c:81,
@@ -2314,7 +2455,7 @@ static int gscon_impl(slu_b200_handle_t H, char norm, const double *anorm, doubl
 int slu_b200_gscon(slu_b200_handle_t H, char norm, double anorm, double *rcond)
 {
     if (!H || !rcond) return fail("null argument");
-    if (refuse_batched(H, SLU_API "gscon")) return -1;
+    if (refuse_batched(H, SLU_API "gscon") || refuse_schur(H, SLU_API "gscon")) return -1;
     if (!H->factored) return fail(SLU_API "gscon needs a successful " SLU_API "factor on this handle first");
     if (H->P2 > 1) return fail(SLU_API "gscon: Pr x Pc > 1 is not supported yet (1 x 1 x Pz only)");
     if (H->comm && !H->coop) return fail(SLU_API "gscon: the Z-distributed solve needs the cooperative schedule (options.reserved[1] = 0)");

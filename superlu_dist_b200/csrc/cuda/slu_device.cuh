@@ -264,6 +264,12 @@ int launch_selinv_logdet(const BatchedLU &d, const int32_t *nodes, int count, do
 int launch_selinv_get(const BatchedLU &d, const val_t *hv, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm,
                       val_t *out, int *err, cudaStream_t s);
 
+// slu_schur.cu (double) / slu_schur_z.cu (doublecomplex): the Schur complement of a partial factorization
+// (slu_b200_schur_get).  S(r - n0, c - n0) = every stored entry (r, c) of the Schur supernodes' panels, into a zeroed s x s
+// column-major buffer (ld s); units[u] = (supernode k, column c): c < ns is column c of L panel k (diagonal block included),
+// c >= ns the skyline segment of packed column c - ns of U panel k.  One launch of nunits CTAs.
+int launch_schur_gather(const DeviceLU &d, const int2 *units, int64_t nunits, int n0, int s, val_t *S, cudaStream_t st);
+
 #ifdef SLU_COMPLEX
 constexpr int SCHUR_BM_BIG = 128, SCHUR_BM_SMALL = 32, SCHUR_BN_SMALL = 16;
 #else

@@ -285,9 +285,22 @@ void postorder(int n, const std::vector<int32_t> &parent, std::vector<int32_t> &
 extern "C" sluh_symb *sluh_symbolic(int n, const int32_t *rowptr, const int32_t *colind,
                                     const int32_t *perm_in, int relax, int maxsup, double amalg)
 {
+    return sluh_symbolic_schur(n, rowptr, colind, perm_in, relax, maxsup, amalg, 0);
+}
+
+// nschur > 0: the columns perm_in sends to n - nschur .. n - 1 (the Schur set) stay there, in the caller's relative order.
+// Every ancestor of a Schur column is a Schur column, so postordering only the elimination forest of the other columns (a
+// column whose parent is a Schur column becomes a root) and appending the Schur columns keeps parent > child.  Column
+// counts and the relaxed / amalgamated partition are computed on that postordered part alone; the Schur block is cut
+// into supernodes of maxsup columns, so no supernode straddles column n - nschur.
+extern "C" sluh_symb *sluh_symbolic_schur(int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm_in,
+                                          int relax, int maxsup, double amalg, int nschur)
+{
+    if (nschur < 0 || nschur > n) return nullptr;
     sluh_symb *S = new sluh_symb;
     S->n = n;
     if (maxsup < 1) maxsup = 1;
+    const int n1 = n - nschur;   // eliminated columns [0, n1)
     std::vector<int32_t> p((size_t)n);
     if (perm_in) std::copy(perm_in, perm_in + n, p.begin());
     else std::iota(p.begin(), p.end(), 0);
@@ -297,7 +310,16 @@ extern "C" sluh_symb *sluh_symbolic(int n, const int32_t *rowptr, const int32_t 
     build_lower(n, rowptr, colind, p.data(), cp, ri);
     transpose_lower(n, cp, ri, rp, ci);
     etree(n, rp, ci, parent);
-    postorder(n, parent, invpost);
+    if (nschur == 0) {
+        postorder(n, parent, invpost);
+    } else {
+        std::vector<int32_t> par1(parent.begin(), parent.begin() + n1);
+        for (int j = 0; j < n1; ++j)
+            if (par1[j] >= n1) par1[j] = -1;
+        postorder(n1, par1, invpost);
+        invpost.resize(n);
+        for (int j = n1; j < n; ++j) invpost[j] = j;
+    }
     bool ident = true;
     for (int i = 0; i < n && ident; ++i) ident = invpost[i] == i;
     if (!ident) {
@@ -309,16 +331,18 @@ extern "C" sluh_symb *sluh_symbolic(int n, const int32_t *rowptr, const int32_t 
     { std::vector<int32_t>().swap(ci); std::vector<int64_t>().swap(rp); }
     S->perm = p;
 
-    // subtree sizes / first descendants (labels are a postorder: parent[j] > j)
+    // subtree sizes / first descendants (labels [0, n1) are a postorder of their forest: parent[j] > j); the Schur
+    // columns' values are not used
     std::vector<int32_t> size(n, 1), first(n);
     for (int j = 0; j < n; ++j)
         if (parent[j] != -1) size[parent[j]] += size[j];
     for (int j = 0; j < n; ++j) first[j] = j - size[j] + 1;
 
-    // column counts of L (Gilbert, Ng & Peyton skeleton algorithm; post = identity)
+    // column counts of L (Gilbert, Ng & Peyton skeleton algorithm; post = identity) of the columns [0, n1): their subtrees
+    // lie in [0, n1), and every count or least common ancestor the walk puts on a Schur column stays outside them
     std::vector<int32_t> cc(n), maxfirst(n, -1), prevleaf(n, -1), anc(n);
     for (int j = 0; j < n; ++j) { cc[j] = size[j] == 1 ? 1 : 0; anc[j] = j; }
-    for (int j = 0; j < n; ++j) {
+    for (int j = 0; j < n1; ++j) {
         if (parent[j] != -1) --cc[parent[j]];
         for (int64_t q = cp[j]; q < cp[j + 1]; ++q) {
             int i = ri[q];  // i > j
@@ -336,7 +360,7 @@ extern "C" sluh_symb *sluh_symbolic(int n, const int32_t *rowptr, const int32_t 
         }
         if (parent[j] != -1) anc[j] = parent[j];
     }
-    for (int j = 0; j < n; ++j)
+    for (int j = 0; j < n1; ++j)
         if (parent[j] != -1) cc[parent[j]] += cc[j];
 
     // supernode partition: relaxed leaf subtrees + fundamental chains, capped at maxsup
@@ -344,14 +368,14 @@ extern "C" sluh_symb *sluh_symbolic(int n, const int32_t *rowptr, const int32_t 
     xsup.clear();
     {
         int j = 0;
-        while (j < n) {
+        while (j < n1) {
             // is j the first column of a maximal subtree with <= relax columns ?
             int root = -1;
             if (relax > 1) {
                 // climb from j while the subtree still starts at j and stays small
                 int r = j;
                 if (first[r] == j) {
-                    while (parent[r] != -1 && first[parent[r]] == j && size[parent[r]] <= relax) r = parent[r];
+                    while (parent[r] != -1 && parent[r] < n1 && first[parent[r]] == j && size[parent[r]] <= relax) r = parent[r];
                     // need the maximal small subtree that STARTS at j: r's subtree is [j, r]
                     if (size[r] <= relax && size[r] > 1) root = r;
                 }
@@ -370,7 +394,7 @@ extern "C" sluh_symb *sluh_symbolic(int n, const int32_t *rowptr, const int32_t 
             // zeros this adds (every earlier column is padded to the structure of column j) stay below
             // the fraction `amalg` of the merged block; amalg = 0 gives exact fundamental supernodes.
             double ent = cc[f];
-            while (j < n && j - f < maxsup && parent[j - 1] == j) {
+            while (j < n1 && j - f < maxsup && parent[j - 1] == j) {
                 double w = j - f + 1;
                 double merged = w * cc[j] + w * (w - 1) / 2, tru = ent + cc[j];
                 if (merged - tru > amalg * merged + 1e-9) break;
@@ -378,6 +402,7 @@ extern "C" sluh_symb *sluh_symbolic(int n, const int32_t *rowptr, const int32_t 
                 ++j;
             }
         }
+        for (int f = n1; f < n; f += maxsup) xsup.push_back(f);
         xsup.push_back(n);
     }
     int nsupers = (int)xsup.size() - 1;

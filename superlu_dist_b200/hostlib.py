@@ -34,6 +34,8 @@ def lib():
     L.sluh_nd_order_graph.argtypes = [C.c_int, i32p, i32p, C.c_int, C.c_int, i32p]
     L.sluh_symbolic.restype = C.c_void_p
     L.sluh_symbolic.argtypes = [C.c_int, i32p, i32p, C.c_void_p, C.c_int, C.c_int, C.c_double]
+    L.sluh_symbolic_schur.restype = C.c_void_p
+    L.sluh_symbolic_schur.argtypes = [C.c_int, i32p, i32p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_int]
     L.sluh_symb_free.argtypes = [C.c_void_p]
     L.sluh_symb_nsupers.restype = C.c_int32
     L.sluh_symb_nsupers.argtypes = [C.c_void_p]
@@ -138,10 +140,38 @@ def nd_order_graph(rowptr, colind, leaf=64, compress_dof=True):
     return perm
 
 
-class Symbolic:
-    """Result of sluh_symbolic: supernode partition + L/U index arenas in the reference layout."""
+def schur_order(rowptr, colind, schur, leaf=64):
+    """A fill-reducing ordering that numbers the Schur unknowns `schur` (distinct indices) last: nested dissection
+    (nd_order_graph) of the pattern with their rows and columns removed, then schur[t] -> n - s + t.  perm[old] = new,
+    for Symbolic / LUProblem.from_matrix with nschur = len(schur)."""
+    rowptr = np.asarray(rowptr, np.int64)
+    colind = np.asarray(colind, np.int64)
+    n = len(rowptr) - 1
+    schur = np.asarray(schur, np.int64)
+    s = len(schur)
+    if s > n or (s and (schur.min() < 0 or schur.max() >= n)) or len(np.unique(schur)) != s:
+        raise ValueError("schur must hold distinct indices in [0, n)")
+    keep = np.ones(n, bool)
+    keep[schur] = False
+    new_of = np.full(n, -1, np.int64)
+    new_of[keep] = np.arange(n - s)
+    perm = np.empty(n, np.int32)
+    perm[schur] = np.arange(n - s, n)
+    if n - s:
+        rows = np.repeat(np.arange(n), np.diff(rowptr))
+        m = keep[rows] & keep[colind]
+        rp = np.concatenate([[0], np.cumsum(np.bincount(new_of[rows[m]], minlength=n - s))]).astype(np.int32)
+        sub = nd_order_graph(rp, new_of[colind[m]].astype(np.int32), leaf)
+        perm[keep] = sub
+    return perm
 
-    def __init__(self, n, rowptr, colind, perm=None, relax=32, maxsup=256, amalg=0.05):
+
+class Symbolic:
+    """Result of sluh_symbolic: supernode partition + L/U index arenas in the reference layout.  nschur > 0
+    (sluh_symbolic_schur): the columns perm sends to n - nschur .. n - 1 stay last, in their order, and form whole
+    supernodes -- the layout of a partial factorization (slu_b200_schur_create)."""
+
+    def __init__(self, n, rowptr, colind, perm=None, relax=32, maxsup=256, amalg=0.05, nschur=0):
         L = lib()
         rowptr = np.ascontiguousarray(rowptr, np.int32)
         colind = np.ascontiguousarray(colind, np.int32)
@@ -149,7 +179,13 @@ class Symbolic:
         if perm is not None:
             perm = np.ascontiguousarray(perm, np.int32)
             pp = perm.ctypes.data_as(C.c_void_p)
-        h = L.sluh_symbolic(n, rowptr, colind, pp, relax, maxsup, amalg)
+        if nschur:
+            h = L.sluh_symbolic_schur(n, rowptr, colind, pp, relax, maxsup, amalg, int(nschur))
+            if not h:
+                raise ValueError(f"nschur = {nschur} must lie in [0, n = {n}]")
+        else:
+            h = L.sluh_symbolic(n, rowptr, colind, pp, relax, maxsup, amalg)
+        self.nschur = int(nschur)
         try:
             self.n = n
             self.nsupers = L.sluh_symb_nsupers(h)

@@ -84,9 +84,11 @@ class LUProblem:
 
     @classmethod
     def from_matrix(cls, rowptr, colind, val, perm=None, relax=32, maxsup=256, npdep=1, layers=(0,),
-                    alloc=None, amalg=0.05):
+                    alloc=None, amalg=0.05, nschur=0):
+        """nschur > 0: the unknowns perm sends to n - nschur .. n - 1 stay last and form whole supernodes (the layout of
+        capi.SchurHandle; hostlib.schur_order makes such a perm)."""
         n = len(rowptr) - 1
-        sym = hostlib.Symbolic(n, rowptr, colind, perm, relax, maxsup, amalg)
+        sym = hostlib.Symbolic(n, rowptr, colind, perm, relax, maxsup, amalg, nschur)
         p = cls.from_symbolic(sym, npdep)
         for z in layers:
             p.add_layer(z, alloc=alloc)
