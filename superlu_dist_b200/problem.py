@@ -67,6 +67,7 @@ class LUProblem:
         self.replace_tiny_pivot = 0
         self.thresh = 0.0
         self.dtype = np.dtype(np.float64)   # complex128 for the doublecomplex mirror (pzgstrf3d)
+        self.nschur = 0                     # the last nschur unknowns form whole supernodes (from_matrix(..., nschur))
         self.layers = {}
 
     # ------------------------------------------------------------------ construction
@@ -90,6 +91,7 @@ class LUProblem:
         n = len(rowptr) - 1
         sym = hostlib.Symbolic(n, rowptr, colind, perm, relax, maxsup, amalg, nschur)
         p = cls.from_symbolic(sym, npdep)
+        p.nschur = int(nschur)
         for z in layers:
             p.add_layer(z, alloc=alloc)
             p.fill_layer(z, rowptr, colind, val)
@@ -289,8 +291,13 @@ class LUProblem:
         return lay
 
     def fill_layer(self, z, rowptr, colind, val):
-        """pddistribute3d + dinit3DLUstructForest: A into the panels; replicated ancestors start at 0."""
+        """pddistribute3d + dinit3DLUstructForest: A into the panels; replicated ancestors start at 0.  float64 only: the
+        host fill writes doubles, so a complex matrix goes into float64 arenas part by part (real, then imaginary) and the
+        two results are combined."""
         lay = self.layers[z]
+        if np.iscomplexobj(val) or np.iscomplexobj(lay.lval) or np.iscomplexobj(lay.uval):
+            raise TypeError("LUProblem.fill_layer fills float64 layers with float64 values; fill a complex matrix part by "
+                            "part (real, then imaginary part into float64 arenas) and combine the two")
         active = np.zeros(self.nsupers, np.int8)
         trees, zero = my_tree_idxs(self.npdep, z), my_zero_tr_idxs(self.npdep, z)
         for f, zr in zip(trees, zero):

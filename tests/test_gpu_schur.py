@@ -1,7 +1,9 @@
 """Partial factorization on one GPU (slu_b200_schur_* and the z twins): S = A22 - A21 A11^-1 A12 against a dense NumPy
 Schur complement and exactly 0 off the stored pattern, condense / expand against dense partial solves and SciPy's
 solution of the whole system, the eliminated panels against a full factorization, determinism, the smaller plan on the
-top-separator case, a singular A22 block the partial factorization never pivots on, and every refusal."""
+top-separator case, a singular A22 block the partial factorization never pivots on, and every refusal.  The host paths
+no other test takes: schur_get and condense / expand into padded host arrays, upload of host panels, and refactoring one
+handle with new values."""
 import ctypes as C
 
 import numpy as np
@@ -12,14 +14,15 @@ import scipy.sparse.linalg as spla
 from superlu_dist_b200 import capi
 from test_scaled_parity import mixed_values, panel_coords
 from test_schur_symbolic_cpu import CASES, dense_F, schur_problem
+from test_unsym_skyline_cpu import fill
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-10
 DTYPES = [np.float64, np.complex128]
 
 
-def make(name, dtype, seed=7):
-    """-> (problem of dtype, (rowptr, colind, values), s, F = P A P^T dense)"""
+def make(name, dtype, seed=7, dense=True):
+    """-> (problem of dtype, (rowptr, colind, values), s, F = P A P^T dense, None unless dense)"""
     prob, (rp, ci, v), schur = schur_problem(name)
     cx = np.dtype(dtype).kind == "c"
     vals = mixed_values(rp, ci, v, seed, cx)
@@ -28,7 +31,7 @@ def make(name, dtype, seed=7):
         for lay in prob.layers.values():
             lay.lval = lay.lval.astype(np.complex128)
             lay.uval = lay.uval.astype(np.complex128)
-    return prob, (rp, ci, vals), len(schur), dense_F(rp, ci, vals, np.asarray(prob.perm))
+    return prob, (rp, ci, vals), len(schur), dense_F(rp, ci, vals, np.asarray(prob.perm)) if dense else None
 
 
 def schur_ref(F, n1):
@@ -212,3 +215,88 @@ def test_refusals(dtype):
             assert b"needs a Schur handle" in L.slu_b200_last_error()
     ho.close()
     bh.close()
+
+
+# the host paths, on a small case and on one with a 256-row Schur panel
+HOST_CASES = ["p8_top", "p16_w256"]
+
+
+def _sentinel(dtype):
+    return np.array(-7.25 + 3.5j if np.dtype(dtype).kind == "c" else -7.25, dtype)
+
+
+@pytest.mark.parametrize("dtype", DTYPES, ids=["d", "z"])
+@pytest.mark.parametrize("name", HOST_CASES)
+def test_schur_get_padded_lds(name, dtype):
+    """lds = s + 3 (a strided device-to-host copy): the s x s block is schur()'s, the padding rows keep their values"""
+    prob, (rp, ci, vals), s, _ = make(name, dtype, dense=False)
+    h = factored(prob, rp, ci, vals, s)
+    S = h.schur()
+    lds = s + 3
+    out = np.full((s, lds), _sentinel(dtype))          # column-major s x s with leading dimension lds: out[j, i] = S(i, j)
+    pre = "slu_b200_z_" if np.dtype(dtype).kind == "c" else "slu_b200_"
+    assert getattr(capi.lib(), pre + "schur_get")(h.h, out.ctypes.data_as(C.c_void_p), lds) == 0
+    assert np.array_equal(out[:, :s].T, S)
+    assert np.all(out[:, s:] == _sentinel(dtype))
+    h.close()
+
+
+@pytest.mark.parametrize("dtype", DTYPES, ids=["d", "z"])
+@pytest.mark.parametrize("name", HOST_CASES)
+def test_condense_expand_padded_ldx(name, dtype):
+    """ldx = n + 5, nrhs = 3: the same result as ldx = n, the padding of every right-hand side untouched"""
+    prob, (rp, ci, vals), s, _ = make(name, dtype, dense=False)
+    h = factored(prob, rp, ci, vals, s)
+    n, nrhs, ldx = prob.n, 3, prob.n + 5
+    rng = np.random.default_rng(5)
+    b = rng.standard_normal((nrhs, n)).astype(dtype)
+    if np.dtype(dtype).kind == "c":
+        b = b + 1j * rng.standard_normal((nrhs, n))
+    pre = "slu_b200_z_" if np.dtype(dtype).kind == "c" else "slu_b200_"
+    for f, x0 in (("condense", b), ("expand", h.condense(b))):
+        want = getattr(h, f)(x0)                                             # ldx = n
+        buf = np.full((nrhs, ldx), _sentinel(dtype))
+        buf[:, :n] = x0
+        assert getattr(capi.lib(), pre + "schur_" + f)(h.h, buf.ctypes.data_as(C.c_void_p), ldx, nrhs) == 0
+        # the update scatter accumulates with atomics, whose order is not fixed: equal up to the last bits
+        assert np.abs(buf[:, :n] - want).max() <= 1e-14 * np.abs(want).max(), f
+        assert np.all(buf[:, n:] == _sentinel(dtype)), f
+    h.close()
+
+
+@pytest.mark.parametrize("dtype", DTYPES, ids=["d", "z"])
+@pytest.mark.parametrize("name", HOST_CASES)
+def test_upload_host_panels(name, dtype):
+    """upload() of panels filled on the host (a complex matrix part by part), then factor(): fill_csr's S"""
+    prob, (rp, ci, vals), s, _ = make(name, dtype, dense=False)
+    h0 = factored(prob, rp, ci, vals, s)
+    S0 = h0.schur()
+    h0.close()
+    fill(prob, rp, ci, vals)             # before the handle: its view points at the layer's arrays
+    h = capi.SchurHandle(prob, s)
+    h.upload()
+    assert h.factor() == 0
+    S = h.schur()
+    assert np.abs(S - S0).max() <= 1e-13 * np.abs(S0).max()
+    h.close()
+
+
+@pytest.mark.parametrize("dtype", DTYPES, ids=["d", "z"])
+@pytest.mark.parametrize("name", HOST_CASES)
+def test_refactor_with_new_values(name, dtype):
+    """fill_csr + factor a second time on one handle (the parameter sweep): the S of a fresh handle for the new values,
+    nothing left of the first"""
+    prob, (rp, ci, v1), s, _ = make(name, dtype, dense=False)
+    fresh, _, _, _ = make(name, dtype, dense=False)
+    v2 = make(name, dtype, seed=8, dense=False)[1][2]
+    h = factored(prob, rp, ci, v1, s)
+    S1 = h.schur()
+    h.fill_csr(rp, ci, v2, prob.perm)
+    assert h.factor() == 0
+    S2 = h.schur()
+    hf = factored(fresh, rp, ci, v2, s)
+    Sf = hf.schur()
+    assert np.abs(S2 - Sf).max() <= 1e-13 * np.abs(Sf).max()
+    assert np.abs(S2 - S1).max() > 0.1 * np.abs(S1).max()
+    h.close()
+    hf.close()

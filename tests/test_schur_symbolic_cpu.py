@@ -7,9 +7,10 @@ import hashlib
 import numpy as np
 import pytest
 
+from oracle import oracle
 from superlu_dist_b200 import LUProblem, hostlib
 from test_scaled_parity import mixed_values, panel_coords
-from test_unsym_skyline_cpu import upwind_matrix
+from test_unsym_skyline_cpu import fill, upwind_matrix
 
 
 # ------------------------------------------------------------------------------------------------------------ the cases
@@ -67,6 +68,44 @@ CASES = {"p8_top": _p8_top, "p8_scattered": _p8_scattered, "fem5_nodes": _fem5_n
          "p8_wide": _p8_wide, "p8_two": _p8_two, "upwind_small": _upwind_small}
 
 
+# the cases at scale: too large for a dense reference (oracle_partial is theirs); Schur panels of 160 to 1024 rows, so the
+# gather walks an L column in several passes, and eliminated supernodes wide enough for the big-tile Schur kernel
+def _p16_w256():
+    """the 256-column top separator of Poisson 16^3, one Schur supernode"""
+    rp, ci, v, perm = _poisson(16, leaf=16)
+    return rp, ci, v, _top(rp, perm, 256), perm, dict(relax=32, maxsup=256), False
+
+
+def _p20_scat():
+    """160 random unknowns of Poisson 20^3: Schur destinations shared by updates from every level"""
+    rp, ci, v, _ = _poisson(20)
+    schur = np.random.default_rng(13).choice(8000, 160, replace=False)
+    return rp, ci, v, schur, None, dict(relax=16, maxsup=128), False
+
+
+def _upwind20():
+    (rp, ci, v), perm = upwind_matrix(N=20, frac=0.5, seed=2)
+    return rp, ci, v, _top(rp, perm, 400), perm, dict(relax=16, maxsup=128, amalg=0.05), True
+
+
+def _fem18_w512():
+    """the top separator of FEM 18^3 x 3 dof (972 unknowns): Schur supernodes of 512 and 460 columns (double only: the
+    doublecomplex path caps supernodes at 256 columns)"""
+    rp, ci, v = hostlib.fem3d(18, dof=3)
+    perm = hostlib.nd_order(18, dof=3, leaf=32)
+    return rp, ci, v, _top(rp, perm, 972), perm, dict(relax=64, maxsup=512), False
+
+
+def _p32_top():
+    """the 1024-unknown top separator of Poisson 32^3 in four 256-column supernodes"""
+    rp, ci, v, perm = _poisson(32, leaf=64)
+    return rp, ci, v, _top(rp, perm, 1024), perm, dict(relax=32, maxsup=256), False
+
+
+SCALE_CASES = {"p16_w256": _p16_w256, "p20_scat": _p20_scat, "upwind20": _upwind20, "fem18_w512": _fem18_w512,
+               "p32_top": _p32_top}
+
+
 def case_perm(rp, ci, schur, perm):
     """perm[old] = new with schur[t] -> n - s + t: the geometric ND itself when it already numbers them last, else
     hostlib.schur_order"""
@@ -77,8 +116,8 @@ def case_perm(rp, ci, schur, perm):
 
 
 def schur_problem(name, layers=(0,)):
-    """-> (LUProblem with nschur, (rowptr, colind, |values|), schur)"""
-    rp, ci, v, schur, perm, kw, prune = CASES[name]()
+    """-> (LUProblem with nschur, (rowptr, colind, |values|), schur); name from CASES or SCALE_CASES"""
+    rp, ci, v, schur, perm, kw, prune = (CASES[name] if name in CASES else SCALE_CASES[name])()
     perm = case_perm(rp, ci, schur, perm)
     prob = LUProblem.from_matrix(rp, ci, v, perm, layers=() if prune else layers, nschur=len(schur), **kw)
     if prune:
@@ -105,6 +144,28 @@ def partial_eliminate(F, n1):
         W[k + 1:, k] /= W[k, k]
         W[k + 1:, k + 1:] -= np.outer(W[k + 1:, k], W[k, k + 1:])
     return W
+
+
+def schur_panels(prob, layer, coords=None):
+    """S (s, s) read from the Schur panels of layer: every stored entry (r, c) with r, c >= n - s (coords: panel_coords)"""
+    n1 = prob.n - prob.nschur
+    lrow, lcol, urow, ucol = panel_coords(prob, layer) if coords is None else coords
+    S = np.zeros((prob.nschur,) * 2, layer.lval.dtype)
+    for r, c, v in ((lrow, lcol, layer.lval), (urow, ucol, layer.uval)):
+        m = (r >= n1) & (c >= n1)
+        S[r[m] - n1, c[m] - n1] = v[m]
+    return S
+
+
+def oracle_partial(prob, rp, ci, vals):
+    """The oracle's partial elimination, a reference that scales: layer 0 filled with vals (float64, or complex128 part by
+    part), its eliminated supernodes 0 .. k1 - 1 (columns 0 .. n - s - 1) factored in place by oracle.factor_nodes, which
+    leaves S = A22 - A21 A11^-1 A12 in the Schur panels.  -> (info, S (s, s), layer)"""
+    fill(prob, rp, ci, vals)
+    lay = prob.layers[0]
+    k1 = int(np.searchsorted(np.asarray(prob.xsup), prob.n - prob.nschur))
+    info, _, _ = oracle.factor_nodes(prob, lay, np.arange(k1))
+    return info, schur_panels(prob, lay), lay
 
 
 # ------------------------------------------------------------------------------------------------------------ the tests
@@ -173,3 +234,68 @@ def test_schur_order_rejects_bad_sets():
         hostlib.schur_order(rp, ci, [64])
     with pytest.raises(ValueError):
         hostlib.Symbolic(64, rp, ci, None, nschur=65)
+
+
+@pytest.mark.parametrize("complex_", [False, True], ids=["d", "z"])
+@pytest.mark.parametrize("name", sorted(CASES))
+def test_oracle_partial_matches_dense(name, complex_):
+    """oracle_partial, the reference of the GPU tests at scale, against the dense A22 - A21 A11^-1 A12 of every small
+    case on sign-indefinite values; S is read from the panels, so every entry off the stored pattern is 0 there too"""
+    prob, (rp, ci, v), schur = schur_problem(name)
+    vals = mixed_values(rp, ci, v, seed=5, complex_=complex_)
+    n1 = prob.n - len(schur)
+    assert prob.nschur == len(schur)
+    info, S, lay = oracle_partial(prob, rp, ci, vals)
+    assert info == 0
+    assert lay.lval.dtype == (np.complex128 if complex_ else np.float64)
+    F = dense_F(rp, ci, vals, np.asarray(prob.perm))
+    Sref = F[n1:, n1:] - F[n1:, :n1] @ np.linalg.solve(F[:n1, :n1], F[:n1, n1:])
+    assert np.abs(S - Sref).max() <= 1e-13 * np.abs(Sref).max(), np.abs(S - Sref).max() / np.abs(Sref).max()
+
+
+def _big_tile_sources(prob, n1):
+    """eliminated supernodes with m, n >= 96 (updates of the big-tile Schur kernel), from the symbolic structure"""
+    ns = np.diff(np.asarray(prob.xsup)).astype(np.int64)
+    m = np.asarray(prob.lidx)[np.asarray(prob.lidx_off)[:-1] + 1].astype(np.int64) - ns
+    nu = np.asarray(prob.uval_len, np.int64) // np.maximum(ns, 1)
+    return int(((m >= 96) & (nu >= 96) & (np.asarray(prob.xsup)[:-1] < n1)).sum())
+
+
+# (s, widths of the Schur supernodes): every case has eliminated sources for the big-tile kernel and a Schur panel of
+# more than 128 rows; the three largest have L columns of more than 512 rows, several passes of the gather's loop
+SCALE_SHAPES = {"p16_w256": (256, [256]), "p20_scat": (160, [128, 32]), "upwind20": (400, [128, 128, 128, 16]),
+                "fem18_w512": (972, [512, 460]), "p32_top": (1024, [256] * 4)}
+
+
+@pytest.mark.parametrize("name", sorted(SCALE_CASES))
+def test_scale_cases_have_their_shape(name):
+    prob, _, schur = schur_problem(name, layers=())
+    s, widths = SCALE_SHAPES[name]
+    n1 = prob.n - s
+    xsup = np.asarray(prob.xsup)
+    assert len(schur) == s and n1 in xsup
+    assert sorted(np.diff(xsup[xsup >= n1]).tolist(), reverse=True) == widths
+    assert _big_tile_sources(prob, n1) > 0
+    nsupr = int(prob.lidx[prob.lidx_off[int(np.searchsorted(xsup, n1))] + 1])     # rows of the first Schur L panel
+    assert nsupr == s and (nsupr > 512) == (s > 512)
+
+
+def test_fill_layer_refuses_complex():
+    """the host fill writes doubles: complex values, or a complex128 layer, would be silently corrupted"""
+    prob, (rp, ci, v), _ = schur_problem("p8_top")
+    vals = mixed_values(rp, ci, v, seed=5, complex_=True)
+    before = prob.layers[0].lval.copy()
+    with pytest.raises(TypeError, match="part by part"):
+        prob.fill_layer(0, rp, ci, vals)
+    assert np.array_equal(prob.layers[0].lval, before)
+    prob.dtype = np.dtype(np.complex128)
+    prob.add_layer(0)
+    with pytest.raises(TypeError, match="part by part"):
+        prob.fill_layer(0, rp, ci, vals.real)
+    # the part-by-part fill gives the values of each part exactly
+    fill(prob, rp, ci, vals)
+    re, im = schur_problem("p8_top")[0], schur_problem("p8_top")[0]
+    re.fill_layer(0, rp, ci, vals.real)
+    im.fill_layer(0, rp, ci, vals.imag)
+    assert np.array_equal(prob.layers[0].lval, re.layers[0].lval + 1j * im.layers[0].lval)
+    assert np.array_equal(prob.layers[0].uval, re.layers[0].uval + 1j * im.layers[0].uval)

@@ -107,8 +107,10 @@ def values(name, complex_=False, seed=0):
 
 
 def fill(prob, rp, ci, vals, z=0):
-    """Layer z of prob holding vals (LUProblem.fill_layer takes float64: a complex matrix goes in part by part)."""
+    """Layer z of prob holding vals (LUProblem.fill_layer takes float64 only: a complex matrix goes in part by part)."""
     lay = prob.add_layer(z) if z not in prob.layers else prob.layers[z]
+    if np.iscomplexobj(lay.lval):       # a complex layer (refilled, or added after an earlier complex fill)
+        lay.lval, lay.uval = np.zeros(len(lay.lval)), np.zeros(len(lay.uval))
     if not np.iscomplexobj(vals):
         prob.fill_layer(z, rp, ci, vals)
         return prob
