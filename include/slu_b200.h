@@ -218,7 +218,8 @@ int slu_b200_logdet(slu_b200_handle_t h, double *logabs, double *sign);
  * with world_size 1 and the int8 tensor-core path is off (options.reserved[4] <= 0; FP64 DMMA only, as on batched handles).
  * A Schur handle takes slu_b200_upload, _fill_csr, _factor, _download, _get_stats, _destroy and the schur_* calls below;
  * factor_host, solve, solve_trans, gscon, selinv, selinv_get, logdet, the batch_* and kernel-export calls fail on it with
- * a message and leave it usable, and the schur_* calls fail on ordinary and batched handles.  factor eliminates the
+ * a message and leave it usable, and the schur_* calls fail on ordinary and batched handles (batched Schur handles:
+ * slu_b200_batch_schur_create and the batch_schur_* calls below).  factor eliminates the
  * non-Schur supernodes only: info = 0 or the 1-based column of the first exact zero pivot among them; ops_fact, ops_schur,
  * nlevels and my_supernodes count the eliminated work.  download writes L11, U11, L21 and U12, and S in the Schur panels,
  * in the reference layout.
@@ -330,6 +331,32 @@ int slu_b200_batch_selinv_get(slu_b200_handle_t h, int n, const int32_t *rowptr,
 /* logabs[batch], sign[batch]: every member's log|det A_j| and sign, as slu_b200_logdet (needs no batch_selinv).  Fails,
  * naming the member, unless every member's last info was 0. */
 int slu_b200_batch_logdet(slu_b200_handle_t h, double *logabs, double *sign);
+/* Partial factorization on batched handles: the slu_b200_schur_* calls for `batch` matrices of one pattern (substructuring
+ * with many same-mesh subdomains, static condensation of many element matrices, Kron reduction of network ensembles,
+ * parameter sweeps of marginal precision matrices).
+ * batch_schur_create: the checks of batch_create and of schur_create (1 <= batch <= 65535, 1 <= nschur < n, n - nschur a
+ * supernode boundary, 1 x 1 x 1 grid with world_size 1, int8 path off), with messages that name batch_schur_create.  The
+ * handle takes batch_fill_csr, batch_factor, batch_download, get_stats, destroy and the four batch_schur_* calls;
+ * batch_solve, batch_solve_trans, batch_gscon, batch_selinv, batch_selinv_get and batch_logdet fail on it with a message
+ * ("Schur handle") and leave it usable, the unbatched schur_* calls fail on it ("batched handle"), and the batch_schur_*
+ * calls fail on ordinary, plain batched and unbatched Schur handles.  batch_factor eliminates A11 of every member in one
+ * launch sequence (the launches of one unbatched Schur factorization, each over batch x the CTAs): info[j] = 0 or the
+ * 1-based column of member j's first exact zero pivot among the eliminated supernodes.  batch_download(j) writes member
+ * j's L11, U11, L21, U12 and S.  Stats: batch x the per-member eliminated work (ops_fact, ops_schur); nlevels and
+ * my_supernodes those of the eliminated part.
+ * batch_schur_get: every member's S, member j's s x s block at S + j*lds*s (lds >= s), as schur_get: one gather launch
+ * over (units, members) into a zeroed batch x s x s HBM buffer (allocated on first use, kept until destroy; if it does not
+ * fit, the call fails with its size and the handle stays usable), then one copy; entries off the stored pattern are
+ * exactly 0 and two calls are bit-identical.  stats.reserved[6] = seconds of the call, [7] = device ms of the gather.
+ * batch_schur_condense / batch_schur_expand: the forward / backward pass of slu_b200_batch_solve over the eliminated
+ * supernodes (as schur_condense / schur_expand for every member); x, ldx, nrhs and the checks as batch_solve (n * nrhs
+ * below 2^31 per member); they set stats.reserved[4] / [5].
+ * All but create fail, naming the member, unless every member's last info was 0. */
+int slu_b200_batch_schur_create(slu_b200_handle_t *h, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt,
+                                int batch, int nschur);
+int slu_b200_batch_schur_get(slu_b200_handle_t h, double *S, int lds);
+int slu_b200_batch_schur_condense(slu_b200_handle_t h, double *x, int ldx, int nrhs);
+int slu_b200_batch_schur_expand(slu_b200_handle_t h, double *x, int ldx, int nrhs);
 /* ---- doublecomplex twins (SRC/complex16/pzgstrf3d.c:120; the reference's z* handle API,
  * SRC/include/superlu_upacked.h:84-97).  Same view/options/stats structs: the Lnzval_bc_ptr / Unzval_br_ptr
  * entries point at arrays of doublecomplex {double r, i} (SRC/include/dcomplex.h:30) and are declared double*
@@ -393,6 +420,13 @@ int slu_b200_z_batch_selinv(slu_b200_zhandle_t h, double out[4]);
 int slu_b200_z_batch_selinv_get(slu_b200_zhandle_t h, int n, const int32_t *rowptr, const int32_t *colind,
                                 const int32_t *perm, double *out);
 int slu_b200_z_batch_logdet(slu_b200_zhandle_t h, double *logabs, double *sign);
+/* as slu_b200_batch_schur_create / _get / _condense / _expand, with the same restrictions and messages; S and x hold
+ * interleaved doublecomplex, lds and ldx count complex elements. */
+int slu_b200_z_batch_schur_create(slu_b200_zhandle_t *h, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt,
+                                  int batch, int nschur);
+int slu_b200_z_batch_schur_get(slu_b200_zhandle_t h, double *S, int lds);
+int slu_b200_z_batch_schur_condense(slu_b200_zhandle_t h, double *x, int ldx, int nrhs);
+int slu_b200_z_batch_schur_expand(slu_b200_zhandle_t h, double *x, int ldx, int nrhs);
 int slu_b200_z_get_stats(slu_b200_zhandle_t h, slu_b200_stats_t *out);
 int slu_b200_z_plan(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, slu_b200_stats_t *stats);
 void slu_b200_z_destroy(slu_b200_zhandle_t h);

@@ -136,6 +136,13 @@ def lib():
         getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_int]
     for f in ("slu_b200_schur_condense", "slu_b200_z_schur_condense", "slu_b200_schur_expand", "slu_b200_z_schur_expand"):
         getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
+    for f in ("slu_b200_batch_schur_create", "slu_b200_z_batch_schur_create"):
+        getattr(L, f).argtypes = [C.POINTER(C.c_void_p), C.POINTER(LUView), C.POINTER(Options), C.c_int, C.c_int]
+    for f in ("slu_b200_batch_schur_get", "slu_b200_z_batch_schur_get"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+    for f in ("slu_b200_batch_schur_condense", "slu_b200_z_batch_schur_condense", "slu_b200_batch_schur_expand",
+              "slu_b200_z_batch_schur_expand"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
     _lib = L
     return L
 
@@ -543,6 +550,53 @@ class BatchHandle:
             self.close()
         except Exception:
             pass
+
+
+class BatchSchurHandle(BatchHandle):
+    """A partial factorization of `batch` matrices with the pattern of `prob` (slu_b200_batch_schur_create /
+    slu_b200_z_batch_schur_create): as SchurHandle for every member, with the values, info and downloads of BatchHandle.
+    fill_csr / factor / download as BatchHandle; schur() returns every member's S, condense / expand the two partial
+    solves.  solve, rcond, selinv, inv_entries, inv_diag and logdet fail on it."""
+
+    def __init__(self, prob, batch, nschur, **opt):
+        require_gpu()
+        self.prob, self.batch, self.nschur = prob, int(batch), int(nschur)
+        self.z_ = _is_complex(prob.dtype)
+        self.view, self._keep = make_view(prob, 0)
+        self.opt = make_options(prob, **opt)
+        self.h = C.c_void_p()
+        _check(_fn("batch_schur_create", self.z_)(C.byref(self.h), C.byref(self.view), C.byref(self.opt), self.batch,
+                                                  self.nschur))
+
+    def schur(self, out=None):
+        """(batch, s, s), float64 or complex128: [j] = S_j, row / column t is unknown n - s + t of the factored ordering;
+        exactly 0 off the stored pattern.  out: a C-contiguous (batch, s, s) array of that dtype to write into instead of a
+        new one (batch x s^2 values: reusing a buffer saves the page faults of fresh host memory on every call)."""
+        s = self.nschur
+        shape = (self.batch, s, s)
+        if out is None:
+            out = np.empty(shape, self._dtype())
+        elif out.shape != shape or out.dtype != self._dtype() or not out.flags.c_contiguous:
+            raise ValueError(f"out must be a C-contiguous {np.dtype(self._dtype()).name} array of shape {shape}")
+        # member j's block is s x s column-major at j * s * s: a C-ordered (batch, s, s) array holds S_j^T in out[j]
+        _check(_fn("batch_schur_get", self.z_)(self.h, out.ctypes.data_as(C.c_void_p), s))
+        return out.transpose(0, 2, 1)
+
+    def _pass(self, name, b):
+        x = np.array(b, self._dtype(), order="C", copy=True)
+        if x.ndim not in (2, 3) or x.shape[0] != self.batch or x.shape[-1] != self.prob.n:
+            raise ValueError(f"b must have shape ({self.batch}, n) or ({self.batch}, nrhs, n) with n = {self.prob.n}")
+        nrhs = 1 if x.ndim == 2 else x.shape[1]
+        _check(_fn(name, self.z_)(self.h, x.ctypes.data_as(C.c_void_p), self.prob.n, nrhs))
+        return x
+
+    def condense(self, b):
+        """b: (batch, n) or (batch, nrhs, n), as SchurHandle.condense for every member"""
+        return self._pass("batch_schur_condense", b)
+
+    def expand(self, y):
+        """y: condense's result with x2 in the last s positions of every member, as SchurHandle.expand"""
+        return self._pass("batch_schur_expand", y)
 
 
 def pdgstrf3d(prob, z=0, **opt):

@@ -56,6 +56,10 @@
 #define slu_b200_schur_get slu_b200_z_schur_get
 #define slu_b200_schur_condense slu_b200_z_schur_condense
 #define slu_b200_schur_expand slu_b200_z_schur_expand
+#define slu_b200_batch_schur_create slu_b200_z_batch_schur_create
+#define slu_b200_batch_schur_get slu_b200_z_batch_schur_get
+#define slu_b200_batch_schur_condense slu_b200_z_batch_schur_condense
+#define slu_b200_batch_schur_expand slu_b200_z_batch_schur_expand
 #define SLU_API "slu_b200_z_"     // name prefix of the exported calls, for error messages
 #else
 #define SLU_API "slu_b200_"
@@ -313,8 +317,8 @@ struct slu_b200_handle_s {
     bool si_ready = false;
     // partial factorization (slu_b200_schur_create): the supernodes from column schur_first = n - nschur on are in no level
     // of the plan, so factor, condense and expand stop at them; d_sunits lists the gather's (supernode, column) units and
-    // d_S is the s x s buffer of slu_b200_schur_get (allocated on first use, freed by destroy).  nschur = 0: not a Schur
-    // handle.
+    // d_S is the s x s buffer of slu_b200_schur_get, batch x s x s on a batched Schur handle (slu_b200_batch_schur_get;
+    // allocated on first use, freed by destroy).  nschur = 0: not a Schur handle.
     int nschur = 0, schur_first = INT_MAX;
     DevBuf<int2> d_sunits;
     DevBuf<val_t> d_S;
@@ -1302,11 +1306,13 @@ int refuse_batched(const slu_b200_handle_s *H, const char *fn)
     return H->batch ? fail("%s on a batched handle (%d members): use the " SLU_API "batch_* calls", fn, H->batch) : 0;
 }
 
-// a Schur handle (slu_b200_schur_create) takes upload, fill_csr, factor, download, get_stats, destroy and the schur_* calls
+// a Schur handle (slu_b200_schur_create) takes upload, fill_csr, factor, download, get_stats, destroy and the schur_* calls;
+// a batched one (slu_b200_batch_schur_create) batch_fill_csr, batch_factor, batch_download, get_stats, destroy and the
+// batch_schur_* calls
 int refuse_schur(const slu_b200_handle_s *H, const char *fn)
 {
-    return H->nschur ? fail("%s on a Schur handle (partial factorization, nschur = %d): its factors are incomplete; use the "
-                            SLU_API "schur_* calls", fn, H->nschur) : 0;
+    return H->nschur ? fail("%s on a Schur handle (partial factorization, nschur = %d): its factors are incomplete; use the %s calls",
+                            fn, H->nschur, H->batch ? SLU_API "batch_schur_*" : SLU_API "schur_*") : 0;
 }
 
 }  // namespace
@@ -1396,14 +1402,15 @@ void slu_b200_destroy(slu_b200_handle_t H)
 }
 
 // batch > 0: a batched handle (slu_b200_batch_create), 1 x 1 x 1 grid, FP64 DMMA kernels only
-// nschur > 0: a Schur handle (slu_b200_schur_create), 1 x 1 x 1 grid, FP64 DMMA kernels only
+// nschur > 0: a Schur handle (slu_b200_schur_create), 1 x 1 x 1 grid, FP64 DMMA kernels only; with batch > 0 a batched one
+// (slu_b200_batch_schur_create)
 static int create_impl(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, int batch, int nschur = 0)
 {
     if (!out || !lu || !opt) return fail("null argument");
     *out = nullptr;
     if (opt->schur_variant != 0) return fail("options.schur_variant is retired and must be 0 (got %d)", opt->schur_variant);
     if (nschur) {
-        const char *fn = SLU_API "schur_create";
+        const char *fn = batch ? SLU_API "batch_schur_create" : SLU_API "schur_create";
         if (nschur < 1 || nschur >= lu->n) return fail("%s: nschur = %d, must satisfy 1 <= nschur < n = %d", fn, nschur, lu->n);
         if (lu->nprow != 1 || lu->npcol != 1 || lu->npdep != 1 || opt->world_size > 1)
             return fail("%s handles 1 x 1 x 1 grids (world_size 1)", fn);
@@ -2111,6 +2118,7 @@ int slu_b200_logdet(slu_b200_handle_t H, double *logabs, double *sign)
 static int schur_refuse(const slu_b200_handle_s *H, const char *fn)
 {
     if (!H->nschur) return fail("%s needs a Schur handle (" SLU_API "schur_create)", fn);
+    if (refuse_batched(H, fn)) return -1;     // a batched Schur handle: the batch_schur_* calls
     if (!H->factored) return fail("%s needs a successful " SLU_API "factor (info = 0) on this handle first", fn);
     return 0;
 }
@@ -2124,19 +2132,21 @@ int slu_b200_schur_create(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, 
     return create_impl(out, lu, opt, 0, nschur);
 }
 
-int slu_b200_schur_get(slu_b200_handle_t H, double *S, int lds)
+// S of every member (one on an unbatched handle) into the host array S: member j's s x s block at S + j * lds * s.  The
+// caller has checked the handle.
+static int schur_get_impl(slu_b200_handle_t H, double *S, int lds, const char *fn)
 {
-    if (!H || !S) return fail("null argument");
-    const char *fn = SLU_API "schur_get";
-    if (schur_refuse(H, fn)) return -1;
-    const int s = H->nschur;
+    const int s = H->nschur, B = H->batch ? H->batch : 1;
     if (lds < s) return fail("%s: lds = %d, must be >= nschur = %d", fn, lds, s);
     const double t0 = now_s();
-    const size_t elems = (size_t)s * s;
+    const size_t elems = (size_t)s * s * B;
     if (!H->d_S.p && H->d_S.alloc(elems)) {
         const std::string why = g_err;
         H->d_S.release();
         cudaGetLastError();
+        if (H->batch)
+            return fail("%s: the %d Schur complements of %d x %d need %.2f GB of HBM: %s", fn, B, s, s,
+                        1e-9 * (double)(elems * sizeof(val_t)), why.c_str());
         return fail("%s: the %d x %d Schur complement needs %.2f GB of HBM: %s", fn, s, s, 1e-9 * (double)(elems * sizeof(val_t)),
                     why.c_str());
     }
@@ -2145,13 +2155,14 @@ int slu_b200_schur_get(slu_b200_handle_t H, double *S, int lds)
     cudaStream_t st = H->stream;
     CU(cudaMemsetAsync(H->d_S.p, 0, elems * sizeof(val_t), st));
     CU(cudaEventRecord(ev[0], st));
-    launch_schur_gather(H->dev, H->d_sunits.p, (int64_t)H->d_sunits.n, H->schur_first, s, H->d_S.p, st);
+    if (H->batch) launch_schur_gather(H->bdev, H->d_sunits.p, (int64_t)H->d_sunits.n, H->schur_first, s, H->d_S.p, st);
+    else launch_schur_gather(H->dev, H->d_sunits.p, (int64_t)H->d_sunits.n, H->schur_first, s, H->d_S.p, st);
     CU(cudaEventRecord(ev[1], st));
     if (lds == s)   // one contiguous copy
         CU(cudaMemcpyAsync(S, H->d_S.p, elems * sizeof(val_t), cudaMemcpyDeviceToHost, st));
-    else
-        CU(cudaMemcpy2DAsync(S, (size_t)lds * sizeof(val_t), H->d_S.p, (size_t)s * sizeof(val_t), (size_t)s * sizeof(val_t), (size_t)s,
-                             cudaMemcpyDeviceToHost, st));
+    else            // the B blocks are B * s columns at pitch lds
+        CU(cudaMemcpy2DAsync(S, (size_t)lds * sizeof(val_t), H->d_S.p, (size_t)s * sizeof(val_t), (size_t)s * sizeof(val_t),
+                             (size_t)s * B, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
     float ms = 0;
@@ -2159,6 +2170,14 @@ int slu_b200_schur_get(slu_b200_handle_t H, double *S, int lds)
     H->st.reserved[6] = now_s() - t0;      // seconds of the call
     H->st.reserved[7] = ms;                // device milliseconds of the gather kernel
     return 0;
+}
+
+int slu_b200_schur_get(slu_b200_handle_t H, double *S, int lds)
+{
+    if (!H || !S) return fail("null argument");
+    const char *fn = SLU_API "schur_get";
+    if (schur_refuse(H, fn)) return -1;
+    return schur_get_impl(H, S, lds, fn);
 }
 
 // condense: the forward pass over the plan; expand: the backward pass.  x: host, n x nrhs (ldx >= n), ordering of F.
@@ -2210,14 +2229,37 @@ static int refuse_unbatched(const slu_b200_handle_s *H, const char *fn)
     return H->batch ? 0 : fail("%s on an unbatched handle: use the " SLU_API "* calls without _batch", fn);
 }
 
+// the calls that read the factors need every member's last batch_factor to have succeeded
+static int refuse_unfactored_members(const slu_b200_handle_s *H, const char *fn)
+{
+    for (int j = 0; j < H->batch; ++j) {
+        if (H->member_info[j] < 0) return fail("%s needs a " SLU_API "batch_factor of the filled members first", fn);
+        if (H->member_info[j] > 0) return fail("%s: member %d has an exact zero pivot in column %d", fn, j, H->member_info[j]);
+    }
+    return 0;
+}
+
+// the batch_schur_* calls (on a batched handle: refuse_unbatched first)
+static int refuse_not_batch_schur(const slu_b200_handle_s *H, const char *fn)
+{
+    return H->nschur ? 0 : fail("%s needs a batched Schur handle (" SLU_API "batch_schur_create)", fn);
+}
+
+// the checks of batch_create and batch_schur_create (fn) before create_impl
+static int batch_create_check(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, int batch, const char *fn)
+{
+    if (batch < 1 || batch > 65535) return fail("%s: batch = %d, must be 1 ... 65535", fn, batch);
+    if (lu->nprow != 1 || lu->npcol != 1 || lu->npdep != 1)
+        return fail("%s: batched handles need a 1 x 1 x 1 grid (got %d x %d x %d)", fn, lu->nprow, lu->npcol, lu->npdep);
+    if (opt->world_size > 1) return fail("%s: batched handles are single-GPU (world_size = %d)", fn, opt->world_size);
+    return 0;
+}
+
 int slu_b200_batch_create(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, int batch)
 {
     if (!out || !lu || !opt) return fail("null argument");
     *out = nullptr;
-    if (batch < 1 || batch > 65535) return fail(SLU_API "batch_create: batch = %d, must be 1 ... 65535", batch);
-    if (lu->nprow != 1 || lu->npcol != 1 || lu->npdep != 1)
-        return fail(SLU_API "batch_create: batched handles need a 1 x 1 x 1 grid (got %d x %d x %d)", lu->nprow, lu->npcol, lu->npdep);
-    if (opt->world_size > 1) return fail(SLU_API "batch_create: batched handles are single-GPU (world_size = %d)", opt->world_size);
+    if (batch_create_check(lu, opt, batch, SLU_API "batch_create")) return -1;
     return create_impl(out, lu, opt, batch);
 }
 
@@ -2322,26 +2364,35 @@ int slu_b200_batch_factor(slu_b200_handle_t H, int *info)
     return 0;
 }
 
+// The passes of a batched solve: both for a solve; on a batched Schur handle the forward one alone is batch_schur_condense,
+// the backward one batch_schur_expand.
+enum { PASS_FORWARD = 1, PASS_BACKWARD = 2, PASS_BOTH = 3 };
+
 // The solve of a batched handle on device vectors, in place in d_x (batch blocks of n x nrhs).  Enqueued on H->stream, not
 // synchronised.  Returns the kernel launches.
-static int batch_solve_dev(slu_b200_handle_t H, int nrhs, int trans)
+static int batch_solve_dev(slu_b200_handle_t H, int nrhs, int trans, int passes = PASS_BOTH)
 {
     const BatchedLU &d = H->bdev;
     val_t *x = H->d_x.p;
     int launches = 0;
-    for (size_t li = 0; li < H->levels.size(); ++li)            // forward: L y = b (U^T y = b)
-        launches += solve_level(H, d, H->levels[li], false, trans, x, H->n, nrhs, H->stream);
-    for (size_t li = H->levels.size(); li-- > 0;)               // backward: U x = y (L^T x = y)
-        launches += solve_level(H, d, H->levels[li], true, trans, x, H->n, nrhs, H->stream);
+    if (passes & PASS_FORWARD)
+        for (size_t li = 0; li < H->levels.size(); ++li)        // forward: L y = b (U^T y = b)
+            launches += solve_level(H, d, H->levels[li], false, trans, x, H->n, nrhs, H->stream);
+    if (passes & PASS_BACKWARD)
+        for (size_t li = H->levels.size(); li-- > 0;)           // backward: U x = y (L^T x = y)
+            launches += solve_level(H, d, H->levels[li], true, trans, x, H->n, nrhs, H->stream);
     return launches;
 }
 
 // x: batch blocks, block j at x + j * ldx * nrhs, each n x nrhs column-major (ldx >= n): b on entry, the solution on return.
-// trans as solve_impl; fn: "batch_solve" or "batch_solve_trans", for the messages
-static int batch_solve_impl(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int trans, const char *fn)
+// trans as solve_impl; fn: "batch_solve", "batch_solve_trans", "batch_schur_condense" or "batch_schur_expand", for the
+// messages.  passes = PASS_BOTH (a solve) needs complete factors, a single pass a batched Schur handle.
+static int batch_solve_impl(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int trans, const char *fn, int passes = PASS_BOTH)
 {
     if (!H || !xh) return fail("null argument");
-    if (refuse_unbatched(H, (std::string(SLU_API) + fn).c_str())) return -1;
+    const std::string name = std::string(SLU_API) + fn;
+    if (refuse_unbatched(H, name.c_str())) return -1;
+    if (passes == PASS_BOTH ? refuse_schur(H, name.c_str()) : refuse_not_batch_schur(H, name.c_str())) return -1;
     if (trans < 0 || trans > 2) return fail(SLU_API "%s: trans = %d, must be 0 (A x = b), 1 (A^T x = b) or 2 (A^H x = b)", fn, trans);
     const int B = H->batch, n = H->n;
     for (int j = 0; j < B; ++j) {
@@ -2358,7 +2409,7 @@ static int batch_solve_impl(slu_b200_handle_t H, double *xh, int ldx, int nrhs, 
     // the B blocks are B * nrhs columns at pitch ldx: one 2D copy each way
     CU(cudaMemcpy2DAsync(x, (size_t)n * sizeof(val_t), xh, (size_t)ldx * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs * B,
                          cudaMemcpyHostToDevice, s));
-    const int launches = batch_solve_dev(H, nrhs, trans);
+    const int launches = batch_solve_dev(H, nrhs, trans, passes);
     CU(cudaMemcpy2DAsync(xh, (size_t)ldx * sizeof(val_t), x, (size_t)n * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs * B,
                          cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
@@ -2465,7 +2516,7 @@ int slu_b200_gscon(slu_b200_handle_t H, char norm, double anorm, double *rcond)
 int slu_b200_batch_gscon(slu_b200_handle_t H, char norm, const double *anorm, double *rcond)
 {
     if (!H || !anorm || !rcond) return fail("null argument");
-    if (refuse_unbatched(H, SLU_API "batch_gscon")) return -1;
+    if (refuse_unbatched(H, SLU_API "batch_gscon") || refuse_schur(H, SLU_API "batch_gscon")) return -1;
     for (int j = 0; j < H->batch; ++j) {
         if (H->member_info[j] < 0) return fail(SLU_API "batch_gscon needs a " SLU_API "batch_factor of the filled members first");
         if (H->member_info[j] > 0) return fail(SLU_API "batch_gscon: member %d has an exact zero pivot in column %d", j, H->member_info[j]);
@@ -2490,12 +2541,8 @@ int slu_b200_batch_download(slu_b200_handle_t H, int member)
 // member_len elements apart as the members' factors are.
 static int batch_selinv_refuse(const slu_b200_handle_s *H, const char *fn)
 {
-    if (refuse_unbatched(H, fn)) return -1;
-    for (int j = 0; j < H->batch; ++j) {
-        if (H->member_info[j] < 0) return fail("%s needs a " SLU_API "batch_factor of the filled members first", fn);
-        if (H->member_info[j] > 0) return fail("%s: member %d has an exact zero pivot in column %d", fn, j, H->member_info[j]);
-    }
-    return 0;
+    if (refuse_unbatched(H, fn) || refuse_schur(H, fn)) return -1;
+    return refuse_unfactored_members(H, fn);
 }
 
 int slu_b200_batch_selinv(slu_b200_handle_t H, double out[4])
@@ -2559,6 +2606,39 @@ int slu_b200_batch_logdet(slu_b200_handle_t H, double *logabs, double *sign)
         for (int c = 0; c < VAL_DOUBLES; ++c) sign[(size_t)j * VAL_DOUBLES + c] = r[(size_t)j * (1 + VAL_DOUBLES) + 1 + c];
     }
     return 0;
+}
+
+// ---- partial factorization on batched handles: a batched handle whose level plan leaves out the Schur supernodes, as an
+// unbatched Schur handle's does.  batch_factor eliminates A11 of every member, the gather runs over (units, members), and
+// condense / expand are the forward / backward pass of batch_solve_impl over the same plan.
+int slu_b200_batch_schur_create(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, int batch,
+                                int nschur)
+{
+    if (!out || !lu || !opt) return fail("null argument");
+    *out = nullptr;
+    const char *fn = SLU_API "batch_schur_create";
+    if (batch_create_check(lu, opt, batch, fn)) return -1;
+    if (nschur < 1 || nschur >= lu->n) return fail("%s: nschur = %d, must satisfy 1 <= nschur < n = %d", fn, nschur, lu->n);
+    return create_impl(out, lu, opt, batch, nschur);
+}
+
+// S: batch blocks of s x s, member j's at S + j * lds * s
+int slu_b200_batch_schur_get(slu_b200_handle_t H, double *S, int lds)
+{
+    if (!H || !S) return fail("null argument");
+    const char *fn = SLU_API "batch_schur_get";
+    if (refuse_unbatched(H, fn) || refuse_not_batch_schur(H, fn) || refuse_unfactored_members(H, fn)) return -1;
+    return schur_get_impl(H, S, lds, fn);
+}
+
+int slu_b200_batch_schur_condense(slu_b200_handle_t H, double *x, int ldx, int nrhs)
+{
+    return batch_solve_impl(H, x, ldx, nrhs, 0, "batch_schur_condense", PASS_FORWARD);
+}
+
+int slu_b200_batch_schur_expand(slu_b200_handle_t H, double *x, int ldx, int nrhs)
+{
+    return batch_solve_impl(H, x, ldx, nrhs, 0, "batch_schur_expand", PASS_BACKWARD);
 }
 
 int slu_b200_get_stats(slu_b200_handle_t H, slu_b200_stats_t *out)

@@ -269,6 +269,9 @@ int launch_selinv_get(const BatchedLU &d, const val_t *hv, int n, const int32_t 
 // column-major buffer (ld s); units[u] = (supernode k, column c): c < ns is column c of L panel k (diagonal block included),
 // c >= ns the skyline segment of packed column c - ns of U panel k.  One launch of nunits CTAs.
 int launch_schur_gather(const DeviceLU &d, const int2 *units, int64_t nunits, int n0, int s, val_t *S, cudaStream_t st);
+// batched (slu_b200_batch_schur_get): the same launch over d.members matrices of one pattern (gridDim.y = members); S holds
+// members blocks of s x s, member j's at S + j * s * s
+int launch_schur_gather(const BatchedLU &d, const int2 *units, int64_t nunits, int n0, int s, val_t *S, cudaStream_t st);
 
 #ifdef SLU_COMPLEX
 constexpr int SCHUR_BM_BIG = 128, SCHUR_BM_SMALL = 32, SCHUR_BN_SMALL = 16;
