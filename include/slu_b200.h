@@ -207,6 +207,20 @@ int slu_b200_selinv_get(slu_b200_handle_t h, int n, const int32_t *rowptr, const
 /* log|det A| and its sign (+1 / -1) from the resident factors: sum of log |U_kk(i,i)| in a fixed order (deterministic),
  * sign from the count of negative pivots; the symmetric permutation does not change det.  Restrictions of selinv. */
 int slu_b200_logdet(slu_b200_handle_t h, double *logabs, double *sign);
+/* Inertia of a real symmetric / complex Hermitian A from the resident factors (MUMPS INFOG(12), PARDISO iparm(22..23)):
+ * F = P A P^T = L U uses a symmetric permutation, no row exchanges and a unit-diagonal L, so U = D L^T (D L^H) and by
+ * Sylvester's law the signs of the pivots u_ii are those of A's eigenvalues; for A - sigma B with B positive definite,
+ * counts[0] is the number of eigenvalues of the pencil below sigma (spectrum slicing, PEXSI's inertia counting, checking
+ * the inertia of a KKT matrix).
+ * counts[0] = pivots with u_ii < 0 (Re u_ii < 0 in doublecomplex), counts[1] = the others (counts[0] + counts[1] = n),
+ * counts[2] = pivots with |u_ii| <= options.thresh (replaced tiny pivots land exactly there), counted in 0/1 as well.
+ * *defect = max_i |Im u_ii| / |u_ii| in doublecomplex (0 for a Hermitian A up to rounding), 0 in double.
+ * The library does not check symmetry: the caller asserts it, and defect is the diagnostic for complex input.  Two limits:
+ * where a tiny pivot was replaced (options.replace_tiny_pivot) the counts describe L U as factored, not A, which is what
+ * counts[2] is for; counts[2] uses options.thresh whether or not replacement is on, so a caller that wants that count must
+ * pass a threshold.  Fixed-order integer reductions (deterministic), 2 kernel launches.  Restrictions and messages of
+ * slu_b200_logdet: a successful factorization, an unbatched handle that is not a Schur handle, a 1 x 1 x 1 grid. */
+int slu_b200_inertia(slu_b200_handle_t h, int64_t counts[3], double *defect);
 /* Partial factorization with a Schur complement (MUMPS ICNTL(19), PARDISO iparm(36)): with F = P A P^T = [A11 A12; A21 A22]
  * and the s = nschur "Schur" unknowns last, eliminate A11 only and keep S = A22 - A21 A11^-1 A12.  Uses: domain
  * decomposition (S is the interface operator), sparse-dense block coupling, Kron reduction, static condensation, marginal
@@ -287,8 +301,8 @@ int slu_b200_k_rerun_schur(slu_b200_handle_t h, int level, int reps, float *ms);
  * exactly as many kernel launches as one unbatched factorization, each over batch x the CTAs (gridDim.y = member).
  * Double precision here and doublecomplex through the slu_b200_z_batch_* twins below; 1 x 1 x 1 grid, FP64 DMMA
  * kernels only (the int8 path is not used; stats.reserved[1] = 0).
- * A batched handle takes only these calls (create, fill_csr, factor, solve, solve_trans, gscon, selinv, selinv_get,
- * logdet and download, each with the batch_ prefix) plus slu_b200_get_stats and slu_b200_destroy; every other call on it
+ * A batched handle takes only these calls (create, fill_csr, fill_affine, factor, solve, solve_trans, gscon, selinv,
+ * selinv_get, logdet, inertia and download, each with the batch_ prefix) plus slu_b200_get_stats and slu_b200_destroy; every other call on it
  * fails, and these fail on an unbatched handle.  Stats describe the whole handle: ops_fact, ops_schur, nnz_l, nnz_u and
  * lu_device_bytes are batch x the per-member values, tiny_pivots is summed over the members, t_factor_s is the device
  * time of the one batched call, stats.reserved[4] / [5] describe the last slu_b200_batch_solve or _batch_solve_trans.
@@ -331,13 +345,28 @@ int slu_b200_batch_selinv_get(slu_b200_handle_t h, int n, const int32_t *rowptr,
 /* logabs[batch], sign[batch]: every member's log|det A_j| and sign, as slu_b200_logdet (needs no batch_selinv).  Fails,
  * naming the member, unless every member's last info was 0. */
 int slu_b200_batch_logdet(slu_b200_handle_t h, double *logabs, double *sign);
+/* every member's inertia, as slu_b200_inertia: member j's counts at counts[3*j + c], its defect at defect[j]; the same two
+ * launches whatever the batch.  Fails, naming the member, unless every member's last info was 0; fails on Schur handles. */
+int slu_b200_batch_inertia(slu_b200_handle_t h, int64_t *counts, double *defect);
+/* Affine families (frequency sweeps K - w^2 M + i w C, shifted pencils A - sigma B, GMRF Q(theta) = sum_t theta_t Q_t):
+ * member j, entry p: v = sum_t coef[j*nterms + t] * terms[t*nnz + p], t = 0 .. nterms-1 in order (v = c_0 V_0, then one
+ * fused multiply-add per term; in doublecomplex the complex product of slu_scalar.cuh).  The nterms x nnz terms cross
+ * PCIe once instead of batch x nnz values, and the slot search runs once per entry, not once per member.  Otherwise as
+ * slu_b200_batch_fill_csr: one CSR pattern (rowptr, colind) and perm shared by all members, the arena zeroed first (fill-in
+ * slots are 0), each slot written once with a plain store (deterministic); entries with no slot fail with their count;
+ * the previous factors, selected inverse and member infos are invalidated (batch_solve fails until batch_factor).  Plain
+ * and Schur batched handles; fails on unbatched handles, unless nterms >= 1, on a mismatched n, a rowptr that does not
+ * start at 0 or decreases, and a colind outside 0 .. n-1.  Offsets are 64-bit. */
+int slu_b200_batch_fill_affine(slu_b200_handle_t h, int n, const int32_t *rowptr, const int32_t *colind, int nterms,
+                               const double *terms, const double *coef, const int32_t *perm);
 /* Partial factorization on batched handles: the slu_b200_schur_* calls for `batch` matrices of one pattern (substructuring
  * with many same-mesh subdomains, static condensation of many element matrices, Kron reduction of network ensembles,
  * parameter sweeps of marginal precision matrices).
  * batch_schur_create: the checks of batch_create and of schur_create (1 <= batch <= 65535, 1 <= nschur < n, n - nschur a
  * supernode boundary, 1 x 1 x 1 grid with world_size 1, int8 path off), with messages that name batch_schur_create.  The
- * handle takes batch_fill_csr, batch_factor, batch_download, get_stats, destroy and the four batch_schur_* calls;
- * batch_solve, batch_solve_trans, batch_gscon, batch_selinv, batch_selinv_get and batch_logdet fail on it with a message
+ * handle takes batch_fill_csr, batch_fill_affine, batch_factor, batch_download, get_stats, destroy and the four
+ * batch_schur_* calls; batch_solve, batch_solve_trans, batch_gscon, batch_selinv, batch_selinv_get, batch_logdet and
+ * batch_inertia fail on it with a message
  * ("Schur handle") and leave it usable, the unbatched schur_* calls fail on it ("batched handle"), and the batch_schur_*
  * calls fail on ordinary, plain batched and unbatched Schur handles.  batch_factor eliminates A11 of every member in one
  * launch sequence (the launches of one unbatched Schur factorization, each over batch x the CTAs): info[j] = 0 or the
@@ -420,6 +449,13 @@ int slu_b200_z_batch_selinv(slu_b200_zhandle_t h, double out[4]);
 int slu_b200_z_batch_selinv_get(slu_b200_zhandle_t h, int n, const int32_t *rowptr, const int32_t *colind,
                                 const int32_t *perm, double *out);
 int slu_b200_z_batch_logdet(slu_b200_zhandle_t h, double *logabs, double *sign);
+/* as slu_b200_inertia / _batch_inertia / _batch_fill_affine with the same restrictions and messages: the sign test is on
+ * Re u_ii, |u_ii| is the modulus and defect the max of |Im u_ii| / |u_ii|; terms and coef of z_batch_fill_affine hold
+ * interleaved doublecomplex, n and nnz count complex elements. */
+int slu_b200_z_inertia(slu_b200_zhandle_t h, int64_t counts[3], double *defect);
+int slu_b200_z_batch_inertia(slu_b200_zhandle_t h, int64_t *counts, double *defect);
+int slu_b200_z_batch_fill_affine(slu_b200_zhandle_t h, int n, const int32_t *rowptr, const int32_t *colind, int nterms,
+                                 const double *terms, const double *coef, const int32_t *perm);
 /* as slu_b200_batch_schur_create / _get / _condense / _expand, with the same restrictions and messages; S and x hold
  * interleaved doublecomplex, lds and ldx count complex elements. */
 int slu_b200_z_batch_schur_create(slu_b200_zhandle_t *h, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt,

@@ -130,6 +130,12 @@ def lib():
         getattr(L, f).argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     for f in ("slu_b200_batch_logdet", "slu_b200_z_batch_logdet"):
         getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    for f in ("slu_b200_inertia", "slu_b200_z_inertia"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_double)]
+    for f in ("slu_b200_batch_inertia", "slu_b200_z_batch_inertia"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    for f in ("slu_b200_batch_fill_affine", "slu_b200_z_batch_fill_affine"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     for f in ("slu_b200_schur_create", "slu_b200_z_schur_create"):
         getattr(L, f).argtypes = [C.POINTER(C.c_void_p), C.POINTER(LUView), C.POINTER(Options), C.c_int]
     for f in ("slu_b200_schur_get", "slu_b200_z_schur_get"):
@@ -386,6 +392,15 @@ class Handle:
         _check(_fn("logdet", self.z_)(self.h, C.byref(la), sg.ctypes.data_as(C.c_void_p)))
         return (complex(sg[0], sg[1]) if self.z_ else float(sg[0])), la.value
 
+    def inertia(self):
+        """Inertia of a symmetric (Hermitian) A from the signs of the resident pivots (slu_b200_inertia / slu_b200_z_inertia)
+        -> (neg, pos, tiny, defect): the pivots with Re u_ii < 0, the others (neg + pos = n), those with |u_ii| <= thresh,
+        and max |Im u_ii| / |u_ii| (0.0 for a real problem).  For A - sigma B with B positive definite, neg is the number
+        of eigenvalues below sigma."""
+        cnt, dfc = np.zeros(3, np.int64), C.c_double(0.0)
+        _check(_fn("inertia", self.z_)(self.h, cnt.ctypes.data_as(C.c_void_p), C.byref(dfc)))
+        return int(cnt[0]), int(cnt[1]), int(cnt[2]), dfc.value
+
     def _dtype(self):
         return np.complex128 if self.z_ else np.float64
 
@@ -531,6 +546,30 @@ class BatchHandle:
         _check(_fn("batch_logdet", self.z_)(self.h, la.ctypes.data_as(C.c_void_p), sg.ctypes.data_as(C.c_void_p)))
         return sg, la
 
+    def inertia(self):
+        """Every member's inertia (slu_b200_batch_inertia), as Handle.inertia -> (neg, pos, tiny, defect): int64 arrays
+        (batch,) and a float64 array (batch,)"""
+        cnt, dfc = np.zeros((self.batch, 3), np.int64), np.zeros(self.batch, np.float64)
+        _check(_fn("batch_inertia", self.z_)(self.h, cnt.ctypes.data_as(C.c_void_p), dfc.ctypes.data_as(C.c_void_p)))
+        return cnt[:, 0].copy(), cnt[:, 1].copy(), cnt[:, 2].copy(), dfc
+
+    def fill_affine(self, rowptr, colind, terms, coef, perm):
+        """An affine family on one CSR pattern (slu_b200_batch_fill_affine): member j's values are
+        sum_t coef[j, t] * terms[t], computed on the device.  terms: (T, nnz), coef: (batch, T), float64 (complex128 for a
+        complex problem); perm[old] = new as in fill_csr."""
+        rp = np.ascontiguousarray(rowptr, np.int32)
+        ci = np.ascontiguousarray(colind, np.int32)
+        tv = np.ascontiguousarray(terms, self._dtype())
+        cv = np.ascontiguousarray(coef, self._dtype())
+        if tv.ndim != 2 or tv.shape[1] != len(ci):
+            raise ValueError(f"terms must have shape (T, {len(ci)}), not {tv.shape}")
+        if cv.shape != (self.batch, tv.shape[0]):
+            raise ValueError(f"coef must have shape ({self.batch}, {tv.shape[0]}), not {cv.shape}")
+        pm = np.ascontiguousarray(perm, np.int32)
+        _check(_fn("batch_fill_affine", self.z_)(self.h, len(rp) - 1, rp.ctypes.data_as(C.c_void_p), ci.ctypes.data_as(C.c_void_p),
+                                                 tv.shape[0], tv.ctypes.data_as(C.c_void_p), cv.ctypes.data_as(C.c_void_p),
+                                                 pm.ctypes.data_as(C.c_void_p)))
+
     def download(self, member):
         """Member `member`'s L and U into prob.layers[0] (the reference layout)."""
         _check(_fn("batch_download", self.z_)(self.h, int(member)))
@@ -555,8 +594,8 @@ class BatchHandle:
 class BatchSchurHandle(BatchHandle):
     """A partial factorization of `batch` matrices with the pattern of `prob` (slu_b200_batch_schur_create /
     slu_b200_z_batch_schur_create): as SchurHandle for every member, with the values, info and downloads of BatchHandle.
-    fill_csr / factor / download as BatchHandle; schur() returns every member's S, condense / expand the two partial
-    solves.  solve, rcond, selinv, inv_entries, inv_diag and logdet fail on it."""
+    fill_csr / fill_affine / factor / download as BatchHandle; schur() returns every member's S, condense / expand the two
+    partial solves.  solve, rcond, selinv, inv_entries, inv_diag, logdet and inertia fail on it."""
 
     def __init__(self, prob, batch, nschur, **opt):
         require_gpu()

@@ -52,6 +52,9 @@
 #define slu_b200_batch_selinv slu_b200_z_batch_selinv
 #define slu_b200_batch_selinv_get slu_b200_z_batch_selinv_get
 #define slu_b200_batch_logdet slu_b200_z_batch_logdet
+#define slu_b200_inertia slu_b200_z_inertia
+#define slu_b200_batch_inertia slu_b200_z_batch_inertia
+#define slu_b200_batch_fill_affine slu_b200_z_batch_fill_affine
 #define slu_b200_schur_create slu_b200_z_schur_create
 #define slu_b200_schur_get slu_b200_z_schur_get
 #define slu_b200_schur_condense slu_b200_z_schur_condense
@@ -2605,6 +2608,102 @@ int slu_b200_batch_logdet(slu_b200_handle_t H, double *logabs, double *sign)
         logabs[j] = r[(size_t)j * (1 + VAL_DOUBLES)];
         for (int c = 0; c < VAL_DOUBLES; ++c) sign[(size_t)j * VAL_DOUBLES + c] = r[(size_t)j * (1 + VAL_DOUBLES) + 1 + c];
     }
+    return 0;
+}
+
+// ---- inertia from the signs of the pivots (slu_b200_inertia, slu_b200_batch_inertia) --------------------------------------
+// F = P A P^T = L U with a symmetric permutation, no row exchanges and a unit-diagonal L: for a real symmetric (complex
+// Hermitian) A, U = D L^T (D L^H), so by Sylvester's law the signs of the u_ii are those of A's eigenvalues.  Two launches
+// over the level plan's supernodes for all members (d = H->dev, or H->bdev with gridDim.y = members); counts[3 j + c] and
+// defect[j] per member.  The checks are the caller's.
+}  // extern "C"
+template <class LU>
+static int inertia_impl(slu_b200_handle_t H, const LU &d, int members, int64_t *counts, double *defect)
+{
+    const int count = (int)H->znodes[0].size();
+    const int nparts = (count + SELINV_VECS - 1) / SELINV_VECS;
+    DevBuf<long long> pcnt, cnt;
+    DevBuf<double> pdef, def;
+    if (pcnt.alloc((size_t)3 * nparts * members) || pdef.alloc((size_t)nparts * members) || cnt.alloc((size_t)3 * members) ||
+        def.alloc((size_t)members))
+        return -1;
+    cudaStream_t s = H->stream;
+    std::vector<long long> c((size_t)3 * members, 0);
+    std::vector<double> m((size_t)members, 0.0);
+    if (launch_inertia(d, H->d_pool_i32.p + H->z_nodes_off[0], count, H->opt.thresh, pcnt.p, pdef.p, cnt.p, def.p, s)) {
+        CU(cudaMemcpyAsync(c.data(), cnt.p, c.size() * sizeof(long long), cudaMemcpyDeviceToHost, s));
+        CU(cudaMemcpyAsync(m.data(), def.p, m.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+    }
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    for (size_t i = 0; i < c.size(); ++i) counts[i] = (int64_t)c[i];
+    for (int j = 0; j < members; ++j) defect[j] = m[j];
+    return 0;
+}
+extern "C" {
+
+int slu_b200_inertia(slu_b200_handle_t H, int64_t counts[3], double *defect)
+{
+    if (!H || !counts || !defect) return fail("null argument");
+    if (selinv_refuse(H, SLU_API "inertia")) return -1;
+    return inertia_impl(H, H->dev, 1, counts, defect);
+}
+
+int slu_b200_batch_inertia(slu_b200_handle_t H, int64_t *counts, double *defect)
+{
+    if (!H || !counts || !defect) return fail("null argument");
+    if (batch_selinv_refuse(H, SLU_API "batch_inertia")) return -1;
+    return inertia_impl(H, H->bdev, H->batch, counts, defect);
+}
+
+// ---- affine families (slu_b200_batch_fill_affine): member j = sum_t coef[j nterms + t] A_t on one pattern.  The T terms
+// cross PCIe once instead of B member value arrays; the slot search runs once per entry, then one launch over (entries,
+// members) combines and scatters.  Otherwise as slu_b200_batch_fill_csr: the arena is zeroed, the factors, inverse and
+// member infos are invalidated.
+int slu_b200_batch_fill_affine(slu_b200_handle_t H, int n, const int32_t *rowptr, const int32_t *colind, int nterms,
+                               const double *terms, const double *coef, const int32_t *perm)
+{
+    if (!H || !rowptr || !colind || !terms || !coef || !perm) return fail("null argument");
+    const char *fn = SLU_API "batch_fill_affine";
+    if (refuse_unbatched(H, fn)) return -1;
+    if (n != H->n) return fail("%s: matrix order %d does not match the handle's %d", fn, n, H->n);
+    if (nterms < 1) return fail("%s: nterms = %d, must be at least 1", fn, nterms);
+    if (rowptr[0] != 0) return fail("%s: bad rowptr (rowptr[0] = %d, must be 0)", fn, rowptr[0]);
+    for (int i = 0; i < n; ++i)
+        if (rowptr[i + 1] < rowptr[i]) return fail("%s: bad rowptr (rowptr[%d] = %d < rowptr[%d] = %d)", fn, i + 1, rowptr[i + 1], i, rowptr[i]);
+    const int64_t nnz = rowptr[n];
+    for (int64_t p = 0; p < nnz; ++p)
+        if (colind[p] < 0 || colind[p] >= n) return fail("%s: colind[%lld] = %d is outside 0 ... %d", fn, (long long)p, colind[p], n - 1);
+    double t0 = now_s();
+    const int B = H->batch;
+    DevBuf<int32_t> drp, dci, dperm;
+    DevBuf<int64_t> ddst;
+    DevBuf<val_t> dterms, dcoef;
+    DevBuf<int8_t> dact;
+    std::vector<int8_t> act(H->nsupers, 0);
+    for (int k : H->znodes[0]) act[k] = 1;
+    if (drp.alloc((size_t)n + 1) || dci.alloc((size_t)nnz) || dperm.alloc((size_t)n) || ddst.alloc((size_t)nnz) ||
+        dterms.alloc((size_t)nnz * nterms) || dcoef.alloc((size_t)B * nterms) || dact.upload(act))
+        return -1;
+    cudaStream_t s = H->stream;
+    int *err = H->d_flags.p + B;
+    CU(cudaMemcpyAsync(drp.p, rowptr, ((size_t)n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(dci.p, colind, (size_t)nnz * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(dperm.p, perm, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(dterms.p, terms, (size_t)nnz * nterms * sizeof(val_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(dcoef.p, coef, (size_t)B * nterms * sizeof(val_t), cudaMemcpyHostToDevice, s));
+    H->si_ready = false;
+    CU(cudaMemsetAsync(H->val.p, 0, H->val.bytes(), s));
+    CU(cudaMemsetAsync(err, 0, sizeof(int), s));
+    launch_fill_affine(H->bdev, n, drp.p, dci.p, dperm.p, dact.p, ddst.p, nnz, nterms, dterms.p, dcoef.p, err, s);
+    int bad = 0;
+    CU(cudaMemcpyAsync(&bad, err, sizeof(int), cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    H->member_info.assign(B, -1);   // the arena was zeroed: no member has factors now
+    H->uploaded = !bad;
+    if (bad) return fail("%s: %d entries of the pattern have no slot in the L/U structure (wrong permutation or symbolic structure)", fn, bad);
+    H->st.t_upload_s = now_s() - t0;
     return 0;
 }
 

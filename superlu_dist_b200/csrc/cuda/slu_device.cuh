@@ -183,6 +183,12 @@ int launch_solve_update(const BatchedLU &d, const Batch &b, int64_t ctas, bool b
                         cudaStream_t s);
 int launch_fill_csr(const BatchedLU &d, int n, const int32_t *rowptr, const int32_t *colind, const val_t *aval, const int32_t *perm,
                     const int8_t *active, int *err, cudaStream_t s);
+// affine fill (slu_b200_batch_fill_affine), 2 launches: dst[p] = the arena offset of CSR entry p (the slot search of fill_csr,
+// once per entry; -1 and a count in *err where it has no slot, -1 in a panel `active` leaves out), then member j's value of
+// entry p, coef[j nterms] terms[p] + sum over t >= 1 of coef[j nterms + t] terms[t nnz + p] in that order, goes to its arena
+// at dst[p]
+int launch_fill_affine(const BatchedLU &d, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm, const int8_t *active,
+                       int64_t *dst, int64_t nnz, int nterms, const val_t *terms, const val_t *coef, int *err, cudaStream_t s);
 
 // slu_cond.cu (double) / slu_cond_z.cu (doublecomplex): the step kernels of the dlacn2 / zlacn2 1-norm estimator
 // (slu_b200_gscon).  One CondState per member: dlacn2's EST, ESTOLD and ISAVE(1..3) as phase, j, iter; kase = the solve
@@ -263,6 +269,13 @@ int launch_selinv_trsm(const BatchedLU &d, const Batch &b, int64_t ctas, int col
 int launch_selinv_logdet(const BatchedLU &d, const int32_t *nodes, int count, double *part, phase_t *pph, double *out, cudaStream_t s);
 int launch_selinv_get(const BatchedLU &d, const val_t *hv, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm,
                       val_t *out, int *err, cudaStream_t s);
+// inertia (slu_b200_inertia, _batch_inertia) over the listed supernodes' pivots u_ii: per member cnt[3 j ...] = the pivots with
+// Re u_ii < 0, the others, those with |u_ii| <= thresh; def[j] = max |Im u_ii| / |u_ii| (0 in double).  pcnt / pdef: members x
+// ceil(count / SELINV_VECS) partials (3 counts each).  2 launches.
+int launch_inertia(const DeviceLU &d, const int32_t *nodes, int count, double thresh, long long *pcnt, double *pdef, long long *cnt,
+                   double *def, cudaStream_t s);
+int launch_inertia(const BatchedLU &d, const int32_t *nodes, int count, double thresh, long long *pcnt, double *pdef, long long *cnt,
+                   double *def, cudaStream_t s);
 
 // slu_schur.cu (double) / slu_schur_z.cu (doublecomplex): the Schur complement of a partial factorization
 // (slu_b200_schur_get).  S(r - n0, c - n0) = every stored entry (r, c) of the Schur supernodes' panels, into a zeroed s x s

@@ -362,6 +362,88 @@ __global__ void __launch_bounds__(SELINV_VECS) selinv_logdet_final_kernel(const 
 }
 
 // ------------------------------------------------------------------------------------------------
+// Inertia: the signs of the pivots, one supernode per thread as in the logdet reduction.  Integer counts (negative real
+// part, the others, |u_ii| <= thresh) and the max of |Im u_ii| / |u_ii|, reduced in a fixed order without atomics.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void inertia_block_reduce(long long (&c)[3], double &def)
+{
+    __shared__ long long sc[SELINV_VECS / 32][3];
+    __shared__ double sd[SELINV_VECS / 32];
+    for (int o = 16; o > 0; o >>= 1) {
+#pragma unroll
+        for (int q = 0; q < 3; ++q) c[q] += __shfl_down_sync(0xffffffffu, c[q], o);
+        def = fmax(def, __shfl_down_sync(0xffffffffu, def, o));
+    }
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (lane == 0) {
+        for (int q = 0; q < 3; ++q) sc[w][q] = c[q];
+        sd[w] = def;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        c[0] = c[1] = c[2] = 0;
+        def = 0.0;
+        for (int i = 0; i < SELINV_VECS / 32; ++i) {
+            for (int q = 0; q < 3; ++q) c[q] += sc[i][q];
+            def = fmax(def, sd[i]);
+        }
+    }
+}
+
+// batched: grid (nparts, members), member j's partials at j * nparts (counts: 3 per partial)
+template <class LU>
+__global__ void __launch_bounds__(SELINV_VECS) inertia_partial_kernel(LU dd, const int32_t *nodes, int count, double thresh,
+                                                                      long long *pcnt, double *pdef)
+{
+    const DeviceLU &d = member_view(dd);
+    pcnt = member_ptr(dd, pcnt, 3 * gridDim.x);
+    pdef = member_ptr(dd, pdef, gridDim.x);
+    const int t = blockIdx.x * SELINV_VECS + threadIdx.x;
+    long long c[3] = {0, 0, 0};
+    double def = 0.0;
+    if (t < count) {
+        const NodeDesc nd = d.nodes[nodes[t]];
+        const val_t *D = d.val + nd.lval;
+        for (int i = 0; i < nd.ns; ++i) {
+            const val_t p = D[(int64_t)i * nd.nsupr + i];
+#ifdef SLU_COMPLEX
+            const double a = hypot(p.x, p.y), re = p.x;
+            if (a > 0.0) def = fmax(def, fabs(p.y) / a);
+#else
+            const double a = fabs(p), re = p;
+#endif
+            c[0] += re < 0.0;
+            c[2] += a <= thresh;
+        }
+        c[1] = nd.ns - c[0];
+    }
+    inertia_block_reduce(c, def);
+    if (threadIdx.x == 0) {
+        for (int q = 0; q < 3; ++q) pcnt[3 * blockIdx.x + q] = c[q];
+        pdef[blockIdx.x] = def;
+    }
+}
+
+// grid (1, members): member j's partials at j * nparts, its counts at cnt + 3 j and its defect at def[j]
+__global__ void __launch_bounds__(SELINV_VECS) inertia_final_kernel(const long long *pcnt, const double *pdef, int nparts,
+                                                                    long long *cnt, double *def)
+{
+    pcnt += (size_t)blockIdx.y * 3 * nparts;
+    pdef += (size_t)blockIdx.y * nparts;
+    long long c[3] = {0, 0, 0};
+    double m = 0.0;
+    for (int i = threadIdx.x; i < nparts; i += SELINV_VECS) {
+        for (int q = 0; q < 3; ++q) c[q] += pcnt[3 * i + q];
+        m = fmax(m, pdef[i]);
+    }
+    inertia_block_reduce(c, m);
+    if (threadIdx.x == 0) {
+        for (int q = 0; q < 3; ++q) cnt[3 * blockIdx.y + q] = c[q];
+        def[blockIdx.y] = m;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // out[p] = A^-1(i, colind[p]) = H(perm[colind[p]], perm[i]): the slot search of fill_csr_kernel with the roles of row and
 // column swapped, reading instead of writing.  One thread per row of the pattern.  Batched: member j's values at
 // out + j * nnz; a missing slot depends on the structure only, so only member 0 counts it.
@@ -434,6 +516,17 @@ static int launch_selinv_logdet_t(const LU &d, const int32_t *nodes, int count, 
 }
 
 template <class LU>
+static int launch_inertia_t(const LU &d, const int32_t *nodes, int count, double thresh, long long *pcnt, double *pdef,
+                            long long *cnt, double *def, cudaStream_t s)
+{
+    const int nparts = (count + SELINV_VECS - 1) / SELINV_VECS;
+    if (nparts <= 0) return 0;
+    inertia_partial_kernel<LU><<<member_grid(d, nparts), SELINV_VECS, 0, s>>>(d, nodes, count, thresh, pcnt, pdef);
+    inertia_final_kernel<<<member_grid(d, 1), SELINV_VECS, 0, s>>>(pcnt, pdef, nparts, cnt, def);
+    return 2;
+}
+
+template <class LU>
 static int launch_selinv_get_t(const LU &d, const val_t *hv, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm,
                                val_t *out, int *err, cudaStream_t s)
 {
@@ -475,6 +568,16 @@ int launch_selinv_get(const BatchedLU &d, const val_t *hv, int n, const int32_t 
                       val_t *out, int *err, cudaStream_t s)
 {
     return launch_selinv_get_t(d, hv, n, rowptr, colind, perm, out, err, s);
+}
+int launch_inertia(const DeviceLU &d, const int32_t *nodes, int count, double thresh, long long *pcnt, double *pdef, long long *cnt,
+                   double *def, cudaStream_t s)
+{
+    return launch_inertia_t(d, nodes, count, thresh, pcnt, pdef, cnt, def, s);
+}
+int launch_inertia(const BatchedLU &d, const int32_t *nodes, int count, double thresh, long long *pcnt, double *pdef, long long *cnt,
+                   double *def, cudaStream_t s)
+{
+    return launch_inertia_t(d, nodes, count, thresh, pcnt, pdef, cnt, def, s);
 }
 
 }  // namespace SLU_NS

@@ -346,6 +346,84 @@ __global__ void fill_csr_kernel(LU dd, int n, const int32_t *__restrict__ rowptr
         }
     }
 }
+
+// ---- affine fill (slu_b200_batch_fill_affine) ----
+// csr_slot: the arena offset of entry (pi, pj) of the permuted matrix; -1 in a panel `active` leaves out, -2 without a slot.
+// The search of fill_csr_kernel, which keeps its own copy: written through this helper, that kernel compiles to other code.
+__device__ __forceinline__ int64_t csr_slot(const DeviceLU &d, int pi, int pj, const int8_t *__restrict__ active)
+{
+    const int ks = d.supno[pj];
+    if (pi >= d.xsup[ks]) {                       // L panel of block column ks (diagonal block included)
+        if (!active[ks]) return -1;
+        const NodeDesc *nd = d.nodes + ks;
+        const int32_t *srow = d.lsrow + nd->lrow;
+        const int q = lower_bound_i32(srow, nd->nsupr, pi);
+        if (q >= nd->nsupr || srow[q] != pi) return -2;
+        return nd->lval + (int64_t)(pj - nd->fsupc) * nd->nsupr + d.lspos[nd->lrow + q];
+    }
+    const int kr = d.supno[pi];                   // U panel of block row supno(i)
+    if (!active[kr]) return -1;
+    const NodeDesc *nd = d.nodes + kr;
+    const int32_t *uc = d.ucols + nd->ucol;
+    const int q = lower_bound_i32(uc, nd->ncols, pj);
+    // above the column's skyline start is dense-packed padding, not a slot
+    if (q >= nd->ncols || uc[q] != pj || pi < d.ufst[nd->ucol + q]) return -2;
+    return nd->uval + (int64_t)q * nd->ns + (pi - nd->fsupc);
+}
+
+// dst[p] = csr_slot of entry p (-1 where it has none, counted in *err): one thread per row, as fill_csr_kernel.  A batched
+// handle fills every panel, so no entry is left out as inactive.
+__global__ void fill_affine_slot_kernel(DeviceLU d, int n, const int32_t *__restrict__ rowptr, const int32_t *__restrict__ colind,
+                                        const int32_t *__restrict__ perm, const int8_t *__restrict__ active, int64_t *__restrict__ dst,
+                                        int *err)
+{
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    const int pi = perm[r];
+    for (int p = rowptr[r]; p < rowptr[r + 1]; ++p) {
+        const int64_t o = csr_slot(d, pi, perm[colind[p]], active);
+        if (o == -2) atomicAdd(err, 1);
+        dst[p] = o < 0 ? -1 : o;
+    }
+}
+
+// grid (entry tiles, members): thread = one entry of member blockIdx.y, v = c_0 V_0 then v = fma(c_t, V_t, v) for t = 1, 2, ...;
+// the member's coefficients are staged in shared memory FA_THREADS at a time, each term is read coalesced, each slot written
+// once with a plain store
+constexpr int FA_THREADS = 256;
+__global__ void __launch_bounds__(FA_THREADS) fill_affine_kernel(BatchedLU dd, int64_t nnz, int nterms, const val_t *__restrict__ terms,
+                                                                 const val_t *__restrict__ coef, const int64_t *__restrict__ dst)
+{
+    __shared__ val_t cs[FA_THREADS];
+    const DeviceLU d = member_view(dd);
+    coef += (int64_t)blockIdx.y * nterms;
+    const int64_t p = (int64_t)blockIdx.x * FA_THREADS + threadIdx.x;
+    val_t v = vzero();
+    for (int t0 = 0; t0 < nterms; t0 += FA_THREADS) {
+        __syncthreads();
+        if (t0 + (int)threadIdx.x < nterms) cs[threadIdx.x] = coef[t0 + threadIdx.x];
+        __syncthreads();
+        if (p >= nnz) continue;
+        const int tn = min(FA_THREADS, nterms - t0);
+        int t = 0;
+        if (t0 == 0) { v = vmul(cs[0], terms[p]); t = 1; }
+        for (; t < tn; ++t) v = vfma(cs[t], terms[(int64_t)(t0 + t) * nnz + p], v);
+    }
+    if (p < nnz) {
+        const int64_t o = dst[p];
+        if (o >= 0) d.val[o] = v;
+    }
+}
+
+int launch_fill_affine(const BatchedLU &d, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm, const int8_t *active,
+                       int64_t *dst, int64_t nnz, int nterms, const val_t *terms, const val_t *coef, int *err, cudaStream_t s)
+{
+    if (n <= 0) return 0;
+    fill_affine_slot_kernel<<<(n + 127) / 128, 128, 0, s>>>(d, n, rowptr, colind, perm, active, dst, err);
+    if (nnz <= 0) return 1;
+    fill_affine_kernel<<<member_grid(d, (unsigned)((nnz + FA_THREADS - 1) / FA_THREADS)), FA_THREADS, 0, s>>>(d, nnz, nterms, terms, coef, dst);
+    return 2;
+}
 template <class LU>
 static int launch_fill_csr_t(const LU &d, int n, const int32_t *rowptr, const int32_t *colind, const val_t *aval, const int32_t *perm,
                              const int8_t *active, int *err, cudaStream_t s)
