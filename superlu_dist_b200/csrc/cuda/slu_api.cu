@@ -693,9 +693,8 @@ int analyze(slu_b200_handle_s *H)
                 L.slab_begin = std::min(L.slab_begin, nd.lval);
                 L.slab_end = std::max(L.slab_end, std::max(nd.lval + (int64_t)nd.nsupr * nd.ns, nd.uval + (int64_t)nd.ns * nd.ncols));
                 L.max_ns = std::max(L.max_ns, nd.ns);
-                const int strip = trsm_strip_of(nd.ns);
-                p_l.push_back(p_l.back() + (nd.m + strip - 1) / strip);
-                p_u.push_back(p_u.back() + (nd.ncols + strip - 1) / strip);
+                p_l.push_back(p_l.back() + (nd.m + TRSM_STRIP - 1) / TRSM_STRIP);
+                p_u.push_back(p_u.back() + (nd.ncols + TRSM_STRIP - 1) / TRSM_STRIP);
                 p_sl.push_back(p_sl.back() + (nd.m + 255) / 256);
                 p_su.push_back(p_su.back() + (nd.ncols + 255) / 256);
                 nd.ws_inv = p_inv.back() * 512;
@@ -2874,7 +2873,7 @@ static int k_trsm(bool ucase, const double *lu_, int ldlu, int ns, double *x_, i
         for (int c = 0; c < nvec; ++c)
             for (int r = 0; r < ns; ++r) h[(size_t)ns * ns + (size_t)c * ns + r] = x[(size_t)c * ldx + r];
     }
-    int64_t ctas = (nvec + trsm_strip_of(ns) - 1) / trsm_strip_of(ns);
+    int64_t ctas = (nvec + TRSM_STRIP - 1) / TRSM_STRIP;
     if (M.init(nd, nval, {0, ctas})) return -1;
     CU(cudaMemcpy(M.val.p, h.data(), nval * sizeof(val_t), cudaMemcpyHostToDevice));
     Batch b{M.ids.p, M.prefix.p, 1};

@@ -115,20 +115,14 @@ struct Batch {               // one kernel launch over several supernodes
 constexpr int DIAG_NB = 16;
 constexpr int TRSM_NB = 16;
 constexpr int MAX_NS = 512;  // MAX_SUPER_SIZE, SRC/include/superlu_defs.h:154
+constexpr int TRSM_STRIP = 32;       // vectors per TRSM CTA, every ns (the CTA prefix of a level batch is built with this)
 #ifdef SLU_COMPLEX
-constexpr int TRSM_STRIP = 32;      // vectors a TRSM CTA keeps in shared memory (16-byte elements)
 constexpr int MAX_NS_HELD = 256;    // widest supernode the kernels accept (the default superlu_maxsup)
-constexpr int TRSM_WIDE_NS = MAX_NS_HELD;   // no half-width strips in the doublecomplex build
 constexpr int SCHUR_BN_TILE = 32;   // columns of a big Schur tile (complex columns: 64 real ones)
 #else
-constexpr int TRSM_STRIP = 64;
 constexpr int MAX_NS_HELD = MAX_NS;  // MAX_SUPER_SIZE
-constexpr int TRSM_WIDE_NS = 416;    // a 64-vector strip of a wider supernode does not fit 227 KB: those use 32-vector strips
 constexpr int SCHUR_BN_TILE = 64;
 #endif
-
-// vectors per TRSM CTA for a supernode of ns columns (the CTA prefix of a level batch is built with this)
-__host__ __device__ inline int trsm_strip_of(int ns) { return ns > TRSM_WIDE_NS ? TRSM_STRIP / 2 : TRSM_STRIP; }
 
 // launchers (slu_kernels.cu).  Every launcher returns the number of kernels it launched.
 // replace_tiny: 0 off, 1 replace and count in d.tiny, 2 replace without counting (replicated copy of a shared forest)

@@ -313,6 +313,12 @@ int launch_diag_lu(const BatchedLU &d, const Batch &b, int max_ns, int replace_t
     return launch_diag_lu_t(d, b, max_ns, replace_tiny, thresh, s);
 }
 
+// Shared images of DMMA.16x8x8 operands (the Hopper main loop and the panel TRSM): rows g and g+8 of a 16-row block
+// are adjacent (row r at prow(r)), and so are k and k+4 of an 8-deep slice (at pk(k)), so that each lane's fragment
+// pairs are 16-byte loads.
+__device__ __forceinline__ int prow(int r) { return (r & ~15) | ((r & 7) << 1) | ((r >> 3) & 1); }
+__device__ __forceinline__ int pk(int k) { return (k & ~7) | ((k & 3) << 1) | ((k >> 2) & 1); }
+
 // ------------------------------------------------------------------------------------------------
 // panel triangular solves on the FP64 tensor cores.
 //   Y <- Y T^-1, T upper triangular ns x ns, blocked by 16 columns (left-looking):
@@ -321,11 +327,7 @@ int launch_diag_lu(const BatchedLU &d, const Batch &b, int max_ns, int replace_t
 //   U case: vectors = packed columns of U(k,:),    T(p,c) = L_kk(c,p) (transposed, unit)
 // The 16x16 diagonal blocks are inverted once per supernode by diag_inv_kernel; everything else is
 // substitution, so the only departure from the reference's dtrsm is inside a 16x16 block.
-// A CTA stages 64 vectors in shared memory; each warp owns 8 of them and walks the column blocks with
-// DMMA m8n8k4 accumulators in registers -- no block-level synchronisation inside the sweep.
 // ------------------------------------------------------------------------------------------------
-constexpr int TRSM_LD = TRSM_STRIP + 4;
-
 template <class LU>
 __global__ void __launch_bounds__(64) diag_inv_kernel(LU dd, Batch b, double *dinv)
 {
@@ -391,150 +393,176 @@ int launch_diag_inv(const BatchedLU &d, const Batch &b, int64_t ctas, double *di
     return launch_diag_inv_t(d, b, ctas, dinv, s);
 }
 
-template <bool UCASE, bool STAGED, int STRIP>
-__device__ __forceinline__ void trsm_body(const DeviceLU &d, const NodeDesc &nd, int strip, const double *dinv, double *Ys)
+// trsm_kernel: one CTA of four warps per strip of TRSM_STRIP = 32 vectors, on DMMA.16x8x8.  Warp (mt, nt) owns vectors
+// 16 mt .. 16 mt + 15 and columns 8 nt .. 8 nt + 7 of every 16-column block j; its sum over p < j0 runs in four
+// independent accumulators (k8 slice q adds into acc[q % 4]), which are added before Y_j - sum is multiplied by
+// inv(T_jj).  The strip stays in shared memory for the whole sweep, vector s at prow(s) of each column, so that A
+// fragments are 16-byte loads; T streams through a double buffer of TRSM_KC x 16 chunks, row p at pk(p).  That is
+// 90 KB of shared memory at ns = 256 (two CTAs per SM) and 162 KB at ns = 512.  Keep it there: with a third T stage
+// (99 KB) or 128-row chunks (110 KB) the kernel was no faster alone and the look-ahead step, where it runs beside the
+// Schur kernel's 88 KB CTAs, was 7 % slower (DESIGN §4d).
+constexpr int TRSM_THREADS = 128, TRSM_KC = 64;
+constexpr int TRSM_LD = TRSM_STRIP + 4;   // == 4 (mod 16) doubles: conflict-free A fragments
+constexpr int TRSM_LDT = TRSM_KC + 8;     // == 8 (mod 16): conflict-free B fragments
+static_assert(TRSM_STRIP == 32 && TRSM_THREADS == 128 && TRSM_KC % 16 == 0, "trsm_kernel thread mapping");
+static size_t trsm_smem(int max_ns)
 {
-    constexpr int LD = STRIP + 4;   // Ys: [ns rounded up to 16][LD] (+ 2 x [16][nsp+4] staged T blocks)
-    const int ns = nd.ns, lda = nd.nsupr, tid = threadIdx.x, nsp = (ns + 15) & ~15;
-    const double *T = d.val + nd.lval;
-    const double *inv = dinv + nd.ws_inv;
-    const int nvec = UCASE ? nd.ncols : nd.m;
-    const int v0 = strip * STRIP, nv = min(STRIP, nvec - v0);
-    double *X = UCASE ? d.val + nd.uval + (size_t)v0 * ns : d.val + nd.lval + ns + v0;
-
-    if (!UCASE) {
-        for (int idx = tid; idx < nsp * STRIP; idx += 256) {
-            int c = idx / STRIP, s = idx - c * STRIP;
-            Ys[c * LD + s] = (s < nv && c < ns) ? X[(size_t)c * lda + s] : 0.0;
-        }
-    } else {
-        for (int idx = tid; idx < nsp * STRIP; idx += 256) {
-            int s = idx / nsp, c = idx - s * nsp;
-            Ys[c * LD + s] = (s < nv && c < ns) ? X[(size_t)s * ns + c] : 0.0;
-        }
-    }
-    __syncthreads();
-
-    const int lane = tid & 31, r0 = (tid >> 5) * 8, lr = lane >> 2, lk = lane & 3;
-    const int LDT = nsp + 4;
-    double *Tb = Ys + (size_t)nsp * LD;  // STAGED: Tb[buf][c][p], T(p, j0 + c) for p < j0
-    auto prefetch = [&](int j0, int buf) {
-        double *dst = Tb + (size_t)buf * 16 * LDT;
-        if (!UCASE) {
-            for (int idx = tid; idx < 16 * j0; idx += 256) {
-                int c = idx / j0, p = idx - c * j0;
-                bool ok = j0 + c < ns;
-                cp_async8(dst + c * LDT + p, ok ? T + (size_t)(j0 + c) * lda + p : T, ok);
-            }
-        } else {
-            for (int idx = tid; idx < 16 * j0; idx += 256) {
-                int p = idx >> 4, c = idx & 15;
-                bool ok = j0 + c < ns;
-                cp_async8(dst + c * LDT + p, ok ? T + (size_t)p * lda + j0 + c : T, ok);
-            }
-        }
-    };
-    if (STAGED) {
-        if (ns > 16) prefetch(16, 1);
-        cp_async_commit();
-    }
-    for (int j0 = 0; j0 < ns; j0 += 16) {
-        const int buf = (j0 >> 4) & 1;
-        if (STAGED) {
-            cp_async_wait<0>();
-            __syncthreads();
-            if (j0 + 16 < ns) prefetch(j0 + 16, buf ^ 1);
-            cp_async_commit();
-        }
-        if (r0 < nv) {
-            const double *ts = Tb + (size_t)buf * 16 * LDT;
-            double acc[2][2];
-#pragma unroll
-            for (int ni = 0; ni < 2; ++ni)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) acc[ni][e] = Ys[(j0 + ni * 8 + 2 * lk + e) * LD + r0 + lr];
-            for (int p0 = 0; p0 < j0; p0 += 4) {
-                const double a = -Ys[(p0 + lk) * LD + r0 + lr];
-#pragma unroll
-                for (int ni = 0; ni < 2; ++ni) {
-                    const int c = j0 + ni * 8 + lr, p = p0 + lk;
-                    double t = 0.0;
-                    if (STAGED) t = ts[(ni * 8 + lr) * LDT + p];
-                    else if (c < ns) t = UCASE ? T[(size_t)p * lda + c] : T[(size_t)c * lda + p];
-                    dmma884(acc[ni][0], acc[ni][1], a, t);
-                }
-            }
-#pragma unroll
-            for (int ni = 0; ni < 2; ++ni)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) Ys[(j0 + ni * 8 + 2 * lk + e) * LD + r0 + lr] = acc[ni][e];
-            __syncwarp();
-            double out[2][2] = {{0.0, 0.0}, {0.0, 0.0}};
-            const double *ib = inv + (size_t)(j0 >> 4) * 512;
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-                const double a = Ys[(j0 + 4 * kk + lk) * LD + r0 + lr];
-#pragma unroll
-                for (int ni = 0; ni < 2; ++ni) {
-                    const int p = 4 * kk + lk, c = ni * 8 + lr;
-                    const double t = UCASE ? ib[256 + p * 16 + c] : ib[c * 16 + p];
-                    dmma884(out[ni][0], out[ni][1], a, t);
-                }
-            }
-            __syncwarp();
-#pragma unroll
-            for (int ni = 0; ni < 2; ++ni)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) Ys[(j0 + ni * 8 + 2 * lk + e) * LD + r0 + lr] = out[ni][e];
-            __syncwarp();
-        }
-    }
-    if (STAGED) cp_async_wait<0>();
-    __syncthreads();
-    if (!UCASE) {
-        for (int idx = tid; idx < ns * STRIP; idx += 256) {
-            int c = idx / STRIP, ss = idx - c * STRIP;
-            if (ss < nv) X[(size_t)c * lda + ss] = Ys[c * LD + ss];
-        }
-    } else {
-        for (int idx = tid; idx < ns * STRIP; idx += 256) {
-            int ss = idx / ns, c = idx - ss * ns;
-            if (ss < nv) X[(size_t)ss * ns + c] = Ys[c * LD + ss];
-        }
-    }
+    return sizeof(double) * ((size_t)((max_ns + 15) & ~15) * TRSM_LD + 2 * 16 * TRSM_LDT);
 }
 
-// Supernodes wider than TRSM_WIDE_NS (up to MAX_SUPER_SIZE = 512) take 32-vector strips (4 of the 8 warps sweep, the
-// strip is 144 KB instead of 272 KB); they only occur with superlu_maxsup raised above its default 256 and always run
-// the un-staged variant.  The CTA prefix of the batch is built with trsm_strip_of(ns) (slu_api.cu).
-template <bool UCASE, bool STAGED, class LU>
-__global__ void __launch_bounds__(256) trsm_kernel(LU dd, Batch b, const double *dinv)
+template <bool UCASE, class LU>
+__global__ void __launch_bounds__(TRSM_THREADS, 2) trsm_kernel(LU dd, Batch b, const double *dinv)
 {
-    extern __shared__ double Ys[];
+    extern __shared__ __align__(16) double Ys[];   // [nsp][TRSM_LD], then Tb[2][16][TRSM_LDT]
     const DeviceLU &d = member_view(dd);
     dinv = member_inv(dd, dinv);
     const int slot = find_slot(b.prefix, b.count, blockIdx.x);
     const NodeDesc nd = d.nodes[b.nodes[slot]];
     const int strip = (int)(blockIdx.x - b.prefix[slot]);
-    if (STAGED || nd.ns <= TRSM_WIDE_NS) trsm_body<UCASE, STAGED, TRSM_STRIP>(d, nd, strip, dinv, Ys);
-    else trsm_body<UCASE, false, TRSM_STRIP / 2>(d, nd, strip, dinv, Ys);
+    const int ns = nd.ns, lda = nd.nsupr, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nsp = (ns + 15) & ~15;
+    const double *T = d.val + nd.lval;
+    const double *inv = dinv + nd.ws_inv;
+    const int nvec = UCASE ? nd.ncols : nd.m;
+    const int v0 = strip * TRSM_STRIP, nv = min(TRSM_STRIP, nvec - v0);
+    double *X = UCASE ? d.val + nd.uval + (size_t)v0 * ns : d.val + nd.lval + ns + v0;
+    double *const Tb = Ys + (size_t)nsp * TRSM_LD;
+
+    // the strip, zero beyond nv vectors and ns columns.  L: X(s, c) = X[c lda + s], lane = s and warp = c mod 4.
+    // U: X(s, c) = X[s ns + c], 16 vectors x 2 columns per warp, so that the shared stores stay conflict-free.
+    const int us = (lane & 15) | (warp & 1) << 4, uc = (lane >> 4) | (warp >> 1) << 1;
+    if (!UCASE) {
+        const bool sv = lane < nv;
+        const double *x = X + (size_t)warp * lda + lane;
+        const size_t step = (size_t)4 * lda;
+        for (int c = warp; c < nsp; c += 4, x += step) {
+            const bool ok = sv && c < ns;
+            cp_async8(Ys + c * TRSM_LD + prow(lane), ok ? x : X, ok);
+        }
+    } else {
+        const bool sv = us < nv;
+        const double *x = X + (size_t)us * ns;
+        for (int c = uc; c < nsp; c += 4) {
+            const bool ok = sv && c < ns;
+            cp_async8(Ys + c * TRSM_LD + prow(us), ok ? x + c : X, ok);
+        }
+    }
+
+    // T chunks in sweep order: block j0 = 16, 32, .. takes rows pn = 0, TRSM_KC, .. < j0 of columns j0 .. j0 + 15.
+    // L: T(p, c) = T[c lda + p], p = tid mod TRSM_KC.  U: T(p, c) = T[p lda + c], 8 rows x 4 columns per warp.
+    int jn = 16, pn = 0;
+    auto fetch = [&](int buf) {
+        if (jn >= ns) return;
+        double *dst = Tb + buf * 16 * TRSM_LDT;
+        constexpr int PASSES = 16 * TRSM_KC / TRSM_THREADS;
+        if (!UCASE) {
+            constexpr int CS = TRSM_THREADS / TRSM_KC;   // columns per pass
+            const int p = tid & (TRSM_KC - 1), c0 = tid / TRSM_KC;
+            const bool pv = pn + p < jn;
+            const double *src = T + (size_t)(jn + c0) * lda + pn + p;
+            const size_t step = (size_t)CS * lda;
+#pragma unroll
+            for (int i = 0; i < PASSES; ++i, src += step) {
+                const bool ok = pv && jn + c0 + CS * i < ns;
+                cp_async8(dst + (c0 + CS * i) * TRSM_LDT + pk(p), ok ? src : T, ok);
+            }
+        } else {
+            const int c = tid >> 3, p0 = tid & 7;
+            const bool cv = jn + c < ns;
+            const double *src = T + (size_t)(pn + p0) * lda + jn + c;
+            const size_t step = (size_t)8 * lda;
+#pragma unroll
+            for (int i = 0; i < PASSES; ++i, src += step) {
+                const bool ok = cv && pn + p0 + 8 * i < jn;
+                cp_async8(dst + c * TRSM_LDT + pk(p0 + 8 * i), ok ? src : T, ok);
+            }
+        }
+        pn += TRSM_KC;
+        if (pn >= jn) { jn += 16; pn = 0; }
+    };
+    cp_async_commit();
+    fetch(0);
+    cp_async_commit();
+    cp_async_wait<0>();
+    __syncthreads();
+
+    const int g = lane >> 2, t = lane & 3, mt = warp & 1, nt = warp >> 1;
+    const double *const ya = Ys + t * TRSM_LD + 16 * mt + 2 * g;         // A fragment of columns p..p+7: ya + p LD
+    double *const yd = Ys + (8 * nt + 2 * t) * TRSM_LD + 16 * mt + 2 * g;  // D tile of block j0: yd + (j0 + e) LD
+    const double *const tb = Tb + (8 * nt + g) * TRSM_LDT + 2 * t;         // B fragment of k8 slice q: tb + 8 q
+    int buf = 0;
+    for (int j0 = 0; j0 < ns; j0 += 16) {
+        const double *ib = inv + (size_t)(j0 >> 4) * 512;   // loaded ahead: the latency hides behind the update
+        double bi[2][2];
+#pragma unroll
+        for (int kk = 0; kk < 2; ++kk)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int p = 8 * kk + 4 * h + t, c = 8 * nt + g;
+                bi[kk][h] = UCASE ? ib[256 + p * 16 + c] : ib[c * 16 + p];
+            }
+        double acc[4][4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) acc[q][0] = acc[q][1] = acc[q][2] = acc[q][3] = 0.0;
+        for (int pc = 0; pc < j0; pc += TRSM_KC) {
+            cp_async_wait<0>();
+            __syncthreads();
+            fetch(buf ^ 1);
+            cp_async_commit();
+            const double *yc = ya + (size_t)pc * TRSM_LD, *tc = tb + buf * 16 * TRSM_LDT;
+            const int nq = min(TRSM_KC, j0 - pc) >> 3;   // even: j0 - pc is a multiple of 16
+#pragma unroll
+            for (int q = 0; q < TRSM_KC / 8; ++q) {
+                if (q < nq) {
+                    const double2 lo = *reinterpret_cast<const double2 *>(yc + 8 * q * TRSM_LD);
+                    const double2 hi = *reinterpret_cast<const double2 *>(yc + (8 * q + 4) * TRSM_LD);
+                    const double2 v = *reinterpret_cast<const double2 *>(tc + 8 * q);
+                    const double a[4] = {lo.x, lo.y, hi.x, hi.y}, bb[2] = {v.x, v.y};
+                    dmma1688(acc[q & 3], a, bb);
+                }
+            }
+            buf ^= 1;
+        }
+        // D = {D(g, 2t), D(g, 2t+1), D(g+8, 2t), D(g+8, 2t+1)}; rows g and g+8 are adjacent in the strip
+        double2 *d0 = reinterpret_cast<double2 *>(yd + (size_t)j0 * TRSM_LD), *d1 = reinterpret_cast<double2 *>(yd + (size_t)(j0 + 1) * TRSM_LD);
+        double sum[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) sum[e] = (acc[0][e] + acc[1][e]) + (acc[2][e] + acc[3][e]);
+        const double2 y0 = *d0, y1 = *d1;
+        *d0 = make_double2(y0.x - sum[0], y0.y - sum[2]);
+        *d1 = make_double2(y1.x - sum[1], y1.y - sum[3]);
+        __syncthreads();   // the product with inv(T_jj) reads both column halves of the block
+        double o[4] = {0.0, 0.0, 0.0, 0.0};
+#pragma unroll
+        for (int kk = 0; kk < 2; ++kk) {
+            const double2 lo = *reinterpret_cast<const double2 *>(ya + (size_t)(j0 + 8 * kk) * TRSM_LD);
+            const double2 hi = *reinterpret_cast<const double2 *>(ya + (size_t)(j0 + 8 * kk + 4) * TRSM_LD);
+            const double a[4] = {lo.x, lo.y, hi.x, hi.y};
+            dmma1688(o, a, bi[kk]);
+        }
+        __syncthreads();
+        *d0 = make_double2(o[0], o[2]);
+        *d1 = make_double2(o[1], o[3]);
+    }
+    __syncthreads();
+    if (!UCASE) {
+        if (lane < nv) {
+            double *x = X + (size_t)warp * lda + lane;
+            const size_t step = (size_t)4 * lda;
+            for (int c = warp; c < ns; c += 4, x += step) *x = Ys[c * TRSM_LD + prow(lane)];
+        }
+    } else if (us < nv) {
+        double *x = X + (size_t)us * ns;
+        for (int c = uc; c < ns; c += 4) x[c] = Ys[c * TRSM_LD + prow(us)];
+    }
 }
 
 template <bool UCASE, class LU>
 static int launch_trsm(const LU &d, const Batch &b, int64_t ctas, int max_ns, const double *dinv, cudaStream_t s)
 {
     if (b.count <= 0 || ctas <= 0) return 0;
-    static std::atomic<unsigned long long> attr_0{0};
-    ensure_dyn_smem(trsm_kernel<UCASE, false, LU>, 227 * 1024, attr_0);
-    static std::atomic<unsigned long long> attr_1{0};
-    ensure_dyn_smem(trsm_kernel<UCASE, true, LU>, 227 * 1024, attr_1);
-    const size_t nsp = (size_t)((max_ns + 15) & ~15);
-    size_t smem = sizeof(double) * nsp * TRSM_LD, staged = smem + sizeof(double) * 2 * 16 * (nsp + 4);
-    if (max_ns > TRSM_WIDE_NS)   // narrower supernodes of the same batch keep their 64-vector strips
-        smem = std::max(sizeof(double) * TRSM_WIDE_NS * TRSM_LD, sizeof(double) * nsp * (TRSM_STRIP / 2 + 4));
-    const dim3 grid = member_grid(d, (unsigned)ctas);
-    if (max_ns <= TRSM_WIDE_NS && staged <= 227 * 1024) trsm_kernel<UCASE, true, LU><<<grid, 256, staged, s>>>(d, b, dinv);
-    else trsm_kernel<UCASE, false, LU><<<grid, 256, smem, s>>>(d, b, dinv);
+    static std::atomic<unsigned long long> attr{0};
+    ensure_dyn_smem(trsm_kernel<UCASE, LU>, (int)trsm_smem(MAX_NS), attr);
+    trsm_kernel<UCASE, LU><<<member_grid(d, (unsigned)ctas), TRSM_THREADS, trsm_smem(max_ns), s>>>(d, b, dinv);
     return 1;
 }
 int launch_trsm_l(const DeviceLU &d, const Batch &b, int64_t ctas, int max_ns, const double *dinv, cudaStream_t s)
@@ -785,8 +813,6 @@ struct HCfg {
     static constexpr size_t SMEM = sizeof(double) * STAGES * (A_STAGE + B_STAGE);
     static_assert(WTM % 16 == 0 && WTN % 8 == 0 && BK % 8 == 0, "tile shape vs m16n8k8");
 };
-__device__ __forceinline__ int prow(int r) { return (r & ~15) | ((r & 7) << 1) | ((r >> 3) & 1); }
-__device__ __forceinline__ int pk(int k) { return (k & ~7) | ((k & 3) << 1) | ((k >> 2) & 1); }
 
 template <int BM, int BN, int WARPS_M, int WARPS_N, int BK, int STAGES>
 __device__ __forceinline__ void gemm_tile_h(const double *__restrict__ A, int lda, const double *__restrict__ B, int ldb,
