@@ -386,6 +386,52 @@ int slu_b200_batch_schur_create(slu_b200_handle_t *h, const slu_b200_lu_view_t *
 int slu_b200_batch_schur_get(slu_b200_handle_t h, double *S, int lds);
 int slu_b200_batch_schur_condense(slu_b200_handle_t h, double *x, int ldx, int nrhs);
 int slu_b200_batch_schur_expand(slu_b200_handle_t h, double *x, int ldx, int nrhs);
+
+/* ---- static pivoting: row permutation and equilibration on the device fill (the pre-processing pdgssvx3d runs in front
+ * of pdgstrf3d: pdgsequ / pdlaqgs, pdgssvx3d.c:695, and the large-diagonal row permutation with its scalings, dldperm_dist
+ * job 5, pdgssvx3d.c:727).  The factorization pivots statically: a matrix with a zero or dominated diagonal (KKT /
+ * saddle-point systems, circuit matrices) needs its large entries moved to the diagonal first.  The matching runs once per
+ * pattern on the host (sluh_large_diag_perm, slu_b200_host.h); the fill, the equilibration and the vector transforms of the
+ * solve run on the device, on every fill and every member.
+ * fill_csr_scaled: as slu_b200_fill_csr, with F = Pc Pr Dr A Dc Pc^T: entry (i, j) of A goes to F(perm[perm_r[i]], perm[j])
+ * with the value (R[i] * a_ij) * C[j], evaluated in that order.  perm_r (perm_r[i] = the row of Pr A that holds row i of
+ * A), R and C may each be NULL (identity, ones); perm must be the final permutation of the pattern of Pr A (ordering and
+ * symbolic factorization run on that pattern).  The arena is zeroed first, each slot gets one plain store (deterministic);
+ * entries with no slot fail with their count.  flags & SLU_B200_FILL_EQUIL: equilibrate M = Pr Dr A Dc on the device with
+ * dgsequ_dist / dlaqgs_dist semantics: row maxima of |M|, column maxima of the row-scaled matrix, smlnum = dmach("S")
+ * clamping, and THRESH = 0.1 with the amax small / large tests choosing rows, columns, both or neither; the chosen factors
+ * are folded into R and C.  The magnitude is slud_z_abs1 (|re| + |im|) in doublecomplex.  The maxima are taken with
+ * integer atomics on the bit patterns, so R and C are bit-identical from run to run.  A zero row or column of A fails,
+ * naming it (dgsequ's info).  4 kernel launches with EQUIL, 2 without.
+ * out (nullable): [0] rowcnd, [1] colcnd, [2] amax, [3] equed (0 none, 1 rows, 2 columns, 3 both); without EQUIL 1, 1,
+ * max |f_ij|, 0.  [4] ||F||_inf as fixed-order row sums (no float atomics), the anorm of slu_b200_gscon(h, 'I', ...); [5]
+ * max |f_ij| ([4], [5] with the modulus).  The handle keeps perm_r, perm[perm_r[.]], perm and the final R and C in HBM until
+ * a later upload, fill_csr, batch_fill_csr or batch_fill_affine, which drops them.
+ * get_scaling: the kept perm_r, R and C (each nullable).
+ * solve_scaled: solve op(A) x = b on the factors of F, x (n x nrhs, ldx >= n) in A's own ordering, b on entry.  trans 0:
+ * b'[perm[perm_r[i]]] = R[i] b[i], F y = b', x[j] = C[j] y[perm[j]]; trans 1 / 2: b'[perm[j]] = C[j] b[j], F^T y = b' (F^H),
+ * x[i] = R[i] y[perm[perm_r[i]]].  Two launches on top of the plain solve, no n-vector work on the host; stats.reserved[4] /
+ * [5] as slu_b200_solve.  Fails unless the last fill was a scaled one and the factorization after it succeeded.
+ * All fail with a message, leaving the handle as it was, on a perm_r or perm that is not a permutation, an R or C entry
+ * that is not finite and > 0, Schur handles, and grids other than 1 x 1 x 1 with world_size 1.
+ * slu_b200_gscon, selinv, logdet and inertia keep describing F: log|det A| = log|det F| - sum log R_i - sum log C_j, the
+ * sign multiplied by sign(perm_r); inertia has no meaning once perm_r is not the identity. */
+#define SLU_B200_FILL_EQUIL 1
+int slu_b200_fill_csr_scaled(slu_b200_handle_t h, int n, const int32_t *rowptr, const int32_t *colind, const double *val,
+                             const int32_t *perm_r, const int32_t *perm, const double *R, const double *C, int flags,
+                             double out[6]);
+int slu_b200_get_scaling(slu_b200_handle_t h, int32_t *perm_r, double *R, double *C);
+int slu_b200_solve_scaled(slu_b200_handle_t h, double *x, int ldx, int nrhs, int trans);
+/* Batched: one perm_r and perm for all members (the reference's SamePattern_SameRowPerm: match a representative member on
+ * the host, equilibrate every member on the device).  val: batch x nnz, member-major; R and C shared (rc_per_member = 0:
+ * n entries) or per member (1: batch x n); out: batch x 6 (nullable).  The equilibration is one launch sequence over (rows,
+ * members), the launches of the unbatched call.  batch_get_scaling returns member `member`'s final R and C;
+ * batch_solve_scaled takes batch_solve's x layout and its per-member info checks. */
+int slu_b200_batch_fill_csr_scaled(slu_b200_handle_t h, int n, const int32_t *rowptr, const int32_t *colind, const double *val,
+                                   const int32_t *perm_r, const int32_t *perm, const double *R, const double *C, int rc_per_member,
+                                   int flags, double *out);
+int slu_b200_batch_get_scaling(slu_b200_handle_t h, int member, double *R, double *C);
+int slu_b200_batch_solve_scaled(slu_b200_handle_t h, double *x, int ldx, int nrhs, int trans);
 /* ---- doublecomplex twins (SRC/complex16/pzgstrf3d.c:120; the reference's z* handle API,
  * SRC/include/superlu_upacked.h:84-97).  Same view/options/stats structs: the Lnzval_bc_ptr / Unzval_br_ptr
  * entries point at arrays of doublecomplex {double r, i} (SRC/include/dcomplex.h:30) and are declared double*
@@ -463,6 +509,18 @@ int slu_b200_z_batch_schur_create(slu_b200_zhandle_t *h, const slu_b200_lu_view_
 int slu_b200_z_batch_schur_get(slu_b200_zhandle_t h, double *S, int lds);
 int slu_b200_z_batch_schur_condense(slu_b200_zhandle_t h, double *x, int ldx, int nrhs);
 int slu_b200_z_batch_schur_expand(slu_b200_zhandle_t h, double *x, int ldx, int nrhs);
+/* as slu_b200_fill_csr_scaled / _get_scaling / _solve_scaled and their batched twins, with the same semantics and
+ * messages: val and x hold interleaved doublecomplex, the scalings R and C are real; the equilibration uses slud_z_abs1. */
+int slu_b200_z_fill_csr_scaled(slu_b200_zhandle_t h, int n, const int32_t *rowptr, const int32_t *colind, const double *val,
+                               const int32_t *perm_r, const int32_t *perm, const double *R, const double *C, int flags,
+                               double out[6]);
+int slu_b200_z_get_scaling(slu_b200_zhandle_t h, int32_t *perm_r, double *R, double *C);
+int slu_b200_z_solve_scaled(slu_b200_zhandle_t h, double *x, int ldx, int nrhs, int trans);
+int slu_b200_z_batch_fill_csr_scaled(slu_b200_zhandle_t h, int n, const int32_t *rowptr, const int32_t *colind,
+                                     const double *val, const int32_t *perm_r, const int32_t *perm, const double *R,
+                                     const double *C, int rc_per_member, int flags, double *out);
+int slu_b200_z_batch_get_scaling(slu_b200_zhandle_t h, int member, double *R, double *C);
+int slu_b200_z_batch_solve_scaled(slu_b200_zhandle_t h, double *x, int ldx, int nrhs, int trans);
 int slu_b200_z_get_stats(slu_b200_zhandle_t h, slu_b200_stats_t *out);
 int slu_b200_z_plan(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, slu_b200_stats_t *stats);
 void slu_b200_z_destroy(slu_b200_zhandle_t h);

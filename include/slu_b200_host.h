@@ -38,6 +38,19 @@ void sluh_nd_order(int nx, int ny, int nz, int dof, int leaf, int32_t *perm);
  * first.  The role of get_perm_c_dist with METIS_AT_PLUS_A (get_perm_c.c:479-560).  perm[old] = new; 0 on success. */
 int sluh_nd_order_graph(int n, const int32_t *rowptr, const int32_t *colind, int leaf, int compress_dof, int32_t *perm);
 
+/* ---- static-pivoting row permutation (the role of dldperm_dist job 5 / LargeDiag_MC64, pdgssvx3d.c:727) ----------- */
+/* Maximum-product matching of the n x n CSR pattern with the scalings of MC64 job 5 (Duff & Koster 2001): absval[p] =
+ * |a_p| (the caller passes the modulus for complex A); explicit zeros are not edges.  perm_r[i] = the row of Pr A that
+ * holds row i of A, so that a_{i, perm_r[i]} lies on the diagonal of Pr A and the product of |diag| is maximal.
+ * R[i] = exp(u_i), C[j] = exp(v_j) / colmax_j from the optimal duals: |R_i a_ij C_j| <= 1 everywhere, = 1 on the
+ * matching (up to rounding).  Greedy start on the tight edges, then successive shortest augmenting paths (Dijkstra on
+ * reduced costs, binary heap); ties go to the smallest row index, so two calls give identical results.
+ * Returns 0; the structural rank r < n if A is structurally singular (perm_r, R, C then unwritten, out[0] = -inf);
+ * -1 on bad input (rowptr not starting at 0 or decreasing, colind outside 0 .. n-1, a negative or non-finite absval).
+ * out (nullable): [0] = sum_i log |a_{i, perm_r[i]}|, [1] = host seconds. */
+int sluh_large_diag_perm(int n, const int32_t *rowptr, const int32_t *colind, const double *absval, int32_t *perm_r,
+                         double *R, double *C, double out[2]);
+
 /* ---- symbolic factorization of P (A + A^T) P^T ----------------------------------------------- */
 typedef struct sluh_symb sluh_symb;
 /* perm_in[old] = new (NULL: identity).  The final permutation is perm_in composed with an etree

@@ -149,6 +149,16 @@ def lib():
     for f in ("slu_b200_batch_schur_condense", "slu_b200_z_batch_schur_condense", "slu_b200_batch_schur_expand",
               "slu_b200_z_batch_schur_expand"):
         getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
+    for f in ("slu_b200_fill_csr_scaled", "slu_b200_z_fill_csr_scaled"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 7 + [C.c_int, C.c_void_p]
+    for f in ("slu_b200_batch_fill_csr_scaled", "slu_b200_z_batch_fill_csr_scaled"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 7 + [C.c_int, C.c_int, C.c_void_p]
+    for f in ("slu_b200_get_scaling", "slu_b200_z_get_scaling"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    for f in ("slu_b200_batch_get_scaling", "slu_b200_z_batch_get_scaling"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    for f in ("slu_b200_solve_scaled", "slu_b200_z_solve_scaled", "slu_b200_batch_solve_scaled", "slu_b200_z_batch_solve_scaled"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
     _lib = L
     return L
 
@@ -185,6 +195,30 @@ def _norm_byte(norm):
     if not (isinstance(norm, str) and len(norm) == 1 and norm.isascii()):
         raise ValueError(f"norm must be '1', 'O' or 'I', not {norm!r}")
     return norm.encode()
+
+
+FILL_EQUIL = 1                      # SLU_B200_FILL_EQUIL
+_SCALED_OUT = ("rowcnd", "colcnd", "amax", "equed", "norm_inf", "max_abs")
+
+
+def _ptr(a):
+    return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def _scaled_args(rowptr, colind, perm, perm_r, R, C_, rc_shape):
+    """The int32 / float64 arrays of a scaled fill (None stays None: identity or ones)"""
+    rp = np.ascontiguousarray(rowptr, np.int32)
+    ci = np.ascontiguousarray(colind, np.int32)
+    pm = np.ascontiguousarray(perm, np.int32)
+    pr = None if perm_r is None else np.ascontiguousarray(perm_r, np.int32)
+    sc = []
+    for name, v in (("R", R), ("C", C_)):
+        if v is not None:
+            v = np.ascontiguousarray(v, np.float64)
+            if v.shape not in rc_shape:
+                raise ValueError(f"{name} must have shape {' or '.join(map(str, rc_shape))}, not {v.shape}")
+        sc.append(v)
+    return rp, ci, pm, pr, sc[0], sc[1]
 
 
 def device_count():
@@ -343,6 +377,36 @@ class Handle:
         _check(_fn("fill_csr", self.z_)(self.h, len(rp) - 1, rp.ctypes.data_as(C.c_void_p), ci.ctypes.data_as(C.c_void_p),
                                         v.ctypes.data_as(C.c_void_p), pm.ctypes.data_as(C.c_void_p)))
 
+    def fill_csr_scaled(self, rowptr, colind, val, perm, perm_r=None, R=None, C=None, equil=True):
+        """Scaled, row-permuted device fill (slu_b200_fill_csr_scaled): F = Pc Pr Dr A Dc Pc^T, entry (i, j) of A to
+        F(perm[perm_r[i]], perm[j]) as (R[i] a_ij) C[j]; perm_r, R, C from hostlib.large_diag_perm (None: identity / ones),
+        perm the ordering of the pattern of Pr A.  equil: equilibrate Pr Dr A Dc on the device (dgsequ / dlaqgs) and fold the
+        factors into R and C.  Replaces upload().  -> dict rowcnd, colcnd, amax, equed (0 none, 1 rows, 2 columns, 3 both),
+        norm_inf (||F||_inf, for rcond(norm_inf, 'I')), max_abs"""
+        rp, ci, pm, pr, Rv, Cv = _scaled_args(rowptr, colind, perm, perm_r, R, C, [(self.prob.n,)])
+        v = np.ascontiguousarray(val, self._dtype())
+        out = np.zeros(6)
+        _check(_fn("fill_csr_scaled", self.z_)(self.h, len(rp) - 1, _ptr(rp), _ptr(ci), _ptr(v), _ptr(pr), _ptr(pm), _ptr(Rv),
+                                               _ptr(Cv), FILL_EQUIL if equil else 0, _ptr(out)))
+        return {k: (int(x) if k == "equed" else float(x)) for k, x in zip(_SCALED_OUT, out)}
+
+    def scaling(self):
+        """(perm_r, R, C) of the last scaled fill, R and C with the equilibration folded in (slu_b200_get_scaling)"""
+        n = self.prob.n
+        pr, Rv, Cv = np.empty(n, np.int32), np.empty(n), np.empty(n)
+        _check(_fn("get_scaling", self.z_)(self.h, _ptr(pr), _ptr(Rv), _ptr(Cv)))
+        return pr, Rv, Cv
+
+    def solve_scaled(self, b, trans="N"):
+        """op(A) x = b in A's own ordering on the factors of a scaled fill (slu_b200_solve_scaled): the row permutation,
+        the scalings and perm are applied on the device.  b: (n,) or (nrhs, n); trans 'N', 'T' or 'H'."""
+        if trans not in _TRANS:
+            raise ValueError(f"trans must be 'N', 'T' or 'H', not {trans!r}")
+        x = np.array(b, self._dtype(), order="C", copy=True)
+        nrhs = 1 if x.ndim == 1 else x.shape[0]
+        _check(_fn("solve_scaled", self.z_)(self.h, _ptr(x), self.prob.n, nrhs, _TRANS[trans]))
+        return x
+
     def solve(self, b, trans="N"):
         """L U x = b on the device-resident factors (slu_b200_solve / slu_b200_z_solve); b: (n,) or (nrhs, n), ordering
         of the factored matrix, complex128 for a complex problem.  Returns x with the same shape and dtype.
@@ -487,6 +551,44 @@ class BatchHandle:
         pm = np.ascontiguousarray(perm, np.int32)
         _check(_fn("batch_fill_csr", self.z_)(self.h, len(rp) - 1, rp.ctypes.data_as(C.c_void_p), ci.ctypes.data_as(C.c_void_p),
                                               v.ctypes.data_as(C.c_void_p), pm.ctypes.data_as(C.c_void_p)))
+
+    def fill_csr_scaled(self, rowptr, colind, vals, perm, perm_r=None, R=None, C=None, equil=True):
+        """Handle.fill_csr_scaled for every member (slu_b200_batch_fill_csr_scaled): one pattern, perm_r and perm; vals
+        (batch, nnz); R and C (n,) shared or (batch, n) per member.  The equilibration runs per member.  -> dict of float64
+        arrays (batch,) with the keys of Handle.fill_csr_scaled (equed int32)"""
+        n, B = self.prob.n, self.batch
+        rp, ci, pm, pr, Rv, Cv = _scaled_args(rowptr, colind, perm, perm_r, R, C, [(n,), (B, n)])
+        per = [x.ndim == 2 for x in (Rv, Cv) if x is not None]
+        if len(set(per)) > 1:
+            raise ValueError("R and C must both be shared (n,) or both per member (batch, n)")
+        v = np.ascontiguousarray(vals, self._dtype())
+        if v.shape != (B, len(ci)):
+            raise ValueError(f"vals must have shape ({B}, {len(ci)}), not {v.shape}")
+        out = np.zeros((B, 6))
+        _check(_fn("batch_fill_csr_scaled", self.z_)(self.h, len(rp) - 1, _ptr(rp), _ptr(ci), _ptr(v), _ptr(pr), _ptr(pm), _ptr(Rv),
+                                                     _ptr(Cv), int(bool(per and per[0])), FILL_EQUIL if equil else 0, _ptr(out)))
+        res = {k: out[:, t].copy() for t, k in enumerate(_SCALED_OUT)}
+        res["equed"] = res["equed"].astype(np.int32)
+        return res
+
+    def scaling(self, member):
+        """(R, C) of member `member` after the last scaled fill (slu_b200_batch_get_scaling)"""
+        n = self.prob.n
+        Rv, Cv = np.empty(n), np.empty(n)
+        _check(_fn("batch_get_scaling", self.z_)(self.h, int(member), _ptr(Rv), _ptr(Cv)))
+        return Rv, Cv
+
+    def solve_scaled(self, b, trans="N"):
+        """Handle.solve_scaled for every member (slu_b200_batch_solve_scaled); b: (batch, n) or (batch, nrhs, n) in A's
+        ordering"""
+        if trans not in _TRANS:
+            raise ValueError(f"trans must be 'N', 'T' or 'H', not {trans!r}")
+        x = np.array(b, self._dtype(), order="C", copy=True)
+        if x.ndim not in (2, 3) or x.shape[0] != self.batch or x.shape[-1] != self.prob.n:
+            raise ValueError(f"b must have shape ({self.batch}, n) or ({self.batch}, nrhs, n) with n = {self.prob.n}")
+        nrhs = 1 if x.ndim == 2 else x.shape[1]
+        _check(_fn("batch_solve_scaled", self.z_)(self.h, _ptr(x), self.prob.n, nrhs, _TRANS[trans]))
+        return x
 
     def factor(self):
         """-> int32 array (batch,): 0, or the 1-based column of the member's first exact zero pivot."""

@@ -63,6 +63,12 @@
 #define slu_b200_batch_schur_get slu_b200_z_batch_schur_get
 #define slu_b200_batch_schur_condense slu_b200_z_batch_schur_condense
 #define slu_b200_batch_schur_expand slu_b200_z_batch_schur_expand
+#define slu_b200_fill_csr_scaled slu_b200_z_fill_csr_scaled
+#define slu_b200_get_scaling slu_b200_z_get_scaling
+#define slu_b200_solve_scaled slu_b200_z_solve_scaled
+#define slu_b200_batch_fill_csr_scaled slu_b200_z_batch_fill_csr_scaled
+#define slu_b200_batch_get_scaling slu_b200_z_batch_get_scaling
+#define slu_b200_batch_solve_scaled slu_b200_z_batch_solve_scaled
 #define SLU_API "slu_b200_z_"     // name prefix of the exported calls, for error messages
 #else
 #define SLU_API "slu_b200_"
@@ -325,6 +331,12 @@ struct slu_b200_handle_s {
     int nschur = 0, schur_first = INT_MAX;
     DevBuf<int2> d_sunits;
     DevBuf<val_t> d_S;
+    // static pivoting (slu_b200_fill_csr_scaled): the last scaled fill's perm_r, its composed row map perm[perm_r[i]], perm,
+    // and the final R and C (batch x n on a batched handle).  `scaled`: they describe the values in the arena (a later
+    // upload, fill_csr, batch_fill_csr or batch_fill_affine clears it).
+    DevBuf<int32_t> d_perm_r, d_rmap, d_cperm;
+    DevBuf<double> d_R, d_C;
+    bool scaled = false;
 };
 
 namespace {
@@ -1400,6 +1412,7 @@ void slu_b200_destroy(slu_b200_handle_t H)
     H->d_cv.release(); H->d_csgn.release(); H->d_cstate.release(); H->d_cpart.release(); H->d_ccount.release();
     H->d_tiny.release(); H->d_oz_i8.release(); H->d_oz_scale.release(); H->d_oz_rexp.release();
     H->d_hinv.release(); H->d_si_pool.release(); H->d_sunits.release(); H->d_S.release();
+    H->d_perm_r.release(); H->d_rmap.release(); H->d_cperm.release(); H->d_R.release(); H->d_C.release();
     delete H;
 }
 
@@ -1540,6 +1553,7 @@ int slu_b200_upload(slu_b200_handle_t H)
     double t0 = now_s();
     H->factored = false;
     H->si_ready = false;
+    H->scaled = false;
     if (transfer(H, true)) return -1;
     H->st.t_upload_s = now_s() - t0;
     H->uploaded = true;
@@ -1716,6 +1730,7 @@ int slu_b200_factor_host(slu_b200_handle_t H, int *info)
     }
     if (H->grouped) {                      // options.reserved[3]: H2D, factorization and D2H all overlapped
         H->factored = false;
+        H->scaled = false;
         if (pipe_prepare(H) || upload_pipe_issue(H)) return -1;
         H->uploaded = true;
         H->st.t_upload_s = 0;
@@ -1741,6 +1756,7 @@ int slu_b200_fill_csr(slu_b200_handle_t H, int n, const int32_t *rowptr, const i
     if (n != H->n) return fail("matrix order %d does not match the handle's %d", n, H->n);
     if (H->P2 > 1) return fail("slu_b200_fill_csr handles 1 x 1 x Pz grids");
     H->si_ready = false;
+    H->scaled = false;
     double t0 = now_s();
     const int64_t nnz = rowptr[n];
     DevBuf<int32_t> drp, dci, dperm;
@@ -2288,6 +2304,7 @@ int slu_b200_batch_fill_csr(slu_b200_handle_t H, int n, const int32_t *rowptr, c
     CU(cudaMemcpyAsync(dv.p, val, (size_t)nnz * B * sizeof(val_t), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(dperm.p, perm, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     H->si_ready = false;
+    H->scaled = false;
     CU(cudaMemsetAsync(H->val.p, 0, H->val.bytes(), s));
     CU(cudaMemsetAsync(err, 0, sizeof(int), s));
     launch_fill_csr(H->bdev, n, drp.p, dci.p, dv.p, dperm.p, dact.p, err, s);
@@ -2692,6 +2709,7 @@ int slu_b200_batch_fill_affine(slu_b200_handle_t H, int n, const int32_t *rowptr
     CU(cudaMemcpyAsync(dterms.p, terms, (size_t)nnz * nterms * sizeof(val_t), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(dcoef.p, coef, (size_t)B * nterms * sizeof(val_t), cudaMemcpyHostToDevice, s));
     H->si_ready = false;
+    H->scaled = false;
     CU(cudaMemsetAsync(H->val.p, 0, H->val.bytes(), s));
     CU(cudaMemsetAsync(err, 0, sizeof(int), s));
     launch_fill_affine(H->bdev, n, drp.p, dci.p, dperm.p, dact.p, ddst.p, nnz, nterms, dterms.p, dcoef.p, err, s);
@@ -2704,6 +2722,234 @@ int slu_b200_batch_fill_affine(slu_b200_handle_t H, int n, const int32_t *rowptr
     if (bad) return fail("%s: %d entries of the pattern have no slot in the L/U structure (wrong permutation or symbolic structure)", fn, bad);
     H->st.t_upload_s = now_s() - t0;
     return 0;
+}
+
+// ---- static pivoting: the row permutation and scalings of pdgssvx3d (pdgssvx3d.c:695-727) around the device routes.
+// The matching runs once per pattern on the host (sluh_large_diag_perm); the scaled, row-permuted fill, the equilibration
+// and the vector transforms of the solve run on the device, per fill and per member.
+static int check_perm(const int32_t *p, int n, std::vector<char> &seen, const char *fn, const char *what)
+{
+    seen.assign(n, 0);
+    for (int i = 0; i < n; ++i) {
+        if (p[i] < 0 || p[i] >= n || seen[p[i]]) return fail("%s: %s is not a permutation of 0 ... %d (entry %d = %d)", fn, what, n - 1, i, p[i]);
+        seen[p[i]] = 1;
+    }
+    return 0;
+}
+
+static int check_scale(const double *v, int64_t len, const char *fn, const char *what)
+{
+    for (int64_t t = 0; t < len; ++t)
+        if (!(std::isfinite(v[t]) && v[t] > 0.0)) return fail("%s: %s[%lld] = %g, must be finite and > 0", fn, what, (long long)t, v[t]);
+    return 0;
+}
+
+// the checks shared by the scaled calls: the handle kind (batched or not), no Schur handle, a 1 x 1 x 1 grid
+static int refuse_scaled(const slu_b200_handle_s *H, bool batched, const char *fn)
+{
+    if (batched ? refuse_unbatched(H, fn) : refuse_batched(H, fn)) return -1;
+    if (refuse_schur(H, fn)) return -1;
+    if (H->view.nprow * H->view.npcol * H->view.npdep != 1 || H->opt.world_size > 1)
+        return fail("%s needs a 1 x 1 x 1 grid with world_size 1 (got %d x %d x %d, world_size %d)", fn, H->view.nprow, H->view.npcol,
+                    H->view.npdep, H->opt.world_size);
+    return 0;
+}
+
+// batched: every member's values (val: members x nnz), R / C shared (rc_per_member = 0) or per member; out: members x 6
+static int fill_scaled_impl(slu_b200_handle_t H, bool batched, int n, const int32_t *rowptr, const int32_t *colind, const double *val,
+                            const int32_t *perm_r, const int32_t *perm, const double *R, const double *C, int rc_per_member, int flags,
+                            double *out, const char *fn)
+{
+    if (!H || !rowptr || !colind || !val || !perm) return fail("null argument");
+    if (refuse_scaled(H, batched, fn)) return -1;
+    if (n != H->n) return fail("%s: matrix order %d does not match the handle's %d", fn, n, H->n);
+    if (flags & ~SLU_B200_FILL_EQUIL) return fail("%s: unknown flags 0x%x", fn, flags);
+    if (rc_per_member != 0 && rc_per_member != 1) return fail("%s: rc_per_member = %d, must be 0 or 1", fn, rc_per_member);
+    if (rowptr[0] != 0) return fail("%s: bad rowptr (rowptr[0] = %d, must be 0)", fn, rowptr[0]);
+    for (int i = 0; i < n; ++i)
+        if (rowptr[i + 1] < rowptr[i]) return fail("%s: bad rowptr (rowptr[%d] = %d < rowptr[%d] = %d)", fn, i + 1, rowptr[i + 1], i, rowptr[i]);
+    const int64_t nnz = rowptr[n];
+    for (int64_t p = 0; p < nnz; ++p)
+        if (colind[p] < 0 || colind[p] >= n) return fail("%s: colind[%lld] = %d is outside 0 ... %d", fn, (long long)p, colind[p], n - 1);
+    std::vector<char> seen;
+    if ((perm_r && check_perm(perm_r, n, seen, fn, "perm_r")) || check_perm(perm, n, seen, fn, "perm")) return -1;
+    const int B = batched ? H->batch : 1;
+    const int64_t rc_len = (int64_t)n * (rc_per_member ? B : 1);
+    if ((R && check_scale(R, rc_len, fn, "R")) || (C && check_scale(C, rc_len, fn, "C"))) return -1;
+    const bool equil = flags & SLU_B200_FILL_EQUIL;
+    double t0 = now_s();
+    std::vector<int32_t> pr(n), rmap(n);
+    for (int i = 0; i < n; ++i) {
+        pr[i] = perm_r ? perm_r[i] : i;
+        rmap[i] = perm[pr[i]];
+    }
+    // every panel of a 1 x 1 x 1 grid is held
+    std::vector<int8_t> act(H->nsupers, 1);
+    std::vector<EquilStat> st0(B, EquilStat{0, 0, 0, 0, 0, 0, INT_MAX, INT_MAX});
+    for (auto &e : st0) {
+        const double big = 1.0 / 2.2250738585072014e-308;   // dgsequ's initial rcmin: bignum = 1 / dmach("S")
+        memcpy(&e.rmin, &big, sizeof big);
+        e.cmin = e.rmin;
+    }
+    DevBuf<int32_t> drp, dci;
+    DevBuf<val_t> dv;
+    DevBuf<double> dRin, dCin, drinv, dout;
+    DevBuf<unsigned long long> dccol;
+    DevBuf<EquilStat> dst;
+    DevBuf<int8_t> dact;
+    const size_t bn = (size_t)B * n;
+    if (drp.alloc((size_t)n + 1) || dci.alloc((size_t)nnz) || dv.alloc((size_t)nnz * B) || dact.upload(act) || dst.upload(st0) ||
+        dout.alloc((size_t)B * 6) || (R && dRin.alloc((size_t)rc_len)) || (C && dCin.alloc((size_t)rc_len)) ||
+        (equil && (drinv.alloc(bn) || dccol.alloc(bn))))
+        return -1;
+    if (H->d_R.n != bn && (H->d_R.alloc(bn) || H->d_C.alloc(bn))) return -1;
+    if (H->d_perm_r.n != (size_t)n && (H->d_perm_r.alloc(n) || H->d_rmap.alloc(n) || H->d_cperm.alloc(n))) return -1;
+    cudaStream_t s = H->stream;
+    int *err = H->d_flags.p + (batched ? B : 1);
+    H->si_ready = false;
+    H->scaled = false;
+    H->uploaded = false;
+    H->factored = false;
+    if (batched) H->member_info.assign(B, -1);
+    CU(cudaMemcpyAsync(drp.p, rowptr, ((size_t)n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(dci.p, colind, (size_t)nnz * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(dv.p, val, (size_t)nnz * B * sizeof(val_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(H->d_perm_r.p, pr.data(), (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(H->d_rmap.p, rmap.data(), (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(H->d_cperm.p, perm, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    if (R) CU(cudaMemcpyAsync(dRin.p, R, (size_t)rc_len * sizeof(double), cudaMemcpyHostToDevice, s));
+    if (C) CU(cudaMemcpyAsync(dCin.p, C, (size_t)rc_len * sizeof(double), cudaMemcpyHostToDevice, s));
+    if (equil) CU(cudaMemsetAsync(dccol.p, 0, bn * sizeof(unsigned long long), s));
+    CU(cudaMemsetAsync(H->val.p, 0, H->val.bytes(), s));
+    CU(cudaMemsetAsync(err, 0, sizeof(int), s));
+    ScaledFill f{};
+    f.n = n;
+    f.rowptr = drp.p; f.colind = dci.p; f.rmap = H->d_rmap.p; f.perm = H->d_cperm.p; f.aval = dv.p;
+    f.R_in = R ? dRin.p : nullptr; f.C_in = C ? dCin.p : nullptr; f.rc_stride = rc_per_member ? n : 0;
+    f.R = H->d_R.p; f.C = H->d_C.p; f.rinv = drinv.p; f.ccol = dccol.p; f.st = dst.p; f.out = dout.p;
+    f.active = dact.p; f.err = err;
+    if (batched) launch_fill_scaled(H->bdev, f, equil, s);
+    else launch_fill_scaled(H->dev, f, equil, s);
+    int bad = 0;
+    std::vector<double> o(equil ? (size_t)B * 6 : 0);
+    CU(cudaMemcpyAsync(&bad, err, sizeof(int), cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(st0.data(), dst.p, (size_t)B * sizeof(EquilStat), cudaMemcpyDeviceToHost, s));
+    if (equil) CU(cudaMemcpyAsync(o.data(), dout.p, o.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    if (bad) return fail("%s: %d entries of A have no slot in the L/U structure (wrong permutation or symbolic structure)", fn, bad);
+    for (int m = 0; equil && m < B; ++m) {   // dgsequ's info: the first exactly zero row, else the first zero column
+        char mem[32] = "";
+        if (batched) snprintf(mem, sizeof mem, " (member %d)", m);
+        if (st0[m].zrow != INT_MAX) return fail("%s: row %d of A%s is exactly zero: cannot equilibrate", fn, st0[m].zrow, mem);
+        if (st0[m].zcol != INT_MAX) return fail("%s: column %d of A%s is exactly zero: cannot equilibrate", fn, st0[m].zcol, mem);
+    }
+    if (out)
+        for (int m = 0; m < B; ++m) {
+            double *om = out + (size_t)m * 6, fn_, fm;
+            memcpy(&fn_, &st0[m].fnorm, sizeof fn_);
+            memcpy(&fm, &st0[m].fmax, sizeof fm);
+            if (equil) for (int k = 0; k < 4; ++k) om[k] = o[(size_t)m * 6 + k];
+            else { om[0] = om[1] = 1.0; om[2] = fm; om[3] = 0.0; }
+            om[4] = fn_;
+            om[5] = fm;
+        }
+    H->st.t_upload_s = now_s() - t0;
+    H->uploaded = true;
+    H->scaled = true;
+    return 0;
+}
+
+static int get_scaling_impl(slu_b200_handle_t H, bool batched, int member, int32_t *perm_r, double *R, double *C, const char *fn)
+{
+    if (!H) return fail("null handle");
+    if (refuse_scaled(H, batched, fn)) return -1;
+    if (!H->scaled) return fail("%s needs a scaled fill on this handle first (a later upload, fill_csr, batch_fill_csr or batch_fill_affine drops the scaling)", fn);
+    if (batched && (member < 0 || member >= H->batch)) return fail("%s: member %d is outside 0 ... %d", fn, member, H->batch - 1);
+    const size_t n = (size_t)H->n, off = (size_t)member * n;
+    if (perm_r) CU(cudaMemcpy(perm_r, H->d_perm_r.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    if (R) CU(cudaMemcpy(R, H->d_R.p + off, n * sizeof(double), cudaMemcpyDeviceToHost));
+    if (C) CU(cudaMemcpy(C, H->d_C.p + off, n * sizeof(double), cudaMemcpyDeviceToHost));
+    return 0;
+}
+
+// x in A's ordering: b' = the row-permuted, scaled b into the solve's input (one scatter launch), the plain solve, x = the
+// scaled, permuted-back solution (one gather launch).  trans 0: b'[rmap[i]] = R[i] b[i], x[j] = C[j] y[perm[j]]; trans 1 / 2:
+// b'[perm[j]] = C[j] b[j], x[i] = R[i] y[rmap[i]] (the scalings are real, so F^H needs nothing more than F^T).
+static int solve_scaled_impl(slu_b200_handle_t H, bool batched, double *xh, int ldx, int nrhs, int trans, const char *fn)
+{
+    if (!H || !xh) return fail("null argument");
+    if (refuse_scaled(H, batched, fn)) return -1;
+    if (trans < 0 || trans > 2) return fail("%s: trans = %d, must be 0 (A x = b), 1 (A^T x = b) or 2 (A^H x = b)", fn, trans);
+    if (!H->scaled) return fail("%s needs a scaled fill on this handle first (a later upload, fill_csr, batch_fill_csr or batch_fill_affine drops the scaling)", fn);
+    const int B = batched ? H->batch : 1, n = H->n;
+    if (batched) {
+        if (refuse_unfactored_members(H, fn)) return -1;
+    } else if (!H->factored) {
+        return fail("%s needs a successful " SLU_API "factor after the scaled fill", fn);
+    }
+    if (nrhs < 1 || ldx < n) return fail("bad nrhs / ldx");
+    if ((int64_t)n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
+    const size_t len = (size_t)n * nrhs * B;
+    if (H->d_x.n < len && H->d_x.alloc(len)) return -1;
+    if (H->d_x2.n < len && H->d_x2.alloc(len)) return -1;
+    cudaStream_t s = H->stream;
+    double t0 = now_s();
+    val_t *in = batched ? H->d_x2.p : H->d_x.p, *b = batched ? H->d_x.p : H->d_x2.p;   // the solve takes b' in d_x / d_x2
+    CU(cudaMemcpy2DAsync(in, (size_t)n * sizeof(val_t), xh, (size_t)ldx * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs * B,
+                         cudaMemcpyHostToDevice, s));
+    int launches = launch_permute_scale(b, in, trans ? H->d_cperm.p : H->d_rmap.p, trans ? H->d_C.p : H->d_R.p, n, nrhs, B, true, s);
+    val_t *y = H->d_x.p;
+    if (batched) {
+        launches += batch_solve_dev(H, nrhs, trans);
+    } else {
+        const int l = solve_dev(H, nrhs, trans, &y);
+        if (l < 0) return -1;
+        launches += l;
+    }
+    val_t *x = H->d_x2.p;
+    launches += launch_permute_scale(x, y, trans ? H->d_rmap.p : H->d_cperm.p, trans ? H->d_R.p : H->d_C.p, n, nrhs, B, false, s);
+    CU(cudaMemcpy2DAsync(xh, (size_t)ldx * sizeof(val_t), x, (size_t)n * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs * B,
+                         cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    H->st.reserved[4] = now_s() - t0;
+    H->st.reserved[5] = (double)launches;
+    return 0;
+}
+
+int slu_b200_fill_csr_scaled(slu_b200_handle_t H, int n, const int32_t *rowptr, const int32_t *colind, const double *val,
+                             const int32_t *perm_r, const int32_t *perm, const double *R, const double *C, int flags, double out[6])
+{
+    return fill_scaled_impl(H, false, n, rowptr, colind, val, perm_r, perm, R, C, 0, flags, out, SLU_API "fill_csr_scaled");
+}
+
+int slu_b200_get_scaling(slu_b200_handle_t H, int32_t *perm_r, double *R, double *C)
+{
+    return get_scaling_impl(H, false, 0, perm_r, R, C, SLU_API "get_scaling");
+}
+
+int slu_b200_solve_scaled(slu_b200_handle_t H, double *x, int ldx, int nrhs, int trans)
+{
+    return solve_scaled_impl(H, false, x, ldx, nrhs, trans, SLU_API "solve_scaled");
+}
+
+int slu_b200_batch_fill_csr_scaled(slu_b200_handle_t H, int n, const int32_t *rowptr, const int32_t *colind, const double *val,
+                                   const int32_t *perm_r, const int32_t *perm, const double *R, const double *C, int rc_per_member,
+                                   int flags, double *out)
+{
+    return fill_scaled_impl(H, true, n, rowptr, colind, val, perm_r, perm, R, C, rc_per_member, flags, out,
+                            SLU_API "batch_fill_csr_scaled");
+}
+
+int slu_b200_batch_get_scaling(slu_b200_handle_t H, int member, double *R, double *C)
+{
+    return get_scaling_impl(H, true, member, nullptr, R, C, SLU_API "batch_get_scaling");
+}
+
+int slu_b200_batch_solve_scaled(slu_b200_handle_t H, double *x, int ldx, int nrhs, int trans)
+{
+    return solve_scaled_impl(H, true, x, ldx, nrhs, trans, SLU_API "batch_solve_scaled");
 }
 
 // ---- partial factorization on batched handles: a batched handle whose level plan leaves out the Schur supernodes, as an

@@ -184,6 +184,38 @@ int launch_fill_csr(const BatchedLU &d, int n, const int32_t *rowptr, const int3
 int launch_fill_affine(const BatchedLU &d, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm, const int8_t *active,
                        int64_t *dst, int64_t nnz, int nterms, const val_t *terms, const val_t *coef, int *err, cudaStream_t s);
 
+// scaled, row-permuted fill (slu_b200_fill_csr_scaled and its batched / z twins): F = Pc Pr Dr A Dc Pc^T, entry (i, j) of A to
+// F(rmap[i], perm[j]) with rmap = perm o perm_r, value (R[i] a_ij) C[j].  Per member: the equilibration reductions (bit
+// patterns of non-negative doubles, which order as unsigned integers) and the norms of F.
+struct EquilStat {
+    unsigned long long rmin, rmax;   // min / max of the row maxima of |Pr Dr A Dc| (rmin starts at bignum, as dgsequ's rcmin)
+    unsigned long long cmin, cmax;   // min / max of the column maxima of the row-scaled matrix
+    unsigned long long fnorm, fmax;  // ||F||_inf and max |f_ij|
+    int zrow, zcol;                  // smallest row / column of A that is exactly zero (INT_MAX: none)
+};
+struct ScaledFill {
+    int n;
+    const int32_t *rowptr, *colind, *rmap, *perm;
+    const val_t *aval;                 // members x nnz values, member-major
+    const double *R_in, *C_in;         // nullptr: ones; else rc_stride elements apart per member (0: shared)
+    int64_t rc_stride;
+    double *R, *C;                     // members x n: the final scalings
+    double *rinv;                      // members x n scratch: dgsequ's row factors
+    unsigned long long *ccol;          // members x n scratch: column maxima (bits)
+    EquilStat *st;                     // [members]
+    double *out;                       // members x 6 (slu_b200_fill_csr_scaled's out[0..3])
+    const int8_t *active;
+    int *err;                          // entries without a slot (member 0's count)
+};
+// equil: 4 launches (row maxima and column maxima, column reductions, the dgsequ / dlaqgs decision folded into R and C, the
+// scatter with the norms); else 2 (R and C copied, the scatter).  Over (rows, members).
+int launch_fill_scaled(const DeviceLU &d, const ScaledFill &f, bool equil, cudaStream_t s);
+int launch_fill_scaled(const BatchedLU &d, const ScaledFill &f, bool equil, cudaStream_t s);
+// the vector transforms of slu_b200_solve_scaled, over (entries, members) with members blocks of n x nrhs (scale: n per
+// member): scatter dst[map[i]] = scale[i] src[i], else gather dst[i] = scale[i] src[map[i]]
+int launch_permute_scale(val_t *dst, const val_t *src, const int32_t *map, const double *scale, int n, int nrhs, int members,
+                         bool scatter, cudaStream_t s);
+
 // slu_cond.cu (double) / slu_cond_z.cu (doublecomplex): the step kernels of the dlacn2 / zlacn2 1-norm estimator
 // (slu_b200_gscon).  One CondState per member: dlacn2's EST, ESTOLD and ISAVE(1..3) as phase, j, iter; kase = the solve
 // the member waits for (1: with B, 2: with B^T / B^H, 0: done); act = the next vector its last step wrote.

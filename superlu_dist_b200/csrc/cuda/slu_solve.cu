@@ -424,6 +424,168 @@ int launch_fill_affine(const BatchedLU &d, int n, const int32_t *rowptr, const i
     fill_affine_kernel<<<member_grid(d, (unsigned)((nnz + FA_THREADS - 1) / FA_THREADS)), FA_THREADS, 0, s>>>(d, nnz, nterms, terms, coef, dst);
     return 2;
 }
+// ---- scaled, row-permuted fill (slu_b200_fill_csr_scaled) ----
+// M = Pr Dr A Dc with the caller's R, C; its equilibration follows dgsequ_dist / dlaqgs_dist (SRC/double/dgsequ_dist.c,
+// dlaqgs_dist.c) with the magnitude of slud_z_abs1 (|re| + |im|) in doublecomplex.  The maxima are order-independent, so
+// the atomics on their bit patterns give the same R and C on every run.  Thread = row i of A (row rmap[i] of F), member
+// blockIdx.y.
+constexpr double EQ_SMLNUM = 2.2250738585072014e-308;           // dmach_dist("S") = DBL_MIN
+constexpr double EQ_BIGNUM = 1.0 / EQ_SMLNUM;
+constexpr double EQ_SMALL = EQ_SMLNUM / 2.220446049250313e-16;  // dlaqgs: dmach("Safe minimum") / dmach("Precision")
+constexpr double EQ_LARGE = 1.0 / EQ_SMALL;
+constexpr double EQ_THRESH = 0.1;
+
+__device__ __forceinline__ double eq_abs1(double v) { return fabs(v); }
+__device__ __forceinline__ double eq_abs1(double2 v) { return fabs(v.x) + fabs(v.y); }
+__device__ __forceinline__ double eq_mod(double v) { return fabs(v); }
+__device__ __forceinline__ double eq_mod(double2 v) { return hypot(v.x, v.y); }
+__device__ __forceinline__ double vscale_d(double s, double v) { return s * v; }
+__device__ __forceinline__ double2 vscale_d(double s, double2 v) { return make_double2(s * v.x, s * v.y); }
+__device__ __forceinline__ unsigned long long dbits(double v) { return (unsigned long long)__double_as_longlong(v); }
+__device__ __forceinline__ double bitsd(unsigned long long b) { return __longlong_as_double((long long)b); }
+// entry p of row i, scaled: (R[i] a) C[j], in that order
+__device__ __forceinline__ val_t scaled_entry(const ScaledFill &f, const val_t *aval, const double *R, const double *C, int i, int64_t p)
+{
+    const double ri = R ? R[i] : 1.0, cj = C ? C[f.colind[p]] : 1.0;
+    return vscale_d(cj, vscale_d(ri, aval[p]));
+}
+
+// row maxima r_i of |M| (stat rmin / rmax / zrow), then the column maxima of |M_ij| / clamp(r_i) into ccol
+__global__ void equil_rows_kernel(ScaledFill f)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x, m = blockIdx.y;
+    if (i >= f.n) return;
+    const int64_t nnz = f.rowptr[f.n];
+    const val_t *aval = f.aval + (int64_t)m * nnz;
+    const double *R = f.R_in ? f.R_in + m * f.rc_stride : nullptr, *C = f.C_in ? f.C_in + m * f.rc_stride : nullptr;
+    double rm = 0.0;
+    for (int64_t p = f.rowptr[i]; p < f.rowptr[i + 1]; ++p) rm = fmax(rm, eq_abs1(scaled_entry(f, aval, R, C, i, p)));
+    EquilStat *st = f.st + m;
+    atomicMin(&st->rmin, dbits(rm));
+    atomicMax(&st->rmax, dbits(rm));
+    if (rm == 0.0) atomicMin(&st->zrow, i);
+    const double r = 1.0 / fmin(fmax(rm, EQ_SMLNUM), EQ_BIGNUM);
+    f.rinv[(int64_t)m * f.n + i] = r;
+    unsigned long long *ccol = f.ccol + (int64_t)m * f.n;
+    for (int64_t p = f.rowptr[i]; p < f.rowptr[i + 1]; ++p)
+        atomicMax(ccol + f.colind[p], dbits(eq_abs1(scaled_entry(f, aval, R, C, i, p)) * r));
+}
+
+// thread = column j: stat cmin / cmax / zcol
+__global__ void equil_cols_kernel(ScaledFill f)
+{
+    const int j = blockIdx.x * blockDim.x + threadIdx.x, m = blockIdx.y;
+    if (j >= f.n) return;
+    const unsigned long long c = f.ccol[(int64_t)m * f.n + j];
+    EquilStat *st = f.st + m;
+    atomicMin(&st->cmin, c);
+    atomicMax(&st->cmax, c);
+    if (c == 0) atomicMin(&st->zcol, j);
+}
+
+// thread = index t: the final R[t] and C[t] of the member.  equil: dgsequ's rowcnd / colcnd / amax and dlaqgs's choice
+// (THRESH, SMALL, LARGE), the chosen factors folded into the caller's; the member's out[0..3].  Else a copy (ones for nullptr).
+template <bool EQUIL>
+__global__ void equil_apply_kernel(ScaledFill f)
+{
+    const int t = blockIdx.x * blockDim.x + threadIdx.x, m = blockIdx.y;
+    if (t >= f.n) return;
+    const double rin = f.R_in ? f.R_in[m * f.rc_stride + t] : 1.0, cin = f.C_in ? f.C_in[m * f.rc_stride + t] : 1.0;
+    const int64_t o = (int64_t)m * f.n + t;
+    if (!EQUIL) {
+        f.R[o] = rin;
+        f.C[o] = cin;
+        return;
+    }
+    const EquilStat st = f.st[m];
+    const double amax = bitsd(st.rmax);
+    const double rowcnd = fmax(bitsd(st.rmin), EQ_SMLNUM) / fmin(amax, EQ_BIGNUM);
+    const double colcnd = fmax(bitsd(st.cmin), EQ_SMLNUM) / fmin(bitsd(st.cmax), EQ_BIGNUM);
+    int equed;   // 0 none, 1 rows, 2 columns, 3 both
+    if (rowcnd >= EQ_THRESH && amax >= EQ_SMALL && amax <= EQ_LARGE) equed = colcnd >= EQ_THRESH ? 0 : 2;
+    else equed = colcnd >= EQ_THRESH ? 1 : 3;
+    f.R[o] = (equed & 1) ? rin * f.rinv[o] : rin;
+    f.C[o] = (equed & 2) ? cin * (1.0 / fmin(fmax(bitsd(f.ccol[o]), EQ_SMLNUM), EQ_BIGNUM)) : cin;
+    if (t == 0) {
+        double *out = f.out + (int64_t)m * 6;
+        out[0] = rowcnd;
+        out[1] = colcnd;
+        out[2] = amax;
+        out[3] = equed;
+    }
+}
+
+// the scatter into the zeroed arena, one plain store per slot; the row's sum of |f_ij| in CSR order (fixed) and its max
+// go to the member's fnorm / fmax
+template <class LU>
+__global__ void fill_scaled_kernel(LU dd, ScaledFill f)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x, m = blockIdx.y;
+    if (i >= f.n) return;
+    const DeviceLU &d = member_view(dd);
+    const int64_t nnz = f.rowptr[f.n];
+    const val_t *aval = f.aval + (int64_t)m * nnz;
+    const double *R = f.R + (int64_t)m * f.n, *C = f.C + (int64_t)m * f.n;
+    const int pi = f.rmap[i];
+    double sum = 0.0, mx = 0.0;
+    for (int64_t p = f.rowptr[i]; p < f.rowptr[i + 1]; ++p) {
+        const val_t v = scaled_entry(f, aval, R, C, i, p);
+        const double a = eq_mod(v);
+        sum += a;
+        mx = fmax(mx, a);
+        const int64_t o = csr_slot(d, pi, f.perm[f.colind[p]], f.active);
+        if (o >= 0) d.val[o] = v;
+        else if (o == -2 && m == 0) atomicAdd(f.err, 1);
+    }
+    atomicMax(&f.st[m].fnorm, dbits(sum));
+    atomicMax(&f.st[m].fmax, dbits(mx));
+}
+
+template <class LU>
+static int launch_fill_scaled_t(const LU &d, const ScaledFill &f, bool equil, cudaStream_t s)
+{
+    if (f.n <= 0) return 0;
+    const dim3 g = member_grid(d, (unsigned)((f.n + 127) / 128));
+    if (equil) {
+        equil_rows_kernel<<<g, 128, 0, s>>>(f);
+        equil_cols_kernel<<<g, 128, 0, s>>>(f);
+        equil_apply_kernel<true><<<g, 128, 0, s>>>(f);
+    } else {
+        equil_apply_kernel<false><<<g, 128, 0, s>>>(f);
+    }
+    fill_scaled_kernel<LU><<<g, 128, 0, s>>>(d, f);
+    return equil ? 4 : 2;
+}
+int launch_fill_scaled(const DeviceLU &d, const ScaledFill &f, bool equil, cudaStream_t s) { return launch_fill_scaled_t(d, f, equil, s); }
+int launch_fill_scaled(const BatchedLU &d, const ScaledFill &f, bool equil, cudaStream_t s) { return launch_fill_scaled_t(d, f, equil, s); }
+
+// thread = entry i of the member blockIdx.y, every right-hand side
+template <bool SCATTER>
+__global__ void permute_scale_kernel(val_t *__restrict__ dst, const val_t *__restrict__ src, const int32_t *__restrict__ map,
+                                     const double *__restrict__ scale, int n, int nrhs)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int64_t base = (int64_t)blockIdx.y * n * nrhs;
+    const double sc = scale[(int64_t)blockIdx.y * n + i];
+    const int k = map[i];
+    for (int r = 0; r < nrhs; ++r) {
+        const int64_t c = base + (int64_t)r * n;
+        if (SCATTER) dst[c + k] = vscale_d(sc, src[c + i]);
+        else dst[c + i] = vscale_d(sc, src[c + k]);
+    }
+}
+
+int launch_permute_scale(val_t *dst, const val_t *src, const int32_t *map, const double *scale, int n, int nrhs, int members,
+                         bool scatter, cudaStream_t s)
+{
+    if (n <= 0) return 0;
+    const dim3 g((unsigned)((n + 255) / 256), (unsigned)members);
+    if (scatter) permute_scale_kernel<true><<<g, 256, 0, s>>>(dst, src, map, scale, n, nrhs);
+    else permute_scale_kernel<false><<<g, 256, 0, s>>>(dst, src, map, scale, n, nrhs);
+    return 1;
+}
+
 template <class LU>
 static int launch_fill_csr_t(const LU &d, int n, const int32_t *rowptr, const int32_t *colind, const val_t *aval, const int32_t *perm,
                              const int8_t *active, int *err, cudaStream_t s)

@@ -53,8 +53,42 @@ def lib():
     L.sluh_matrix_export_csr.argtypes = [C.c_void_p, i32p, i32p, f64p]
     L.sluh_matrix_free.argtypes = [C.c_void_p]
     L.sluh_write_binary.argtypes = [C.c_char_p, C.c_int32, C.c_int32, i32p, i32p, f64p]
+    L.sluh_large_diag_perm.argtypes = [C.c_int, i32p, i32p, f64p, i32p, f64p, f64p, f64p]
     _lib = L
     return L
+
+
+def large_diag_perm(rowptr, colind, val):
+    """Maximum-product matching with the MC64 job-5 scalings (sluh_large_diag_perm) -> (perm_r, R, C, logprod):
+    perm_r[i] = the row of Pr A that holds row i of A, |R_i a_ij C_j| <= 1 with equality on the matching, logprod =
+    sum_i log |a_{i, perm_r[i]}|.  val may be complex (the modulus is matched).  Raises ValueError, naming the
+    structural rank, if A is structurally singular."""
+    rp = np.ascontiguousarray(rowptr, np.int32)
+    ci = np.ascontiguousarray(colind, np.int32)
+    av = np.ascontiguousarray(np.abs(np.asarray(val)), np.float64)
+    n = len(rp) - 1
+    perm_r = np.empty(n, np.int32)
+    R, Cs, out = np.empty(n), np.empty(n), np.zeros(2)
+    rc = lib().sluh_large_diag_perm(n, rp, ci, av, perm_r, R, Cs, out)
+    if rc < 0:
+        raise ValueError("sluh_large_diag_perm: bad CSR input (rowptr, colind outside 0 .. n-1, or a non-finite value)")
+    if rc > 0 or out[0] == -np.inf:
+        raise ValueError(f"A is structurally singular: structural rank {rc} < n = {n}")
+    return perm_r, R, Cs, float(out[0])
+
+
+def row_permute(rowptr, colind, val, perm_r):
+    """CSR of Pr A: row i of A becomes row perm_r[i] (columns and their order within a row kept)."""
+    rp = np.asarray(rowptr, np.int64)
+    ci, v = np.asarray(colind), np.asarray(val)
+    perm_r = np.asarray(perm_r, np.int64)
+    n = len(rp) - 1
+    inv = np.empty(n, np.int64)
+    inv[perm_r] = np.arange(n)
+    cnt = np.diff(rp)[inv]
+    nrp = np.concatenate([[0], np.cumsum(cnt)])
+    src = np.repeat(rp[:-1][inv] - nrp[:-1], cnt) + np.arange(nrp[-1])
+    return nrp.astype(np.int32), ci[src].astype(np.int32), v[src]
 
 
 def read_matrix(path, fmt=None, layout="csr"):
