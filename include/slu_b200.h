@@ -118,8 +118,8 @@ typedef struct {
     int32_t my_supernodes;        /* supernodes this rank factored                           */
     double reserved[8];           /* [0] ms spent slicing (verbose >= 2), [1] Schur flops taken by the */
                                   /* tcgen05 path, [2] bytes of its int8 workspace, [3] slices in use,  */
-                                  /* [4] seconds of the last slu_b200_solve or _solve_trans, [5] its    */
-                                  /* kernel launches, [6] seconds of the last slu_b200_gscon or         */
+                                  /* [4] seconds of the last slu_b200_solve, _solve_trans, _solve_scaled */
+                                  /* or _gsrfs, [5] its kernel launches, [6] seconds of the last slu_b200_gscon or         */
                                   /* _batch_gscon, [7] the solve rounds it ran                          */
 } slu_b200_stats_t;
 
@@ -406,7 +406,9 @@ int slu_b200_batch_schur_expand(slu_b200_handle_t h, double *x, int ldx, int nrh
  * out (nullable): [0] rowcnd, [1] colcnd, [2] amax, [3] equed (0 none, 1 rows, 2 columns, 3 both); without EQUIL 1, 1,
  * max |f_ij|, 0.  [4] ||F||_inf as fixed-order row sums (no float atomics), the anorm of slu_b200_gscon(h, 'I', ...); [5]
  * max |f_ij| ([4], [5] with the modulus).  The handle keeps perm_r, perm[perm_r[.]], perm and the final R and C in HBM until
- * a later upload, fill_csr, batch_fill_csr or batch_fill_affine, which drops them.
+ * a later upload, fill_csr, batch_fill_csr or batch_fill_affine, which drops them.  It keeps A as well, for slu_b200_gsrfs:
+ * rowptr, colind and the values as given, 4 (n + 1) + 4 nnz + 8 nnz batch bytes (16 per value in doublecomplex), reused by
+ * the next scaled fill of the same nnz and dropped with the scalings.
  * get_scaling: the kept perm_r, R and C (each nullable).
  * solve_scaled: solve op(A) x = b on the factors of F, x (n x nrhs, ldx >= n) in A's own ordering, b on entry.  trans 0:
  * b'[perm[perm_r[i]]] = R[i] b[i], F y = b', x[j] = C[j] y[perm[j]]; trans 1 / 2: b'[perm[j]] = C[j] b[j], F^T y = b' (F^H),
@@ -432,6 +434,32 @@ int slu_b200_batch_fill_csr_scaled(slu_b200_handle_t h, int n, const int32_t *ro
                                    int flags, double *out);
 int slu_b200_batch_get_scaling(slu_b200_handle_t h, int member, double *R, double *C);
 int slu_b200_batch_solve_scaled(slu_b200_handle_t h, double *x, int ldx, int nrhs, int trans);
+/* ---- iterative refinement with error bounds on the factors of a scaled fill: pdgsrfs (pdgsrfs.c:198-251) for op(A) = A in
+ * A's own ordering, the step static pivoting relies on to recover the accuracy lost to replaced tiny pivots.  The scaled
+ * fill keeps A in HBM for it (see fill_csr_scaled); a plain fill_csr user gets the same fill from fill_csr_scaled with NULL
+ * perm_r, R and C and no flags.
+ * b (n x nrhs, ldb >= n): the right-hand sides.  x (ldx >= n): the caller's solution on entry (typically solve_scaled's),
+ * the refined one on return.  Per column j and step: r = b - A x, w = |A| |x| + |b| with the kept A, berr = max_i |r_i| / w_i
+ * ((safe1 + |r_i|) / w_i where w_i <= safe2, rows with w_i = 0 skipped; safe1 = (n + 1) dmach("S"), safe2 = safe1 / eps);
+ * while berr > eps, 2 berr <= the last step's berr (3 at the start) and fewer than 20 steps: x += the scaled solve of r.
+ * berr[j] (required) is the berr of the returned x, steps[j] (nullable) the steps taken.  The columns are independent, as in
+ * the reference's per-column loop: each step solves the whole block, a column that has stopped is left exactly as it was.
+ * ferr[j] (nullable): dgerfs's forward error bound, est ||A^-1 diag(W)||_inf / max_i |x_i| with W_i = |r_i| + (n + 1) eps w_i
+ * (+ safe1 where w_i <= safe2) of the returned x, estimated by the dlacn2 of slu_b200_gscon (divided only where max |x_i| > 0).
+ * In doublecomplex |.| is cabs1 (|re| + |im|), as pzgsrfs and zgerfs, and the estimate solves with A^H.
+ * The residual walks each row's entries in CSR order with unfused multiplies and adds, and the maxima are integer atomics on
+ * bit patterns: berr is a pure function of (A, b, x), bit for bit.  The solves sum with atomic adds, so the steps taken and
+ * the refined x can differ between runs at the eps level.  b and x go up once and x comes back once; per step the host reads
+ * the count of columns still active.  stats.reserved[4] / [5] = seconds and kernel launches of the whole call.
+ * Fails with a message, leaving the handle usable, without a scaled fill (or after a later upload, fill_csr, batch_fill_csr
+ * or batch_fill_affine) and a successful factor after it, on Schur handles, grids other than 1 x 1 x 1 with world_size 1,
+ * ldb or ldx < n, nrhs < 1, n * nrhs >= 2^31, and null b, x or berr.
+ * batch_gsrfs: b and x in batch_solve_scaled's layout (ldb / ldx apart, nrhs columns per member); berr, ferr and steps hold
+ * batch x nrhs entries, member-major; fails, naming the member, unless every member's last info was 0. */
+int slu_b200_gsrfs(slu_b200_handle_t h, const double *b, int ldb, double *x, int ldx, int nrhs, double *berr, double *ferr,
+                   int32_t *steps);
+int slu_b200_batch_gsrfs(slu_b200_handle_t h, const double *b, int ldb, double *x, int ldx, int nrhs, double *berr,
+                         double *ferr, int32_t *steps);
 /* ---- doublecomplex twins (SRC/complex16/pzgstrf3d.c:120; the reference's z* handle API,
  * SRC/include/superlu_upacked.h:84-97).  Same view/options/stats structs: the Lnzval_bc_ptr / Unzval_br_ptr
  * entries point at arrays of doublecomplex {double r, i} (SRC/include/dcomplex.h:30) and are declared double*
@@ -521,6 +549,12 @@ int slu_b200_z_batch_fill_csr_scaled(slu_b200_zhandle_t h, int n, const int32_t 
                                      const double *C, int rc_per_member, int flags, double *out);
 int slu_b200_z_batch_get_scaling(slu_b200_zhandle_t h, int member, double *R, double *C);
 int slu_b200_z_batch_solve_scaled(slu_b200_zhandle_t h, double *x, int ldx, int nrhs, int trans);
+/* as slu_b200_gsrfs / _batch_gsrfs: b and x hold interleaved doublecomplex (ldb, ldx count complex elements), berr and ferr
+ * are real; |.| is cabs1 and the forward error estimate solves with A^H */
+int slu_b200_z_gsrfs(slu_b200_zhandle_t h, const double *b, int ldb, double *x, int ldx, int nrhs, double *berr, double *ferr,
+                     int32_t *steps);
+int slu_b200_z_batch_gsrfs(slu_b200_zhandle_t h, const double *b, int ldb, double *x, int ldx, int nrhs, double *berr,
+                           double *ferr, int32_t *steps);
 int slu_b200_z_get_stats(slu_b200_zhandle_t h, slu_b200_stats_t *out);
 int slu_b200_z_plan(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, slu_b200_stats_t *stats);
 void slu_b200_z_destroy(slu_b200_zhandle_t h);

@@ -159,6 +159,8 @@ def lib():
         getattr(L, f).argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     for f in ("slu_b200_solve_scaled", "slu_b200_z_solve_scaled", "slu_b200_batch_solve_scaled", "slu_b200_z_batch_solve_scaled"):
         getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
+    for f in ("slu_b200_gsrfs", "slu_b200_z_gsrfs", "slu_b200_batch_gsrfs", "slu_b200_z_batch_gsrfs"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 3
     _lib = L
     return L
 
@@ -219,6 +221,15 @@ def _scaled_args(rowptr, colind, perm, perm_r, R, C_, rc_shape):
                 raise ValueError(f"{name} must have shape {' or '.join(map(str, rc_shape))}, not {v.shape}")
         sc.append(v)
     return rp, ci, pm, pr, sc[0], sc[1]
+
+
+def _gsrfs(name, complex_, h, b, x, n, nrhs, cols, ferr):
+    """slu_b200_[z_][batch_]gsrfs on C-ordered b and x of the same shape, x refined in place (one row of n per column)
+    -> (berr, steps, ferr or None), each (cols,)"""
+    berr, steps = np.zeros(cols), np.zeros(cols, np.int32)
+    fe = np.zeros(cols) if ferr else None
+    _check(_fn(name, complex_)(h, _ptr(b), n, _ptr(x), n, nrhs, _ptr(berr), _ptr(fe), _ptr(steps)))
+    return berr, steps, fe
 
 
 def device_count():
@@ -407,6 +418,21 @@ class Handle:
         _check(_fn("solve_scaled", self.z_)(self.h, _ptr(x), self.prob.n, nrhs, _TRANS[trans]))
         return x
 
+    def refine(self, b, x, ferr=True):
+        """Iterative refinement of x for A x = b on the factors of a scaled fill and the A it kept (slu_b200_gsrfs), as
+        pdgsrfs; b and x: (n,) or (nrhs, n) in A's ordering, x typically from solve_scaled.  -> (refined x, berr, steps,
+        ferr or None): berr the componentwise backward error of the refined x, steps the refinement steps, ferr dgerfs's
+        forward error bound (ferr=False skips its estimate), one per right-hand side ((nrhs,) arrays, scalars for (n,))"""
+        bb = np.ascontiguousarray(b, self._dtype())
+        xx = np.array(x, self._dtype(), order="C", copy=True)
+        if bb.shape != xx.shape or bb.ndim not in (1, 2) or bb.shape[-1] != self.prob.n:
+            raise ValueError(f"b and x must both have shape (n,) or (nrhs, n) with n = {self.prob.n}")
+        nrhs = 1 if bb.ndim == 1 else bb.shape[0]
+        berr, steps, fe = _gsrfs("gsrfs", self.z_, self.h, bb, xx, self.prob.n, nrhs, nrhs, ferr)
+        if bb.ndim == 1:
+            return xx, float(berr[0]), int(steps[0]), None if fe is None else float(fe[0])
+        return xx, berr, steps, fe
+
     def solve(self, b, trans="N"):
         """L U x = b on the device-resident factors (slu_b200_solve / slu_b200_z_solve); b: (n,) or (nrhs, n), ordering
         of the factored matrix, complex128 for a complex problem.  Returns x with the same shape and dtype.
@@ -589,6 +615,18 @@ class BatchHandle:
         nrhs = 1 if x.ndim == 2 else x.shape[1]
         _check(_fn("batch_solve_scaled", self.z_)(self.h, _ptr(x), self.prob.n, nrhs, _TRANS[trans]))
         return x
+
+    def refine(self, b, x, ferr=True):
+        """Handle.refine for every member (slu_b200_batch_gsrfs); b and x: (batch, n) or (batch, nrhs, n) in A's ordering.
+        -> (refined x, berr, steps, ferr or None) with berr, steps, ferr of shape (batch,) or (batch, nrhs)"""
+        bb = np.ascontiguousarray(b, self._dtype())
+        xx = np.array(x, self._dtype(), order="C", copy=True)
+        if bb.shape != xx.shape or bb.ndim not in (2, 3) or bb.shape[0] != self.batch or bb.shape[-1] != self.prob.n:
+            raise ValueError(f"b and x must both have shape ({self.batch}, n) or ({self.batch}, nrhs, n) with n = {self.prob.n}")
+        nrhs = 1 if bb.ndim == 2 else bb.shape[1]
+        berr, steps, fe = _gsrfs("batch_gsrfs", self.z_, self.h, bb, xx, self.prob.n, nrhs, self.batch * nrhs, ferr)
+        shape = bb.shape[:-1]
+        return xx, berr.reshape(shape), steps.reshape(shape), None if fe is None else fe.reshape(shape)
 
     def factor(self):
         """-> int32 array (batch,): 0, or the 1-based column of the member's first exact zero pivot."""

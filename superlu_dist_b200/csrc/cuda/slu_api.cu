@@ -69,6 +69,8 @@
 #define slu_b200_batch_fill_csr_scaled slu_b200_z_batch_fill_csr_scaled
 #define slu_b200_batch_get_scaling slu_b200_z_batch_get_scaling
 #define slu_b200_batch_solve_scaled slu_b200_z_batch_solve_scaled
+#define slu_b200_gsrfs slu_b200_z_gsrfs
+#define slu_b200_batch_gsrfs slu_b200_z_batch_gsrfs
 #define SLU_API "slu_b200_z_"     // name prefix of the exported calls, for error messages
 #else
 #define SLU_API "slu_b200_"
@@ -337,9 +339,27 @@ struct slu_b200_handle_s {
     DevBuf<int32_t> d_perm_r, d_rmap, d_cperm;
     DevBuf<double> d_R, d_C;
     bool scaled = false;
+    // iterative refinement (slu_b200_gsrfs): A as the last scaled fill received it (rowptr, colind, batch x nnz values; kept
+    // and dropped with the scaling), the right-hand sides and the solution being refined, dgerfs's W and the per-column state
+    DevBuf<int32_t> d_arp, d_aci;
+    DevBuf<val_t> d_aval;
+    DevBuf<val_t> d_rb, d_rx;
+    DevBuf<double> d_rw;
+    DevBuf<RefineState> d_rst;
+    DevBuf<int> d_ract;
 };
 
 namespace {
+
+// an upload, fill_csr, batch_fill_csr or batch_fill_affine: the scalings no longer describe the arena, and the A kept for
+// refinement goes with them
+void drop_scaling(slu_b200_handle_s *H)
+{
+    H->scaled = false;
+    H->d_arp.release();
+    H->d_aci.release();
+    H->d_aval.release();
+}
 
 int device_setup(const slu_b200_options_t *opt)
 {
@@ -1553,7 +1573,7 @@ int slu_b200_upload(slu_b200_handle_t H)
     double t0 = now_s();
     H->factored = false;
     H->si_ready = false;
-    H->scaled = false;
+    drop_scaling(H);
     if (transfer(H, true)) return -1;
     H->st.t_upload_s = now_s() - t0;
     H->uploaded = true;
@@ -1730,7 +1750,7 @@ int slu_b200_factor_host(slu_b200_handle_t H, int *info)
     }
     if (H->grouped) {                      // options.reserved[3]: H2D, factorization and D2H all overlapped
         H->factored = false;
-        H->scaled = false;
+        drop_scaling(H);
         if (pipe_prepare(H) || upload_pipe_issue(H)) return -1;
         H->uploaded = true;
         H->st.t_upload_s = 0;
@@ -1756,7 +1776,7 @@ int slu_b200_fill_csr(slu_b200_handle_t H, int n, const int32_t *rowptr, const i
     if (n != H->n) return fail("matrix order %d does not match the handle's %d", n, H->n);
     if (H->P2 > 1) return fail("slu_b200_fill_csr handles 1 x 1 x Pz grids");
     H->si_ready = false;
-    H->scaled = false;
+    drop_scaling(H);
     double t0 = now_s();
     const int64_t nnz = rowptr[n];
     DevBuf<int32_t> drp, dci, dperm;
@@ -2304,7 +2324,7 @@ int slu_b200_batch_fill_csr(slu_b200_handle_t H, int n, const int32_t *rowptr, c
     CU(cudaMemcpyAsync(dv.p, val, (size_t)nnz * B * sizeof(val_t), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(dperm.p, perm, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     H->si_ready = false;
-    H->scaled = false;
+    drop_scaling(H);
     CU(cudaMemsetAsync(H->val.p, 0, H->val.bytes(), s));
     CU(cudaMemsetAsync(err, 0, sizeof(int), s));
     launch_fill_csr(H->bdev, n, drp.p, dci.p, dv.p, dperm.p, dact.p, err, s);
@@ -2461,6 +2481,37 @@ int slu_b200_batch_solve_trans(slu_b200_handle_t H, double *xh, int ldx, int nrh
 // takes its right-hand side (in place over the solution along Z, where the solve ends in d_x2).
 constexpr int COND_MAX_ROUNDS = 64;     // dlacn2 makes at most 11 solves; lock-step at most doubles that
 
+}  // extern "C"
+// The rounds of dlacn2 / zlacn2 over `members` vectors of n elements, shared by gscon and the forward error bound of gsrfs:
+// v holds the pending vectors; apply(kase, &x) enqueues the operator of kase on them and points x at the result.  Ends when
+// no member waits; the estimates are then in d_cstate.  *rounds counts the applications.
+template <class Apply>
+static int cond_rounds(slu_b200_handle_t H, int n, int members, val_t *v, Apply apply, int *rounds, const char *fn)
+{
+    const size_t len = (size_t)n * members;
+    const size_t parts = (size_t)((n + COND_CHUNK - 1) / COND_CHUNK) * members;
+    if (VAL_DOUBLES == 1 && H->d_csgn.n < len && H->d_csgn.alloc(len)) return -1;     // the real repeated-sign test
+    if (H->d_cstate.n < (size_t)members && (H->d_cstate.alloc(members) || H->d_cpart.alloc(parts) || H->d_ccount.alloc(2))) return -1;
+    cudaStream_t s = H->stream;
+    launch_cond_init(H->d_cstate.p, v, n, members, s);
+    for (int kase = 1;;) {
+        if (*rounds == COND_MAX_ROUNDS) return fail("%s: the estimator did not finish in %d solves", fn, *rounds);
+        val_t *x = nullptr;
+        if (apply(kase, &x) < 0) return -1;
+        CU(cudaMemsetAsync(H->d_ccount.p, 0, 2 * sizeof(int), s));
+        launch_cond_step(H->d_cstate.p, kase, x, v, H->d_csgn.p, H->d_cpart.p, H->d_ccount.p, n, members, s);
+        int waiting[2] = {0, 0};                      // members waiting for kase 1 / kase 2
+        CU(cudaMemcpyAsync(waiting, H->d_ccount.p, sizeof waiting, cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+        ++*rounds;
+        if (waiting[2 - kase] > 0) kase = 3 - kase;
+        else if (waiting[kase - 1] == 0) break;
+    }
+    CU(cudaGetLastError());
+    return 0;
+}
+extern "C" {
+
 // the preconditions of the matching solve are checked by the caller; B = 1 member on an unbatched handle
 static int gscon_impl(slu_b200_handle_t H, char norm, const double *anorm, double *rcond, const char *fn)
 {
@@ -2483,34 +2534,19 @@ static int gscon_impl(slu_b200_handle_t H, char norm, const double *anorm, doubl
     }
     if (any) {
         const size_t len = (size_t)n * B;
-        const size_t parts = (size_t)((n + COND_CHUNK - 1) / COND_CHUNK) * B;
         if (batched && H->d_cv.n < len && H->d_cv.alloc(len)) return -1;
-        if (VAL_DOUBLES == 1 && H->d_csgn.n < len && H->d_csgn.alloc(len)) return -1;     // the real repeated-sign test
-        if (H->d_cstate.n < (size_t)B && (H->d_cstate.alloc(B) || H->d_cpart.alloc(parts) || H->d_ccount.alloc(2))) return -1;
         if (batched ? (H->d_x.n < len && H->d_x.alloc(len)) : (H->d_x.n < len && (H->d_x.alloc(len) || H->d_x2.alloc(len)))) return -1;
         cudaStream_t s = H->stream;
         val_t *v = batched ? H->d_cv.p : H->d_x2.p;       // the pending vectors
-        launch_cond_init(H->d_cstate.p, v, n, B, s);
-        for (int kase = 1;;) {
-            if (rounds == COND_MAX_ROUNDS) return fail("%s: the estimator did not finish in %d solves", fn, rounds);
+        auto apply = [&](int kase, val_t **x) -> int {
             const int trans = (kase == 1) == one ? 0 : (VAL_DOUBLES == 2 ? 2 : 1);
-            val_t *x = H->d_x.p;
-            if (batched) {
-                CU(cudaMemcpyAsync(x, v, len * sizeof(val_t), cudaMemcpyDeviceToDevice, s));
-                batch_solve_dev(H, 1, trans);
-            } else if (solve_dev(H, 1, trans, &x) < 0) {
-                return -1;
-            }
-            CU(cudaMemsetAsync(H->d_ccount.p, 0, 2 * sizeof(int), s));
-            launch_cond_step(H->d_cstate.p, kase, x, v, H->d_csgn.p, H->d_cpart.p, H->d_ccount.p, n, B, s);
-            int waiting[2] = {0, 0};                      // members waiting for kase 1 / kase 2
-            CU(cudaMemcpyAsync(waiting, H->d_ccount.p, sizeof waiting, cudaMemcpyDeviceToHost, s));
-            CU(cudaStreamSynchronize(s));
-            ++rounds;
-            if (waiting[2 - kase] > 0) kase = 3 - kase;
-            else if (waiting[kase - 1] == 0) break;
-        }
-        CU(cudaGetLastError());
+            *x = H->d_x.p;
+            if (!batched) return solve_dev(H, 1, trans, x) < 0 ? -1 : 0;
+            CU(cudaMemcpyAsync(*x, v, len * sizeof(val_t), cudaMemcpyDeviceToDevice, s));
+            batch_solve_dev(H, 1, trans);
+            return 0;
+        };
+        if (cond_rounds(H, n, B, v, apply, &rounds, fn)) return -1;
         std::vector<CondState> st(B);
         CU(cudaMemcpy(st.data(), H->d_cstate.p, B * sizeof(CondState), cudaMemcpyDeviceToHost));
         for (int j = 0; j < B; ++j)
@@ -2709,7 +2745,7 @@ int slu_b200_batch_fill_affine(slu_b200_handle_t H, int n, const int32_t *rowptr
     CU(cudaMemcpyAsync(dterms.p, terms, (size_t)nnz * nterms * sizeof(val_t), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(dcoef.p, coef, (size_t)B * nterms * sizeof(val_t), cudaMemcpyHostToDevice, s));
     H->si_ready = false;
-    H->scaled = false;
+    drop_scaling(H);
     CU(cudaMemsetAsync(H->val.p, 0, H->val.bytes(), s));
     CU(cudaMemsetAsync(err, 0, sizeof(int), s));
     launch_fill_affine(H->bdev, n, drp.p, dci.p, dperm.p, dact.p, ddst.p, nnz, nterms, dterms.p, dcoef.p, err, s);
@@ -2791,14 +2827,17 @@ static int fill_scaled_impl(slu_b200_handle_t H, bool batched, int n, const int3
         memcpy(&e.rmin, &big, sizeof big);
         e.cmin = e.rmin;
     }
-    DevBuf<int32_t> drp, dci;
-    DevBuf<val_t> dv;
+    // A stays in HBM for slu_b200_gsrfs: 4 (n + 1) + 4 nnz + 8 nnz batch bytes (16 per value in complex), reused by the next
+    // scaled fill of the same nnz
+    DevBuf<int32_t> &drp = H->d_arp, &dci = H->d_aci;
+    DevBuf<val_t> &dv = H->d_aval;
     DevBuf<double> dRin, dCin, drinv, dout;
     DevBuf<unsigned long long> dccol;
     DevBuf<EquilStat> dst;
     DevBuf<int8_t> dact;
     const size_t bn = (size_t)B * n;
-    if (drp.alloc((size_t)n + 1) || dci.alloc((size_t)nnz) || dv.alloc((size_t)nnz * B) || dact.upload(act) || dst.upload(st0) ||
+    if ((drp.n != (size_t)n + 1 && drp.alloc((size_t)n + 1)) || (dci.n != (size_t)nnz && dci.alloc((size_t)nnz)) ||
+        (dv.n != (size_t)nnz * B && dv.alloc((size_t)nnz * B)) || dact.upload(act) || dst.upload(st0) ||
         dout.alloc((size_t)B * 6) || (R && dRin.alloc((size_t)rc_len)) || (C && dCin.alloc((size_t)rc_len)) ||
         (equil && (drinv.alloc(bn) || dccol.alloc(bn))))
         return -1;
@@ -2876,6 +2915,30 @@ static int get_scaling_impl(slu_b200_handle_t H, bool batched, int member, int32
 // x in A's ordering: b' = the row-permuted, scaled b into the solve's input (one scatter launch), the plain solve, x = the
 // scaled, permuted-back solution (one gather launch).  trans 0: b'[rmap[i]] = R[i] b[i], x[j] = C[j] y[perm[j]]; trans 1 / 2:
 // b'[perm[j]] = C[j] b[j], x[i] = R[i] y[rmap[i]] (the scalings are real, so F^H needs nothing more than F^T).
+// Where solve_scaled_dev takes b: d_x2 on a batched handle, d_x on an unbatched one (the scatter writes b' where the plain
+// solve takes its right-hand side)
+static val_t *scaled_in(slu_b200_handle_t H, bool batched) { return batched ? H->d_x2.p : H->d_x.p; }
+
+// The device part of solve_scaled: b in scaled_in(H), x in d_x2 (both buffers hold batch x n x nrhs).  Enqueued on H->stream,
+// not synchronised.  Returns the kernel launches, < 0 on an error.
+static int solve_scaled_dev(slu_b200_handle_t H, bool batched, int nrhs, int trans)
+{
+    const int B = batched ? H->batch : 1, n = H->n;
+    cudaStream_t s = H->stream;
+    val_t *in = scaled_in(H, batched), *b = batched ? H->d_x.p : H->d_x2.p;
+    int launches = launch_permute_scale(b, in, trans ? H->d_cperm.p : H->d_rmap.p, trans ? H->d_C.p : H->d_R.p, n, nrhs, B, true, s);
+    val_t *y = H->d_x.p;
+    if (batched) {
+        launches += batch_solve_dev(H, nrhs, trans);
+    } else {
+        const int l = solve_dev(H, nrhs, trans, &y);
+        if (l < 0) return -1;
+        launches += l;
+    }
+    launches += launch_permute_scale(H->d_x2.p, y, trans ? H->d_rmap.p : H->d_cperm.p, trans ? H->d_R.p : H->d_C.p, n, nrhs, B, false, s);
+    return launches;
+}
+
 static int solve_scaled_impl(slu_b200_handle_t H, bool batched, double *xh, int ldx, int nrhs, int trans, const char *fn)
 {
     if (!H || !xh) return fail("null argument");
@@ -2895,21 +2958,11 @@ static int solve_scaled_impl(slu_b200_handle_t H, bool batched, double *xh, int 
     if (H->d_x2.n < len && H->d_x2.alloc(len)) return -1;
     cudaStream_t s = H->stream;
     double t0 = now_s();
-    val_t *in = batched ? H->d_x2.p : H->d_x.p, *b = batched ? H->d_x.p : H->d_x2.p;   // the solve takes b' in d_x / d_x2
-    CU(cudaMemcpy2DAsync(in, (size_t)n * sizeof(val_t), xh, (size_t)ldx * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs * B,
-                         cudaMemcpyHostToDevice, s));
-    int launches = launch_permute_scale(b, in, trans ? H->d_cperm.p : H->d_rmap.p, trans ? H->d_C.p : H->d_R.p, n, nrhs, B, true, s);
-    val_t *y = H->d_x.p;
-    if (batched) {
-        launches += batch_solve_dev(H, nrhs, trans);
-    } else {
-        const int l = solve_dev(H, nrhs, trans, &y);
-        if (l < 0) return -1;
-        launches += l;
-    }
-    val_t *x = H->d_x2.p;
-    launches += launch_permute_scale(x, y, trans ? H->d_rmap.p : H->d_cperm.p, trans ? H->d_R.p : H->d_C.p, n, nrhs, B, false, s);
-    CU(cudaMemcpy2DAsync(xh, (size_t)ldx * sizeof(val_t), x, (size_t)n * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs * B,
+    CU(cudaMemcpy2DAsync(scaled_in(H, batched), (size_t)n * sizeof(val_t), xh, (size_t)ldx * sizeof(val_t), (size_t)n * sizeof(val_t),
+                         (size_t)nrhs * B, cudaMemcpyHostToDevice, s));
+    const int launches = solve_scaled_dev(H, batched, nrhs, trans);
+    if (launches < 0) return -1;
+    CU(cudaMemcpy2DAsync(xh, (size_t)ldx * sizeof(val_t), H->d_x2.p, (size_t)n * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs * B,
                          cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     CU(cudaGetLastError());
@@ -2950,6 +3003,114 @@ int slu_b200_batch_get_scaling(slu_b200_handle_t H, int member, double *R, doubl
 int slu_b200_batch_solve_scaled(slu_b200_handle_t H, double *x, int ldx, int nrhs, int trans)
 {
     return solve_scaled_impl(H, true, x, ldx, nrhs, trans, SLU_API "batch_solve_scaled");
+}
+
+// ---- iterative refinement with error bounds: pdgsrfs (pdgsrfs.c:198-251) for op(A) = A in A's own ordering, on the factors
+// and scalings of the last scaled fill and the A it kept; the forward error bound of LAPACK dgerfs.  Each step runs the
+// residual kernel over every (row, column, member), the decide kernel and one read of the count of columns still active, then
+// one scaled solve of the whole block of residuals and the update.  ferr: dlacn2 through cond_rounds, each (member, column)
+// one estimator member: kase 1 solves with A^T (A^H) and multiplies by W, kase 2 multiplies by W and solves with A.
+static int gsrfs_impl(slu_b200_handle_t H, bool batched, const double *bh, int ldb, double *xh, int ldx, int nrhs, double *berr,
+                      double *ferr, int32_t *steps, const char *fn)
+{
+    if (!H || !bh || !xh || !berr) return fail("%s: null argument (b, x and berr are required)", fn);
+    if (refuse_scaled(H, batched, fn)) return -1;
+    if (!H->scaled)
+        return fail("%s needs a scaled fill on this handle first (a later upload, fill_csr, batch_fill_csr or batch_fill_affine drops "
+                    "the scaling and the kept A)", fn);
+    if (batched) {
+        if (refuse_unfactored_members(H, fn)) return -1;
+    } else if (!H->factored) {
+        return fail("%s needs a successful " SLU_API "factor after the scaled fill", fn);
+    }
+    const int B = batched ? H->batch : 1, n = H->n;
+    if (nrhs < 1) return fail("%s: nrhs = %d, must be >= 1", fn, nrhs);
+    if (ldb < n || ldx < n) return fail("%s: ldb = %d and ldx = %d must be >= n = %d", fn, ldb, ldx, n);
+    if ((int64_t)n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
+    const int cols = B * nrhs;
+    const size_t len = (size_t)n * cols;
+    if ((H->d_x.n < len && H->d_x.alloc(len)) || (H->d_x2.n < len && H->d_x2.alloc(len)) || (H->d_rb.n < len && H->d_rb.alloc(len)) ||
+        (H->d_rx.n < len && H->d_rx.alloc(len)) || (H->d_rst.n < (size_t)cols && H->d_rst.alloc(cols)) ||
+        (!H->d_ract.p && H->d_ract.alloc(1)) || (ferr && ((H->d_rw.n < len && H->d_rw.alloc(len)) || (H->d_cv.n < len && H->d_cv.alloc(len)))))
+        return -1;
+    cudaStream_t s = H->stream;
+    const double t0 = now_s();
+    const size_t w = (size_t)n * sizeof(val_t);
+    CU(cudaMemcpy2DAsync(H->d_rb.p, w, bh, (size_t)ldb * sizeof(val_t), w, (size_t)cols, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpy2DAsync(H->d_rx.p, w, xh, (size_t)ldx * sizeof(val_t), w, (size_t)cols, cudaMemcpyHostToDevice, s));
+    std::vector<RefineState> st(cols, RefineState{3.0, 0.0, 0, 0, 1});   // pdgsrfs: lstres = 3, count = 0
+    CU(cudaMemcpyAsync(H->d_rst.p, st.data(), cols * sizeof(RefineState), cudaMemcpyHostToDevice, s));
+    const RefineArgs a{n, nrhs, B, (int64_t)H->d_aci.n, H->d_arp.p, H->d_aci.p, H->d_aval.p, H->d_rb.p, H->d_rst.p,
+                       ferr ? H->d_rw.p : nullptr};
+    val_t *in = scaled_in(H, batched), *x = H->d_rx.p;
+    int launches = 0;
+    for (int step = 0;; ++step) {
+        if (step > REFINE_ITMAX) return fail("%s: the refinement did not stop after %d steps", fn, REFINE_ITMAX);
+        launches += launch_refine_residual(a, x, in, s);
+        CU(cudaMemsetAsync(H->d_ract.p, 0, sizeof(int), s));
+        launches += launch_refine_decide(a, H->d_ract.p, s);
+        int active = 0;
+        CU(cudaMemcpyAsync(&active, H->d_ract.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+        if (active == 0) break;
+        const int l = solve_scaled_dev(H, batched, nrhs, 0);    // dx = A^-1 r in d_x2
+        if (l < 0) return -1;
+        launches += l + launch_refine_update(a, x, H->d_x2.p, s);
+    }
+    if (ferr) {
+        int rounds = 0;
+        val_t *v = H->d_cv.p;
+        const double *W = H->d_rw.p;
+        auto apply = [&](int kase, val_t **res) -> int {
+            *res = H->d_x2.p;
+            int l;
+            if (kase == 2) {                                    // A^-1 diag(W) v
+                launches += launch_refine_scale(in, v, W, (int64_t)len, s);
+                l = solve_scaled_dev(H, batched, nrhs, 0);
+            } else {                                            // diag(W) A^-T v
+                CU(cudaMemcpyAsync(in, v, len * sizeof(val_t), cudaMemcpyDeviceToDevice, s));
+                l = solve_scaled_dev(H, batched, nrhs, VAL_DOUBLES == 2 ? 2 : 1);
+                launches += launch_refine_scale(*res, *res, W, (int64_t)len, s);
+            }
+            if (l < 0) return -1;
+            launches += l;
+            return 0;
+        };
+        if (cond_rounds(H, n, cols, v, apply, &rounds, fn)) return -1;
+    }
+    CU(cudaMemcpy2DAsync(xh, (size_t)ldx * sizeof(val_t), x, w, w, (size_t)cols, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(st.data(), H->d_rst.p, cols * sizeof(RefineState), cudaMemcpyDeviceToHost, s));
+    std::vector<CondState> est(ferr ? cols : 0);
+    if (ferr) CU(cudaMemcpyAsync(est.data(), H->d_cstate.p, cols * sizeof(CondState), cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    for (int c = 0; c < cols; ++c) {
+        berr[c] = st[c].berr;
+        if (steps) steps[c] = st[c].count;
+        if (!ferr) continue;
+        double xmax = 0.0;                                      // dgerfs: divide by max |x_i| unless it is 0 (cabs1 in complex)
+        const double *xc = xh + (size_t)c * ldx * VAL_DOUBLES;
+        for (int i = 0; i < n; ++i) {
+            double ai = std::fabs(xc[(size_t)i * VAL_DOUBLES]);
+            if (VAL_DOUBLES == 2) ai += std::fabs(xc[(size_t)i * VAL_DOUBLES + 1]);
+            xmax = std::max(xmax, ai);
+        }
+        ferr[c] = xmax != 0.0 ? est[c].est / xmax : est[c].est;
+    }
+    H->st.reserved[4] = now_s() - t0;
+    H->st.reserved[5] = (double)launches;
+    return 0;
+}
+
+int slu_b200_gsrfs(slu_b200_handle_t H, const double *b, int ldb, double *x, int ldx, int nrhs, double *berr, double *ferr, int32_t *steps)
+{
+    return gsrfs_impl(H, false, b, ldb, x, ldx, nrhs, berr, ferr, steps, SLU_API "gsrfs");
+}
+
+int slu_b200_batch_gsrfs(slu_b200_handle_t H, const double *b, int ldb, double *x, int ldx, int nrhs, double *berr, double *ferr,
+                         int32_t *steps)
+{
+    return gsrfs_impl(H, true, b, ldb, x, ldx, nrhs, berr, ferr, steps, SLU_API "batch_gsrfs");
 }
 
 // ---- partial factorization on batched handles: a batched handle whose level plan leaves out the Schur supernodes, as an

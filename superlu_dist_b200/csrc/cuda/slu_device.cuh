@@ -235,6 +235,32 @@ int launch_cond_init(CondState *st, val_t *v, int n, int members, cudaStream_t s
 int launch_cond_step(CondState *st, int kase, const val_t *x, val_t *v, val_t *sgn, CondPart *part, int *counts, int n, int members,
                      cudaStream_t s);
 
+// slu_refine.cu (double) / slu_refine_z.cu (doublecomplex): the step kernels of iterative refinement (slu_b200_gsrfs), pdgsrfs's
+// loop per column.  One RefineState per column, members x nrhs of them, member-major; vectors: members blocks of n x nrhs.
+constexpr int REFINE_ITMAX = 20;      // pdgsrfs.c ITMAX
+struct RefineState {
+    double lstres, berr;              // pdgsrfs's lstres (3 at the start), the berr of the last residual
+    unsigned long long berr_bits;     // this step's max_i |r_i| / w_i as bits (atomicMax; zeroed by the decide kernel)
+    int32_t count, active;            // steps taken; 1 while the column is refined
+};
+struct RefineArgs {
+    int n, nrhs, members;
+    int64_t nnz;
+    const int32_t *rowptr, *colind;
+    const val_t *aval;                // members x nnz, member-major: A as the scaled fill received it
+    const val_t *b;                   // right-hand sides
+    RefineState *st;
+    double *W;                        // nullptr, or dgerfs's W of every active column (the forward error estimate)
+};
+// r = b - A x for the active columns (0 elsewhere), their berr bits and W
+int launch_refine_residual(const RefineArgs &a, const val_t *x, val_t *r, cudaStream_t s);
+// berr of the step, pdgsrfs's test; *active (zeroed by the caller) receives the columns that take another step
+int launch_refine_decide(const RefineArgs &a, int *active, cudaStream_t s);
+// x += dx on the active columns
+int launch_refine_update(const RefineArgs &a, val_t *x, const val_t *dx, cudaStream_t s);
+// dst[t] = W[t] src[t], t < len
+int launch_refine_scale(val_t *dst, const val_t *src, const double *W, int64_t len, cudaStream_t s);
+
 #ifndef SLU_COMPLEX
 // slu_ozaki.cu: the Schur update of wide supernodes on wgmma (int8 slices, exact int32 accumulation in registers)
 constexpr int OZ_NT = 32;             // columns of one CTA's int8 Schur tile (rows: 128)
