@@ -1,0 +1,412 @@
+"""Componentwise backward error of the kernels, factorizations and solves (test infrastructure, imported like util).
+
+A correctly rounded algorithm of the same shape as the reference's meets each bound here whatever the condition number
+of its input, so these checks need no oracle and stay sharp on graded, indefinite and tiny-pivot inputs, where the
+normwise checks (rel_err against the oracle) are either blind to small entries or too loose to mean anything.
+
+Every ratio is |R| / D elementwise.  R is computed in extended precision (np.longdouble: 64-bit significand on x86), so
+that the residual of a double-precision result is exact to far below the bounds; D, a sum of non-negative terms, is
+accurate to a few ulps in double.  R != 0 where D == 0 counts as infinity: a
+write to a position that no product touches fails.  In doublecomplex |.| is the modulus and every bound doubles.
+
+    operation                  residual R                     scale D                 bound
+    diag LU (k_diag_lu)        A - L U                        |L| |U|                 4 ns u
+    trsm L case (X U = B)      X U - B                        |X| |U|                 4 ns u
+    trsm U case (L X = B)      L X - B                        |L| |X|                 4 ns u
+    gemm_sub (C - A B)         C_out - (C - A B)              |C| + |A| |B|           2 (k + 1) u
+    factorization              F - L U on pattern(F, L U)     |L| |U|                 4 k_max u
+    solve, op = N / T / H      b - op(L U) x, per row         op(|L| |U|) |x|         4 k_max u
+
+u = 2^-53.  k_max is the largest panel height (nsupr) of the problem.  The bounds are fixed formulas in u: none is
+tuned to what a GPU returns.  Pivots replaced by +-thresh (static pivoting) are excluded from the factorization ratio
+at their own diagonal position; the callers check that their count is the kernel's tiny-pivot count."""
+import numpy as np
+import scipy.sparse as sp
+
+from test_scaled_parity import panel_coords
+
+U = 2.0 ** -53
+LD, CLD = np.longdouble, np.clongdouble
+
+
+def ext(a):
+    """a in extended precision (long double, complex long double for complex a)"""
+    return a.astype(CLD if np.iscomplexobj(a) else LD)
+
+
+def cfactor(dtype):
+    """2 for doublecomplex, 1 for double: every bound doubles in complex"""
+    return 2 if np.dtype(dtype).kind == "c" else 1
+
+
+def ratio(r, d):
+    """max |r| / d elementwise (arrays of the same shape, d >= 0); r != 0 with d == 0 is infinity, 0 / 0 is 0"""
+    r = np.abs(np.asarray(r))
+    d = np.asarray(d)
+    if r.size == 0:
+        return 0.0
+    bad = (d == 0) & (r != 0)
+    q = np.where(d > 0, r / np.where(d > 0, d, 1), 0)
+    return float(np.inf) if bad.any() else float(q.max())
+
+
+# ------------------------------------------------------------------------------------------------- kernel inputs
+# The widths cross the 16-column blocks of the TRSM and its inverses, the 32-column slabs and the 65..256 range of the
+# cluster diagonal LU, and the 64-row T chunks; the vector counts cross the 32-vector TRSM strip.
+WIDTHS = [1, 15, 16, 17, 31, 32, 33, 63, 64, 65, 96, 97, 255, 256, 257, 416, 417, 512]
+ZWIDTHS = [w for w in WIDTHS if w <= 256]
+VECS = [1, 31, 32, 33, 95, 1000]
+# dominant: the inputs of test_gpu_kernels.py.  nondom: |u_ii| in [0.5, 2], off-diagonal entries that outweigh it
+# (|l| <= 1 in the unit lower factor).  graded: rows scaled log-uniformly over [1e-6, 1], the first 16 columns swept over
+# the whole range.  tiny: exact tiny pivots at block and slab boundaries.  scaled: rows and columns scaled by powers of
+# two up to 2^+-300.  zpivots (complex): pivots with |Im| / |Re| = 1e+-12, purely imaginary ones and |pivot| = 2^+-600,
+# where a naive |a|^2 overflows.
+FAMILIES = ["dominant", "nondom", "graded", "tiny", "scaled"]
+ZFAMILIES = FAMILIES + ["zpivots"]
+TINY_COLS = (0, 15, 16, 31, 32, 63, 64, 255, 256)
+TINY_PIVOT = 1e-30      # planted in the diagonal LU's input, below THRESH: replaced
+THRESH = 2.0 ** -26     # the replacement value; the triangles of the TRSM take it as their tiny pivots
+
+
+def vecs_for(ns, family):
+    """One vector count per (width, family), rotating through VECS; 1000 vectors only up to 128 columns (95 past it),
+    which keeps every extended-precision residual under a second"""
+    m = VECS[(WIDTHS.index(ns) + ZFAMILIES.index(family)) % len(VECS)]
+    return 95 if m == 1000 and ns > 128 else m
+
+
+def _rand(rng, shape, z, kind="normal"):
+    draw = (lambda: rng.standard_normal(shape)) if kind == "normal" else (lambda: rng.uniform(-1.0, 1.0, shape))
+    return draw() + 1j * draw() if z else draw()
+
+
+def _pivots(rng, ns, z):
+    mag = rng.uniform(0.5, 2.0, ns)
+    return mag * (np.exp(2j * np.pi * rng.uniform(size=ns)) if z else rng.choice([-1.0, 1.0], ns))
+
+
+def _special(ns, family):
+    """columns whose pivot is planted (their row of the unit lower factor is zero left of the diagonal)"""
+    if family == "tiny":
+        return [c for c in TINY_COLS if c < ns]
+    if family == "zpivots":
+        return list(range(0, ns, 3))
+    return []
+
+
+def _graded(rng, ns):
+    d = 10.0 ** rng.uniform(-6.0, 0.0, ns)
+    w = min(16, ns)
+    d[:w] = 10.0 ** (-6.0 * np.arange(w) / 15)
+    return d
+
+
+def upper(family, ns, rng, z, pivot_tiny=THRESH, scale_rows=True):
+    """An upper triangle of `family` (the U of X U = B, or U0 of a diagonal LU input).  zpivots: scale_rows puts the
+    2^+-600 moduli on the whole row (a TRSM stays in range: one column of X scales), else on the pivot alone (the
+    diagonal LU's multipliers below it stay O(1), and the reciprocal of the pivot must not overflow)."""
+    if family == "dominant":
+        return np.triu(_rand(rng, (ns, ns), z)) + ns * np.eye(ns)
+    u = np.triu(_rand(rng, (ns, ns), z, "uniform"), 1) / np.sqrt(ns)
+    p = _pivots(rng, ns, z)
+    rs = np.ones(ns)
+    if family == "graded":
+        rs = _graded(rng, ns)
+    elif family == "scaled":
+        rs = 2.0 ** rng.integers(-300, 301, ns)
+    elif family == "tiny":
+        for c in _special(ns, family):
+            p[c] = pivot_tiny * (-1.0 if c % 2 else 1.0) * (np.exp(0.25j * np.pi) if z else 1.0)
+    elif family == "zpivots":
+        kinds = [np.exp(1j * np.arctan(1e-12)), np.exp(1j * np.arctan(1e12)), 1j, -1j, 1.0, 1.0]
+        scale = [1.0, 1.0, 1.0, 1.0, 2.0 ** 600, 2.0 ** -600]
+        for t, c in enumerate(_special(ns, family)):
+            p[c] = abs(p[c]) * kinds[t % 6] * (1.0 if scale_rows else scale[t % 6])
+            rs[c] = scale[t % 6] if scale_rows else 1.0
+            u[:c, c] = 0.0   # with row c of L0 zero, the pivot of A = L0 U0 is exactly p[c] and nothing cancels
+    u = u + np.diag(p)
+    if family == "scaled":
+        u = u * 2.0 ** rng.integers(-300, 301, ns)[None, :]
+    return rs[:, None] * u
+
+
+def unit_lower(family, ns, rng, z, special=()):
+    """A unit lower triangle of `family` (the L of L X = B, or L0 of a diagonal LU input); rows in `special` are zero
+    left of the diagonal"""
+    if family == "dominant":
+        return np.tril(_rand(rng, (ns, ns), z), -1) / ns + np.eye(ns)
+    lo = np.tril(_rand(rng, (ns, ns), z, "uniform"), -1) / np.sqrt(ns)
+    lo[list(special)] = 0.0
+    if family == "graded":
+        d = _graded(rng, ns)
+        lo = d[:, None] * lo / d[None, :]
+    elif family == "scaled":
+        d = 2.0 ** rng.integers(-150, 151, ns)
+        lo = d[:, None] * lo / d[None, :]
+    return lo + np.eye(ns)
+
+
+def diag_lu_input(family, ns, extra, seed, z=False):
+    """(ns + extra) x ns: A = L0 U0 on top (randn + ns I for dominant), random rows below.  scaled: Dr (L0 U0) Dc with
+    the non-dominant L0 and U0, whose LU is Dr L0 Dr^-1 and Dr U0 Dc exactly in binary floating point."""
+    rng = np.random.default_rng(seed)
+    if family == "dominant":
+        top = _rand(rng, (ns, ns), z) + ns * np.eye(ns)
+    elif family == "scaled":
+        top = unit_lower("nondom", ns, rng, z) @ upper("nondom", ns, rng, z)
+        top = 2.0 ** rng.integers(-300, 301, ns)[:, None] * top * 2.0 ** rng.integers(-300, 301, ns)[None, :]
+    else:
+        top = unit_lower(family, ns, rng, z, _special(ns, family)) @ upper(family, ns, rng, z, TINY_PIVOT, False)
+    return np.vstack([top, _rand(rng, (extra, ns), z)])
+
+
+def trsm_l_input(family, ns, m, seed, z=False):
+    """(U, B) of X U = B; B's rows scaled by powers of two up to 2^+-300 in the scaled family"""
+    rng = np.random.default_rng(seed)
+    u = upper(family, ns, rng, z)
+    b = _rand(rng, (m, ns), z)
+    if family == "scaled":
+        b = b * 2.0 ** rng.integers(-300, 301, m)[:, None]
+    return u, b
+
+
+def trsm_u_input(family, ns, nc, seed, z=False):
+    """(L, B) of L X = B (the unit lower triangle of the first; its diagonal is not read)"""
+    rng = np.random.default_rng(seed)
+    lo = unit_lower(family, ns, rng, z)
+    b = _rand(rng, (ns, nc), z)
+    if family == "scaled":
+        b = b * 2.0 ** rng.integers(-300, 301, nc)[None, :]
+    return lo, b
+
+
+GEMM_SHAPES = [(1, 1, 1), (33, 31, 7), (96, 97, 17), (128, 130, 100), (257, 131, 137), (200, 97, 256), (129, 300, 513)]
+GEMM_FAMILIES = ["random", "cancel", "scaled"]
+
+
+def gemm_input(family, m, n, k, seed, z=False):
+    """(A, B, C) of C - A B.  cancel: C = fl(A B) plus a perturbation of 2^-40 of it; scaled: rows of A and C by 2^+-200"""
+    rng = np.random.default_rng(seed)
+    a, b, c = _rand(rng, (m, k), z), _rand(rng, (k, n), z), _rand(rng, (m, n), z)
+    if family == "cancel":
+        c = a @ b
+        c = c + 2.0 ** -40 * c * rng.uniform(-1.0, 1.0, c.shape)
+    elif family == "scaled":
+        r = 2.0 ** rng.integers(-200, 201, m)[:, None]
+        a, c = a * r, c * r
+    return a, b, c
+
+
+# ---------------------------------------------------------------------------------------------------- restatements
+def lu_nopivot_ld(a, thresh=None):
+    """Right-looking LU without pivoting in extended precision, rounded to the input's dtype; tiny pivots replaced by
+    +-thresh as the kernels do (pdgstrf2.c: |p| < thresh; pzgstrf2.c: |re| + |im| < thresh with both parts non-zero)
+    -> (factored block, replaced count)"""
+    w = ext(np.array(a))
+    ns, tiny, z = w.shape[1], 0, np.iscomplexobj(a)
+    for j in range(ns):
+        p = w[j, j]
+        small = (abs(p.real) + abs(p.imag) < thresh and p.real != 0 and p.imag != 0) if z else abs(p) < thresh
+        if thresh is not None and small:
+            w[j, j] = -thresh if p.real < 0 else thresh
+            tiny += 1
+        if w[j, j] != 0:
+            w[j + 1:ns, j] /= w[j, j]
+        w[j + 1:ns, j + 1:] -= np.outer(w[j + 1:ns, j], w[j, j + 1:])
+    return w.astype(a.dtype), tiny
+
+
+def _inv_upper16(t):
+    """Inverse of an upper triangle, column by column from the diagonal up, dividing by the pivot (diag_inv_kernel)"""
+    m = t.shape[0]
+    x = np.zeros_like(t)
+    for r in range(m - 1, -1, -1):
+        s = (np.arange(m) == r).astype(t.dtype)
+        for q in range(r + 1, m):
+            s = s - t[r, q] * x[q]
+        x[r] = np.where(np.arange(m) >= r, s / t[r, r], 0)
+    return x
+
+
+def _inv_unit_lower16(lo):
+    """Inverse of a unit lower triangle, column by column downwards (diag_inv_kernel)"""
+    m = lo.shape[0]
+    x = np.eye(m, dtype=lo.dtype)
+    for r in range(1, m):
+        s = np.zeros(m, lo.dtype)
+        for q in range(r):
+            s = s - lo[r, q] * x[q]
+        x[r] = np.where(np.arange(m) < r, s, x[r])
+    return x
+
+
+def trsm_blocked(t, b, unit):
+    """trsm_kernel's algorithm in NumPy: Y <- Y T^-1 blocked by 16 columns, Y_j <- (Y_j - sum_{p<j} Y_p T_pj) inv(T_jj)
+    with the explicit 16 x 16 inverses of diag_inv_kernel.  unit: T = L^T of a unit lower L (the U case)."""
+    ns = t.shape[0]
+    y = b.copy()
+    for j0 in range(0, ns, 16):
+        j1 = min(ns, j0 + 16)
+        inv = _inv_unit_lower16(t[j0:j1, j0:j1].T).T if unit else _inv_upper16(t[j0:j1, j0:j1])
+        y[:, j0:j1] = (y[:, j0:j1] - y[:, :j0] @ t[:j0, j0:j1]) @ inv
+    return y
+
+
+# --------------------------------------------------------------------------------------------------- dense (kernels)
+def diag_lu_ratio(a, out, thresh=None):
+    """k_diag_lu: A (ns + extra) x ns in, the factored block out -> (ratio on the ns x ns block, replaced pivots).
+    Diagonal positions where |u_kk| == thresh (pivots replaced by +-thresh) are excluded."""
+    ns = a.shape[1]
+    L = np.tril(out[:ns], -1) + np.eye(ns)
+    Uf = np.triu(out[:ns])
+    R = ext(a[:ns]) - ext(L) @ ext(Uf)
+    D = np.abs(L) @ np.abs(Uf)
+    rep = np.zeros(ns, bool) if thresh is None else np.abs(np.diag(out[:ns])) == thresh
+    R[np.diag_indices(ns)] = np.where(rep, 0, np.diag(R))
+    return ratio(R, D), int(rep.sum())
+
+
+def trsm_l_ratio(u, b, x):
+    """X U = B, U the upper triangle of u (non-unit)"""
+    Ut = np.triu(u)
+    return ratio(ext(x) @ ext(Ut) - ext(b), np.abs(x) @ np.abs(Ut))
+
+
+def trsm_u_ratio(lo, b, x):
+    """L X = B, L the strict lower triangle of lo plus the unit diagonal"""
+    Lt = np.tril(lo, -1) + np.eye(lo.shape[0])
+    return ratio(ext(Lt) @ ext(x) - ext(b), np.abs(Lt) @ np.abs(x))
+
+
+def gemm_sub_ratio(a, b, c, out):
+    return ratio(ext(out) - (ext(c) - ext(a) @ ext(b)), np.abs(c) + np.abs(a) @ np.abs(b))
+
+
+def kernel_bound(ns, dtype):
+    return 4 * ns * U * cfactor(dtype)
+
+
+def gemm_bound(k, dtype):
+    return 2 * (k + 1) * U * cfactor(dtype)
+
+
+# ---------------------------------------------------------------------------------------------- sparse (factorizations)
+def _csr(rows, cols, vals, n):
+    m = sp.csr_matrix((vals, (rows, cols)), shape=(n, n))
+    m.sum_duplicates()
+    return m
+
+
+def panel_matrix(prob, layer):
+    """The unfactored layer (F = P A P^T as the panels hold it) as CSR"""
+    lrow, lcol, urow, ucol = panel_coords(prob, layer)
+    lk, uk = lrow >= 0, urow >= 0
+    return _csr(np.concatenate([lrow[lk], urow[uk]]), np.concatenate([lcol[lk], ucol[uk]]),
+                np.concatenate([layer.lval[lk], layer.uval[uk]]), prob.n)
+
+
+def factors(prob, layer, n_elim=None):
+    """(L, U) of one factored layer as CSR: L unit lower (the identity added), U upper, the walk of LUProblem.dense.
+    n_elim: only the first n_elim columns were eliminated (a partial factorization); the panels of the later columns
+    are left out, and L gets the identity there."""
+    n = prob.n
+    n_elim = n if n_elim is None else n_elim
+    lrow, lcol, urow, ucol = panel_coords(prob, layer)
+    lk = (lrow >= 0) & (lcol < n_elim)
+    uk = (urow >= 0) & (urow < n_elim)
+    lr, lc, lv = lrow[lk], lcol[lk], layer.lval[lk]
+    low = lr > lc
+    eye = np.arange(n)
+    L = _csr(np.concatenate([lr[low], eye]), np.concatenate([lc[low], eye]),
+             np.concatenate([lv[low], np.ones(n, lv.dtype)]), n)
+    Uf = _csr(np.concatenate([lr[~low], urow[uk]]), np.concatenate([lc[~low], ucol[uk]]),
+              np.concatenate([lv[~low], layer.uval[uk]]), n)
+    return L, Uf
+
+
+def csr_values(rp, ci, vals, perm, n, rperm=None):
+    """F(perm[rperm[i]], perm[j]) = a_ij of the CSR matrix (rperm: row permutation applied first, None the identity)"""
+    rows = np.repeat(np.arange(n), np.diff(rp))
+    perm = np.asarray(perm)
+    ri = rows if rperm is None else np.asarray(rperm)[rows]
+    return _csr(perm[ri], perm[np.asarray(ci)], np.asarray(vals), n)
+
+
+def k_max(prob):
+    """The largest panel height nsupr: every dot product of the factorization and the solves is at most this long"""
+    return int(np.asarray(prob.lidx)[np.asarray(prob.lidx_off)[:-1] + 1].max())
+
+
+def factor_bound(prob):
+    return 4 * k_max(prob) * U * cfactor(prob.dtype)
+
+
+def _keys(m):
+    m = m.tocoo()
+    return m.row.astype(np.int64) * m.shape[1] + m.col, m.data
+
+
+def factor_ratio(F, L, Uf, thresh=None):
+    """max |F - L U| / (|L| |U|) over pattern(F) and pattern(L U), in extended precision -> (ratio, replaced pivots).
+    thresh: exclude the diagonal positions where |u_kk| == thresh (pivots replaced by +-thresh)."""
+    R = (ext(F).tocsr() - ext(L).tocsr() @ ext(Uf).tocsr()).tocsr()
+    D = (abs(L) @ abs(Uf)).tocsr()
+    d = Uf.diagonal()
+    rep = np.zeros(F.shape[0], bool) if thresh is None else np.abs(d) == thresh
+    rk, rv = _keys(R)
+    n = F.shape[0]
+    drop = np.isin(rk, np.nonzero(rep)[0] * (n + 1))
+    rk, rv = rk[~drop], rv[~drop]
+    dk, dv = _keys(D)
+    o = np.argsort(dk)
+    dk, dv = dk[o], dv[o]
+    q = np.minimum(np.searchsorted(dk, rk), max(len(dk) - 1, 0))
+    hit = (dk[q] == rk) if len(dk) else np.zeros(len(rk), bool)
+    den = np.where(hit, dv[q] if len(dv) else 0, 0)
+    return ratio(rv, den), int(rep.sum())
+
+
+def _op(M, trans):
+    return {"N": M, "T": M.T, "H": M.conj().T}[trans]
+
+
+def solve_ratio(L, Uf, x, b, trans="N"):
+    """max over right-hand sides and rows of |b - op(L U) x| / (op(|L| |U|) |x|); x, b: (n,) or (nrhs, n)"""
+    Le, Ue = ext(L).tocsr(), ext(Uf).tocsr()
+    x, b = np.atleast_2d(x).T, np.atleast_2d(b).T
+    X, B = ext(x), ext(b)
+    if trans == "N":
+        R = B - Le @ (Ue @ X)
+        D = abs(L) @ (abs(Uf) @ np.abs(x))
+    else:
+        R = B - _op(Ue, trans) @ (_op(Le, trans) @ X)
+        D = abs(Uf).T @ (abs(L).T @ np.abs(x))
+    return ratio(R, D)
+
+
+# ------------------------------------------------------------------------------------------ factorization problems
+# Poisson 12^3 (maxsup 128); the 256-column top separator of Poisson 16^3; fem 6^3 x 3 (supernodes up to 200 columns);
+# supernodes of at most 8 columns, so that the 64-column Schur tiles span eight or more destination panels (Poisson
+# 16^3: 1524 such tiles, the layout of test_gpu_schur_destinations.py at a size whose residual takes seconds).
+PROBLEMS = {"poisson12": dict(N=12, leaf=8, relax=16, maxsup=128),
+            "top256": dict(N=16, leaf=16, relax=32, maxsup=256),
+            "fem6": dict(N=6, leaf=4, relax=8, maxsup=200, fem=3),
+            "narrow": dict(N=16, leaf=8, relax=8, maxsup=8)}
+ZPROBLEMS = {"z32": dict(N=8, leaf=4, relax=8, maxsup=32),
+             "z200": dict(N=6, leaf=4, relax=8, maxsup=200, fem=3)}
+# a dyadic shift of Poisson 12^3 between two eigenvalues (test_inertia_cpu.gap_shifts): mixed-sign, small pivots
+SHIFT_N, SHIFT_KW = 12, dict(N=12, leaf=8, relax=16, maxsup=128)
+
+
+def shift_sigma():
+    from test_inertia_cpu import gap_shifts, spectrum
+    return gap_shifts(spectrum(SHIFT_N), 7)[3]
+
+
+def kkt_matrix():
+    """The KKT matrix of test_gpu_static_pivot.py: zero (2, 2) block, no unpivoted LU in the natural order"""
+    from test_static_pivot_cpu import kkt
+    return kkt(16, 40, 3)
+
+
+KKT_THRESH = 0.625   # above the smallest pivots of the matched, scaled KKT matrix (0.57..): some are replaced
