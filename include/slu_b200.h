@@ -133,7 +133,11 @@ const char *slu_b200_last_error(void);
 /* number of visible CUDA devices (0 if none / driver missing); never throws */
 int slu_b200_device_count(void);
 
-/* Analyse the structure, allocate HBM, build device index structures.  Values are not read. */
+/* Analyse the structure, allocate HBM, build device index structures.  Values are not read.
+ * Every handle call that writes the values in HBM (an upload, any fill, a factorization) first discards what the handle
+ * knew about them: a call of these that fails leaves the handle with no factors (and, for an upload or fill, no values
+ * to factor either).  The calls that read the factors then refuse, with a message, until a successful fill and
+ * factorization. */
 int slu_b200_create(slu_b200_handle_t *h, const slu_b200_lu_view_t *lu,
                     const slu_b200_options_t *opt);
 /* H2D: copy the view's Lnzval/Unzval (for the supernodes of my forests) into HBM. */

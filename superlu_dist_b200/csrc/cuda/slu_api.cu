@@ -278,7 +278,6 @@ struct slu_b200_handle_s {
     bool tc_force_off = false, tc_alloc_failed = false;   // slice workspace did not fit: analysed again without the int8 tensor-core path
     DevBuf<val_t> d_x, d_x2;              // triangular solve: right-hand sides / solution
     std::vector<int64_t> z_nodes_off;     // [zl] offset into d_pool_i32 of the forest's node list (solve masks)
-    bool factored = false;
     DevBuf<int> d_flags;                  // [0]=info [1]=err
     DevBuf<unsigned long long> d_tiny;
     DeviceLU dev{};
@@ -313,7 +312,9 @@ struct slu_b200_handle_s {
     int batch = 0;                        // 0: an ordinary handle
     int64_t member_len = 0, inv_len = 0;  // elements of one member's arena / diag-inverse workspace
     BatchedLU bdev{};
-    std::vector<int> member_info;         // info of every member after the last slu_b200_batch_factor
+    // info of every member (one on an unbatched handle): -1 no factors since the last fill or upload, 0 factored, > 0 the
+    // first zero pivot (1-based column)
+    std::vector<int> member_info;
     // condition estimation (slu_b200_gscon): per member the pending vector (batched handles only), the last real sign
     // vector, the state; the reduction partials and the two kase counters
     DevBuf<val_t> d_cv, d_csgn;
@@ -351,14 +352,80 @@ struct slu_b200_handle_s {
 
 namespace {
 
-// an upload, fill_csr, batch_fill_csr or batch_fill_affine: the scalings no longer describe the arena, and the A kept for
-// refinement goes with them
-void drop_scaling(slu_b200_handle_s *H)
+// The handle's state in one place.  Every call that writes the arena first says so here, after its argument checks and
+// before its first write, and sets the state it establishes only once it has succeeded: a call that fails on the way
+// leaves a handle whose factors (and values, for a fill) the calls that read them refuse.
+
+// a factorization is about to overwrite the arena: no member has factors, and the inverse no longer describes them
+void factors_replaced(slu_b200_handle_s *H)
 {
+    std::fill(H->member_info.begin(), H->member_info.end(), -1);
+    H->si_ready = false;
+}
+
+// an upload or a fill is about to overwrite the arena: no values to factor either, and the scaling no longer describes
+// them.  The A kept for refinement goes with the scaling, except on a scaled fill (keep_a), which reuses its buffers.
+void values_replaced(slu_b200_handle_s *H, bool keep_a = false)
+{
+    factors_replaced(H);
+    H->uploaded = false;
     H->scaled = false;
+    if (keep_a) return;
     H->d_arp.release();
     H->d_aci.release();
     H->d_aval.release();
+}
+
+// What a call needs of the handle (check): one bit per condition
+enum Need : unsigned {
+    UNBATCHED = 1u << 0,      // kind: slu_b200_create / schur_create
+    BATCHED = 1u << 1,        //       slu_b200_batch_create / batch_schur_create
+    NOT_SCHUR = 1u << 2,      // complete factors: not a Schur handle
+    SCHUR = 1u << 3,          // a Schur handle
+    GRID_Z = 1u << 4,         // 1 x 1 x Pz
+    GRID_SOLVE = 1u << 5,     // 1 x 1 x Pz, cooperative along Z
+    GRID_1 = 1u << 6,         // 1 x 1 x 1, world_size 1
+    UPLOADED = 1u << 7,       // values from a successful upload or fill
+    SCALED = 1u << 8,         // the scaling of a successful scaled fill
+    FACTORED = 1u << 9,       // every member factored with info 0
+    SI_READY = 1u << 10,      // the inverse of selinv on the current factors
+};
+
+// Refuses a call on a handle that does not give it what it needs, with a message that starts with fn, the call's exported
+// name.  Kind, then Schur, then grid, then state; except that an unbatched schur_* call names a missing Schur handle first.
+int check(const slu_b200_handle_s *H, const char *fn, unsigned need)
+{
+    if ((need & SCHUR) && (need & UNBATCHED) && !H->nschur) return fail("%s needs a Schur handle (" SLU_API "schur_create)", fn);
+    if ((need & UNBATCHED) && H->batch)
+        return fail("%s on a batched handle (%d members): use the " SLU_API "batch_* calls", fn, H->batch);
+    if ((need & BATCHED) && !H->batch) return fail("%s on an unbatched handle: use the " SLU_API "* calls without _batch", fn);
+    if ((need & NOT_SCHUR) && H->nschur)
+        return fail("%s on a Schur handle (partial factorization, nschur = %d): its factors are incomplete; use the %s calls", fn,
+                    H->nschur, H->batch ? SLU_API "batch_schur_*" : SLU_API "schur_*");
+    if ((need & SCHUR) && !H->nschur) return fail("%s needs a batched Schur handle (" SLU_API "batch_schur_create)", fn);
+    if ((need & (GRID_Z | GRID_SOLVE)) && H->P2 > 1) return fail("%s handles 1 x 1 x Pz grids (Pr x Pc = %d)", fn, H->P2);
+    if ((need & GRID_SOLVE) && H->comm && !H->coop)
+        return fail("%s: the Z-distributed solve needs the cooperative schedule (options.reserved[1] = 0)", fn);
+    if ((need & GRID_1) && (H->view.nprow * H->view.npcol * H->view.npdep != 1 || H->opt.world_size > 1))
+        return fail("%s needs a 1 x 1 x 1 grid with world_size 1 (got %d x %d x %d, world_size %d)", fn, H->view.nprow, H->view.npcol,
+                    H->view.npdep, H->opt.world_size);
+    if ((need & UPLOADED) && !H->uploaded)
+        return fail("%s before a successful %s", fn, H->batch ? SLU_API "batch_fill_csr" : SLU_API "upload or " SLU_API "fill_csr");
+    if ((need & SCALED) && !H->scaled)
+        return fail("%s needs a scaled fill on this handle first (a later upload or plain fill drops the scaling and the kept A)", fn);
+    if (need & FACTORED)
+        for (size_t j = 0; j < H->member_info.size(); ++j) {
+            const int info = H->member_info[j];
+            if (info == 0) continue;
+            if (!H->batch)
+                return fail("%s needs a successful " SLU_API "factor %s", fn, (need & SCALED) ? "after the scaled fill" : "(info = 0) on this handle first");
+            if (info < 0) return fail("%s needs a " SLU_API "batch_factor of the filled members first", fn);
+            return fail("%s: member %zu has an exact zero pivot in column %d", fn, j, info);
+        }
+    if ((need & SI_READY) && !H->si_ready)
+        return fail("%s needs %s on the current factors first (a later fill, upload or factorization invalidates it)", fn,
+                    H->batch ? SLU_API "batch_selinv" : SLU_API "selinv");
+    return 0;
 }
 
 int device_setup(const slu_b200_options_t *opt)
@@ -1334,19 +1401,23 @@ int upload_pipe_issue(slu_b200_handle_s *H)
     return 0;
 }
 
-// a batched handle (slu_b200_batch_create) only takes the slu_b200_batch_* calls, get_stats and destroy
-int refuse_batched(const slu_b200_handle_s *H, const char *fn)
+// The panel work of one level: diagonal LU, the inverses of the 16x16 diagonal blocks, the two panel solves and the
+// destination maps of the Schur update (value-independent: built once on H->dev for every member).  marks: nullptr, or
+// two profiling events recorded after the diagonal LU and after the panel solves.  Returns the kernel launches.
+template <class LU>
+int panel_work(const slu_b200_handle_s *H, const LU &d, const LevelPlan &L, int replace_tiny, cudaStream_t s,
+               const cudaEvent_t *marks = nullptr)
 {
-    return H->batch ? fail("%s on a batched handle (%d members): use the " SLU_API "batch_* calls", fn, H->batch) : 0;
-}
-
-// a Schur handle (slu_b200_schur_create) takes upload, fill_csr, factor, download, get_stats, destroy and the schur_* calls;
-// a batched one (slu_b200_batch_schur_create) batch_fill_csr, batch_factor, batch_download, get_stats, destroy and the
-// batch_schur_* calls
-int refuse_schur(const slu_b200_handle_s *H, const char *fn)
-{
-    return H->nschur ? fail("%s on a Schur handle (partial factorization, nschur = %d): its factors are incomplete; use the %s calls",
-                            fn, H->nschur, H->batch ? SLU_API "batch_schur_*" : SLU_API "schur_*") : 0;
+    const int32_t *nodes = H->d_pool_i32.p + L.nodes_off;
+    const int64_t *p64 = H->d_pool_i64.p;
+    int launches = launch_diag_lu(d, Batch{nodes, p64 + L.trsml_prefix, L.count}, L.max_ns, replace_tiny, H->opt.thresh, s);
+    if (marks) cudaEventRecord(marks[0], s);
+    launches += launch_diag_inv(d, Batch{nodes, p64 + L.inv_prefix, L.count}, L.inv_ctas, H->d_inv.p, s);
+    launches += launch_trsm_l(d, Batch{nodes, p64 + L.trsml_prefix, L.count}, L.trsml_ctas, L.max_ns, H->d_inv.p, s);
+    launches += launch_trsm_u(d, Batch{nodes, p64 + L.trsmu_prefix, L.count}, L.trsmu_ctas, L.max_ns, H->d_inv.p, s);
+    if (marks) cudaEventRecord(marks[1], s);
+    launches += launch_schur_setup(H->dev, Batch{nodes, p64 + L.setup_prefix, L.count}, L.setup_ctas, s);
+    return launches;
 }
 
 }  // namespace
@@ -1424,16 +1495,7 @@ void slu_b200_destroy(slu_b200_handle_t H)
     for (auto e : H->ev_up) if (e) cudaEventDestroy(e);
     for (auto e : H->ev_panel) if (e) cudaEventDestroy(e);
     for (auto e : H->ev_bulk) if (e) cudaEventDestroy(e);
-    H->val.release(); H->stage.release(); H->d_inv.release(); H->d_nodes.release(); H->d_xsup.release(); H->d_supno.release();
-    H->d_lrows.release(); H->d_lsrow.release(); H->d_lspos.release(); H->d_ucols.release(); H->d_ufst.release();
-    H->d_useg.release(); H->d_pool_i32.release(); H->d_pool_i64.release(); H->d_lrel.release(); H->d_urel.release();
-    H->d_lblk.release(); H->d_ublk.release(); H->d_rowinfo.release(); H->d_colinfo.release(); H->d_flags.release();
-    H->d_x.release(); H->d_x2.release();
-    H->d_cv.release(); H->d_csgn.release(); H->d_cstate.release(); H->d_cpart.release(); H->d_ccount.release();
-    H->d_tiny.release(); H->d_oz_i8.release(); H->d_oz_scale.release(); H->d_oz_rexp.release();
-    H->d_hinv.release(); H->d_si_pool.release(); H->d_sunits.release(); H->d_S.release();
-    H->d_perm_r.release(); H->d_rmap.release(); H->d_cperm.release(); H->d_R.release(); H->d_C.release();
-    delete H;
+    delete H;                                   // every DevBuf frees its HBM
 }
 
 // batch > 0: a batched handle (slu_b200_batch_create), 1 x 1 x 1 grid, FP64 DMMA kernels only
@@ -1537,8 +1599,8 @@ static int create_impl(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, con
         H->bdev.val_stride = H->member_len;
         H->bdev.inv_stride = H->inv_len;
         H->bdev.members = batch;
-        H->member_info.assign(batch, -1);
     }
+    H->member_info.assign(batch ? batch : 1, -1);
     {
         int lo = 0, hi = 0;
         cudaDeviceGetStreamPriorityRange(&lo, &hi);  // hi = numerically lowest = highest priority
@@ -1569,11 +1631,9 @@ int slu_b200_create(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, const 
 int slu_b200_upload(slu_b200_handle_t H)
 {
     if (!H) return fail("null handle");
-    if (refuse_batched(H, SLU_API "upload")) return -1;
+    if (check(H, SLU_API "upload", UNBATCHED)) return -1;
     double t0 = now_s();
-    H->factored = false;
-    H->si_ready = false;
-    drop_scaling(H);
+    values_replaced(H);
     if (transfer(H, true)) return -1;
     H->st.t_upload_s = now_s() - t0;
     H->uploaded = true;
@@ -1583,7 +1643,7 @@ int slu_b200_upload(slu_b200_handle_t H)
 int slu_b200_download(slu_b200_handle_t H)
 {
     if (!H) return fail("null handle");
-    if (refuse_batched(H, SLU_API "download")) return -1;
+    if (check(H, SLU_API "download", UNBATCHED)) return -1;
     double t0 = now_s();
     if (transfer(H, false)) return -1;
     H->st.t_download_s = now_s() - t0;
@@ -1593,9 +1653,8 @@ int slu_b200_download(slu_b200_handle_t H)
 static int factor_impl(slu_b200_handle_t H, int *info, bool pipelined, bool up_pipe = false)
 {
     if (!H || !info) return fail("null argument");
-    if (refuse_batched(H, SLU_API "factor")) return -1;
-    if (!H->uploaded) return fail("slu_b200_factor before slu_b200_upload");
-    H->si_ready = false;
+    if (check(H, SLU_API "factor", UNBATCHED | UPLOADED)) return -1;
+    factors_replaced(H);
     if (pipelined && pipe_prepare(H)) return -1;
     cudaStream_t s = H->stream;
     const DeviceLU &d = H->dev;
@@ -1628,9 +1687,7 @@ static int factor_impl(slu_b200_handle_t H, int *info, bool pipelined, bool up_p
             if (L.zlvl < zl) continue;
             if (first == (size_t)-1) first = li;
             last = li;
-            const int32_t *nodes = H->d_pool_i32.p + L.nodes_off;
             const int64_t *p64 = H->d_pool_i64.p;
-            Batch all{nodes, p64 + L.trsml_prefix, L.count};
             if (lookahead && li >= first + 2) CU(cudaStreamWaitEvent(s, H->ev_bulk[li - 2], 0));
             if (up_pipe) CU(cudaStreamWaitEvent(s, H->ev_up[li], 0));  // this level's A values are in the arena
             if (coopz && L.slab_end > L.slab_begin) {
@@ -1647,13 +1704,7 @@ static int factor_impl(slu_b200_handle_t H, int *info, bool pipelined, bool up_p
             // copies of a cooperative group) and by one rank of its 2D grid (stat->TinyPivots is MPI_SUMmed there,
             // pdgssvx3d.c:1149)
             const bool count_tiny = !H->my_zero[zl] && (H->P2 == 1 || (H->view.myrow == 0 && H->view.mycol == 0));
-            H->st.gpu_launches += launch_diag_lu(d, all, L.max_ns, H->opt.replace_tiny_pivot ? (count_tiny ? 1 : 2) : 0, H->opt.thresh, s);
-            if (prof) cudaEventRecord(pe[1], s);
-            H->st.gpu_launches += launch_diag_inv(d, Batch{nodes, p64 + L.inv_prefix, L.count}, L.inv_ctas, H->d_inv.p, s);
-            H->st.gpu_launches += launch_trsm_l(d, Batch{nodes, p64 + L.trsml_prefix, L.count}, L.trsml_ctas, L.max_ns, H->d_inv.p, s);
-            H->st.gpu_launches += launch_trsm_u(d, Batch{nodes, p64 + L.trsmu_prefix, L.count}, L.trsmu_ctas, L.max_ns, H->d_inv.p, s);
-            if (prof) cudaEventRecord(pe[2], s);
-            H->st.gpu_launches += launch_schur_setup(d, Batch{nodes, p64 + L.setup_prefix, L.count}, L.setup_ctas, s);
+            H->st.gpu_launches += panel_work(H, d, L, H->opt.replace_tiny_pivot ? (count_tiny ? 1 : 2) : 0, s, prof ? &pe[1] : nullptr);
 #ifndef SLU_COMPLEX
             const int32_t *tcn = H->d_pool_i32.p + L.tc_nodes;
             if (L.tc_count > 0)      // int8 slices of the level's wide panels (final after the TRSMs above)
@@ -1724,8 +1775,7 @@ static int factor_impl(slu_b200_handle_t H, int *info, bool pipelined, bool up_p
     }
     H->st.tiny_pivots = (int64_t)tiny;
     if (flags[1]) return fail("%d Schur-update destinations were not found in the L/U structure", flags[1]);
-    *info = flags[0] == INT_MAX ? 0 : flags[0];
-    H->factored = *info == 0;
+    *info = H->member_info[0] = flags[0] == INT_MAX ? 0 : flags[0];
     return 0;
 }
 
@@ -1734,7 +1784,7 @@ int slu_b200_factor(slu_b200_handle_t H, int *info) { return factor_impl(H, info
 int slu_b200_factor_host(slu_b200_handle_t H, int *info)
 {
     if (!H || !info) return fail("null argument");
-    if (refuse_batched(H, SLU_API "factor_host") || refuse_schur(H, SLU_API "factor_host")) return -1;
+    if (check(H, SLU_API "factor_host", UNBATCHED | NOT_SCHUR)) return -1;
     // The overlapped transfers move whole panels between the caller's arrays and the arena, which needs the U
     // skylines to equal their dense-packed form (symmetric patterns) and 1 x 1 x Pz pieces.  Anything else -- the
     // unsymmetric patterns SuperLU exists for, Pr x Pc pieces -- takes the plain path: upload (with the skyline
@@ -1749,8 +1799,7 @@ int slu_b200_factor_host(slu_b200_handle_t H, int *info)
         return rc2 ? rc2 : slu_b200_download(H);
     }
     if (H->grouped) {                      // options.reserved[3]: H2D, factorization and D2H all overlapped
-        H->factored = false;
-        drop_scaling(H);
+        values_replaced(H);
         if (pipe_prepare(H) || upload_pipe_issue(H)) return -1;
         H->uploaded = true;
         H->st.t_upload_s = 0;
@@ -1768,42 +1817,51 @@ int slu_b200_factor_host(slu_b200_handle_t H, int *info)
 // ScalePermstruct->perm_c after sp_colorder), is copied to HBM once (12 bytes per nonzero instead of 8 bytes per FACTOR
 // entry; 20 instead of 16 in doublecomplex, where val holds (re, im) pairs) and scattered into the panels by a kernel --
 // what pddistribute3d does on the host.  Replicated ancestors of other layers start at zero (dinit3DLUstructForest,
-// pdgssvx3d.c:948).  Replaces slu_b200_upload.
-int slu_b200_fill_csr(slu_b200_handle_t H, int n, const int32_t *rowptr, const int32_t *colind, const double *val, const int32_t *perm)
+// pdgssvx3d.c:948).  Replaces slu_b200_upload.  On a batched handle (slu_b200_batch_fill_csr) val holds batch x nnz values,
+// member-major.
+static int fill_csr_impl(slu_b200_handle_t H, bool batched, int n, const int32_t *rowptr, const int32_t *colind, const double *val,
+                         const int32_t *perm, const char *fn)
 {
     if (!H || !rowptr || !colind || !val || !perm) return fail("null argument");
-    if (refuse_batched(H, SLU_API "fill_csr")) return -1;
-    if (n != H->n) return fail("matrix order %d does not match the handle's %d", n, H->n);
-    if (H->P2 > 1) return fail("slu_b200_fill_csr handles 1 x 1 x Pz grids");
-    H->si_ready = false;
-    drop_scaling(H);
+    if (check(H, fn, batched ? BATCHED : (UNBATCHED | GRID_Z))) return -1;
+    if (n != H->n) return fail("%s: matrix order %d does not match the handle's %d", fn, n, H->n);
     double t0 = now_s();
+    const int B = batched ? H->batch : 1;
     const int64_t nnz = rowptr[n];
     DevBuf<int32_t> drp, dci, dperm;
     DevBuf<val_t> dv;
     DevBuf<int8_t> dact;
     std::vector<int8_t> act(H->nsupers, 0);
-    for (int zl = 0; zl < H->max_lvl; ++zl)
-        if (!H->my_zero[zl])
+    for (int zl = 0; zl < H->max_lvl; ++zl)      // the panels this layer holds (a batched handle has one level: znodes[0])
+        if (batched || !H->my_zero[zl])
             for (int k : H->znodes[zl]) act[k] = 1;
-    if (drp.alloc((size_t)n + 1) || dci.alloc((size_t)nnz) || dv.alloc((size_t)nnz) || dperm.alloc((size_t)n) || dact.upload(act)) return -1;
+    if (drp.alloc((size_t)n + 1) || dci.alloc((size_t)nnz) || dv.alloc((size_t)nnz * B) || dperm.alloc((size_t)n) || dact.upload(act))
+        return -1;
     cudaStream_t s = H->stream;
     CU(cudaMemcpyAsync(drp.p, rowptr, ((size_t)n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(dci.p, colind, (size_t)nnz * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(dv.p, val, (size_t)nnz * sizeof(val_t), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(dv.p, val, (size_t)nnz * B * sizeof(val_t), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(dperm.p, perm, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    values_replaced(H);
     CU(cudaMemsetAsync(H->val.p, 0, H->val.bytes(), s));
-    CU(cudaMemsetAsync(H->d_flags.p + 1, 0, sizeof(int), s));
-    launch_fill_csr(H->dev, n, drp.p, dci.p, dv.p, dperm.p, dact.p, H->d_flags.p + 1, s);
+    CU(cudaMemsetAsync(H->dev.err, 0, sizeof(int), s));
+    if (batched) launch_fill_csr(H->bdev, n, drp.p, dci.p, dv.p, dperm.p, dact.p, H->dev.err, s);
+    else launch_fill_csr(H->dev, n, drp.p, dci.p, dv.p, dperm.p, dact.p, H->dev.err, s);
     int bad = 0;
-    CU(cudaMemcpyAsync(&bad, H->d_flags.p + 1, sizeof(int), cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&bad, H->dev.err, sizeof(int), cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     CU(cudaGetLastError());
-    if (bad) return fail("%d entries of A have no slot in the L/U structure (wrong permutation or symbolic structure)", bad);
+    if (bad)
+        return fail("%s: %d entries of %s have no slot in the L/U structure (wrong permutation or symbolic structure)", fn, bad,
+                    batched ? "the members" : "A");
     H->st.t_upload_s = now_s() - t0;
     H->uploaded = true;
-    H->factored = false;
     return 0;
+}
+
+int slu_b200_fill_csr(slu_b200_handle_t H, int n, const int32_t *rowptr, const int32_t *colind, const double *val, const int32_t *perm)
+{
+    return fill_csr_impl(H, false, n, rowptr, colind, val, perm, SLU_API "fill_csr");
 }
 
 // Triangular solves on the resident factors (the job of pdgstrs3d, SRC/double/pdgstrs3d.c:6604, for factors that never
@@ -1833,6 +1891,26 @@ static int solve_level(const slu_b200_handle_s *H, const LU &d, const LevelPlan 
     if (!backward) launches += launch_solve_diag(d, nodes, L.count, false, trans, x, n, nrhs, s);
     launches += launch_solve_update(d, b, upanel ? L.su_ctas : L.sl_ctas, backward, trans, x, n, nrhs, s);
     if (backward) launches += launch_solve_diag(d, nodes, L.count, true, trans, x, n, nrhs, s);
+    return launches;
+}
+
+// The passes of a solve over the whole level plan: both for a solve; on a Schur handle the forward one alone is condense, the
+// backward one expand.
+enum { PASS_FORWARD = 1, PASS_BACKWARD = 2, PASS_BOTH = 3 };
+
+// The passes on device LU d (H->dev, or H->bdev for every member of a batched handle) of a 1 x 1 x 1 grid, in place in d_x
+// (one n x nrhs block per member).  Enqueued on H->stream, not synchronised.  Returns the kernel launches.
+template <class LU>
+static int solve_passes(slu_b200_handle_t H, const LU &d, int nrhs, int trans, int passes = PASS_BOTH)
+{
+    val_t *x = H->d_x.p;
+    int launches = 0;
+    if (passes & PASS_FORWARD)
+        for (size_t li = 0; li < H->levels.size(); ++li)        // forward: L y = b (U^T y = b)
+            launches += solve_level(H, d, H->levels[li], false, trans, x, H->n, nrhs, H->stream);
+    if (passes & PASS_BACKWARD)
+        for (size_t li = H->levels.size(); li-- > 0;)           // backward: U x = y (L^T x = y)
+            launches += solve_level(H, d, H->levels[li], true, trans, x, H->n, nrhs, H->stream);
     return launches;
 }
 extern "C" {
@@ -1898,27 +1976,30 @@ static int solve_dev(slu_b200_handle_t H, int nrhs, int trans, val_t **result)
     return launches;
 }
 
-// fn: "solve" or "solve_trans", for the messages
-static int solve_impl(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int trans, const char *fn)
+// Every solve on host vectors: solve, solve_trans, schur_condense / expand and their batched twins (fn, with what they need
+// of the handle).  x: one n x nrhs block per member (ldx >= n), block j at x + j * ldx * nrhs: b on entry, the result on
+// return.  The complete unbatched solve is solve_dev (b in d_x2), everything else the passes in place in d_x.
+static int solve_host(slu_b200_handle_t H, const char *fn, unsigned need, double *xh, int ldx, int nrhs, int trans, int passes)
 {
     if (!H || !xh) return fail("null argument");
-    if (refuse_batched(H, (std::string(SLU_API) + fn).c_str()) || refuse_schur(H, (std::string(SLU_API) + fn).c_str())) return -1;
-    if (trans < 0 || trans > 2) return fail(SLU_API "%s: trans = %d, must be 0 (A x = b), 1 (A^T x = b) or 2 (A^H x = b)", fn, trans);
-    if (!H->factored) return fail("slu_b200_%s needs a successful slu_b200_factor on this handle first", fn);
-    if (nrhs < 1 || ldx < H->n) return fail("bad nrhs / ldx");
-    if (H->P2 > 1) return fail("slu_b200_%s: Pr x Pc > 1 is not supported yet (1 x 1 x Pz only)", fn);
-    if (H->comm && !H->coop) return fail("slu_b200_%s: the Z-distributed solve needs the cooperative schedule (options.reserved[1] = 0)", fn);
-    const int n = H->n;
-    const size_t len = (size_t)n * nrhs;
-    if (H->d_x.n < len && (H->d_x.alloc(len) || H->d_x2.alloc(len))) return -1;
+    if (check(H, fn, need)) return -1;
+    if (trans < 0 || trans > 2) return fail("%s: trans = %d, must be 0 (A x = b), 1 (A^T x = b) or 2 (A^H x = b)", fn, trans);
+    const bool batched = H->batch > 0, full = !batched && passes == PASS_BOTH;
+    const int B = batched ? H->batch : 1, n = H->n;
+    if (nrhs < 1 || ldx < n) return fail("%s: bad nrhs / ldx", fn);
+    if (batched && (int64_t)n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
+    const size_t len = (size_t)n * nrhs * B;
+    if (H->d_x.n < len && (H->d_x.alloc(len) || (!batched && H->d_x2.alloc(len)))) return -1;
     cudaStream_t s = H->stream;
     double t0 = now_s();
-    CU(cudaMemcpy2DAsync(H->d_x2.p, (size_t)n * sizeof(val_t), xh, (size_t)ldx * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs,
-                         cudaMemcpyHostToDevice, s));
-    val_t *result = nullptr;
-    const int launches = solve_dev(H, nrhs, trans, &result);
+    val_t *result = H->d_x.p;
+    // the blocks are B * nrhs columns at pitch ldx: one 2D copy each way
+    CU(cudaMemcpy2DAsync(full ? H->d_x2.p : result, (size_t)n * sizeof(val_t), xh, (size_t)ldx * sizeof(val_t), (size_t)n * sizeof(val_t),
+                         (size_t)nrhs * B, cudaMemcpyHostToDevice, s));
+    const int launches = full ? solve_dev(H, nrhs, trans, &result)
+                              : batched ? solve_passes(H, H->bdev, nrhs, trans, passes) : solve_passes(H, H->dev, nrhs, trans, passes);
     if (launches < 0) return -1;
-    CU(cudaMemcpy2DAsync(xh, (size_t)ldx * sizeof(val_t), result, (size_t)n * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs,
+    CU(cudaMemcpy2DAsync(xh, (size_t)ldx * sizeof(val_t), result, (size_t)n * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs * B,
                          cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     CU(cudaGetLastError());
@@ -1929,12 +2010,12 @@ static int solve_impl(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int tr
 
 int slu_b200_solve(slu_b200_handle_t H, double *xh, int ldx, int nrhs)
 {
-    return solve_impl(H, xh, ldx, nrhs, 0, "solve");
+    return solve_host(H, SLU_API "solve", UNBATCHED | NOT_SCHUR | GRID_SOLVE | FACTORED, xh, ldx, nrhs, 0, PASS_BOTH);
 }
 
 int slu_b200_solve_trans(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int trans)
 {
-    return solve_impl(H, xh, ldx, nrhs, trans, "solve_trans");
+    return solve_host(H, SLU_API "solve_trans", UNBATCHED | NOT_SCHUR | GRID_SOLVE | FACTORED, xh, ldx, nrhs, trans, PASS_BOTH);
 }
 
 #ifndef SLU_COMPLEX
@@ -1946,7 +2027,7 @@ int slu_b200_solve_trans(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int
 int slu_b200_k_level_export(slu_b200_handle_t H, int level, void *device_lu, int device_lu_bytes, int32_t *nodes, int max_nodes)
 {
     if (!H || level < 0 || level >= (int)H->levels.size()) return fail("bad handle / level");
-    if (refuse_batched(H, "slu_b200_k_level_export") || refuse_schur(H, "slu_b200_k_level_export")) return -1;
+    if (check(H, "slu_b200_k_level_export", UNBATCHED | NOT_SCHUR)) return -1;
     if (device_lu && device_lu_bytes == (int)sizeof(DeviceLU)) memcpy(device_lu, &H->dev, sizeof(DeviceLU));
     else if (device_lu) return fail("DeviceLU is %d bytes", (int)sizeof(DeviceLU));
     const LevelPlan &L = H->levels[level];
@@ -1964,7 +2045,7 @@ int slu_b200_k_level_export(slu_b200_handle_t H, int level, void *device_lu, int
 int slu_b200_k_rerun_schur(slu_b200_handle_t H, int level, int reps, float *ms)
 {
     if (!H || level < 0 || level >= (int)H->levels.size() || reps < 1 || !ms) return fail("bad argument");
-    if (refuse_batched(H, "slu_b200_k_rerun_schur") || refuse_schur(H, "slu_b200_k_rerun_schur")) return -1;
+    if (check(H, "slu_b200_k_rerun_schur", UNBATCHED | NOT_SCHUR)) return -1;
     const LevelPlan &L = H->levels[level];
     cudaStream_t s = H->stream;
     const DeviceLU &d = H->dev;
@@ -1997,13 +2078,6 @@ int slu_b200_k_rerun_schur(slu_b200_handle_t H, int level, int reps, float *ms)
 // level, so its gathered block M = H(R, C) is final.  Per level 7 launches: the destination maps and the 16x16
 // diagonal-block inverses are rebuilt in the factorization's per-level workspaces, then three products and two
 // triangular solves; a level with no Schur update (the root) has no maps to build and makes 6.
-static int selinv_refuse(const slu_b200_handle_s *H, const char *fn)
-{
-    if (refuse_batched(H, fn) || refuse_schur(H, fn)) return -1;
-    if (H->opt.world_size > 1 || H->max_lvl > 1 || H->P2 > 1) return fail("%s handles 1 x 1 x 1 grids (world_size 1)", fn);
-    if (!H->factored) return fail("%s needs a successful " SLU_API "factor (info = 0) on this handle first", fn);
-    return 0;
-}
 
 // CTA prefixes of the selinv kernels, from the level plan: built once per handle.  Product tiles are SELINV_TILE_M rows
 // by SELINV_TILE_N val_t columns (64 x 64 real outputs: 32 complex columns in doublecomplex).
@@ -2097,54 +2171,76 @@ extern "C" {
 int slu_b200_selinv(slu_b200_handle_t H, double out[4])
 {
     if (!H) return fail("null handle");
-    if (selinv_refuse(H, SLU_API "selinv")) return -1;
+    if (check(H, SLU_API "selinv", UNBATCHED | NOT_SCHUR | GRID_1 | FACTORED)) return -1;
     return selinv_sweep(H, H->dev, 1, SLU_API "selinv", out);
 }
 
-int slu_b200_selinv_get(slu_b200_handle_t H, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm, double *out)
+// The entries of A^-1 on A's pattern from the inverse of the last selinv, for every member (one on an unbatched handle):
+// out holds members x nnz values, member j's at out + j * nnz.  need: what the call (fn) needs of the handle.
+static int selinv_get_impl(slu_b200_handle_t H, const char *fn, unsigned need, int n, const int32_t *rowptr, const int32_t *colind,
+                           const int32_t *perm, double *out)
 {
     if (!H || !rowptr || !colind || !perm || !out) return fail("null argument");
-    if (selinv_refuse(H, SLU_API "selinv_get")) return -1;
-    if (!H->si_ready) return fail(SLU_API "selinv_get needs " SLU_API "selinv on the current factors first (a later upload, fill_csr or factor invalidates it)");
-    if (n != H->n) return fail(SLU_API "selinv_get: matrix order %d does not match the handle's %d", n, H->n);
+    if (check(H, fn, need)) return -1;
+    if (n != H->n) return fail("%s: matrix order %d does not match the handle's %d", fn, n, H->n);
     const int64_t nnz = rowptr[n];
-    if (rowptr[0] != 0 || nnz < 0) return fail(SLU_API "selinv_get: bad rowptr");
+    if (rowptr[0] != 0 || nnz < 0) return fail("%s: bad rowptr", fn);
+    const int B = H->batch ? H->batch : 1;
     DevBuf<int32_t> drp, dci, dperm;
     DevBuf<val_t> dout;
-    if (drp.alloc((size_t)n + 1) || dci.alloc((size_t)nnz) || dperm.alloc((size_t)n) || dout.alloc((size_t)nnz)) return -1;
+    if (drp.alloc((size_t)n + 1) || dci.alloc((size_t)nnz) || dperm.alloc((size_t)n) || dout.alloc((size_t)nnz * B)) return -1;
     cudaStream_t s = H->stream;
     CU(cudaMemcpyAsync(drp.p, rowptr, ((size_t)n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(dci.p, colind, (size_t)nnz * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(dperm.p, perm, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    CU(cudaMemsetAsync(H->d_flags.p + 1, 0, sizeof(int), s));
-    launch_selinv_get(H->dev, H->d_hinv.p, n, drp.p, dci.p, dperm.p, dout.p, H->d_flags.p + 1, s);
+    CU(cudaMemsetAsync(H->dev.err, 0, sizeof(int), s));
+    if (H->batch) launch_selinv_get(H->bdev, H->d_hinv.p, n, drp.p, dci.p, dperm.p, dout.p, H->dev.err, s);
+    else launch_selinv_get(H->dev, H->d_hinv.p, n, drp.p, dci.p, dperm.p, dout.p, H->dev.err, s);
     int bad = 0;
-    CU(cudaMemcpyAsync(out, dout.p, (size_t)nnz * sizeof(val_t), cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(&bad, H->d_flags.p + 1, sizeof(int), cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(out, dout.p, (size_t)nnz * B * sizeof(val_t), cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&bad, H->dev.err, sizeof(int), cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     CU(cudaGetLastError());
-    if (bad) return fail(SLU_API "selinv_get: %d entries have no slot in the L/U structure (A^-1 is known on the pattern of L+U only)", bad);
+    if (bad) return fail("%s: %d entries have no slot in the L/U structure (A^-1 is known on the pattern of L+U only)", fn, bad);
+    return 0;
+}
+
+int slu_b200_selinv_get(slu_b200_handle_t H, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm, double *out)
+{
+    return selinv_get_impl(H, SLU_API "selinv_get", UNBATCHED | NOT_SCHUR | GRID_1 | FACTORED | SI_READY, n, rowptr, colind, perm, out);
+}
+
+// log |det| and the sign of every member (one on an unbatched handle): logabs[members]; sign[members] (double) or
+// sign[2 * members] = exp(i theta_j) as (re, im) pairs (doublecomplex).  need: what the call (fn) needs of the handle.
+static int logdet_impl(slu_b200_handle_t H, const char *fn, unsigned need, double *logabs, double *sign)
+{
+    if (!H || !logabs || !sign) return fail("null argument");
+    if (check(H, fn, need)) return -1;
+    const int B = H->batch ? H->batch : 1;
+    const int count = (int)H->znodes[0].size();
+    const int nparts = (count + SELINV_VECS - 1) / SELINV_VECS;
+    DevBuf<double> part, res;
+    DevBuf<phase_t> ph;
+    if (part.alloc((size_t)nparts * B) || ph.alloc((size_t)nparts * B) || res.alloc((size_t)(1 + VAL_DOUBLES) * B)) return -1;
+    cudaStream_t s = H->stream;
+    const int32_t *nodes = H->d_pool_i32.p + H->z_nodes_off[0];
+    if (H->batch) launch_selinv_logdet(H->bdev, nodes, count, part.p, ph.p, res.p, s);
+    else launch_selinv_logdet(H->dev, nodes, count, part.p, ph.p, res.p, s);
+    std::vector<double> r((size_t)(1 + VAL_DOUBLES) * B, 0.0);
+    for (int j = 0; j < B; ++j) r[(size_t)j * (1 + VAL_DOUBLES) + 1] = 1.0;   // no supernode: log |det| 0, sign 1
+    if (nparts > 0) CU(cudaMemcpyAsync(r.data(), res.p, r.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    for (int j = 0; j < B; ++j) {
+        logabs[j] = r[(size_t)j * (1 + VAL_DOUBLES)];
+        for (int c = 0; c < VAL_DOUBLES; ++c) sign[(size_t)j * VAL_DOUBLES + c] = r[(size_t)j * (1 + VAL_DOUBLES) + 1 + c];
+    }
     return 0;
 }
 
 int slu_b200_logdet(slu_b200_handle_t H, double *logabs, double *sign)
 {
-    if (!H || !logabs || !sign) return fail("null argument");
-    if (selinv_refuse(H, SLU_API "logdet")) return -1;
-    const int count = (int)H->znodes[0].size();
-    const int nparts = (count + SELINV_VECS - 1) / SELINV_VECS;
-    DevBuf<double> part, res;
-    DevBuf<phase_t> ph;
-    if (part.alloc((size_t)nparts) || ph.alloc((size_t)nparts) || res.alloc(1 + VAL_DOUBLES)) return -1;
-    cudaStream_t s = H->stream;
-    launch_selinv_logdet(H->dev, H->d_pool_i32.p + H->z_nodes_off[0], count, part.p, ph.p, res.p, s);
-    double r[1 + VAL_DOUBLES] = {0.0, 1.0};   // log |det|, then the sign: +-1, or exp(i theta) as (re, im)
-    CU(cudaMemcpyAsync(r, res.p, sizeof r, cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    CU(cudaGetLastError());
-    *logabs = r[0];
-    for (int c = 0; c < VAL_DOUBLES; ++c) sign[c] = r[1 + c];
-    return 0;
+    return logdet_impl(H, SLU_API "logdet", UNBATCHED | NOT_SCHUR | GRID_1 | FACTORED, logabs, sign);
 }
 
 // ---- partial factorization: the Schur complement and the two partial solves ------------------------------------------
@@ -2153,14 +2249,6 @@ int slu_b200_logdet(slu_b200_handle_t H, double *logabs, double *sign)
 // start as A22 and end as S = A22 - A21 A11^-1 A12 on the symbolic pattern.  The forward pass of the solve over the same
 // plan is condense (its update scatter subtracts L21 y1 from the Schur rows), the backward pass with x2 in the Schur
 // positions is expand.
-static int schur_refuse(const slu_b200_handle_s *H, const char *fn)
-{
-    if (!H->nschur) return fail("%s needs a Schur handle (" SLU_API "schur_create)", fn);
-    if (refuse_batched(H, fn)) return -1;     // a batched Schur handle: the batch_schur_* calls
-    if (!H->factored) return fail("%s needs a successful " SLU_API "factor (info = 0) on this handle first", fn);
-    return 0;
-}
-
 int slu_b200_schur_create(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, int nschur)
 {
     if (!out || !lu || !opt) return fail("null argument");
@@ -2214,45 +2302,19 @@ int slu_b200_schur_get(slu_b200_handle_t H, double *S, int lds)
 {
     if (!H || !S) return fail("null argument");
     const char *fn = SLU_API "schur_get";
-    if (schur_refuse(H, fn)) return -1;
+    if (check(H, fn, UNBATCHED | SCHUR | FACTORED)) return -1;
     return schur_get_impl(H, S, lds, fn);
 }
 
 // condense: the forward pass over the plan; expand: the backward pass.  x: host, n x nrhs (ldx >= n), ordering of F.
-static int schur_pass(slu_b200_handle_t H, double *xh, int ldx, int nrhs, bool backward, const char *fn)
-{
-    if (!H || !xh) return fail("null argument");
-    if (schur_refuse(H, fn)) return -1;
-    if (nrhs < 1 || ldx < H->n) return fail("%s: bad nrhs / ldx", fn);
-    const int n = H->n;
-    const size_t len = (size_t)n * nrhs;
-    if (H->d_x.n < len && (H->d_x.alloc(len) || H->d_x2.alloc(len))) return -1;
-    cudaStream_t s = H->stream;
-    const double t0 = now_s();
-    CU(cudaMemcpy2DAsync(H->d_x.p, (size_t)n * sizeof(val_t), xh, (size_t)ldx * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs,
-                         cudaMemcpyHostToDevice, s));
-    int launches = 0;
-    if (!backward)
-        for (size_t li = 0; li < H->levels.size(); ++li) launches += solve_level(H, H->dev, H->levels[li], false, 0, H->d_x.p, n, nrhs, s);
-    else
-        for (size_t li = H->levels.size(); li-- > 0;) launches += solve_level(H, H->dev, H->levels[li], true, 0, H->d_x.p, n, nrhs, s);
-    CU(cudaMemcpy2DAsync(xh, (size_t)ldx * sizeof(val_t), H->d_x.p, (size_t)n * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs,
-                         cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    CU(cudaGetLastError());
-    H->st.reserved[4] = now_s() - t0;
-    H->st.reserved[5] = (double)launches;
-    return 0;
-}
-
 int slu_b200_schur_condense(slu_b200_handle_t H, double *x, int ldx, int nrhs)
 {
-    return schur_pass(H, x, ldx, nrhs, false, SLU_API "schur_condense");
+    return solve_host(H, SLU_API "schur_condense", UNBATCHED | SCHUR | FACTORED, x, ldx, nrhs, 0, PASS_FORWARD);
 }
 
 int slu_b200_schur_expand(slu_b200_handle_t H, double *x, int ldx, int nrhs)
 {
-    return schur_pass(H, x, ldx, nrhs, true, SLU_API "schur_expand");
+    return solve_host(H, SLU_API "schur_expand", UNBATCHED | SCHUR | FACTORED, x, ldx, nrhs, 0, PASS_BACKWARD);
 }
 
 // ---- batched handles: many matrices of one sparsity pattern (pdgssvx3d_csc_batch, SRC/double/pdgssvx3d_csc_batch.c:81,
@@ -2262,26 +2324,6 @@ int slu_b200_schur_expand(slu_b200_handle_t H, double *x, int ldx, int nrhs)
 // the LBlk/UBlk tables, the look-ahead split and the RowInfo/ColInfo/lrel/urel maps (built once per level by
 // schur_setup_kernel).  Each member has its own value arena, d_inv slice and info flag; every batched launch is the
 // unbatched one with gridDim.y = members, so a batched factorization takes exactly as many launches as one matrix.
-static int refuse_unbatched(const slu_b200_handle_s *H, const char *fn)
-{
-    return H->batch ? 0 : fail("%s on an unbatched handle: use the " SLU_API "* calls without _batch", fn);
-}
-
-// the calls that read the factors need every member's last batch_factor to have succeeded
-static int refuse_unfactored_members(const slu_b200_handle_s *H, const char *fn)
-{
-    for (int j = 0; j < H->batch; ++j) {
-        if (H->member_info[j] < 0) return fail("%s needs a " SLU_API "batch_factor of the filled members first", fn);
-        if (H->member_info[j] > 0) return fail("%s: member %d has an exact zero pivot in column %d", fn, j, H->member_info[j]);
-    }
-    return 0;
-}
-
-// the batch_schur_* calls (on a batched handle: refuse_unbatched first)
-static int refuse_not_batch_schur(const slu_b200_handle_s *H, const char *fn)
-{
-    return H->nschur ? 0 : fail("%s needs a batched Schur handle (" SLU_API "batch_schur_create)", fn);
-}
 
 // the checks of batch_create and batch_schur_create (fn) before create_impl
 static int batch_create_check(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, int batch, const char *fn)
@@ -2305,38 +2347,7 @@ int slu_b200_batch_create(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, 
 int slu_b200_batch_fill_csr(slu_b200_handle_t H, int n, const int32_t *rowptr, const int32_t *colind, const double *val,
                             const int32_t *perm)
 {
-    if (!H || !rowptr || !colind || !val || !perm) return fail("null argument");
-    if (refuse_unbatched(H, SLU_API "batch_fill_csr")) return -1;
-    if (n != H->n) return fail("matrix order %d does not match the handle's %d", n, H->n);
-    double t0 = now_s();
-    const int B = H->batch;
-    const int64_t nnz = rowptr[n];
-    DevBuf<int32_t> drp, dci, dperm;
-    DevBuf<val_t> dv;
-    DevBuf<int8_t> dact;
-    std::vector<int8_t> act(H->nsupers, 0);
-    for (int k : H->znodes[0]) act[k] = 1;
-    if (drp.alloc((size_t)n + 1) || dci.alloc((size_t)nnz) || dv.alloc((size_t)nnz * B) || dperm.alloc((size_t)n) || dact.upload(act)) return -1;
-    cudaStream_t s = H->stream;
-    int *err = H->d_flags.p + B;
-    CU(cudaMemcpyAsync(drp.p, rowptr, ((size_t)n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(dci.p, colind, (size_t)nnz * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(dv.p, val, (size_t)nnz * B * sizeof(val_t), cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(dperm.p, perm, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    H->si_ready = false;
-    drop_scaling(H);
-    CU(cudaMemsetAsync(H->val.p, 0, H->val.bytes(), s));
-    CU(cudaMemsetAsync(err, 0, sizeof(int), s));
-    launch_fill_csr(H->bdev, n, drp.p, dci.p, dv.p, dperm.p, dact.p, err, s);
-    int bad = 0;
-    CU(cudaMemcpyAsync(&bad, err, sizeof(int), cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    CU(cudaGetLastError());
-    if (bad) return fail("%d entries of the members have no slot in the L/U structure (wrong permutation or symbolic structure)", bad);
-    H->st.t_upload_s = now_s() - t0;
-    H->uploaded = true;
-    H->member_info.assign(B, -1);
-    return 0;
+    return fill_csr_impl(H, true, n, rowptr, colind, val, perm, SLU_API "batch_fill_csr");
 }
 
 // factor_impl's level loop on a 1 x 1 x 1 grid, every launch over all members (look-ahead streams and events as there:
@@ -2344,9 +2355,8 @@ int slu_b200_batch_fill_csr(slu_b200_handle_t H, int n, const int32_t *rowptr, c
 int slu_b200_batch_factor(slu_b200_handle_t H, int *info)
 {
     if (!H || !info) return fail("null argument");
-    if (refuse_unbatched(H, SLU_API "batch_factor")) return -1;
-    if (!H->uploaded) return fail(SLU_API "batch_factor before " SLU_API "batch_fill_csr");
-    H->si_ready = false;
+    if (check(H, SLU_API "batch_factor", BATCHED | UPLOADED)) return -1;
+    factors_replaced(H);
     const int B = H->batch;
     cudaStream_t s = H->stream, s2 = H->stream2;
     const BatchedLU &d = H->bdev;
@@ -2362,14 +2372,10 @@ int slu_b200_batch_factor(slu_b200_handle_t H, int *info)
     CU(cudaEventRecord(H->ev0, s));
     for (size_t li = 0; li < H->levels.size(); ++li) {
         const LevelPlan &L = H->levels[li];
-        const int32_t *nodes = H->d_pool_i32.p + L.nodes_off, *bign = H->d_pool_i32.p + L.big_nodes;
+        const int32_t *bign = H->d_pool_i32.p + L.big_nodes;
         const Batch small{H->d_pool_i32.p + L.small_nodes, p64 + L.small_prefix, L.small_count};
         if (lookahead && li >= 2) CU(cudaStreamWaitEvent(s, H->ev_bulk[li - 2], 0));
-        launches += launch_diag_lu(d, Batch{nodes, p64 + L.trsml_prefix, L.count}, L.max_ns, replace_tiny, H->opt.thresh, s);
-        launches += launch_diag_inv(d, Batch{nodes, p64 + L.inv_prefix, L.count}, L.inv_ctas, H->d_inv.p, s);
-        launches += launch_trsm_l(d, Batch{nodes, p64 + L.trsml_prefix, L.count}, L.trsml_ctas, L.max_ns, H->d_inv.p, s);
-        launches += launch_trsm_u(d, Batch{nodes, p64 + L.trsmu_prefix, L.count}, L.trsmu_ctas, L.max_ns, H->d_inv.p, s);
-        launches += launch_schur_setup(H->dev, Batch{nodes, p64 + L.setup_prefix, L.count}, L.setup_ctas, s);
+        launches += panel_work(H, d, L, replace_tiny, s);
         if (lookahead) {
             CU(cudaEventRecord(H->ev_panel[li], s));
             launches += launch_schur(d, Batch{bign, p64 + L.urg_prefix, L.big_count}, L.urg_ctas, 1, 1, s);
@@ -2403,75 +2409,20 @@ int slu_b200_batch_factor(slu_b200_handle_t H, int *info)
     return 0;
 }
 
-// The passes of a batched solve: both for a solve; on a batched Schur handle the forward one alone is batch_schur_condense,
-// the backward one batch_schur_expand.
-enum { PASS_FORWARD = 1, PASS_BACKWARD = 2, PASS_BOTH = 3 };
-
-// The solve of a batched handle on device vectors, in place in d_x (batch blocks of n x nrhs).  Enqueued on H->stream, not
-// synchronised.  Returns the kernel launches.
-static int batch_solve_dev(slu_b200_handle_t H, int nrhs, int trans, int passes = PASS_BOTH)
-{
-    const BatchedLU &d = H->bdev;
-    val_t *x = H->d_x.p;
-    int launches = 0;
-    if (passes & PASS_FORWARD)
-        for (size_t li = 0; li < H->levels.size(); ++li)        // forward: L y = b (U^T y = b)
-            launches += solve_level(H, d, H->levels[li], false, trans, x, H->n, nrhs, H->stream);
-    if (passes & PASS_BACKWARD)
-        for (size_t li = H->levels.size(); li-- > 0;)           // backward: U x = y (L^T x = y)
-            launches += solve_level(H, d, H->levels[li], true, trans, x, H->n, nrhs, H->stream);
-    return launches;
-}
-
-// x: batch blocks, block j at x + j * ldx * nrhs, each n x nrhs column-major (ldx >= n): b on entry, the solution on return.
-// trans as solve_impl; fn: "batch_solve", "batch_solve_trans", "batch_schur_condense" or "batch_schur_expand", for the
-// messages.  passes = PASS_BOTH (a solve) needs complete factors, a single pass a batched Schur handle.
-static int batch_solve_impl(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int trans, const char *fn, int passes = PASS_BOTH)
-{
-    if (!H || !xh) return fail("null argument");
-    const std::string name = std::string(SLU_API) + fn;
-    if (refuse_unbatched(H, name.c_str())) return -1;
-    if (passes == PASS_BOTH ? refuse_schur(H, name.c_str()) : refuse_not_batch_schur(H, name.c_str())) return -1;
-    if (trans < 0 || trans > 2) return fail(SLU_API "%s: trans = %d, must be 0 (A x = b), 1 (A^T x = b) or 2 (A^H x = b)", fn, trans);
-    const int B = H->batch, n = H->n;
-    for (int j = 0; j < B; ++j) {
-        if (H->member_info[j] < 0) return fail(SLU_API "%s needs a " SLU_API "batch_factor of the filled members first", fn);
-        if (H->member_info[j] > 0) return fail(SLU_API "%s: member %d has an exact zero pivot in column %d", fn, j, H->member_info[j]);
-    }
-    if (nrhs < 1 || ldx < n) return fail("bad nrhs / ldx");
-    if ((int64_t)n * nrhs > INT_MAX) return fail(SLU_API "%s: n * nrhs must stay below 2^31 per member", fn);
-    const size_t len = (size_t)n * nrhs * B;
-    if (H->d_x.n < len && H->d_x.alloc(len)) return -1;
-    cudaStream_t s = H->stream;
-    val_t *x = H->d_x.p;
-    double t0 = now_s();
-    // the B blocks are B * nrhs columns at pitch ldx: one 2D copy each way
-    CU(cudaMemcpy2DAsync(x, (size_t)n * sizeof(val_t), xh, (size_t)ldx * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs * B,
-                         cudaMemcpyHostToDevice, s));
-    const int launches = batch_solve_dev(H, nrhs, trans, passes);
-    CU(cudaMemcpy2DAsync(xh, (size_t)ldx * sizeof(val_t), x, (size_t)n * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs * B,
-                         cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    CU(cudaGetLastError());
-    H->st.reserved[4] = now_s() - t0;
-    H->st.reserved[5] = (double)launches;
-    return 0;
-}
-
 int slu_b200_batch_solve(slu_b200_handle_t H, double *xh, int ldx, int nrhs)
 {
-    return batch_solve_impl(H, xh, ldx, nrhs, 0, "batch_solve");
+    return solve_host(H, SLU_API "batch_solve", BATCHED | NOT_SCHUR | FACTORED, xh, ldx, nrhs, 0, PASS_BOTH);
 }
 
 int slu_b200_batch_solve_trans(slu_b200_handle_t H, double *xh, int ldx, int nrhs, int trans)
 {
-    return batch_solve_impl(H, xh, ldx, nrhs, trans, "batch_solve_trans");
+    return solve_host(H, SLU_API "batch_solve_trans", BATCHED | NOT_SCHUR | FACTORED, xh, ldx, nrhs, trans, PASS_BOTH);
 }
 
 // ---- condition estimation on the resident factors (LAPACK dgecon / zgecon, sequential SuperLU dgscon / zgscon) --------
 // dlacn2 / zlacn2 estimate ||B||_1 for B = F^-1 (norm '1') or B = F^-T / F^-H (norm 'I'), F = P A P^T, by reverse
 // communication: "kase 1" asks for B x, "kase 2" for B^T x (B^H x).  Each round here is one solve of every member on
-// device vectors (solve_dev / batch_solve_dev, exactly the launches of a solve) and the step kernels of slu_cond.cu; the
+// device vectors (solve_dev / solve_passes, exactly the launches of a solve) and the step kernels of slu_cond.cu; the
 // host only reads back how many members wait for kase 1 and for kase 2.  The next round takes the kase other than the
 // last one if any member waits for it, else the same one: with one member these are exactly dlacn2's solves, and in a
 // batch no member waits more than one round.
@@ -2543,7 +2494,7 @@ static int gscon_impl(slu_b200_handle_t H, char norm, const double *anorm, doubl
             *x = H->d_x.p;
             if (!batched) return solve_dev(H, 1, trans, x) < 0 ? -1 : 0;
             CU(cudaMemcpyAsync(*x, v, len * sizeof(val_t), cudaMemcpyDeviceToDevice, s));
-            batch_solve_dev(H, 1, trans);
+            solve_passes(H, H->bdev, 1, trans);
             return 0;
         };
         if (cond_rounds(H, n, B, v, apply, &rounds, fn)) return -1;
@@ -2561,21 +2512,14 @@ static int gscon_impl(slu_b200_handle_t H, char norm, const double *anorm, doubl
 int slu_b200_gscon(slu_b200_handle_t H, char norm, double anorm, double *rcond)
 {
     if (!H || !rcond) return fail("null argument");
-    if (refuse_batched(H, SLU_API "gscon") || refuse_schur(H, SLU_API "gscon")) return -1;
-    if (!H->factored) return fail(SLU_API "gscon needs a successful " SLU_API "factor on this handle first");
-    if (H->P2 > 1) return fail(SLU_API "gscon: Pr x Pc > 1 is not supported yet (1 x 1 x Pz only)");
-    if (H->comm && !H->coop) return fail(SLU_API "gscon: the Z-distributed solve needs the cooperative schedule (options.reserved[1] = 0)");
+    if (check(H, SLU_API "gscon", UNBATCHED | NOT_SCHUR | GRID_SOLVE | FACTORED)) return -1;
     return gscon_impl(H, norm, &anorm, rcond, SLU_API "gscon");
 }
 
 int slu_b200_batch_gscon(slu_b200_handle_t H, char norm, const double *anorm, double *rcond)
 {
     if (!H || !anorm || !rcond) return fail("null argument");
-    if (refuse_unbatched(H, SLU_API "batch_gscon") || refuse_schur(H, SLU_API "batch_gscon")) return -1;
-    for (int j = 0; j < H->batch; ++j) {
-        if (H->member_info[j] < 0) return fail(SLU_API "batch_gscon needs a " SLU_API "batch_factor of the filled members first");
-        if (H->member_info[j] > 0) return fail(SLU_API "batch_gscon: member %d has an exact zero pivot in column %d", j, H->member_info[j]);
-    }
+    if (check(H, SLU_API "batch_gscon", BATCHED | NOT_SCHUR | FACTORED)) return -1;
     return gscon_impl(H, norm, anorm, rcond, SLU_API "batch_gscon");
 }
 
@@ -2583,7 +2527,7 @@ int slu_b200_batch_gscon(slu_b200_handle_t H, char norm, const double *anorm, do
 int slu_b200_batch_download(slu_b200_handle_t H, int member)
 {
     if (!H) return fail("null handle");
-    if (refuse_unbatched(H, SLU_API "batch_download")) return -1;
+    if (check(H, SLU_API "batch_download", BATCHED)) return -1;
     if (member < 0 || member >= H->batch) return fail(SLU_API "batch_download: member %d out of range (batch of %d)", member, H->batch);
     double t0 = now_s();
     if (transfer(H, false, member)) return -1;
@@ -2594,73 +2538,22 @@ int slu_b200_batch_download(slu_b200_handle_t H, int member)
 // ---- selected inversion and log-determinants on batched handles: selinv_sweep over H->bdev, so the sweep makes exactly the
 // launches of one unbatched sweep, each over every member (gridDim.y = member).  The H arena holds `batch` member arenas,
 // member_len elements apart as the members' factors are.
-static int batch_selinv_refuse(const slu_b200_handle_s *H, const char *fn)
-{
-    if (refuse_unbatched(H, fn) || refuse_schur(H, fn)) return -1;
-    return refuse_unfactored_members(H, fn);
-}
-
 int slu_b200_batch_selinv(slu_b200_handle_t H, double out[4])
 {
     if (!H) return fail("null handle");
-    if (batch_selinv_refuse(H, SLU_API "batch_selinv")) return -1;
+    if (check(H, SLU_API "batch_selinv", BATCHED | NOT_SCHUR | FACTORED)) return -1;
     return selinv_sweep(H, H->bdev, H->batch, SLU_API "batch_selinv", out);
 }
 
-// out: batch x nnz values, member j's at out + j * nnz
 int slu_b200_batch_selinv_get(slu_b200_handle_t H, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm,
                               double *out)
 {
-    if (!H || !rowptr || !colind || !perm || !out) return fail("null argument");
-    if (batch_selinv_refuse(H, SLU_API "batch_selinv_get")) return -1;
-    if (!H->si_ready)
-        return fail(SLU_API "batch_selinv_get needs " SLU_API "batch_selinv on the current factors first (a later batch_fill_csr or "
-                    "batch_factor invalidates it)");
-    if (n != H->n) return fail(SLU_API "batch_selinv_get: matrix order %d does not match the handle's %d", n, H->n);
-    const int64_t nnz = rowptr[n];
-    if (rowptr[0] != 0 || nnz < 0) return fail(SLU_API "batch_selinv_get: bad rowptr");
-    const int B = H->batch;
-    DevBuf<int32_t> drp, dci, dperm;
-    DevBuf<val_t> dout;
-    if (drp.alloc((size_t)n + 1) || dci.alloc((size_t)nnz) || dperm.alloc((size_t)n) || dout.alloc((size_t)nnz * B)) return -1;
-    cudaStream_t s = H->stream;
-    CU(cudaMemcpyAsync(drp.p, rowptr, ((size_t)n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(dci.p, colind, (size_t)nnz * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(dperm.p, perm, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    CU(cudaMemsetAsync(H->dev.err, 0, sizeof(int), s));
-    launch_selinv_get(H->bdev, H->d_hinv.p, n, drp.p, dci.p, dperm.p, dout.p, H->dev.err, s);
-    int bad = 0;
-    CU(cudaMemcpyAsync(out, dout.p, (size_t)nnz * B * sizeof(val_t), cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(&bad, H->dev.err, sizeof(int), cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    CU(cudaGetLastError());
-    if (bad) return fail(SLU_API "batch_selinv_get: %d entries have no slot in the L/U structure (A^-1 is known on the pattern of L+U only)", bad);
-    return 0;
+    return selinv_get_impl(H, SLU_API "batch_selinv_get", BATCHED | NOT_SCHUR | FACTORED | SI_READY, n, rowptr, colind, perm, out);
 }
 
-// logabs[batch]; sign[batch] (double) or sign[2 * batch] = exp(i theta_j) as (re, im) pairs (doublecomplex)
 int slu_b200_batch_logdet(slu_b200_handle_t H, double *logabs, double *sign)
 {
-    if (!H || !logabs || !sign) return fail("null argument");
-    if (batch_selinv_refuse(H, SLU_API "batch_logdet")) return -1;
-    const int B = H->batch;
-    const int count = (int)H->znodes[0].size();
-    const int nparts = (count + SELINV_VECS - 1) / SELINV_VECS;
-    DevBuf<double> part, res;
-    DevBuf<phase_t> ph;
-    if (part.alloc((size_t)nparts * B) || ph.alloc((size_t)nparts * B) || res.alloc((size_t)(1 + VAL_DOUBLES) * B)) return -1;
-    cudaStream_t s = H->stream;
-    launch_selinv_logdet(H->bdev, H->d_pool_i32.p + H->z_nodes_off[0], count, part.p, ph.p, res.p, s);
-    std::vector<double> r((size_t)(1 + VAL_DOUBLES) * B, 0.0);
-    for (int j = 0; j < B; ++j) r[(size_t)j * (1 + VAL_DOUBLES) + 1] = 1.0;   // no supernode: log |det| 0, sign 1
-    if (nparts > 0) CU(cudaMemcpyAsync(r.data(), res.p, r.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    CU(cudaGetLastError());
-    for (int j = 0; j < B; ++j) {
-        logabs[j] = r[(size_t)j * (1 + VAL_DOUBLES)];
-        for (int c = 0; c < VAL_DOUBLES; ++c) sign[(size_t)j * VAL_DOUBLES + c] = r[(size_t)j * (1 + VAL_DOUBLES) + 1 + c];
-    }
-    return 0;
+    return logdet_impl(H, SLU_API "batch_logdet", BATCHED | NOT_SCHUR | FACTORED, logabs, sign);
 }
 
 // ---- inertia from the signs of the pivots (slu_b200_inertia, slu_b200_batch_inertia) --------------------------------------
@@ -2697,14 +2590,14 @@ extern "C" {
 int slu_b200_inertia(slu_b200_handle_t H, int64_t counts[3], double *defect)
 {
     if (!H || !counts || !defect) return fail("null argument");
-    if (selinv_refuse(H, SLU_API "inertia")) return -1;
+    if (check(H, SLU_API "inertia", UNBATCHED | NOT_SCHUR | GRID_1 | FACTORED)) return -1;
     return inertia_impl(H, H->dev, 1, counts, defect);
 }
 
 int slu_b200_batch_inertia(slu_b200_handle_t H, int64_t *counts, double *defect)
 {
     if (!H || !counts || !defect) return fail("null argument");
-    if (batch_selinv_refuse(H, SLU_API "batch_inertia")) return -1;
+    if (check(H, SLU_API "batch_inertia", BATCHED | NOT_SCHUR | FACTORED)) return -1;
     return inertia_impl(H, H->bdev, H->batch, counts, defect);
 }
 
@@ -2717,7 +2610,7 @@ int slu_b200_batch_fill_affine(slu_b200_handle_t H, int n, const int32_t *rowptr
 {
     if (!H || !rowptr || !colind || !terms || !coef || !perm) return fail("null argument");
     const char *fn = SLU_API "batch_fill_affine";
-    if (refuse_unbatched(H, fn)) return -1;
+    if (check(H, fn, BATCHED)) return -1;
     if (n != H->n) return fail("%s: matrix order %d does not match the handle's %d", fn, n, H->n);
     if (nterms < 1) return fail("%s: nterms = %d, must be at least 1", fn, nterms);
     if (rowptr[0] != 0) return fail("%s: bad rowptr (rowptr[0] = %d, must be 0)", fn, rowptr[0]);
@@ -2744,8 +2637,7 @@ int slu_b200_batch_fill_affine(slu_b200_handle_t H, int n, const int32_t *rowptr
     CU(cudaMemcpyAsync(dperm.p, perm, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(dterms.p, terms, (size_t)nnz * nterms * sizeof(val_t), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(dcoef.p, coef, (size_t)B * nterms * sizeof(val_t), cudaMemcpyHostToDevice, s));
-    H->si_ready = false;
-    drop_scaling(H);
+    values_replaced(H);
     CU(cudaMemsetAsync(H->val.p, 0, H->val.bytes(), s));
     CU(cudaMemsetAsync(err, 0, sizeof(int), s));
     launch_fill_affine(H->bdev, n, drp.p, dci.p, dperm.p, dact.p, ddst.p, nnz, nterms, dterms.p, dcoef.p, err, s);
@@ -2753,10 +2645,9 @@ int slu_b200_batch_fill_affine(slu_b200_handle_t H, int n, const int32_t *rowptr
     CU(cudaMemcpyAsync(&bad, err, sizeof(int), cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     CU(cudaGetLastError());
-    H->member_info.assign(B, -1);   // the arena was zeroed: no member has factors now
-    H->uploaded = !bad;
     if (bad) return fail("%s: %d entries of the pattern have no slot in the L/U structure (wrong permutation or symbolic structure)", fn, bad);
     H->st.t_upload_s = now_s() - t0;
+    H->uploaded = true;
     return 0;
 }
 
@@ -2780,16 +2671,8 @@ static int check_scale(const double *v, int64_t len, const char *fn, const char 
     return 0;
 }
 
-// the checks shared by the scaled calls: the handle kind (batched or not), no Schur handle, a 1 x 1 x 1 grid
-static int refuse_scaled(const slu_b200_handle_s *H, bool batched, const char *fn)
-{
-    if (batched ? refuse_unbatched(H, fn) : refuse_batched(H, fn)) return -1;
-    if (refuse_schur(H, fn)) return -1;
-    if (H->view.nprow * H->view.npcol * H->view.npdep != 1 || H->opt.world_size > 1)
-        return fail("%s needs a 1 x 1 x 1 grid with world_size 1 (got %d x %d x %d, world_size %d)", fn, H->view.nprow, H->view.npcol,
-                    H->view.npdep, H->opt.world_size);
-    return 0;
-}
+// what every scaled call needs of the handle: the kind its name says, no Schur handle, a 1 x 1 x 1 grid
+static unsigned scaled_need(bool batched) { return (batched ? BATCHED : UNBATCHED) | NOT_SCHUR | GRID_1; }
 
 // batched: every member's values (val: members x nnz), R / C shared (rc_per_member = 0) or per member; out: members x 6
 static int fill_scaled_impl(slu_b200_handle_t H, bool batched, int n, const int32_t *rowptr, const int32_t *colind, const double *val,
@@ -2797,7 +2680,7 @@ static int fill_scaled_impl(slu_b200_handle_t H, bool batched, int n, const int3
                             double *out, const char *fn)
 {
     if (!H || !rowptr || !colind || !val || !perm) return fail("null argument");
-    if (refuse_scaled(H, batched, fn)) return -1;
+    if (check(H, fn, scaled_need(batched))) return -1;
     if (n != H->n) return fail("%s: matrix order %d does not match the handle's %d", fn, n, H->n);
     if (flags & ~SLU_B200_FILL_EQUIL) return fail("%s: unknown flags 0x%x", fn, flags);
     if (rc_per_member != 0 && rc_per_member != 1) return fail("%s: rc_per_member = %d, must be 0 or 1", fn, rc_per_member);
@@ -2812,6 +2695,7 @@ static int fill_scaled_impl(slu_b200_handle_t H, bool batched, int n, const int3
     const int B = batched ? H->batch : 1;
     const int64_t rc_len = (int64_t)n * (rc_per_member ? B : 1);
     if ((R && check_scale(R, rc_len, fn, "R")) || (C && check_scale(C, rc_len, fn, "C"))) return -1;
+    values_replaced(H, true);   // before the buffers of the scaling and the kept A are resized
     const bool equil = flags & SLU_B200_FILL_EQUIL;
     double t0 = now_s();
     std::vector<int32_t> pr(n), rmap(n);
@@ -2845,11 +2729,6 @@ static int fill_scaled_impl(slu_b200_handle_t H, bool batched, int n, const int3
     if (H->d_perm_r.n != (size_t)n && (H->d_perm_r.alloc(n) || H->d_rmap.alloc(n) || H->d_cperm.alloc(n))) return -1;
     cudaStream_t s = H->stream;
     int *err = H->d_flags.p + (batched ? B : 1);
-    H->si_ready = false;
-    H->scaled = false;
-    H->uploaded = false;
-    H->factored = false;
-    if (batched) H->member_info.assign(B, -1);
     CU(cudaMemcpyAsync(drp.p, rowptr, ((size_t)n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(dci.p, colind, (size_t)nnz * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(dv.p, val, (size_t)nnz * B * sizeof(val_t), cudaMemcpyHostToDevice, s));
@@ -2902,8 +2781,7 @@ static int fill_scaled_impl(slu_b200_handle_t H, bool batched, int n, const int3
 static int get_scaling_impl(slu_b200_handle_t H, bool batched, int member, int32_t *perm_r, double *R, double *C, const char *fn)
 {
     if (!H) return fail("null handle");
-    if (refuse_scaled(H, batched, fn)) return -1;
-    if (!H->scaled) return fail("%s needs a scaled fill on this handle first (a later upload, fill_csr, batch_fill_csr or batch_fill_affine drops the scaling)", fn);
+    if (check(H, fn, scaled_need(batched) | SCALED)) return -1;
     if (batched && (member < 0 || member >= H->batch)) return fail("%s: member %d is outside 0 ... %d", fn, member, H->batch - 1);
     const size_t n = (size_t)H->n, off = (size_t)member * n;
     if (perm_r) CU(cudaMemcpy(perm_r, H->d_perm_r.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost));
@@ -2929,7 +2807,7 @@ static int solve_scaled_dev(slu_b200_handle_t H, bool batched, int nrhs, int tra
     int launches = launch_permute_scale(b, in, trans ? H->d_cperm.p : H->d_rmap.p, trans ? H->d_C.p : H->d_R.p, n, nrhs, B, true, s);
     val_t *y = H->d_x.p;
     if (batched) {
-        launches += batch_solve_dev(H, nrhs, trans);
+        launches += solve_passes(H, H->bdev, nrhs, trans);
     } else {
         const int l = solve_dev(H, nrhs, trans, &y);
         if (l < 0) return -1;
@@ -2942,16 +2820,10 @@ static int solve_scaled_dev(slu_b200_handle_t H, bool batched, int nrhs, int tra
 static int solve_scaled_impl(slu_b200_handle_t H, bool batched, double *xh, int ldx, int nrhs, int trans, const char *fn)
 {
     if (!H || !xh) return fail("null argument");
-    if (refuse_scaled(H, batched, fn)) return -1;
+    if (check(H, fn, scaled_need(batched) | SCALED | FACTORED)) return -1;
     if (trans < 0 || trans > 2) return fail("%s: trans = %d, must be 0 (A x = b), 1 (A^T x = b) or 2 (A^H x = b)", fn, trans);
-    if (!H->scaled) return fail("%s needs a scaled fill on this handle first (a later upload, fill_csr, batch_fill_csr or batch_fill_affine drops the scaling)", fn);
     const int B = batched ? H->batch : 1, n = H->n;
-    if (batched) {
-        if (refuse_unfactored_members(H, fn)) return -1;
-    } else if (!H->factored) {
-        return fail("%s needs a successful " SLU_API "factor after the scaled fill", fn);
-    }
-    if (nrhs < 1 || ldx < n) return fail("bad nrhs / ldx");
+    if (nrhs < 1 || ldx < n) return fail("%s: bad nrhs / ldx", fn);
     if ((int64_t)n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
     const size_t len = (size_t)n * nrhs * B;
     if (H->d_x.n < len && H->d_x.alloc(len)) return -1;
@@ -3014,15 +2886,7 @@ static int gsrfs_impl(slu_b200_handle_t H, bool batched, const double *bh, int l
                       double *ferr, int32_t *steps, const char *fn)
 {
     if (!H || !bh || !xh || !berr) return fail("%s: null argument (b, x and berr are required)", fn);
-    if (refuse_scaled(H, batched, fn)) return -1;
-    if (!H->scaled)
-        return fail("%s needs a scaled fill on this handle first (a later upload, fill_csr, batch_fill_csr or batch_fill_affine drops "
-                    "the scaling and the kept A)", fn);
-    if (batched) {
-        if (refuse_unfactored_members(H, fn)) return -1;
-    } else if (!H->factored) {
-        return fail("%s needs a successful " SLU_API "factor after the scaled fill", fn);
-    }
+    if (check(H, fn, scaled_need(batched) | SCALED | FACTORED)) return -1;
     const int B = batched ? H->batch : 1, n = H->n;
     if (nrhs < 1) return fail("%s: nrhs = %d, must be >= 1", fn, nrhs);
     if (ldb < n || ldx < n) return fail("%s: ldb = %d and ldx = %d must be >= n = %d", fn, ldb, ldx, n);
@@ -3115,7 +2979,7 @@ int slu_b200_batch_gsrfs(slu_b200_handle_t H, const double *b, int ldb, double *
 
 // ---- partial factorization on batched handles: a batched handle whose level plan leaves out the Schur supernodes, as an
 // unbatched Schur handle's does.  batch_factor eliminates A11 of every member, the gather runs over (units, members), and
-// condense / expand are the forward / backward pass of batch_solve_impl over the same plan.
+// condense / expand are the forward / backward pass of solve_host over the same plan.
 int slu_b200_batch_schur_create(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, int batch,
                                 int nschur)
 {
@@ -3132,18 +2996,18 @@ int slu_b200_batch_schur_get(slu_b200_handle_t H, double *S, int lds)
 {
     if (!H || !S) return fail("null argument");
     const char *fn = SLU_API "batch_schur_get";
-    if (refuse_unbatched(H, fn) || refuse_not_batch_schur(H, fn) || refuse_unfactored_members(H, fn)) return -1;
+    if (check(H, fn, BATCHED | SCHUR | FACTORED)) return -1;
     return schur_get_impl(H, S, lds, fn);
 }
 
 int slu_b200_batch_schur_condense(slu_b200_handle_t H, double *x, int ldx, int nrhs)
 {
-    return batch_solve_impl(H, x, ldx, nrhs, 0, "batch_schur_condense", PASS_FORWARD);
+    return solve_host(H, SLU_API "batch_schur_condense", BATCHED | SCHUR | FACTORED, x, ldx, nrhs, 0, PASS_FORWARD);
 }
 
 int slu_b200_batch_schur_expand(slu_b200_handle_t H, double *x, int ldx, int nrhs)
 {
-    return batch_solve_impl(H, x, ldx, nrhs, 0, "batch_schur_expand", PASS_BACKWARD);
+    return solve_host(H, SLU_API "batch_schur_expand", BATCHED | SCHUR | FACTORED, x, ldx, nrhs, 0, PASS_BACKWARD);
 }
 
 int slu_b200_get_stats(slu_b200_handle_t H, slu_b200_stats_t *out)
