@@ -464,6 +464,36 @@ int slu_b200_gsrfs(slu_b200_handle_t h, const double *b, int ldb, double *x, int
                    int32_t *steps);
 int slu_b200_batch_gsrfs(slu_b200_handle_t h, const double *b, int ldb, double *x, int ldx, int nrhs, double *berr,
                          double *ferr, int32_t *steps);
+/* ---- device-resident refill and solves on the caller's CUDA stream: the loop of pdgssvx3d's Fact = SamePattern_SameRowPerm
+ * (Newton and time-stepping loops, parameter and shift sweeps) for values and right-hand sides that are already on the GPU.
+ * stream: a cudaStream_t passed as void* (NULL = the legacy default stream).  val and x must be device or managed memory on
+ * the handle's device (checked with cudaPointerGetAttributes before anything is enqueued; host memory or another device's
+ * memory is refused, naming the argument); keeping x + ldx * nrhs (* batch) in bounds is the caller's job.  Each call makes
+ * the handle's stream wait for the work already on `stream` before it reads val or x, and `stream` wait for the handle's
+ * work before it returns, with events: the caller may overwrite or free val and read x in `stream` order right after the
+ * call.  No host synchronisation and no PCIe copy, except where a buffer grows (a larger nrhs) and in the first refill after
+ * each scaled fill, which builds the slot map and waits for it.  stats.reserved[5] = the call's kernel launches;
+ * stats.reserved[4] (and t_upload_s for a refill) = 0: no host clock measures work that is not waited for.
+ * refill: new values of the pattern of the handle's last successful scaled fill (fill_csr_scaled, batch_fill_csr_scaled),
+ * val: nnz values in that fill's CSR entry order (batch x nnz, member-major, on a batched handle).  The arena is zeroed and
+ * F = Pc Pr Dr A Dc Pc^T written with the kept perm_r, perm, R and C: (R[i] * a_ij) * C[j], one plain store per slot, bit
+ * for bit what fill_csr_scaled writes with the same R and C and no EQUIL.  The equilibration is not redone (R and C stay
+ * those of the scaled fill, per member).  val also replaces the kept A, so gsrfs refines against the new matrix.  The
+ * first refill after a scaled fill builds the slot map: 8 bytes per entry for the arena offset and 4 for the row, shared by
+ * the members, dropped with the scaling.  Then 1 launch: thread = entry, no search.  After it the handle has values and
+ * its scaling and no factors: factor / batch_factor follow, on the handle's stream after the refill.  Fails with a message,
+ * leaving the handle as it was, without a scaled fill (or after a later upload or plain fill, which drop it), on Schur
+ * handles and on grids other than 1 x 1 x 1 with world_size 1.
+ * solve_device / solve_scaled_device: slu_b200_solve and _solve_trans (trans 0, 1 or 2, F's ordering) and
+ * slu_b200_solve_scaled (A's ordering) on device x, with their layout, ldx / nrhs checks (n * nrhs < 2^31) and state
+ * checks; the same device work, with device-to-device 2D copies in place of the H2D and D2H ones.  1 x 1 x 1 grids only.
+ * The batched twins take the batched layout (member j's block at x + j * ldx * nrhs) and check every member's info. */
+int slu_b200_refill(slu_b200_handle_t h, const double *val, void *stream);
+int slu_b200_batch_refill(slu_b200_handle_t h, const double *val, void *stream);
+int slu_b200_solve_device(slu_b200_handle_t h, double *x, int ldx, int nrhs, int trans, void *stream);
+int slu_b200_batch_solve_device(slu_b200_handle_t h, double *x, int ldx, int nrhs, int trans, void *stream);
+int slu_b200_solve_scaled_device(slu_b200_handle_t h, double *x, int ldx, int nrhs, int trans, void *stream);
+int slu_b200_batch_solve_scaled_device(slu_b200_handle_t h, double *x, int ldx, int nrhs, int trans, void *stream);
 /* ---- doublecomplex twins (SRC/complex16/pzgstrf3d.c:120; the reference's z* handle API,
  * SRC/include/superlu_upacked.h:84-97).  Same view/options/stats structs: the Lnzval_bc_ptr / Unzval_br_ptr
  * entries point at arrays of doublecomplex {double r, i} (SRC/include/dcomplex.h:30) and are declared double*
@@ -559,6 +589,14 @@ int slu_b200_z_gsrfs(slu_b200_zhandle_t h, const double *b, int ldb, double *x, 
                      int32_t *steps);
 int slu_b200_z_batch_gsrfs(slu_b200_zhandle_t h, const double *b, int ldb, double *x, int ldx, int nrhs, double *berr,
                            double *ferr, int32_t *steps);
+/* as slu_b200_refill / _solve_device / _solve_scaled_device and their batched twins: val and x point at interleaved
+ * doublecomplex on the device, nnz and ldx count complex elements */
+int slu_b200_z_refill(slu_b200_zhandle_t h, const double *val, void *stream);
+int slu_b200_z_batch_refill(slu_b200_zhandle_t h, const double *val, void *stream);
+int slu_b200_z_solve_device(slu_b200_zhandle_t h, double *x, int ldx, int nrhs, int trans, void *stream);
+int slu_b200_z_batch_solve_device(slu_b200_zhandle_t h, double *x, int ldx, int nrhs, int trans, void *stream);
+int slu_b200_z_solve_scaled_device(slu_b200_zhandle_t h, double *x, int ldx, int nrhs, int trans, void *stream);
+int slu_b200_z_batch_solve_scaled_device(slu_b200_zhandle_t h, double *x, int ldx, int nrhs, int trans, void *stream);
 int slu_b200_z_get_stats(slu_b200_zhandle_t h, slu_b200_stats_t *out);
 int slu_b200_z_plan(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, slu_b200_stats_t *stats);
 void slu_b200_z_destroy(slu_b200_zhandle_t h);

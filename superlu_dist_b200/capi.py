@@ -6,6 +6,7 @@ compute entry point is called, this module raises.
 import ctypes as C
 import os
 import re
+import sys
 
 import numpy as np
 
@@ -161,6 +162,12 @@ def lib():
         getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
     for f in ("slu_b200_gsrfs", "slu_b200_z_gsrfs", "slu_b200_batch_gsrfs", "slu_b200_z_batch_gsrfs"):
         getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 3
+    # device-resident refill and solves on the caller's stream (a cudaStream_t as void*)
+    for f in ("slu_b200_refill", "slu_b200_z_refill", "slu_b200_batch_refill", "slu_b200_z_batch_refill"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    for f in ("solve_device", "batch_solve_device", "solve_scaled_device", "batch_solve_scaled_device"):
+        for pre in ("slu_b200_", "slu_b200_z_"):
+            getattr(L, pre + f).argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
     _lib = L
     return L
 
@@ -230,6 +237,42 @@ def _gsrfs(name, complex_, h, b, x, n, nrhs, cols, ferr):
     fe = np.zeros(cols) if ferr else None
     _check(_fn(name, complex_)(h, _ptr(b), n, _ptr(x), n, nrhs, _ptr(berr), _ptr(fe), _ptr(steps)))
     return berr, steps, fe
+
+
+def _is_tensor(a):
+    """a torch tensor?  Without importing torch: a program that never imported it has none."""
+    torch = sys.modules.get("torch")
+    return torch is not None and isinstance(a, torch.Tensor)
+
+
+def _device_args(t, complex_, shape, what):
+    """A torch CUDA tensor of `shape` (None: any) -> (contiguous tensor of the handle's dtype, the raw cudaStream_t of the current stream
+    of its device)"""
+    import torch
+    if not t.is_cuda:
+        raise ValueError(f"{what} must be a CUDA tensor (numpy arrays take the host path)")
+    dt = torch.complex128 if complex_ else torch.float64
+    if t.dtype != dt:
+        raise ValueError(f"{what} must be {dt} for this handle, not {t.dtype}")
+    if shape is not None and tuple(t.shape) not in shape:
+        raise ValueError(f"{what} must have shape {' or '.join(map(str, shape))}, not {tuple(t.shape)}")
+    return t.contiguous(), C.c_void_p(torch.cuda.current_stream(t.device).cuda_stream)
+
+
+def _solve_device(name, complex_, h, b, n, batch, trans):
+    """slu_b200_[z_][batch_]solve[_scaled]_device on a copy of CUDA tensor b: (n,) or (nrhs, n), (batch, n) or (batch, nrhs,
+    n) with batch -> a new tensor of b's shape, ordered on the current stream of b's device"""
+    if trans not in _TRANS:
+        raise ValueError(f"trans must be 'N', 'T' or 'H', not {trans!r}")
+    lead = () if batch is None else (batch,)
+    nd = len(lead) + 1
+    if b.dim() not in (nd, nd + 1) or tuple(b.shape[:len(lead)]) != lead or b.shape[-1] != n:
+        raise ValueError(f"b must have shape {lead + (n,)} or {lead + ('nrhs', n)}, not {tuple(b.shape)}")
+    b, stream = _device_args(b, complex_, None, "b")
+    x = b.clone()
+    nrhs = 1 if b.dim() == nd else b.shape[-2]
+    _check(_fn(name, complex_)(h, C.c_void_p(x.data_ptr()), n, nrhs, _TRANS[trans], stream))
+    return x
 
 
 def device_count():
@@ -399,7 +442,16 @@ class Handle:
         out = np.zeros(6)
         _check(_fn("fill_csr_scaled", self.z_)(self.h, len(rp) - 1, _ptr(rp), _ptr(ci), _ptr(v), _ptr(pr), _ptr(pm), _ptr(Rv),
                                                _ptr(Cv), FILL_EQUIL if equil else 0, _ptr(out)))
+        self._nnz = len(ci)
         return {k: (int(x) if k == "equed" else float(x)) for k, x in zip(_SCALED_OUT, out)}
+
+    def refill(self, val):
+        """New values of the last scaled fill's pattern from the device (slu_b200_refill): val a torch CUDA tensor (nnz,),
+        float64 (complex128 for a complex problem), in that fill's CSR entry order.  F is written with the kept perm_r, perm,
+        R and C (no equilibration), ordered after the work on the current stream of val's device, which waits for it in turn:
+        val may be overwritten right after.  factor() follows as after any fill."""
+        v, stream = _device_args(val, self.z_, [(getattr(self, "_nnz", val.shape[0]),)], "val")
+        _check(_fn("refill", self.z_)(self.h, C.c_void_p(v.data_ptr()), stream))
 
     def scaling(self):
         """(perm_r, R, C) of the last scaled fill, R and C with the equilibration folded in (slu_b200_get_scaling)"""
@@ -410,7 +462,10 @@ class Handle:
 
     def solve_scaled(self, b, trans="N"):
         """op(A) x = b in A's own ordering on the factors of a scaled fill (slu_b200_solve_scaled): the row permutation,
-        the scalings and perm are applied on the device.  b: (n,) or (nrhs, n); trans 'N', 'T' or 'H'."""
+        the scalings and perm are applied on the device.  b: (n,) or (nrhs, n); trans 'N', 'T' or 'H'.  A torch CUDA tensor
+        b is solved on the device, on the current stream of its device (slu_b200_solve_scaled_device): x is a new tensor."""
+        if _is_tensor(b):
+            return _solve_device("solve_scaled_device", self.z_, self.h, b, self.prob.n, None, trans)
         if trans not in _TRANS:
             raise ValueError(f"trans must be 'N', 'T' or 'H', not {trans!r}")
         x = np.array(b, self._dtype(), order="C", copy=True)
@@ -436,7 +491,11 @@ class Handle:
     def solve(self, b, trans="N"):
         """L U x = b on the device-resident factors (slu_b200_solve / slu_b200_z_solve); b: (n,) or (nrhs, n), ordering
         of the factored matrix, complex128 for a complex problem.  Returns x with the same shape and dtype.
-        trans = 'T' solves A^T x = b, 'H' A^H x = b (slu_b200_solve_trans / slu_b200_z_solve_trans) on the same factors."""
+        trans = 'T' solves A^T x = b, 'H' A^H x = b (slu_b200_solve_trans / slu_b200_z_solve_trans) on the same factors.
+        A torch CUDA tensor b is solved on the device, on the current stream of its device (slu_b200_solve_device): x is a
+        new tensor."""
+        if _is_tensor(b):
+            return _solve_device("solve_device", self.z_, self.h, b, self.prob.n, None, trans)
         fn, extra = _solve_call("solve", self.z_, trans)
         x = np.array(b, self._dtype(), order="C", copy=True)
         nrhs = 1 if x.ndim == 1 else x.shape[0]
@@ -593,9 +652,17 @@ class BatchHandle:
         out = np.zeros((B, 6))
         _check(_fn("batch_fill_csr_scaled", self.z_)(self.h, len(rp) - 1, _ptr(rp), _ptr(ci), _ptr(v), _ptr(pr), _ptr(pm), _ptr(Rv),
                                                      _ptr(Cv), int(bool(per and per[0])), FILL_EQUIL if equil else 0, _ptr(out)))
+        self._nnz = len(ci)
         res = {k: out[:, t].copy() for t, k in enumerate(_SCALED_OUT)}
         res["equed"] = res["equed"].astype(np.int32)
         return res
+
+    def refill(self, vals):
+        """Handle.refill for every member (slu_b200_batch_refill): vals a torch CUDA tensor (batch, nnz); each member keeps
+        its own R and C"""
+        nnz = getattr(self, "_nnz", vals.shape[-1])
+        v, stream = _device_args(vals, self.z_, [(self.batch, nnz)], "vals")
+        _check(_fn("batch_refill", self.z_)(self.h, C.c_void_p(v.data_ptr()), stream))
 
     def scaling(self, member):
         """(R, C) of member `member` after the last scaled fill (slu_b200_batch_get_scaling)"""
@@ -606,7 +673,9 @@ class BatchHandle:
 
     def solve_scaled(self, b, trans="N"):
         """Handle.solve_scaled for every member (slu_b200_batch_solve_scaled); b: (batch, n) or (batch, nrhs, n) in A's
-        ordering"""
+        ordering; a torch CUDA tensor on the device (slu_b200_batch_solve_scaled_device)"""
+        if _is_tensor(b):
+            return _solve_device("batch_solve_scaled_device", self.z_, self.h, b, self.prob.n, self.batch, trans)
         if trans not in _TRANS:
             raise ValueError(f"trans must be 'N', 'T' or 'H', not {trans!r}")
         x = np.array(b, self._dtype(), order="C", copy=True)
@@ -636,7 +705,10 @@ class BatchHandle:
 
     def solve(self, b, trans="N"):
         """L_j U_j x_j = b_j for every member; b: (batch, n) or (batch, nrhs, n), ordering of the factored matrix.
-        trans = 'T' / 'H' solves A_j^T x_j = b_j / A_j^H x_j = b_j (slu_b200_batch_solve_trans)."""
+        trans = 'T' / 'H' solves A_j^T x_j = b_j / A_j^H x_j = b_j (slu_b200_batch_solve_trans).  A torch CUDA tensor b is
+        solved on the device (slu_b200_batch_solve_device), as Handle.solve."""
+        if _is_tensor(b):
+            return _solve_device("batch_solve_device", self.z_, self.h, b, self.prob.n, self.batch, trans)
         fn, extra = _solve_call("batch_solve", self.z_, trans)
         x = np.array(b, self._dtype(), order="C", copy=True)
         if x.ndim not in (2, 3) or x.shape[0] != self.batch or x.shape[-1] != self.prob.n:

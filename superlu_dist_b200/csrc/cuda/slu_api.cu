@@ -71,6 +71,12 @@
 #define slu_b200_batch_solve_scaled slu_b200_z_batch_solve_scaled
 #define slu_b200_gsrfs slu_b200_z_gsrfs
 #define slu_b200_batch_gsrfs slu_b200_z_batch_gsrfs
+#define slu_b200_refill slu_b200_z_refill
+#define slu_b200_batch_refill slu_b200_z_batch_refill
+#define slu_b200_solve_device slu_b200_z_solve_device
+#define slu_b200_batch_solve_device slu_b200_z_batch_solve_device
+#define slu_b200_solve_scaled_device slu_b200_z_solve_scaled_device
+#define slu_b200_batch_solve_scaled_device slu_b200_z_batch_solve_scaled_device
 #define SLU_API "slu_b200_z_"     // name prefix of the exported calls, for error messages
 #else
 #define SLU_API "slu_b200_"
@@ -348,6 +354,15 @@ struct slu_b200_handle_s {
     DevBuf<double> d_rw;
     DevBuf<RefineState> d_rst;
     DevBuf<int> d_ract;
+    // refill (slu_b200_refill): the arena offset and the row of every entry of the kept A, built by the first refill after a
+    // scaled fill (amap_ready) and shared by the members; dropped with the scaling
+    DevBuf<int64_t> d_amap;
+    DevBuf<int32_t> d_arow;
+    bool amap_ready = false;
+    // the calls on the caller's stream: the handle's device, and the events that order the handle's stream after the caller's
+    // work (ev_in) and the caller's stream after the handle's (ev_out)
+    int device = 0;
+    cudaEvent_t ev_in = nullptr, ev_out = nullptr;
 };
 
 namespace {
@@ -364,16 +379,20 @@ void factors_replaced(slu_b200_handle_s *H)
 }
 
 // an upload or a fill is about to overwrite the arena: no values to factor either, and the scaling no longer describes
-// them.  The A kept for refinement goes with the scaling, except on a scaled fill (keep_a), which reuses its buffers.
+// them.  The A kept for refinement and the refill's slot map go with the scaling, except on a scaled fill (keep_a), which
+// reuses their buffers (the map is rebuilt by the next refill).
 void values_replaced(slu_b200_handle_s *H, bool keep_a = false)
 {
     factors_replaced(H);
     H->uploaded = false;
     H->scaled = false;
+    H->amap_ready = false;
     if (keep_a) return;
     H->d_arp.release();
     H->d_aci.release();
     H->d_aval.release();
+    H->d_amap.release();
+    H->d_arow.release();
 }
 
 // What a call needs of the handle (check): one bit per condition
@@ -1488,6 +1507,8 @@ void slu_b200_destroy(slu_b200_handle_t H)
     // the NCCL communicators belong to the per-process cache (slu_b200_comm_cache_clear)
     if (H->ev0) cudaEventDestroy(H->ev0);
     if (H->ev1) cudaEventDestroy(H->ev1);
+    if (H->ev_in) cudaEventDestroy(H->ev_in);
+    if (H->ev_out) cudaEventDestroy(H->ev_out);
     if (H->stream) cudaStreamDestroy(H->stream);
     if (H->stream2) cudaStreamDestroy(H->stream2);
     if (H->s_down) cudaStreamDestroy(H->s_down);
@@ -1537,8 +1558,9 @@ static int create_impl(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, con
     if (lu->npdep < 1 || (lu->npdep & (lu->npdep - 1)) || H->P2 < 1) { slu_b200_destroy(H); return fail("bad process grid"); }
     H->max_lvl = 1;
     while ((1 << (H->max_lvl - 1)) < lu->npdep) ++H->max_lvl;
-    if (cudaStreamCreate(&H->stream) != cudaSuccess || cudaEventCreate(&H->ev0) != cudaSuccess ||
-        cudaEventCreate(&H->ev1) != cudaSuccess) {
+    if (cudaGetDevice(&H->device) != cudaSuccess || cudaStreamCreate(&H->stream) != cudaSuccess || cudaEventCreate(&H->ev0) != cudaSuccess ||
+        cudaEventCreate(&H->ev1) != cudaSuccess || cudaEventCreateWithFlags(&H->ev_in, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&H->ev_out, cudaEventDisableTiming) != cudaSuccess) {
         slu_b200_destroy(H);
         return fail("cannot create stream/events");
     }
@@ -2975,6 +2997,135 @@ int slu_b200_batch_gsrfs(slu_b200_handle_t H, const double *b, int ldb, double *
                          int32_t *steps)
 {
     return gsrfs_impl(H, true, b, ldb, x, ldx, nrhs, berr, ferr, steps, SLU_API "batch_gsrfs");
+}
+
+// ---- device-resident refill and solves on the caller's stream (pdgssvx3d's Fact = SamePattern_SameRowPerm for values that
+// already live in HBM).  Every call checks its pointers before it enqueues anything, orders the handle's stream after the
+// work already on the caller's stream, and the caller's stream after its own work, with events: no host wait, no PCIe copy.
+static int check_device_ptr(slu_b200_handle_t H, const void *p, const char *fn, const char *what)
+{
+    cudaPointerAttributes a{};
+    const cudaError_t e = cudaPointerGetAttributes(&a, p);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return fail("%s: %s is not a pointer CUDA knows (%s)", fn, what, cudaGetErrorString(e));
+    }
+    if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged)
+        return fail("%s: %s must point at device or managed memory on device %d, not at %s memory", fn, what, H->device,
+                    a.type == cudaMemoryTypeHost ? "pinned host" : "host");
+    if (a.device != H->device) return fail("%s: %s points at memory of device %d, the handle's device is %d", fn, what, a.device, H->device);
+    return 0;
+}
+
+static int stream_enter(slu_b200_handle_t H, cudaStream_t caller)
+{
+    CU(cudaEventRecord(H->ev_in, caller));
+    CU(cudaStreamWaitEvent(H->stream, H->ev_in, 0));
+    return 0;
+}
+
+static int stream_leave(slu_b200_handle_t H, cudaStream_t caller)
+{
+    CU(cudaEventRecord(H->ev_out, H->stream));
+    CU(cudaStreamWaitEvent(caller, H->ev_out, 0));
+    return 0;
+}
+
+// New values of the last scaled fill's pattern, val on the device (batch x nnz on a batched handle): the arena zeroed, then
+// F = Pc Pr Dr A Dc Pc^T with the kept perm_r, perm, R and C, bit for bit the scaled fill's values; val also replaces the
+// kept A.  The first refill after a scaled fill builds the slot map (allocates, and waits for it once).
+static int refill_impl(slu_b200_handle_t H, bool batched, const double *val, void *stream, const char *fn)
+{
+    if (!H || !val) return fail("%s: null argument", fn);
+    if (check(H, fn, scaled_need(batched) | SCALED)) return -1;
+    if (check_device_ptr(H, val, fn, "val")) return -1;
+    const cudaStream_t caller = (cudaStream_t)stream, s = H->stream;
+    const int n = H->n;
+    const int64_t nnz = (int64_t)H->d_aci.n;
+    int launches = 0;
+    if (!H->amap_ready) {
+        DevBuf<int8_t> act;                       // every panel of a 1 x 1 x 1 grid is held
+        if ((H->d_amap.n != (size_t)nnz && (H->d_amap.alloc(nnz) || H->d_arow.alloc(nnz))) || act.alloc(H->nsupers)) return -1;
+        CU(cudaMemsetAsync(act.p, 1, act.bytes(), s));
+        launches += launch_refill_slots(H->dev, n, H->d_arp.p, H->d_aci.p, H->d_rmap.p, H->d_cperm.p, act.p, H->d_amap.p, H->d_arow.p, s);
+        CU(cudaStreamSynchronize(s));
+        CU(cudaGetLastError());
+        H->amap_ready = true;
+    }
+    factors_replaced(H);
+    H->uploaded = false;
+    if (stream_enter(H, caller)) return -1;
+    CU(cudaMemsetAsync(H->val.p, 0, H->val.bytes(), s));
+    const Refill r{n, nnz, (const val_t *)val, H->d_amap.p, H->d_arow.p, H->d_aci.p, H->d_R.p, H->d_C.p, H->d_aval.p};
+    launches += batched ? launch_refill(H->bdev, r, s) : launch_refill(H->dev, r, s);
+    CU(cudaGetLastError());
+    if (stream_leave(H, caller)) return -1;
+    H->st.t_upload_s = 0;
+    H->st.reserved[4] = 0;
+    H->st.reserved[5] = (double)launches;
+    H->uploaded = true;
+    return 0;
+}
+
+// solve / solve_trans (scaled = false: F's ordering) and solve_scaled (A's ordering) on device x, with the host twins' layout
+// and checks; the same device work, with device-to-device copies in place of the H2D and D2H ones.  1 x 1 x 1 grids.
+static int solve_device_impl(slu_b200_handle_t H, bool batched, bool scaled, double *xd, int ldx, int nrhs, int trans, void *stream,
+                             const char *fn)
+{
+    if (!H || !xd) return fail("%s: null argument", fn);
+    if (check(H, fn, scaled_need(batched) | (scaled ? SCALED : 0) | FACTORED)) return -1;
+    if (trans < 0 || trans > 2) return fail("%s: trans = %d, must be 0 (A x = b), 1 (A^T x = b) or 2 (A^H x = b)", fn, trans);
+    const int B = batched ? H->batch : 1, n = H->n;
+    if (nrhs < 1 || ldx < n) return fail("%s: bad nrhs / ldx", fn);
+    if ((int64_t)n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
+    if (check_device_ptr(H, xd, fn, "x")) return -1;
+    const size_t len = (size_t)n * nrhs * B;
+    if ((H->d_x.n < len && H->d_x.alloc(len)) || ((scaled || !batched) && H->d_x2.n < len && H->d_x2.alloc(len))) return -1;
+    const cudaStream_t caller = (cudaStream_t)stream, s = H->stream;
+    if (stream_enter(H, caller)) return -1;
+    // b goes where each solve takes it: scaled_in, d_x2 for solve_dev, d_x for the batched passes
+    val_t *in = scaled ? scaled_in(H, batched) : batched ? H->d_x.p : H->d_x2.p, *result = scaled ? H->d_x2.p : H->d_x.p;
+    const size_t w = (size_t)n * sizeof(val_t), pitch = (size_t)ldx * sizeof(val_t);
+    CU(cudaMemcpy2DAsync(in, w, xd, pitch, w, (size_t)nrhs * B, cudaMemcpyDeviceToDevice, s));
+    const int launches = scaled ? solve_scaled_dev(H, batched, nrhs, trans)
+                                : batched ? solve_passes(H, H->bdev, nrhs, trans) : solve_dev(H, nrhs, trans, &result);
+    if (launches < 0) return -1;
+    CU(cudaMemcpy2DAsync(xd, pitch, result, w, w, (size_t)nrhs * B, cudaMemcpyDeviceToDevice, s));
+    CU(cudaGetLastError());
+    if (stream_leave(H, caller)) return -1;
+    H->st.reserved[4] = 0;
+    H->st.reserved[5] = (double)launches;
+    return 0;
+}
+
+int slu_b200_refill(slu_b200_handle_t H, const double *val, void *stream)
+{
+    return refill_impl(H, false, val, stream, SLU_API "refill");
+}
+
+int slu_b200_batch_refill(slu_b200_handle_t H, const double *val, void *stream)
+{
+    return refill_impl(H, true, val, stream, SLU_API "batch_refill");
+}
+
+int slu_b200_solve_device(slu_b200_handle_t H, double *x, int ldx, int nrhs, int trans, void *stream)
+{
+    return solve_device_impl(H, false, false, x, ldx, nrhs, trans, stream, SLU_API "solve_device");
+}
+
+int slu_b200_batch_solve_device(slu_b200_handle_t H, double *x, int ldx, int nrhs, int trans, void *stream)
+{
+    return solve_device_impl(H, true, false, x, ldx, nrhs, trans, stream, SLU_API "batch_solve_device");
+}
+
+int slu_b200_solve_scaled_device(slu_b200_handle_t H, double *x, int ldx, int nrhs, int trans, void *stream)
+{
+    return solve_device_impl(H, false, true, x, ldx, nrhs, trans, stream, SLU_API "solve_scaled_device");
+}
+
+int slu_b200_batch_solve_scaled_device(slu_b200_handle_t H, double *x, int ldx, int nrhs, int trans, void *stream)
+{
+    return solve_device_impl(H, true, true, x, ldx, nrhs, trans, stream, SLU_API "batch_solve_scaled_device");
 }
 
 // ---- partial factorization on batched handles: a batched handle whose level plan leaves out the Schur supernodes, as an

@@ -211,6 +211,23 @@ struct ScaledFill {
 // scatter with the norms); else 2 (R and C copied, the scatter).  Over (rows, members).
 int launch_fill_scaled(const DeviceLU &d, const ScaledFill &f, bool equil, cudaStream_t s);
 int launch_fill_scaled(const BatchedLU &d, const ScaledFill &f, bool equil, cudaStream_t s);
+// refill of a scaled fill's pattern with new values (slu_b200_refill and its batched / z twins).  The slot map, once per
+// scaled fill: slot[p] = the arena offset of CSR entry p at (rmap[i], perm[colind[p]]) (-1 without one), row[p] = its row i;
+// 1 launch over rows.  The refill: member j's value a of entry p goes to its arena at slot[p] as (R[i] a) C[j], exactly the
+// value of launch_fill_scaled's scatter, and to aval; 1 launch over (entries, members), no search.
+int launch_refill_slots(const DeviceLU &d, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *rmap, const int32_t *perm,
+                        const int8_t *active, int64_t *slot, int32_t *row, cudaStream_t s);
+struct Refill {
+    int n;
+    int64_t nnz;
+    const val_t *val;                  // members x nnz new values, member-major
+    const int64_t *slot;
+    const int32_t *row, *colind;
+    const double *R, *C;               // members x n: the kept scalings
+    val_t *aval;                       // members x nnz: the kept A, receives val
+};
+int launch_refill(const DeviceLU &d, const Refill &r, cudaStream_t s);
+int launch_refill(const BatchedLU &d, const Refill &r, cudaStream_t s);
 // the vector transforms of slu_b200_solve_scaled, over (entries, members) with members blocks of n x nrhs (scale: n per
 // member): scatter dst[map[i]] = scale[i] src[i], else gather dst[i] = scale[i] src[map[i]]
 int launch_permute_scale(val_t *dst, const val_t *src, const int32_t *map, const double *scale, int n, int nrhs, int members,

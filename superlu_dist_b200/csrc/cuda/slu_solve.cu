@@ -559,6 +559,59 @@ static int launch_fill_scaled_t(const LU &d, const ScaledFill &f, bool equil, cu
 int launch_fill_scaled(const DeviceLU &d, const ScaledFill &f, bool equil, cudaStream_t s) { return launch_fill_scaled_t(d, f, equil, s); }
 int launch_fill_scaled(const BatchedLU &d, const ScaledFill &f, bool equil, cudaStream_t s) { return launch_fill_scaled_t(d, f, equil, s); }
 
+// ---- refill of a scaled fill's pattern (slu_b200_refill) ----
+// slot[p] = csr_slot of entry p at (rmap[i], perm[colind[p]]) (-1 where it has none), row[p] = i: one thread per row, the
+// search of fill_scaled_kernel done once per pattern
+__global__ void refill_slot_kernel(DeviceLU d, int n, const int32_t *__restrict__ rowptr, const int32_t *__restrict__ colind,
+                                   const int32_t *__restrict__ rmap, const int32_t *__restrict__ perm, const int8_t *__restrict__ active,
+                                   int64_t *__restrict__ slot, int32_t *__restrict__ row)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int pi = rmap[i];
+    for (int64_t p = rowptr[i]; p < rowptr[i + 1]; ++p) {
+        const int64_t o = csr_slot(d, pi, perm[colind[p]], active);
+        slot[p] = o < 0 ? -1 : o;
+        row[p] = i;
+    }
+}
+
+int launch_refill_slots(const DeviceLU &d, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *rmap, const int32_t *perm,
+                        const int8_t *active, int64_t *slot, int32_t *row, cudaStream_t s)
+{
+    if (n <= 0) return 0;
+    refill_slot_kernel<<<(n + 127) / 128, 128, 0, s>>>(d, n, rowptr, colind, rmap, perm, active, slot, row);
+    return 1;
+}
+
+// grid (entry tiles, members): thread = entry p of member blockIdx.y.  Coalesced reads of the value, its slot, row and
+// column, the value of fill_scaled_kernel ((R[i] a) C[j], in that order), one scattered store into the zeroed arena and
+// one coalesced store of a into the kept A
+constexpr int REFILL_THREADS = 256;
+template <class LU>
+__global__ void __launch_bounds__(REFILL_THREADS) refill_kernel(LU dd, Refill r)
+{
+    const int64_t p = (int64_t)blockIdx.x * REFILL_THREADS + threadIdx.x;
+    if (p >= r.nnz) return;
+    const DeviceLU &d = member_view(dd);
+    const int64_t m = blockIdx.y, e = m * r.nnz + p;
+    const val_t a = r.val[e];
+    const int64_t o = r.slot[p];
+    const val_t v = vscale_d(r.C[m * r.n + r.colind[p]], vscale_d(r.R[m * r.n + r.row[p]], a));
+    r.aval[e] = a;
+    if (o >= 0) d.val[o] = v;
+}
+
+template <class LU>
+static int launch_refill_t(const LU &d, const Refill &r, cudaStream_t s)
+{
+    if (r.nnz <= 0) return 0;
+    refill_kernel<LU><<<member_grid(d, (unsigned)((r.nnz + REFILL_THREADS - 1) / REFILL_THREADS)), REFILL_THREADS, 0, s>>>(d, r);
+    return 1;
+}
+int launch_refill(const DeviceLU &d, const Refill &r, cudaStream_t s) { return launch_refill_t(d, r, s); }
+int launch_refill(const BatchedLU &d, const Refill &r, cudaStream_t s) { return launch_refill_t(d, r, s); }
+
 // thread = entry i of the member blockIdx.y, every right-hand side
 template <bool SCATTER>
 __global__ void permute_scale_kernel(val_t *__restrict__ dst, const val_t *__restrict__ src, const int32_t *__restrict__ map,
