@@ -94,7 +94,14 @@ typedef struct {
                                   /* [4] tcgen05 path for wide supernodes: int8 slices per operand    */
                                   /* (0 = default: off, 5..8 opt in, < 0 = off: FP64 DMMA only; needs  */
                                   /* balanced pivot-row scales, e.g. an equilibrated A), [5] narrowest */
-                                  /* supernode that takes the tcgen05 path (0 = default 128)          */
+                                  /* supernode that takes the tcgen05 path (0 = default 128), [6] the  */
+                                  /* most supernode panels one Schur GEMM takes (0 = default 4, 1 =    */
+                                  /* off, up to 4; DESIGN 4a): a child whose structure is its parent's */
+                                  /* columns followed by its parent's structure leaves the rest of its */
+                                  /* update to its parent's, as more K.  The environment variable      */
+                                  /* SLU_B200_SCHUR_DEPTH overrides it.  Always 1 in doublecomplex, on */
+                                  /* the int8 path, on Pr x Pc > 1 and on Pz > 1.  Results change only */
+                                  /* in summation order; the flop counts do not change.                */
 } slu_b200_options_t;
 
 typedef struct {
@@ -297,6 +304,10 @@ int slu_b200_k_gemm_sub(int m, int n, int k, const double *a, int lda, const dou
  * Returns their count (< 0 on error). */
 int slu_b200_k_level_export(slu_b200_handle_t h, int level, void *device_lu, int device_lu_bytes, int32_t *nodes, int max_nodes);
 int slu_b200_k_rerun_schur(slu_b200_handle_t h, int level, int reps, float *ms);
+/* the deferred Schur updates the analysis plans (options.reserved[6]), without a device: out[0] = supernodes whose update
+ * is carried by their parent's, out[1] / out[2] = destination updates (RED.ADD.F64) of one factorization without and with
+ * them.  variant 35 of slu_b200_k_gemm_sub (SLU_B200_GEMM_VARIANT) runs the same segmented K loop. */
+int slu_b200_k_schur_merge(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, double out[3]);
 
 /* ---- batched handles: many matrices of ONE sparsity pattern (the reference's pdgssvx3d_csc_batch /
  * dsparseTreeFactorBatchGPU): per-cell implicit solves, parameter sweeps, ensemble members.  The structure analysis,

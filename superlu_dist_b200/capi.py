@@ -90,6 +90,7 @@ def lib():
     L.pdgstrf3d_b200.argtypes = [C.POINTER(LUView), C.POINTER(Options), C.POINTER(Stats), C.POINTER(C.c_int)]
     L.slu_b200_plan.argtypes = [C.POINTER(LUView), C.POINTER(Options), C.POINTER(Stats)]
     L.slu_b200_z_plan.argtypes = [C.POINTER(LUView), C.POINTER(Options), C.POINTER(Stats)]
+    L.slu_b200_k_schur_merge.argtypes = [C.POINTER(LUView), C.POINTER(Options), C.POINTER(C.c_double)]
     # doublecomplex twins (same structs; value arrays hold (re, im) pairs)
     L.slu_b200_z_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(LUView), C.POINTER(Options)]
     for f in ("slu_b200_z_upload", "slu_b200_z_download"):
@@ -356,7 +357,7 @@ def pdgstrf3d_2d(prob, local, z, **opt):
 
 
 def make_options(prob, device=-1, verbose=0, world_size=1, world_rank=0, nccl_id=None, pinned=0, schur_variant=0,
-                 no_lookahead=0, no_coop=0, pipeline=0, overlap_h2d=0, tc_slices=0, tc_min_ns=0):
+                 no_lookahead=0, no_coop=0, pipeline=0, overlap_h2d=0, tc_slices=0, tc_min_ns=0, schur_depth=0):
     o = Options()
     o.device = device
     o.replace_tiny_pivot = int(prob.replace_tiny_pivot)
@@ -370,6 +371,7 @@ def make_options(prob, device=-1, verbose=0, world_size=1, world_rank=0, nccl_id
     o.reserved[3] = overlap_h2d    # 1: level-by-level arena; factor_host also overlaps the upload (opt-in, DESIGN 9)
     o.reserved[4] = tc_slices      # int8 tensor-core path: int8 slices per operand (0 default: off, < 0 off, 5..8)
     o.reserved[5] = tc_min_ns      # narrowest supernode on the int8 tensor-core path (0: default)
+    o.reserved[6] = schur_depth    # most supernode panels per Schur GEMM (deferred chain updates; 0: default, 1: off)
     o.world_size, o.world_rank = world_size, world_rank
     if nccl_id is not None:
         C.memmove(o.nccl_id, bytes(nccl_id), 128)
@@ -384,6 +386,17 @@ def plan(prob, z=0, **opt):
     _check(_fn("plan", _is_complex(prob.dtype))(C.byref(view), C.byref(o), C.byref(st)))
     del keep
     return st
+
+
+def schur_merge(prob, z=0, **opt):
+    """slu_b200_k_schur_merge: the deferred Schur updates of the analysis of layer z, without a device
+    -> (deferred children, destination REDs without deferral, REDs with it)."""
+    view, keep = make_view(prob, z)
+    o = make_options(prob, **opt)
+    out = (C.c_double * 3)()
+    _check(lib().slu_b200_k_schur_merge(C.byref(view), C.byref(o), out))
+    del keep
+    return int(out[0]), int(out[1]), int(out[2])
 
 
 def nccl_unique_id():

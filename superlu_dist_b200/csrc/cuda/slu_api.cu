@@ -96,6 +96,7 @@
 #include <cstdio>
 #include <cstring>
 #include <string>
+#include <functional>
 #include <vector>
 
 using namespace SLU_NS;
@@ -272,6 +273,8 @@ struct slu_b200_handle_s {
     DevBuf<NodeDesc> d_nodes;
     DevBuf<int32_t> d_xsup, d_supno, d_lrows, d_lsrow, d_lspos, d_ucols, d_ufst, d_useg, d_pool_i32, d_lrel, d_urel;
     DevBuf<int64_t> d_pool_i64;
+    DevBuf<KSeg> d_kseg;                  // K segments of deferred child updates (NodeDesc.kseg_off)
+    double merge[3] = {0, 0, 0};          // deferred children, destination REDs at depth 1 and at the planned depth
     DevBuf<LBlk> d_lblk;
     DevBuf<UBlk> d_ublk;
     DevBuf<RowInfo> d_rowinfo;
@@ -768,6 +771,55 @@ int analyze(slu_b200_handle_s *H)
     if (getenv("SLU_B200_TC_MIN_NS")) H->tc_min_ns = std::max(1, atoi(getenv("SLU_B200_TC_MIN_NS")));
     if (H->tc_force_off) H->tc_slices = 0;
 #endif
+    // Deferred Schur updates along supernode chains (DESIGN 4a).  When the structure of supernode k is exactly the columns
+    // of its parent p followed by the structure of p (L rows and packed U columns, position by position), the part of k's
+    // update below and right of p's columns has p's region and destination maps: it runs inside p's update as more K
+    // segments of one GEMM, and k keeps only its panel tiles (those that write p).  options.reserved[6] or
+    // SLU_B200_SCHUR_DEPTH = the most panels one GEMM takes (1: off).
+    int depth = H->opt.reserved[6] > 0 ? H->opt.reserved[6] : SCHUR_DEPTH_DEFAULT;
+    if (getenv("SLU_B200_SCHUR_DEPTH")) depth = atoi(getenv("SLU_B200_SCHUR_DEPTH"));
+    depth = std::min(SCHUR_DEPTH_MAX, std::max(1, depth));
+#ifdef SLU_COMPLEX
+    depth = 1;   // slu_kernels_z.cu has no segmented K loop
+#endif
+    if (H->tc_slices > 0 || H->P2 > 1 || max_lvl > 1) depth = 1;   // int8 route, 2D layers, Z-split tile dealing: DESIGN 8
+    std::vector<KSeg> kseg;
+    {
+        std::vector<std::vector<KSeg>> carried(nsupers);   // segments of nested children each supernode's update carries
+        std::vector<int32_t> panels(nsupers, 1);
+        int64_t deferred = 0;
+        double reds = 0, saved = 0;
+        for (int k = 0; k < nsupers; ++k) {   // children before parents: a parent's id is larger
+            NodeDesc &nd = H->nodes[k];
+            if (!nd.held || xsup[k] >= H->schur_first || H->my_zero[zl_of[k]] || nd.m <= 0 || nd.ncols <= 0) continue;
+            reds += (double)nd.m * nd.ncols;
+            if (depth < 2 || nd.m < 96 || nd.ncols < 96) continue;
+            const int p = supno[lrows[nd.lrow + nd.ns]];
+            const NodeDesc &pd = H->nodes[p];
+            if (!pd.held || zl_of[p] != zl_of[k] || xsup[p] >= H->schur_first || pd.m < 96 || pd.ncols < 96) continue;
+            if (nd.m != pd.ns + pd.m || nd.ncols != pd.ns + pd.ncols || panels[k] + panels[p] > depth) continue;
+            bool nest = true;
+            for (int i = 0; i < nd.m && nest; ++i)
+                nest = lrows[nd.lrow + nd.ns + i] == (i < pd.ns ? xsup[p] + i : lrows[pd.lrow + i]);
+            for (int j = 0; j < nd.ncols && nest; ++j)
+                nest = ucols[nd.ucol + j] == (j < pd.ns ? xsup[p] + j : ucols[pd.ucol + j - pd.ns]);
+            if (!nest) continue;
+            nd.defer = 1;
+            panels[p] += panels[k];
+            // row ns_p of k's update is row 0 of p's: every carried segment starts ns_p rows / packed columns further on
+            carried[p].push_back(KSeg{nd.lval + nd.ns + pd.ns, nd.uval + (int64_t)pd.ns * nd.ns, nd.nsupr, nd.ns, nd.ns, 0});
+            for (const KSeg &q : carried[k]) carried[p].push_back(KSeg{q.a + pd.ns, q.b + (int64_t)pd.ns * q.ldb, q.lda, q.ldb, q.k, 0});
+            ++deferred;
+            saved += (double)pd.m * pd.ncols;
+        }
+        for (int k = 0; k < nsupers; ++k)
+            if (!carried[k].empty()) {
+                H->nodes[k].kseg_off = (int64_t)kseg.size();
+                H->nodes[k].nkseg = (int)carried[k].size();
+                kseg.insert(kseg.end(), carried[k].begin(), carried[k].end());
+            }
+        H->merge[0] = (double)deferred; H->merge[1] = reds; H->merge[2] = reds - saved;
+    }
     H->levels.clear();
     for (int zl = 0; zl < max_lvl; ++zl) {
         int maxlev = -1;
@@ -832,6 +884,16 @@ int analyze(slu_b200_handle_s *H)
 #endif
                         (use_tc ? tc : big).push_back(k);
                         const int64_t tiles_m = (nd.m + SCHUR_BM_BIG - 1) / SCHUR_BM_BIG, tiles_n = (nd.ncols + bn - 1) / bn;
+                        if (nd.defer) {   // only the panel tiles (the kernel takes them as mode 1 in every launch)
+                            const int np = H->nodes[supno[lrows[nd.lrow + nd.ns]]].ns;
+                            const int64_t tru = (np + SCHUR_BM_BIG - 1) / SCHUR_BM_BIG, tcu = (np + bn - 1) / bn;
+                            const int64_t urg = tiles_m * tcu + tru * (tiles_n - tcu);
+                            nd.urg_rows = np; nd.urg_cols = np;
+                            p_big.push_back(p_big.back() + urg);
+                            p_urg.push_back(p_urg.back() + urg);
+                            p_bulk.push_back(p_bulk.back());
+                            continue;
+                        }
                         p_big.push_back(p_big.back() + tiles_m * tiles_n);
                         // look-ahead: which destinations are factored at the very next level of this forest?
                         int r1 = 0, c1 = 0;
@@ -932,7 +994,7 @@ int analyze(slu_b200_handle_s *H)
         H->d_lrows.upload(lrows) || H->d_lsrow.upload(lsrow) || H->d_lspos.upload(lspos) ||
         H->d_ucols.upload(ucols) || H->d_ufst.upload(ufst) || H->d_useg.upload(useg) ||
         H->d_lblk.upload(lblk) || H->d_ublk.upload(ublk) || H->d_pool_i32.upload(pool_i32) ||
-        H->d_pool_i64.upload(pool_i64))
+        H->d_pool_i64.upload(pool_i64) || H->d_kseg.upload(kseg))
         return -1;
     if (H->d_rowinfo.alloc((size_t)ws_row_max * 2) || H->d_colinfo.alloc((size_t)ws_col_max * 2) ||
         H->d_lrel.alloc((size_t)ws_lrel_max * 2) || H->d_urel.alloc((size_t)ws_urel_max * 2) || H->d_flags.alloc((size_t)members + 1) ||
@@ -957,6 +1019,7 @@ int analyze(slu_b200_handle_s *H)
     d.lblk = H->d_lblk.p; d.ublk = H->d_ublk.p; d.rowinfo = H->d_rowinfo.p; d.colinfo = H->d_colinfo.p;
     d.oz_i8 = H->d_oz_i8.p; d.oz_scale = H->d_oz_scale.p; d.oz_rexp = H->d_oz_rexp.p;
     d.lrel = H->d_lrel.p; d.urel = H->d_urel.p; d.info = H->d_flags.p; d.err = H->d_flags.p + members; d.tiny = H->d_tiny.p;
+    d.kseg = H->d_kseg.p;
 
     slu_b200_stats_t &st = H->st;
     st.ops_fact = ops; st.ops_schur = ops_schur; st.schur_bytes = bytes_schur;
@@ -3188,7 +3251,7 @@ int pdgstrf3d_b200(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, 
 // Analysis only, no device needed: HBM bytes, flops in the reference's accounting, level count ... for one rank of a
 // 1 x 1 x Pz grid -- what a caller needs to size a run for 180 GB GPUs before it allocates them.  Also checks the
 // level-by-level layout that the overlapped upload (options.reserved[3]) relies on.
-int slu_b200_plan(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, slu_b200_stats_t *stats)
+static int plan_impl(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, slu_b200_stats_t *stats, double *merge)
 {
     if (!lu || !opt || !stats) return fail("null argument");
     if (opt->schur_variant != 0) return fail("options.schur_variant is retired and must be 0 (got %d)", opt->schur_variant);
@@ -3217,9 +3280,22 @@ int slu_b200_plan(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, s
             if (!rc && off != L.slab_end) rc = fail("level %zu: slab end mismatch", li);
         }
     if (!rc) *stats = H->st;
+    if (!rc && merge) std::copy(H->merge, H->merge + 3, merge);
     delete H;
     return rc;
 }
+int slu_b200_plan(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, slu_b200_stats_t *stats)
+{
+    return plan_impl(lu, opt, stats, nullptr);
+}
+#ifndef SLU_COMPLEX
+int slu_b200_k_schur_merge(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, double out[3])
+{
+    if (!out) return fail("null argument");
+    slu_b200_stats_t st{};
+    return plan_impl(lu, opt, &st, out);
+}
+#endif
 
 // ---- kernel-level entry points -----------------------------------------------------------------
 namespace {
@@ -3335,12 +3411,42 @@ int slu_b200_k_gemm_sub(int m, int n, int k, const double *a, int lda, const dou
     if (ev.create()) return fail("cannot create events");
     cudaEvent_t e0 = ev[0], e1 = ev[1];
 #ifndef SLU_COMPLEX
-    auto launch_gemm_sub = [](int m_, int n_, int k_, const val_t *a_, int lda_, const val_t *b_, int ldb_, val_t *c_, int ldc_,
-                              int variant_, cudaStream_t s_) {
+    std::function<int(int, int, int, const val_t *, int, const val_t *, int, val_t *, int, int, cudaStream_t)> launch_gemm_sub =
+        [](int m_, int n_, int k_, const val_t *a_, int lda_, const val_t *b_, int ldb_, val_t *c_, int ldc_, int variant_, cudaStream_t s_) {
         if (variant_ >= 100) return launch_gemm_sub_ozaki(m_, n_, k_, a_, lda_, b_, ldb_, c_, ldc_, variant_, s_);
         return SLU_NS::launch_gemm_sub(m_, n_, k_, a_, lda_, b_, ldb_, c_, ldc_, variant_, s_);
     };
     if (variant >= 100 && k > 512) return fail("the int8 tensor-core path handles k <= 512 (MAX_SUPER_SIZE)");
+    // variant 35: schur_kernel_h's segmented K loop; K cut into three segments (k1 = k / 3 | 1, k2 = k / 3, the rest), the
+    // second and third repacked with leading dimensions lda + 2q + 1 and their own depth + q + 1 (operands after da / db)
+    DevBuf<val_t> dseg;
+    DevBuf<KSeg> dks;
+    if (variant == 35) {
+        const int k1 = std::min(k, (k / 3) | 1), k2 = std::min(k - k1, k / 3), kq[3] = {k1, k2, k - k1 - k2};
+        std::vector<KSeg> ks;
+        std::vector<val_t> h;
+        int kstart = k1;
+        for (int q = 1; q < 3; ++q) {
+            const int la = lda + 2 * q + 1, lb = kq[q] + q + 1;
+            if (kq[q] <= 0) continue;
+            KSeg g{(int64_t)h.size(), 0, la, lb, kq[q], 0};
+            h.resize(h.size() + (size_t)la * kq[q], 0.0);
+            for (int c = 0; c < kq[q]; ++c)
+                for (int r = 0; r < m; ++r) h[g.a + (size_t)c * la + r] = a[(size_t)(kstart + c) * lda + r];
+            g.b = (int64_t)h.size();
+            h.resize(h.size() + (size_t)lb * n, 0.0);
+            for (int c = 0; c < n; ++c)
+                for (int r = 0; r < kq[q]; ++r) h[g.b + (size_t)c * lb + r] = b[(size_t)c * ldb + kstart + r];
+            ks.push_back(g);
+            kstart += kq[q];
+        }
+        if (dseg.upload(h) || dks.upload(ks)) return -1;
+        // k1 and the segment count by value: the launcher outlives this block (timed repetitions below)
+        launch_gemm_sub = [k1, nks = (int)ks.size(), &dseg, &dks](int m_, int n_, int, const val_t *a_, int lda_, const val_t *b_, int ldb_,
+                                                                 val_t *c_, int ldc_, int, cudaStream_t s_) {
+            return launch_gemm_sub_seg(m_, n_, k1, a_, lda_, b_, ldb_, dseg.p, dks.p, nks, c_, ldc_, s_);
+        };
+    }
 #endif
     launch_gemm_sub(m, n, k, da.p, lda, db.p, ldb, dc.p, ldc, variant, 0);
     CU(cudaDeviceSynchronize());

@@ -51,6 +51,19 @@ struct NodeDesc {            // one per supernode (indexed by global supernode i
     // int8 tensor-core path (slu_ozaki.cu): per-level workspace of this supernode's int8 slices and scales
     int64_t ws_oza, ws_ozb;      // byte offsets into oz_i8: A tiles [rt][ks][s][4096], B tiles [ct][ks][s][OZ_NT*32]
     int64_t ws_ozs;              // element offset into oz_scale / oz_rexp: row scales [0, 128*RT), column scales after
+    // deferred Schur updates along supernode chains (DESIGN 4a): kseg[kseg_off ...] = the nkseg K segments of nested
+    // children that this supernode's update carries after its own; defer = 1: this supernode's update beyond the first
+    // urg_rows rows and urg_cols columns (its parent's columns) is carried by its parent's update
+    int64_t kseg_off;
+    int32_t nkseg, defer;
+};
+
+// deferred Schur updates (DESIGN 4a): panels per GEMM when options.reserved[6] is 0, and the most it accepts
+constexpr int SCHUR_DEPTH_DEFAULT = 4, SCHUR_DEPTH_MAX = 4;
+
+struct KSeg {                // one K segment of a Schur GEMM: A = val + a (lda), B = val + b (ldb), depth k
+    int64_t a, b;
+    int32_t lda, ldb, k, pad;
 };
 
 struct LBlk {                // an off-diagonal L block of panel k
@@ -95,6 +108,7 @@ struct DeviceLU {            // everything the kernels need, passed by value
     int *info;               // min over zero pivots of (1-based global column); INT_MAX if none
     unsigned long long *tiny;
     int *err;                // debug: count of destination lookups that failed
+    const KSeg *kseg;        // the K segments of deferred child updates (NodeDesc.kseg_off)
 };
 
 // Several matrices of one sparsity pattern factored together (slu_b200_batch_*): every structure-only object of
@@ -147,6 +161,11 @@ struct UpSeg { int64_t dst, src, len; };  // a transfer chunk: arena offset, (un
 // standalone kernel tests
 int launch_gemm_sub(int m, int n, int k, const val_t *a, int lda, const val_t *b, int ldb, val_t *c,
                     int ldc, int variant, cudaStream_t s);
+#ifndef SLU_COMPLEX
+// C -= A B + sum over q of A_q B_q on schur_kernel_h's tile and segmented K loop (A_q = base + seg[q].a, device array seg)
+int launch_gemm_sub_seg(int m, int n, int k, const double *a, int lda, const double *b, int ldb, const double *base, const KSeg *seg,
+                        int nseg, double *c, int ldc, cudaStream_t s);
+#endif
 
 // slu_solve.cu (double) / slu_solve_z.cu (doublecomplex): triangular solves on the resident factors.
 // x: device, n x nrhs elements of val_t, ordering of the factored matrix.  trans: 0 solves A x = b (forward pass with L,

@@ -817,7 +817,8 @@ struct HCfg {
 template <int BM, int BN, int WARPS_M, int WARPS_N, int BK, int STAGES>
 __device__ __forceinline__ void gemm_tile_h(const double *__restrict__ A, int lda, const double *__restrict__ B, int ldb,
                                             int M, int N, int K, int m0, int n0, double *sm,
-                                            double (&acc)[BM / WARPS_M / 16][BN / WARPS_N / 8][4])
+                                            double (&acc)[BM / WARPS_M / 16][BN / WARPS_N / 8][4],
+                                            const double *base = nullptr, const KSeg *seg = nullptr, int nseg = 0)
 {
     using C = HCfg<BM, BN, WARPS_M, WARPS_N, BK, STAGES>;
     constexpr int NW = C::NT / 32;
@@ -827,11 +828,14 @@ __device__ __forceinline__ void gemm_tile_h(const double *__restrict__ A, int ld
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
     const int wm0 = (warp % WARPS_M) * C::WTM, wn0 = (warp / WARPS_M) * C::WTN;
     double *As = sm, *Bs = sm + STAGES * C::A_STAGE;
-    const int KT = (K + BK - 1) / BK;
-    const int KF = ((m0 + BM <= M) && (n0 + BN <= N)) ? K / BK : 0;  // k-steps the unpredicated loader serves
+    // K runs over segments: (A, B, K) first, then seg[0 .. nseg) (A = base + a ...).  Each segment takes
+    // ceil(k / BK) k-steps, its tail on the predicated loader; the pipeline runs straight across the boundaries.
+    int KT = (K + BK - 1) / BK;
+    for (int q = 0; q < nseg; ++q) KT += (seg[q].k + BK - 1) / BK;
+    const bool full = (m0 + BM <= M) && (n0 + BN <= N);  // whole k-steps of a full tile take the unpredicated loader
+    int k0 = 0, sg = 0;                                    // the loader is at depth k0 of segment sg (0: the first)
 
-    auto load = [&](int st, int kt) {  // edge tiles and the K tail: predicated, zero-filled
-        const int k0 = kt * BK;
+    auto load = [&](int st) {  // edge tiles and the K tail: predicated, zero-filled
         double *as = As + st * C::A_STAGE, *bs = Bs + st * C::B_STAGE;
 #pragma unroll
         for (int idx = tid; idx < BK * BM; idx += C::NT) {
@@ -850,9 +854,9 @@ __device__ __forceinline__ void gemm_tile_h(const double *__restrict__ A, int ld
     // 32-row column slices of A, so the permuted destinations are a per-lane constant plus immediates
     const double *pa = A + (size_t)warp * lda + m0 + lane;
     const double *pb = B + (size_t)(n0 + tid / BK) * ldb + (tid % BK);
-    const size_t a_col = (size_t)NW * lda, a_step = (size_t)BK * lda, b_col = (size_t)CB * ldb;
     double *const sa = As + warp * C::LDA + prow(lane), *const sb = Bs + (tid / BK) * C::LDB + pk(tid % BK);
     auto load_fast = [&](int st) {
+        const size_t a_col = (size_t)NW * lda, a_step = (size_t)BK * lda, b_col = (size_t)CB * ldb;
         double *as = sa + st * C::A_STAGE, *bs = sb + st * C::B_STAGE;
         const double *p = pa;
 #pragma unroll
@@ -870,20 +874,27 @@ __device__ __forceinline__ void gemm_tile_h(const double *__restrict__ A, int ld
         pa += a_step;
         pb += BK;
     };
-    auto issue = [&](int st, int kt) {
-        if (kt < KF) load_fast(st);
-        else load(st, kt);
+    auto issue = [&](int st) {  // the next k-step (they are issued in order)
+        if (k0 >= K) {          // re-seat the loader on the next segment
+            const KSeg q = seg[sg++];
+            A = base + q.a; lda = q.lda; B = base + q.b; ldb = q.ldb; K = q.k; k0 = 0;
+            pa = A + (size_t)warp * lda + m0 + lane;
+            pb = B + (size_t)(n0 + tid / BK) * ldb + (tid % BK);
+        }
+        if (full && k0 + BK <= K) load_fast(st);
+        else load(st);
+        k0 += BK;
     };
 
 #pragma unroll
     for (int s = 0; s < STAGES - 1; ++s) {
-        if (s < KT) issue(s, s);
+        if (s < KT) issue(s);
         cp_async_commit();
     }
     for (int kt = 0; kt < KT; ++kt) {
         cp_async_wait<STAGES - 2>();
         __syncthreads();
-        if (kt + STAGES - 1 < KT) issue((kt + STAGES - 1) % STAGES, kt + STAGES - 1);
+        if (kt + STAGES - 1 < KT) issue((kt + STAGES - 1) % STAGES);
         cp_async_commit();
         const double *as = As + (kt % STAGES) * C::A_STAGE + t * C::LDA + wm0 + 2 * g;
         const double *bs = Bs + (kt % STAGES) * C::B_STAGE + (wn0 + g) * C::LDB + 2 * t;
@@ -925,7 +936,8 @@ __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, MINB)
     const int k = b.nodes[slot];
     const NodeDesc nd = d.nodes[k];
     int tm, tn;
-    schur_tile_of<BM, BN>(nd, (int)(gt - b.prefix[slot]), mode, tm, tn);
+    // a deferred child has only its panel tiles (mode 1 with urg = its parent's columns), whatever the launch
+    schur_tile_of<BM, BN>(nd, (int)(gt - b.prefix[slot]), nd.defer ? 1 : mode, tm, tn);
     const int m0 = tm * BM, n0 = tn * BN;
 
     double acc[C::MT][C::NT8][4];
@@ -934,10 +946,12 @@ __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, MINB)
 #pragma unroll
         for (int nt = 0; nt < C::NT8; ++nt) acc[mt][nt][0] = acc[mt][nt][1] = acc[mt][nt][2] = acc[mt][nt][3] = 0.0;
     gemm_tile_h<BM, BN, WARPS_M, WARPS_N, BK, STAGES>(d.val + nd.lval + nd.ns, nd.nsupr, d.val + nd.uval, nd.ns, nd.m,
-                                                      nd.ncols, nd.ns, m0, n0, sm, acc);
+                                                      nd.ncols, nd.ns, m0, n0, sm, acc, d.val, d.kseg + nd.kseg_off, nd.nkseg);
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int wm0 = m0 + (warp % WARPS_M) * C::WTM + (lane >> 2), wn0 = n0 + (warp / WARPS_M) * C::WTN + 2 * (lane & 3);
+    // a deferred child leaves the elements below and right of its parent's columns to its parent's update
+    const int defer_i = nd.defer ? nd.urg_rows : nd.m, defer_j = nd.defer ? nd.urg_cols : nd.ncols;
     const RowInfo *rinfo = d.rowinfo + nd.ws_row;
     const ColInfo *cinfo = d.colinfo + nd.ws_col;
 #pragma unroll
@@ -962,8 +976,8 @@ __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, MINB)
 #pragma unroll
                 for (int mt = 0; mt < C::MT; ++mt) {
                     idx[e][mt] = -1;
-                    if (!cok || !rok[mt]) continue;
                     const int i = wm0 + 16 * mt + 8 * h;
+                    if (!cok || !rok[mt] || (i >= defer_i && j >= defer_j)) continue;
                     if (ri[mt].ib >= cj.jb) {
                         const int p = d.lrel[cj.lrel_off + i];
                         if (p >= 0) idx[e][mt] = cj.lbase + p;
@@ -1068,7 +1082,8 @@ static int launch_gemm_sub_t(int m, int n, int k, const double *a, int lda, cons
 // the same on the Hopper main loop (gemm_tile_h)
 template <int BM, int BN, int WARPS_M, int WARPS_N, int BK, int STAGES, int MINB>
 __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, MINB)
-    gemm_sub_kernel_h(int M, int N, int K, const double *A, int lda, const double *B, int ldb, double *Cm, int ldc)
+    gemm_sub_kernel_h(int M, int N, int K, const double *A, int lda, const double *B, int ldb, double *Cm, int ldc,
+                      const double *base, const KSeg *seg, int nseg)
 {
     using C = HCfg<BM, BN, WARPS_M, WARPS_N, BK, STAGES>;
     extern __shared__ __align__(16) double sm[];
@@ -1079,7 +1094,7 @@ __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, MINB)
     for (int mt = 0; mt < C::MT; ++mt)
 #pragma unroll
         for (int nt = 0; nt < C::NT8; ++nt) acc[mt][nt][0] = acc[mt][nt][1] = acc[mt][nt][2] = acc[mt][nt][3] = 0.0;
-    gemm_tile_h<BM, BN, WARPS_M, WARPS_N, BK, STAGES>(A, lda, B, ldb, M, N, K, m0, n0, sm, acc);
+    gemm_tile_h<BM, BN, WARPS_M, WARPS_N, BK, STAGES>(A, lda, B, ldb, M, N, K, m0, n0, sm, acc, base, seg, nseg);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int wm0 = m0 + (warp % WARPS_M) * C::WTM + (lane >> 2), wn0 = n0 + (warp / WARPS_M) * C::WTN + 2 * (lane & 3);
 #pragma unroll
@@ -1100,14 +1115,22 @@ __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N, MINB)
 
 template <int BM, int BN, int WARPS_M, int WARPS_N, int BK, int STAGES, int MINB>
 static int launch_gemm_sub_h(int m, int n, int k, const double *a, int lda, const double *b, int ldb, double *c, int ldc,
-                             cudaStream_t s)
+                             cudaStream_t s, const double *base = nullptr, const KSeg *seg = nullptr, int nseg = 0)
 {
     using C = HCfg<BM, BN, WARPS_M, WARPS_N, BK, STAGES>;
     static std::atomic<unsigned long long> attr_0{0};
     ensure_dyn_smem(gemm_sub_kernel_h<BM, BN, WARPS_M, WARPS_N, BK, STAGES, MINB>, (int)C::SMEM, attr_0);
     const int64_t ctas = (int64_t)((m + BM - 1) / BM) * ((n + BN - 1) / BN);
-    gemm_sub_kernel_h<BM, BN, WARPS_M, WARPS_N, BK, STAGES, MINB><<<(unsigned)ctas, C::NT, C::SMEM, s>>>(m, n, k, a, lda, b, ldb, c, ldc);
+    gemm_sub_kernel_h<BM, BN, WARPS_M, WARPS_N, BK, STAGES, MINB><<<(unsigned)ctas, C::NT, C::SMEM, s>>>(m, n, k, a, lda, b, ldb, c, ldc,
+                                                                                                       base, seg, nseg);
     return 1;
+}
+
+int launch_gemm_sub_seg(int m, int n, int k, const double *a, int lda, const double *b, int ldb, const double *base, const KSeg *seg,
+                        int nseg, double *c, int ldc, cudaStream_t s)
+{
+    if (m <= 0 || n <= 0) return 0;
+    return launch_gemm_sub_h<SCHUR_H_TILE>(m, n, k, a, lda, b, ldb, c, ldc, s, base, seg, nseg);
 }
 
 int launch_gemm_sub(int m, int n, int k, const double *a, int lda, const double *b, int ldb, double *c, int ldc,
