@@ -505,6 +505,44 @@ int slu_b200_solve_device(slu_b200_handle_t h, double *x, int ldx, int nrhs, int
 int slu_b200_batch_solve_device(slu_b200_handle_t h, double *x, int ldx, int nrhs, int trans, void *stream);
 int slu_b200_solve_scaled_device(slu_b200_handle_t h, double *x, int ldx, int nrhs, int trans, void *stream);
 int slu_b200_batch_solve_scaled_device(slu_b200_handle_t h, double *x, int ldx, int nrhs, int trans, void *stream);
+/* ---- factorization on the caller's CUDA stream, and CUDA graphs of refill -> factor -> solve.
+ * factor_device / batch_factor_device: slu_b200_factor / _batch_factor (the same plan, kernels, look-ahead streams, deferred
+ * chains and int8 route), ordered on `stream` as the calls above, for 1 x 1 x 1 grids and handles that are not Schur handles;
+ * refused, with a message, before a successful fill, upload or refill.  No host wait, no host copy and no allocation.  info:
+ * 1 (batch) int32 in device memory on the handle's device (checked as val / x above), written in `stream` order with each
+ * member's status: 0 factored; > 0 the 1-based column of the first exact zero pivot, as slu_b200_factor's info; -1 when
+ * Schur-update destinations were missing from the L/U structure (slu_b200_factor fails with a message there).  The handle
+ * keeps the same status on the device.  stats.gpu_launches counts the call's kernels (2 more than slu_b200_factor: the status
+ * reset and the status write); stats.t_factor_s = 0.
+ * Deferred status: until the host has read it, the handle's factors are "pending".  The calls on `stream` (solve_device,
+ * solve_scaled_device and their batched twins) take pending factors as they are, without a wait.  Every host-synchronous
+ * call that needs factors (solve, solve_trans, solve_scaled, gscon, gsrfs, selinv, logdet, inertia and their batched
+ * twins) and get_stats first synchronise the handle's stream and read the status: they then refuse, and report
+ * stats.tiny_pivots, exactly as after slu_b200_factor.
+ * get_stats while the handle's stream is being captured (after a captured call, before the capture ends) does not wait:
+ * it returns the stats as the host last saw them.
+ * Solves after a failed member: a device solve cannot refuse what the host has not seen.  solve_device and
+ * solve_scaled_device (both precisions, batched or not) overwrite every column of x (rows 0 .. n-1) of each member whose
+ * status is not 0 with quiet NaN (both parts in doublecomplex); the other members' x are the solutions.  On a handle
+ * with a captured call, whose status a replay may change behind the host's back, the device solves accept any status and
+ * leave it to this guard.
+ * CUDA graphs: refill, factor_device, solve_device and solve_scaled_device (and their batched / z twins) may be captured
+ * (cudaStreamBeginCapture on `stream`, any capture mode; torch.cuda.CUDAGraph).  Under capture a call that would allocate,
+ * grow a buffer or wait on the host is refused before it enqueues anything, leaving the capture valid: the first refill
+ * after a scaled fill, and a solve with more right-hand sides (nrhs * batch) than any solve before.  Make such a call once
+ * outside capture first.  A graph holds the addresses of the handle's buffers: from the first captured call on, a call that
+ * would reallocate one of them (a solve, gscon or gsrfs with more right-hand sides than any before, a scaled fill with
+ * another nnz) is refused, naming the captured graph, until slu_b200_destroy; an upload or plain fill keeps the kept A's
+ * buffers instead of freeing them.  A replay runs on the stream it is launched on, not on the handle's stream: a
+ * host-synchronous call after a replay needs the caller to have synchronised that stream first (the status it reads is
+ * then the replay's, and a selinv inverse from before a replayed factorization is refused as after slu_b200_factor); a
+ * call on the same stream is ordered after the replay without that.  Destroying the handle while
+ * a graph that uses it is alive is the caller's error, as with any CUDA library workspace. */
+int slu_b200_factor_device(slu_b200_handle_t h, int32_t *info, void *stream);
+int slu_b200_batch_factor_device(slu_b200_handle_t h, int32_t *info, void *stream);
+/* the CUDA device the handle was created on (options.device, or the current device when that was < 0): where the
+ * device-memory arguments of the calls above must live */
+int slu_b200_get_device(slu_b200_handle_t h, int *device);
 /* ---- doublecomplex twins (SRC/complex16/pzgstrf3d.c:120; the reference's z* handle API,
  * SRC/include/superlu_upacked.h:84-97).  Same view/options/stats structs: the Lnzval_bc_ptr / Unzval_br_ptr
  * entries point at arrays of doublecomplex {double r, i} (SRC/include/dcomplex.h:30) and are declared double*
@@ -608,6 +646,9 @@ int slu_b200_z_solve_device(slu_b200_zhandle_t h, double *x, int ldx, int nrhs, 
 int slu_b200_z_batch_solve_device(slu_b200_zhandle_t h, double *x, int ldx, int nrhs, int trans, void *stream);
 int slu_b200_z_solve_scaled_device(slu_b200_zhandle_t h, double *x, int ldx, int nrhs, int trans, void *stream);
 int slu_b200_z_batch_solve_scaled_device(slu_b200_zhandle_t h, double *x, int ldx, int nrhs, int trans, void *stream);
+int slu_b200_z_factor_device(slu_b200_zhandle_t h, int32_t *info, void *stream);
+int slu_b200_z_batch_factor_device(slu_b200_zhandle_t h, int32_t *info, void *stream);
+int slu_b200_z_get_device(slu_b200_zhandle_t h, int *device);
 int slu_b200_z_get_stats(slu_b200_zhandle_t h, slu_b200_stats_t *out);
 int slu_b200_z_plan(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, slu_b200_stats_t *stats);
 void slu_b200_z_destroy(slu_b200_zhandle_t h);

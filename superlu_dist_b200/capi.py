@@ -169,6 +169,10 @@ def lib():
     for f in ("solve_device", "batch_solve_device", "solve_scaled_device", "batch_solve_scaled_device"):
         for pre in ("slu_b200_", "slu_b200_z_"):
             getattr(L, pre + f).argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
+    for f in ("slu_b200_factor_device", "slu_b200_z_factor_device", "slu_b200_batch_factor_device", "slu_b200_z_batch_factor_device"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    for f in ("slu_b200_get_device", "slu_b200_z_get_device"):
+        getattr(L, f).argtypes = [C.c_void_p, C.c_void_p]
     _lib = L
     return L
 
@@ -274,6 +278,28 @@ def _solve_device(name, complex_, h, b, n, batch, trans):
     nrhs = 1 if b.dim() == nd else b.shape[-2]
     _check(_fn(name, complex_)(h, C.c_void_p(x.data_ptr()), n, nrhs, _TRANS[trans], stream))
     return x
+
+
+def _handle_device(complex_, h):
+    """the CUDA device the handle lives on (slu_b200_[z_]get_device)"""
+    d = C.c_int(0)
+    _check(_fn("get_device", complex_)(h, C.byref(d)))
+    return d.value
+
+
+def _factor_device(name, complex_, h, info, count):
+    """slu_b200_[z_][batch_]factor_device on the current stream of the handle's device -> info, an int32 CUDA tensor (count,)
+    on that device (a new one without info), written in stream order"""
+    import torch
+    dev = torch.device("cuda", _handle_device(complex_, h))
+    if info is None:
+        info = torch.empty(count, dtype=torch.int32, device=dev)
+    elif not (_is_tensor(info) and info.device == dev and info.dtype == torch.int32 and tuple(info.shape) == (count,)
+              and info.is_contiguous()):
+        raise ValueError(f"info must be a contiguous int32 tensor of shape ({count},) on {dev}, the handle's device")
+    stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    _check(_fn(name, complex_)(h, C.c_void_p(info.data_ptr()), stream))
+    return info
 
 
 def device_count():
@@ -424,6 +450,13 @@ class Handle:
         info = C.c_int(0)
         _check(_fn("factor", self.z_)(self.h, C.byref(info)))
         return info.value
+
+    def factor_device(self, info=None):
+        """factor() on the device, enqueued on the current stream with no host wait (slu_b200_factor_device) -> an int32
+        CUDA tensor (1,): 0, the 1-based column of the first exact zero pivot, or -1 (missing Schur-update destinations),
+        written in stream order.  info: a caller-owned tensor to write instead (what a captured CUDA graph needs).  Solves
+        on torch tensors follow without a wait; host calls wait for the status and refuse as after factor()."""
+        return _factor_device("factor_device", self.z_, self.h, info, 1)
 
     def factor_host(self):
         """upload + factor + download with the transfers overlapped (slu_b200_factor_host)."""
@@ -715,6 +748,11 @@ class BatchHandle:
         info = np.zeros(self.batch, np.int32)
         _check(_fn("batch_factor", self.z_)(self.h, info.ctypes.data_as(C.c_void_p)))
         return info
+
+    def factor_device(self, info=None):
+        """factor() on the device for every member (slu_b200_batch_factor_device), as Handle.factor_device -> an int32 CUDA
+        tensor (batch,)"""
+        return _factor_device("batch_factor_device", self.z_, self.h, info, self.batch)
 
     def solve(self, b, trans="N"):
         """L_j U_j x_j = b_j for every member; b: (batch, n) or (batch, nrhs, n), ordering of the factored matrix.

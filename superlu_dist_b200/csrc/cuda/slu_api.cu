@@ -77,6 +77,9 @@
 #define slu_b200_batch_solve_device slu_b200_z_batch_solve_device
 #define slu_b200_solve_scaled_device slu_b200_z_solve_scaled_device
 #define slu_b200_batch_solve_scaled_device slu_b200_z_batch_solve_scaled_device
+#define slu_b200_factor_device slu_b200_z_factor_device
+#define slu_b200_batch_factor_device slu_b200_z_batch_factor_device
+#define slu_b200_get_device slu_b200_z_get_device
 #define SLU_API "slu_b200_z_"     // name prefix of the exported calls, for error messages
 #else
 #define SLU_API "slu_b200_"
@@ -366,6 +369,16 @@ struct slu_b200_handle_s {
     // work (ev_in) and the caller's stream after the handle's (ev_out)
     int device = 0;
     cudaEvent_t ev_in = nullptr, ev_out = nullptr;
+    // factor_device: every member's info on the device, as member_info holds it (written by every factorization), and
+    // whether member_info waits for it (status_on_device; settle)
+    DevBuf<int32_t> d_info;
+    bool status_on_device = false;
+    // the device factorizations so far, counted by factor_info_kernel (a replay counts too): epoch is the count the last
+    // settle read, si_epoch the count selinv inverted
+    DevBuf<unsigned long long> d_epoch;
+    unsigned long long epoch = 0, si_epoch = 0;
+    // a call on the caller's stream has been captured into a CUDA graph: the buffers those calls use are pinned (grow)
+    bool captured = false;
 };
 
 namespace {
@@ -374,28 +387,36 @@ namespace {
 // before its first write, and sets the state it establishes only once it has succeeded: a call that fails on the way
 // leaves a handle whose factors (and values, for a fill) the calls that read them refuse.
 
-// a factorization is about to overwrite the arena: no member has factors, and the inverse no longer describes them
-void factors_replaced(slu_b200_handle_s *H)
+// member_info after a device factorization (factor_device) until settle reads the status it left on the device
+constexpr int INFO_PENDING = INT_MIN;
+
+// a factorization is about to overwrite the arena: no member has factors, and the inverse no longer describes them.  d_info
+// says the same in the handle's stream order (a captured refill carries it into every replay).
+int factors_replaced(slu_b200_handle_s *H)
 {
     std::fill(H->member_info.begin(), H->member_info.end(), -1);
+    H->status_on_device = false;
     H->si_ready = false;
+    CU(cudaMemsetAsync(H->d_info.p, 0xff, H->d_info.bytes(), H->stream));
+    return 0;
 }
 
 // an upload or a fill is about to overwrite the arena: no values to factor either, and the scaling no longer describes
 // them.  The A kept for refinement and the refill's slot map go with the scaling, except on a scaled fill (keep_a), which
 // reuses their buffers (the map is rebuilt by the next refill).
-void values_replaced(slu_b200_handle_s *H, bool keep_a = false)
+int values_replaced(slu_b200_handle_s *H, bool keep_a = false)
 {
-    factors_replaced(H);
+    const int rc = factors_replaced(H);
     H->uploaded = false;
     H->scaled = false;
     H->amap_ready = false;
-    if (keep_a) return;
+    if (keep_a || H->captured) return rc;    // a captured refill reads them (grow)
     H->d_arp.release();
     H->d_aci.release();
     H->d_aval.release();
     H->d_amap.release();
     H->d_arow.release();
+    return rc;
 }
 
 // What a call needs of the handle (check): one bit per condition
@@ -411,11 +432,37 @@ enum Need : unsigned {
     SCALED = 1u << 8,         // the scaling of a successful scaled fill
     FACTORED = 1u << 9,       // every member factored with info 0
     SI_READY = 1u << 10,      // the inverse of selinv on the current factors
+    DEVICE_ORDERED = 1u << 11, // with FACTORED: a call on the caller's stream, which takes a pending status as it is (and
+                               // on a captured handle any status: a replay may have changed it, and the guard covers it)
 };
+
+// The status a device factorization left in d_info and d_tiny, read into member_info and stats.tiny_pivots once the handle's
+// stream has drained: what a host-synchronous call sees, exactly as after slu_b200_factor.  On a captured handle it is read
+// every time, since a replay of the graph may have rewritten it (every fill, refill and factorization writes d_info), and
+// the inverse of selinv goes when a factorization has run since it (the epoch moved).  While the handle's stream is being
+// captured nothing is read: a wait would end the capture.
+int settle(slu_b200_handle_s *H)
+{
+    if (!H->status_on_device && !H->captured) return 0;
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    CU(cudaStreamIsCapturing(H->stream, &cs));
+    if (cs != cudaStreamCaptureStatusNone) return 0;
+    std::vector<int32_t> info(H->member_info.size());
+    unsigned long long tiny = 0;
+    CU(cudaStreamSynchronize(H->stream));
+    CU(cudaMemcpy(info.data(), H->d_info.p, info.size() * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(&tiny, H->d_tiny.p, sizeof tiny, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(&H->epoch, H->d_epoch.p, sizeof H->epoch, cudaMemcpyDeviceToHost));
+    std::copy(info.begin(), info.end(), H->member_info.begin());
+    H->st.tiny_pivots = (int64_t)tiny;
+    H->status_on_device = false;
+    if (H->captured && H->epoch != H->si_epoch) H->si_ready = false;
+    return 0;
+}
 
 // Refuses a call on a handle that does not give it what it needs, with a message that starts with fn, the call's exported
 // name.  Kind, then Schur, then grid, then state; except that an unbatched schur_* call names a missing Schur handle first.
-int check(const slu_b200_handle_s *H, const char *fn, unsigned need)
+int check(slu_b200_handle_s *H, const char *fn, unsigned need)
 {
     if ((need & SCHUR) && (need & UNBATCHED) && !H->nschur) return fail("%s needs a Schur handle (" SLU_API "schur_create)", fn);
     if ((need & UNBATCHED) && H->batch)
@@ -435,10 +482,11 @@ int check(const slu_b200_handle_s *H, const char *fn, unsigned need)
         return fail("%s before a successful %s", fn, H->batch ? SLU_API "batch_fill_csr" : SLU_API "upload or " SLU_API "fill_csr");
     if ((need & SCALED) && !H->scaled)
         return fail("%s needs a scaled fill on this handle first (a later upload or plain fill drops the scaling and the kept A)", fn);
+    if ((need & FACTORED) && !(need & DEVICE_ORDERED) && settle(H)) return -1;
     if (need & FACTORED)
         for (size_t j = 0; j < H->member_info.size(); ++j) {
             const int info = H->member_info[j];
-            if (info == 0) continue;
+            if (info == 0 || ((need & DEVICE_ORDERED) && (info == INFO_PENDING || H->captured))) continue;
             if (!H->batch)
                 return fail("%s needs a successful " SLU_API "factor %s", fn, (need & SCALED) ? "after the scaled fill" : "(info = 0) on this handle first");
             if (info < 0) return fail("%s needs a " SLU_API "batch_factor of the filled members first", fn);
@@ -448,6 +496,30 @@ int check(const slu_b200_handle_s *H, const char *fn, unsigned need)
         return fail("%s needs %s on the current factors first (a later fill, upload or factorization invalidates it)", fn,
                     H->batch ? SLU_API "batch_selinv" : SLU_API "selinv");
     return 0;
+}
+
+// A CUDA graph captured from the calls on the caller's stream holds raw pointers to the buffers they use: d_x, d_x2, and the
+// kept A and the slot map of the refill.  Once one of those calls has been captured (H->captured), none of them is freed
+// or moved again until slu_b200_destroy; moves: the call would do so.
+int pin_check(const slu_b200_handle_s *H, bool moves, const char *fn)
+{
+    if (moves && H->captured)
+        return fail("%s would reallocate a buffer that a captured CUDA graph uses: after a capture the handle's buffers keep "
+                    "their sizes until " SLU_API "destroy", fn);
+    return 0;
+}
+
+// Every growth of those buffers (exact: resized to len, else grown to at least len).  capturing: the call is being captured,
+// where an allocation is not allowed: it is refused before anything is enqueued.
+template <class T>
+int grow(const slu_b200_handle_s *H, DevBuf<T> &b, size_t len, bool exact, bool capturing, const char *fn)
+{
+    if (exact ? b.n == len : b.n >= len) return 0;
+    if (capturing)
+        return fail("%s would allocate device buffers while the stream is capturing a CUDA graph: make this call once outside "
+                    "capture first", fn);
+    if (pin_check(H, true, fn)) return -1;
+    return b.alloc(len);
 }
 
 int device_setup(const slu_b200_options_t *opt)
@@ -1502,6 +1574,123 @@ int panel_work(const slu_b200_handle_s *H, const LU &d, const LevelPlan &L, int 
     return launches;
 }
 
+// the Schur launch of the level loop: the cooperative split of an unbatched handle; a batched handle has none
+int schur_launch(const DeviceLU &d, const Batch &b, int64_t ctas, int big, int mode, int split_n, int split_i, cudaStream_t s)
+{
+    return launch_schur(d, b, ctas, big, mode, split_n, split_i, s);
+}
+int schur_launch(const BatchedLU &d, const Batch &b, int64_t ctas, int big, int mode, int, int, cudaStream_t s)
+{
+    return launch_schur(d, b, ctas, big, mode, s);
+}
+
+// The level loop of a factorization, enqueued on H->stream (the bulk Schur tiles on stream2 with look-ahead, joined back
+// before it returns) after the caller has reset the info flags and d_tiny: slu_b200_factor, factor_host, batch_factor and
+// the factor_device twins.  d = H->dev, or H->bdev with every launch over the members (a batched handle has a 1 x 1 x 1
+// grid and no int8 levels: tc_count = 0).  prof: the per-level timings of options.verbose >= 2, which wait for every
+// level; pipelined / up_pipe: factor_host's overlapped D2H / H2D.  Without them and on one rank, no host wait, no
+// allocation and no host copy: the loop can be captured into a CUDA graph.  Returns the kernel launches, < 0 on an error.
+template <class LU>
+int64_t factor_levels(slu_b200_handle_s *H, const LU &d, bool prof, bool pipelined, bool up_pipe)
+{
+    float t_diag = 0, t_trsm = 0, t_setup = 0, t_schur = 0, t_red = 0;
+    EventSet pe;
+    if (prof && pe.create()) return fail("cannot create the profiling events");
+    const cudaStream_t s = H->stream, s2 = H->stream2;
+    int64_t launches = 0;
+    // Look-ahead (the role of dsparseTreeFactor_ASYNC's pipeline, dtreeFactorization.c:430-454,598-706): the
+    // critical path (panel work of level l, then the "urgent" Schur tiles that feed the panels of level l+1) runs on
+    // a high-priority stream; the bulk of the Schur update of level l runs on a second stream, concurrently with the
+    // panel work of level l+1.  All updates are atomic adds, so bulk(l) and anything of level l+1 commute; the only
+    // ordering needed is panel(l) after bulk(l-2) (in-order stream: after every earlier bulk).
+    const bool lookahead = !prof && !H->opt.reserved[0];
+    size_t li = 0;
+    for (int zl = 0; zl < H->max_lvl; ++zl) {
+        const bool coopz = H->coop && (zl >= 1 || H->P2 > 1);
+        if (H->my_zero[zl] && !coopz) continue;  // pdgstrf3d.c:336
+        const int split_n = coopz ? (H->P2 << zl) : 1;
+        const int split_i = coopz ? ((H->view.mydep & ((1 << zl) - 1)) * H->P2 + H->view.myrow * H->view.npcol + H->view.mycol) : 0;
+        size_t first = (size_t)-1, last = (size_t)-1;
+        for (; li < H->levels.size() && H->levels[li].zlvl <= zl; ++li) {
+            const LevelPlan &L = H->levels[li];
+            if (L.zlvl < zl) continue;
+            if (first == (size_t)-1) first = li;
+            last = li;
+            const int64_t *p64 = H->d_pool_i64.p;
+            if (lookahead && li >= first + 2) CU(cudaStreamWaitEvent(s, H->ev_bulk[li - 2], 0));
+            if (up_pipe) CU(cudaStreamWaitEvent(s, H->ev_up[li], 0));  // this level's A values are in the arena
+            if (coopz && L.slab_end > L.slab_begin) {
+                // every rank of the Z group holds a partial sum of this level's panels (its own Schur contributions,
+                // plus A on the group leader): one in-place all-reduce makes them complete and identical everywhere.
+                // Replaces dreduceAllAncestors3d's pairwise Send/Recv (pd3dcomm.c:1046-1081) for this forest.
+                if (prof) cudaEventRecord(pe[5], s);
+                NC(g_nccl.AllReduce(H->val.p + L.slab_begin, H->val.p + L.slab_begin, (size_t)(L.slab_end - L.slab_begin) * VAL_DOUBLES,
+                                    NCCL_FLOAT64, NCCL_SUM, H->gcomm[zl], s));
+                if (prof) { cudaEventRecord(pe[0], s); cudaEventSynchronize(pe[0]); float ms; cudaEventElapsedTime(&ms, pe[5], pe[0]); t_red += ms; }
+            }
+            if (prof) cudaEventRecord(pe[0], s);
+            // tiny-pivot replacements are counted once: by the layer that owns the forest (not by the replicated
+            // copies of a cooperative group) and by one rank of its 2D grid (stat->TinyPivots is MPI_SUMmed there,
+            // pdgssvx3d.c:1149)
+            const bool count_tiny = !H->my_zero[zl] && (H->P2 == 1 || (H->view.myrow == 0 && H->view.mycol == 0));
+            launches += panel_work(H, d, L, H->opt.replace_tiny_pivot ? (count_tiny ? 1 : 2) : 0, s, prof ? &pe[1] : nullptr);
+#ifndef SLU_COMPLEX
+            const int32_t *tcn = H->d_pool_i32.p + L.tc_nodes;
+            if (L.tc_count > 0)      // int8 slices of the level's wide panels (final after the TRSMs above)
+                launches += launch_oz_slice(d, tcn, L.tc_count, p64 + L.tc_p_rt, L.tc_n_rt, p64 + L.tc_p_ak, L.tc_n_ak,
+                                            p64 + L.tc_p_b, L.tc_n_b, H->tc_slices, s);
+#endif
+            if (prof) cudaEventRecord(pe[3], s);
+            const int32_t *bign = H->d_pool_i32.p + L.big_nodes;
+            if (lookahead || pipelined) CU(cudaEventRecord(H->ev_panel[li], s));
+            if (pipelined && pipe_download_level(H, li)) return -1;
+            if (lookahead) {
+                launches += schur_launch(d, Batch{bign, p64 + L.urg_prefix, L.big_count}, L.urg_ctas, 1, 1, split_n, split_i, s);
+                launches += schur_launch(d, Batch{H->d_pool_i32.p + L.small_nodes, p64 + L.small_prefix, L.small_count}, L.small_ctas, 0, 0, split_n, split_i, s);
+#ifndef SLU_COMPLEX
+                launches += launch_oz_schur(d, Batch{tcn, p64 + L.tc_urg_prefix, L.tc_count}, L.tc_urg_ctas, 1, split_n, split_i, H->tc_slices, s);
+#endif
+                CU(cudaStreamWaitEvent(s2, H->ev_panel[li], 0));
+#ifndef SLU_COMPLEX
+                launches += launch_oz_schur(d, Batch{tcn, p64 + L.tc_bulk_prefix, L.tc_count}, L.tc_bulk_ctas, 2, split_n, split_i, H->tc_slices, s2);
+#endif
+                launches += schur_launch(d, Batch{bign, p64 + L.bulk_prefix, L.big_count}, L.bulk_ctas, 1, 2, split_n, split_i, s2);
+                CU(cudaEventRecord(H->ev_bulk[li], s2));
+            } else {
+#ifndef SLU_COMPLEX
+                launches += launch_oz_schur(d, Batch{tcn, p64 + L.tc_prefix, L.tc_count}, L.tc_ctas, 0, split_n, split_i, H->tc_slices, s);
+#endif
+                launches += schur_launch(d, Batch{bign, p64 + L.big_prefix, L.big_count}, L.big_ctas, 1, 0, split_n, split_i, s);
+                launches += schur_launch(d, Batch{H->d_pool_i32.p + L.small_nodes, p64 + L.small_prefix, L.small_count}, L.small_ctas, 0, 0, split_n, split_i, s);
+            }
+            if (prof) {
+                cudaEventRecord(pe[4], s);
+                cudaEventSynchronize(pe[4]);
+                float ms;
+                cudaEventElapsedTime(&ms, pe[0], pe[1]); t_diag += ms;
+                cudaEventElapsedTime(&ms, pe[1], pe[2]); t_trsm += ms;
+                cudaEventElapsedTime(&ms, pe[2], pe[3]); t_setup += ms;
+                cudaEventElapsedTime(&ms, pe[3], pe[4]); t_schur += ms;
+            }
+        }
+        if (lookahead && last != (size_t)-1) {  // join the bulk stream before anything that reads the ancestors
+            CU(cudaStreamWaitEvent(s, H->ev_bulk[last], 0));
+            if (last > first) CU(cudaStreamWaitEvent(s, H->ev_bulk[last - 1], 0));
+        }
+        if (zl < H->max_lvl - 1 && !H->coop) {
+            if (prof) cudaEventRecord(pe[0], s);
+            // the pairwise reduction adds non-atomically: every upload into the ancestors must have landed
+            if (up_pipe && !H->ev_up.empty()) CU(cudaStreamWaitEvent(s, H->ev_up.back(), 0));
+            if (reduce_ancestors(H, zl)) return -1;
+            if (prof) { cudaEventRecord(pe[1], s); cudaEventSynchronize(pe[1]); float ms; cudaEventElapsedTime(&ms, pe[0], pe[1]); t_red += ms; }
+        }
+    }
+    if (prof) {
+        H->st.t_diag_ms = t_diag; H->st.t_trsm_ms = t_trsm; H->st.t_schur_setup_ms = t_setup; H->st.t_schur_ms = t_schur; H->st.t_reduce_ms = t_red;
+    }
+    return launches;
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -1686,6 +1875,11 @@ static int create_impl(slu_b200_handle_t *out, const slu_b200_lu_view_t *lu, con
         H->bdev.members = batch;
     }
     H->member_info.assign(batch ? batch : 1, -1);
+    if (H->d_info.alloc(H->member_info.size()) || cudaMemset(H->d_info.p, 0xff, H->d_info.bytes()) != cudaSuccess ||
+        H->d_epoch.alloc(1) || cudaMemset(H->d_epoch.p, 0, H->d_epoch.bytes()) != cudaSuccess) {
+        slu_b200_destroy(H);
+        return fail("cannot allocate the device status");
+    }
     {
         int lo = 0, hi = 0;
         cudaDeviceGetStreamPriorityRange(&lo, &hi);  // hi = numerically lowest = highest priority
@@ -1718,7 +1912,7 @@ int slu_b200_upload(slu_b200_handle_t H)
     if (!H) return fail("null handle");
     if (check(H, SLU_API "upload", UNBATCHED)) return -1;
     double t0 = now_s();
-    values_replaced(H);
+    if (values_replaced(H)) return -1;
     if (transfer(H, true)) return -1;
     H->st.t_upload_s = now_s() - t0;
     H->uploaded = true;
@@ -1739,108 +1933,18 @@ static int factor_impl(slu_b200_handle_t H, int *info, bool pipelined, bool up_p
 {
     if (!H || !info) return fail("null argument");
     if (check(H, SLU_API "factor", UNBATCHED | UPLOADED)) return -1;
-    factors_replaced(H);
+    if (factors_replaced(H)) return -1;
     if (pipelined && pipe_prepare(H)) return -1;
     cudaStream_t s = H->stream;
-    const DeviceLU &d = H->dev;
     int init[2] = {INT_MAX, 0};
     CU(cudaMemcpyAsync(H->d_flags.p, init, sizeof init, cudaMemcpyHostToDevice, s));
     CU(cudaMemsetAsync(H->d_tiny.p, 0, sizeof(unsigned long long), s));
-    H->st.gpu_launches = 0;
+    H->st.gpu_launches = 0;                // the pairwise reduction of the level loop adds its launches here too
     const bool prof = H->opt.verbose >= 2 && !pipelined;
-    float t_diag = 0, t_trsm = 0, t_setup = 0, t_schur = 0, t_red = 0;
-
-    EventSet pe;
-    if (prof && pe.create()) return fail("cannot create the profiling events");
     CU(cudaEventRecord(H->ev0, s));
-    // Look-ahead (the role of dsparseTreeFactor_ASYNC's pipeline, dtreeFactorization.c:430-454,598-706): the
-    // critical path (panel work of level l, then the "urgent" Schur tiles that feed the panels of level l+1) runs on
-    // a high-priority stream; the bulk of the Schur update of level l runs on a second stream, concurrently with the
-    // panel work of level l+1.  All updates are atomic adds, so bulk(l) and anything of level l+1 commute; the only
-    // ordering needed is panel(l) after bulk(l-2) (in-order stream: after every earlier bulk).
-    const bool lookahead = !prof && !H->opt.reserved[0];
-    cudaStream_t s2 = H->stream2;
-    size_t li = 0;
-    for (int zl = 0; zl < H->max_lvl; ++zl) {
-        const bool coopz = H->coop && (zl >= 1 || H->P2 > 1);
-        if (H->my_zero[zl] && !coopz) continue;  // pdgstrf3d.c:336
-        const int split_n = coopz ? (H->P2 << zl) : 1;
-        const int split_i = coopz ? ((H->view.mydep & ((1 << zl) - 1)) * H->P2 + H->view.myrow * H->view.npcol + H->view.mycol) : 0;
-        size_t first = (size_t)-1, last = (size_t)-1;
-        for (; li < H->levels.size() && H->levels[li].zlvl <= zl; ++li) {
-            const LevelPlan &L = H->levels[li];
-            if (L.zlvl < zl) continue;
-            if (first == (size_t)-1) first = li;
-            last = li;
-            const int64_t *p64 = H->d_pool_i64.p;
-            if (lookahead && li >= first + 2) CU(cudaStreamWaitEvent(s, H->ev_bulk[li - 2], 0));
-            if (up_pipe) CU(cudaStreamWaitEvent(s, H->ev_up[li], 0));  // this level's A values are in the arena
-            if (coopz && L.slab_end > L.slab_begin) {
-                // every rank of the Z group holds a partial sum of this level's panels (its own Schur contributions,
-                // plus A on the group leader): one in-place all-reduce makes them complete and identical everywhere.
-                // Replaces dreduceAllAncestors3d's pairwise Send/Recv (pd3dcomm.c:1046-1081) for this forest.
-                if (prof) cudaEventRecord(pe[5], s);
-                NC(g_nccl.AllReduce(H->val.p + L.slab_begin, H->val.p + L.slab_begin, (size_t)(L.slab_end - L.slab_begin) * VAL_DOUBLES,
-                                    NCCL_FLOAT64, NCCL_SUM, H->gcomm[zl], s));
-                if (prof) { cudaEventRecord(pe[0], s); cudaEventSynchronize(pe[0]); float ms; cudaEventElapsedTime(&ms, pe[5], pe[0]); t_red += ms; }
-            }
-            if (prof) cudaEventRecord(pe[0], s);
-            // tiny-pivot replacements are counted once: by the layer that owns the forest (not by the replicated
-            // copies of a cooperative group) and by one rank of its 2D grid (stat->TinyPivots is MPI_SUMmed there,
-            // pdgssvx3d.c:1149)
-            const bool count_tiny = !H->my_zero[zl] && (H->P2 == 1 || (H->view.myrow == 0 && H->view.mycol == 0));
-            H->st.gpu_launches += panel_work(H, d, L, H->opt.replace_tiny_pivot ? (count_tiny ? 1 : 2) : 0, s, prof ? &pe[1] : nullptr);
-#ifndef SLU_COMPLEX
-            const int32_t *tcn = H->d_pool_i32.p + L.tc_nodes;
-            if (L.tc_count > 0)      // int8 slices of the level's wide panels (final after the TRSMs above)
-                H->st.gpu_launches += launch_oz_slice(d, tcn, L.tc_count, p64 + L.tc_p_rt, L.tc_n_rt, p64 + L.tc_p_ak, L.tc_n_ak,
-                                                      p64 + L.tc_p_b, L.tc_n_b, H->tc_slices, s);
-#endif
-            if (prof) cudaEventRecord(pe[3], s);
-            const int32_t *bign = H->d_pool_i32.p + L.big_nodes;
-            if (lookahead || pipelined) CU(cudaEventRecord(H->ev_panel[li], s));
-            if (pipelined && pipe_download_level(H, li)) return -1;
-            if (lookahead) {
-                H->st.gpu_launches += launch_schur(d, Batch{bign, p64 + L.urg_prefix, L.big_count}, L.urg_ctas, 1, 1, split_n, split_i, s);
-                H->st.gpu_launches += launch_schur(d, Batch{H->d_pool_i32.p + L.small_nodes, p64 + L.small_prefix, L.small_count}, L.small_ctas, 0, 0, split_n, split_i, s);
-#ifndef SLU_COMPLEX
-                H->st.gpu_launches += launch_oz_schur(d, Batch{tcn, p64 + L.tc_urg_prefix, L.tc_count}, L.tc_urg_ctas, 1, split_n, split_i, H->tc_slices, s);
-#endif
-                CU(cudaStreamWaitEvent(s2, H->ev_panel[li], 0));
-#ifndef SLU_COMPLEX
-                H->st.gpu_launches += launch_oz_schur(d, Batch{tcn, p64 + L.tc_bulk_prefix, L.tc_count}, L.tc_bulk_ctas, 2, split_n, split_i, H->tc_slices, s2);
-#endif
-                H->st.gpu_launches += launch_schur(d, Batch{bign, p64 + L.bulk_prefix, L.big_count}, L.bulk_ctas, 1, 2, split_n, split_i, s2);
-                CU(cudaEventRecord(H->ev_bulk[li], s2));
-            } else {
-#ifndef SLU_COMPLEX
-                H->st.gpu_launches += launch_oz_schur(d, Batch{tcn, p64 + L.tc_prefix, L.tc_count}, L.tc_ctas, 0, split_n, split_i, H->tc_slices, s);
-#endif
-                H->st.gpu_launches += launch_schur(d, Batch{bign, p64 + L.big_prefix, L.big_count}, L.big_ctas, 1, 0, split_n, split_i, s);
-                H->st.gpu_launches += launch_schur(d, Batch{H->d_pool_i32.p + L.small_nodes, p64 + L.small_prefix, L.small_count}, L.small_ctas, 0, 0, split_n, split_i, s);
-            }
-            if (prof) {
-                cudaEventRecord(pe[4], s);
-                cudaEventSynchronize(pe[4]);
-                float ms;
-                cudaEventElapsedTime(&ms, pe[0], pe[1]); t_diag += ms;
-                cudaEventElapsedTime(&ms, pe[1], pe[2]); t_trsm += ms;
-                cudaEventElapsedTime(&ms, pe[2], pe[3]); t_setup += ms;
-                cudaEventElapsedTime(&ms, pe[3], pe[4]); t_schur += ms;
-            }
-        }
-        if (lookahead && last != (size_t)-1) {  // join the bulk stream before anything that reads the ancestors
-            CU(cudaStreamWaitEvent(s, H->ev_bulk[last], 0));
-            if (last > first) CU(cudaStreamWaitEvent(s, H->ev_bulk[last - 1], 0));
-        }
-        if (zl < H->max_lvl - 1 && !H->coop) {
-            if (prof) cudaEventRecord(pe[0], s);
-            // the pairwise reduction adds non-atomically: every upload into the ancestors must have landed
-            if (up_pipe && !H->ev_up.empty()) CU(cudaStreamWaitEvent(s, H->ev_up.back(), 0));
-            if (reduce_ancestors(H, zl)) return -1;
-            if (prof) { cudaEventRecord(pe[1], s); cudaEventSynchronize(pe[1]); float ms; cudaEventElapsedTime(&ms, pe[0], pe[1]); t_red += ms; }
-        }
-    }
+    const int64_t launches = factor_levels(H, H->dev, prof, pipelined, up_pipe);
+    if (launches < 0) return -1;
+    H->st.gpu_launches += launches;
     if (H->comm)  // pdgstrf3d.c:388-392: MPI_Allreduce(info, MIN) over the 3D grid
         NC(g_nccl.AllReduce(H->d_flags.p, H->d_flags.p, 1, NCCL_INT32, NCCL_MIN, H->comm, s));
     CU(cudaEventRecord(H->ev1, s));
@@ -1855,12 +1959,10 @@ static int factor_impl(slu_b200_handle_t H, int *info, bool pipelined, bool up_p
     unsigned long long tiny = 0;
     CU(cudaMemcpy(flags, H->d_flags.p, sizeof flags, cudaMemcpyDeviceToHost));
     CU(cudaMemcpy(&tiny, H->d_tiny.p, sizeof tiny, cudaMemcpyDeviceToHost));
-    if (prof) {
-        H->st.t_diag_ms = t_diag; H->st.t_trsm_ms = t_trsm; H->st.t_schur_setup_ms = t_setup; H->st.t_schur_ms = t_schur; H->st.t_reduce_ms = t_red;
-    }
     H->st.tiny_pivots = (int64_t)tiny;
     if (flags[1]) return fail("%d Schur-update destinations were not found in the L/U structure", flags[1]);
     *info = H->member_info[0] = flags[0] == INT_MAX ? 0 : flags[0];
+    CU(cudaMemcpy(H->d_info.p, H->member_info.data(), sizeof(int32_t), cudaMemcpyHostToDevice));   // for the device solves
     return 0;
 }
 
@@ -1884,7 +1986,7 @@ int slu_b200_factor_host(slu_b200_handle_t H, int *info)
         return rc2 ? rc2 : slu_b200_download(H);
     }
     if (H->grouped) {                      // options.reserved[3]: H2D, factorization and D2H all overlapped
-        values_replaced(H);
+        if (values_replaced(H)) return -1;
         if (pipe_prepare(H) || upload_pipe_issue(H)) return -1;
         H->uploaded = true;
         H->st.t_upload_s = 0;
@@ -1927,7 +2029,7 @@ static int fill_csr_impl(slu_b200_handle_t H, bool batched, int n, const int32_t
     CU(cudaMemcpyAsync(dci.p, colind, (size_t)nnz * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(dv.p, val, (size_t)nnz * B * sizeof(val_t), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(dperm.p, perm, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    values_replaced(H);
+    if (values_replaced(H)) return -1;
     CU(cudaMemsetAsync(H->val.p, 0, H->val.bytes(), s));
     CU(cudaMemsetAsync(H->dev.err, 0, sizeof(int), s));
     if (batched) launch_fill_csr(H->bdev, n, drp.p, dci.p, dv.p, dperm.p, dact.p, H->dev.err, s);
@@ -2074,7 +2176,7 @@ static int solve_host(slu_b200_handle_t H, const char *fn, unsigned need, double
     if (nrhs < 1 || ldx < n) return fail("%s: bad nrhs / ldx", fn);
     if (batched && (int64_t)n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
     const size_t len = (size_t)n * nrhs * B;
-    if (H->d_x.n < len && (H->d_x.alloc(len) || (!batched && H->d_x2.alloc(len)))) return -1;
+    if (grow(H, H->d_x, len, false, false, fn) || (!batched && grow(H, H->d_x2, len, false, false, fn))) return -1;
     cudaStream_t s = H->stream;
     double t0 = now_s();
     val_t *result = H->d_x.p;
@@ -2243,6 +2345,7 @@ static int selinv_sweep(slu_b200_handle_t H, const LU &d, int members, const cha
     CU(cudaGetLastError());
     if (bad) return fail("%s: %d Schur-update destinations were not found in the L/U structure", fn, bad);
     H->si_ready = true;
+    H->si_epoch = H->epoch;                // selinv's check settled the handle: the factorizations counted so far
     if (out) {
         out[0] = now_s() - t0;
         out[1] = flops * members;
@@ -2441,43 +2544,17 @@ int slu_b200_batch_factor(slu_b200_handle_t H, int *info)
 {
     if (!H || !info) return fail("null argument");
     if (check(H, SLU_API "batch_factor", BATCHED | UPLOADED)) return -1;
-    factors_replaced(H);
+    if (factors_replaced(H)) return -1;
     const int B = H->batch;
-    cudaStream_t s = H->stream, s2 = H->stream2;
-    const BatchedLU &d = H->bdev;
+    cudaStream_t s = H->stream;
     std::vector<int> flags(B + 1, INT_MAX);
     flags[B] = 0;
     CU(cudaMemcpyAsync(H->d_flags.p, flags.data(), flags.size() * sizeof(int), cudaMemcpyHostToDevice, s));
     CU(cudaMemsetAsync(H->d_tiny.p, 0, sizeof(unsigned long long), s));
     CU(cudaStreamSynchronize(s));   // `flags` is pageable host memory reused below
-    int64_t launches = 0;
-    const bool lookahead = !H->opt.reserved[0];
-    const int replace_tiny = H->opt.replace_tiny_pivot ? 1 : 0;
-    const int64_t *p64 = H->d_pool_i64.p;
     CU(cudaEventRecord(H->ev0, s));
-    for (size_t li = 0; li < H->levels.size(); ++li) {
-        const LevelPlan &L = H->levels[li];
-        const int32_t *bign = H->d_pool_i32.p + L.big_nodes;
-        const Batch small{H->d_pool_i32.p + L.small_nodes, p64 + L.small_prefix, L.small_count};
-        if (lookahead && li >= 2) CU(cudaStreamWaitEvent(s, H->ev_bulk[li - 2], 0));
-        launches += panel_work(H, d, L, replace_tiny, s);
-        if (lookahead) {
-            CU(cudaEventRecord(H->ev_panel[li], s));
-            launches += launch_schur(d, Batch{bign, p64 + L.urg_prefix, L.big_count}, L.urg_ctas, 1, 1, s);
-            launches += launch_schur(d, small, L.small_ctas, 0, 0, s);
-            CU(cudaStreamWaitEvent(s2, H->ev_panel[li], 0));
-            launches += launch_schur(d, Batch{bign, p64 + L.bulk_prefix, L.big_count}, L.bulk_ctas, 1, 2, s2);
-            CU(cudaEventRecord(H->ev_bulk[li], s2));
-        } else {
-            launches += launch_schur(d, Batch{bign, p64 + L.big_prefix, L.big_count}, L.big_ctas, 1, 0, s);
-            launches += launch_schur(d, small, L.small_ctas, 0, 0, s);
-        }
-    }
-    const size_t nl = H->levels.size();
-    if (lookahead && nl > 0) {
-        CU(cudaStreamWaitEvent(s, H->ev_bulk[nl - 1], 0));
-        if (nl > 1) CU(cudaStreamWaitEvent(s, H->ev_bulk[nl - 2], 0));
-    }
+    const int64_t launches = factor_levels(H, H->bdev, false, false, false);
+    if (launches < 0) return -1;
     CU(cudaEventRecord(H->ev1, s));
     CU(cudaStreamSynchronize(s));
     CU(cudaGetLastError());
@@ -2491,6 +2568,7 @@ int slu_b200_batch_factor(slu_b200_handle_t H, int *info)
     H->st.tiny_pivots = (int64_t)tiny;   // summed over the members
     if (flags[B]) return fail("%d Schur-update destinations were not found in the L/U structure", flags[B]);
     for (int j = 0; j < B; ++j) info[j] = H->member_info[j] = flags[j] == INT_MAX ? 0 : flags[j];
+    CU(cudaMemcpy(H->d_info.p, H->member_info.data(), (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice));
     return 0;
 }
 
@@ -2571,7 +2649,7 @@ static int gscon_impl(slu_b200_handle_t H, char norm, const double *anorm, doubl
     if (any) {
         const size_t len = (size_t)n * B;
         if (batched && H->d_cv.n < len && H->d_cv.alloc(len)) return -1;
-        if (batched ? (H->d_x.n < len && H->d_x.alloc(len)) : (H->d_x.n < len && (H->d_x.alloc(len) || H->d_x2.alloc(len)))) return -1;
+        if (grow(H, H->d_x, len, false, false, fn) || (!batched && grow(H, H->d_x2, len, false, false, fn))) return -1;
         cudaStream_t s = H->stream;
         val_t *v = batched ? H->d_cv.p : H->d_x2.p;       // the pending vectors
         auto apply = [&](int kase, val_t **x) -> int {
@@ -2722,7 +2800,7 @@ int slu_b200_batch_fill_affine(slu_b200_handle_t H, int n, const int32_t *rowptr
     CU(cudaMemcpyAsync(dperm.p, perm, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(dterms.p, terms, (size_t)nnz * nterms * sizeof(val_t), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(dcoef.p, coef, (size_t)B * nterms * sizeof(val_t), cudaMemcpyHostToDevice, s));
-    values_replaced(H);
+    if (values_replaced(H)) return -1;
     CU(cudaMemsetAsync(H->val.p, 0, H->val.bytes(), s));
     CU(cudaMemsetAsync(err, 0, sizeof(int), s));
     launch_fill_affine(H->bdev, n, drp.p, dci.p, dperm.p, dact.p, ddst.p, nnz, nterms, dterms.p, dcoef.p, err, s);
@@ -2780,7 +2858,8 @@ static int fill_scaled_impl(slu_b200_handle_t H, bool batched, int n, const int3
     const int B = batched ? H->batch : 1;
     const int64_t rc_len = (int64_t)n * (rc_per_member ? B : 1);
     if ((R && check_scale(R, rc_len, fn, "R")) || (C && check_scale(C, rc_len, fn, "C"))) return -1;
-    values_replaced(H, true);   // before the buffers of the scaling and the kept A are resized
+    if (pin_check(H, H->d_aci.n != (size_t)nnz || H->d_aval.n != (size_t)nnz * B, fn)) return -1;
+    if (values_replaced(H, true)) return -1;   // before the buffers of the scaling and the kept A are resized
     const bool equil = flags & SLU_B200_FILL_EQUIL;
     double t0 = now_s();
     std::vector<int32_t> pr(n), rmap(n);
@@ -2805,8 +2884,8 @@ static int fill_scaled_impl(slu_b200_handle_t H, bool batched, int n, const int3
     DevBuf<EquilStat> dst;
     DevBuf<int8_t> dact;
     const size_t bn = (size_t)B * n;
-    if ((drp.n != (size_t)n + 1 && drp.alloc((size_t)n + 1)) || (dci.n != (size_t)nnz && dci.alloc((size_t)nnz)) ||
-        (dv.n != (size_t)nnz * B && dv.alloc((size_t)nnz * B)) || dact.upload(act) || dst.upload(st0) ||
+    if ((drp.n != (size_t)n + 1 && drp.alloc((size_t)n + 1)) || grow(H, dci, (size_t)nnz, true, false, fn) ||
+        grow(H, dv, (size_t)nnz * B, true, false, fn) || dact.upload(act) || dst.upload(st0) ||
         dout.alloc((size_t)B * 6) || (R && dRin.alloc((size_t)rc_len)) || (C && dCin.alloc((size_t)rc_len)) ||
         (equil && (drinv.alloc(bn) || dccol.alloc(bn))))
         return -1;
@@ -2911,8 +2990,7 @@ static int solve_scaled_impl(slu_b200_handle_t H, bool batched, double *xh, int 
     if (nrhs < 1 || ldx < n) return fail("%s: bad nrhs / ldx", fn);
     if ((int64_t)n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
     const size_t len = (size_t)n * nrhs * B;
-    if (H->d_x.n < len && H->d_x.alloc(len)) return -1;
-    if (H->d_x2.n < len && H->d_x2.alloc(len)) return -1;
+    if (grow(H, H->d_x, len, false, false, fn) || grow(H, H->d_x2, len, false, false, fn)) return -1;
     cudaStream_t s = H->stream;
     double t0 = now_s();
     CU(cudaMemcpy2DAsync(scaled_in(H, batched), (size_t)n * sizeof(val_t), xh, (size_t)ldx * sizeof(val_t), (size_t)n * sizeof(val_t),
@@ -2978,7 +3056,7 @@ static int gsrfs_impl(slu_b200_handle_t H, bool batched, const double *bh, int l
     if ((int64_t)n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
     const int cols = B * nrhs;
     const size_t len = (size_t)n * cols;
-    if ((H->d_x.n < len && H->d_x.alloc(len)) || (H->d_x2.n < len && H->d_x2.alloc(len)) || (H->d_rb.n < len && H->d_rb.alloc(len)) ||
+    if (grow(H, H->d_x, len, false, false, fn) || grow(H, H->d_x2, len, false, false, fn) || (H->d_rb.n < len && H->d_rb.alloc(len)) ||
         (H->d_rx.n < len && H->d_rx.alloc(len)) || (H->d_rst.n < (size_t)cols && H->d_rst.alloc(cols)) ||
         (!H->d_ract.p && H->d_ract.alloc(1)) || (ferr && ((H->d_rw.n < len && H->d_rw.alloc(len)) || (H->d_cv.n < len && H->d_cv.alloc(len)))))
         return -1;
@@ -3094,6 +3172,17 @@ static int stream_leave(slu_b200_handle_t H, cudaStream_t caller)
     return 0;
 }
 
+// Whether the caller's stream is capturing a CUDA graph: 1 yes, 0 no, < 0 an error.  Every call on the caller's stream asks
+// before it enqueues anything, refuses under capture what would allocate or wait on the host, and marks the handle as
+// captured (pin_check) once it is sure to enqueue.
+static int capturing(slu_b200_handle_t H, cudaStream_t caller, const char *fn)
+{
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    const cudaError_t e = cudaStreamIsCapturing(caller, &cs);
+    if (e != cudaSuccess) return fail("%s: cudaStreamIsCapturing: %s", fn, cudaGetErrorString(e));
+    return cs != cudaStreamCaptureStatusNone;
+}
+
 // New values of the last scaled fill's pattern, val on the device (batch x nnz on a batched handle): the arena zeroed, then
 // F = Pc Pr Dr A Dc Pc^T with the kept perm_r, perm, R and C, bit for bit the scaled fill's values; val also replaces the
 // kept A.  The first refill after a scaled fill builds the slot map (allocates, and waits for it once).
@@ -3103,21 +3192,27 @@ static int refill_impl(slu_b200_handle_t H, bool batched, const double *val, voi
     if (check(H, fn, scaled_need(batched) | SCALED)) return -1;
     if (check_device_ptr(H, val, fn, "val")) return -1;
     const cudaStream_t caller = (cudaStream_t)stream, s = H->stream;
+    const int cap = capturing(H, caller, fn);
+    if (cap < 0) return -1;
+    if (cap && !H->amap_ready)
+        return fail("%s: the first refill after a scaled fill builds the slot map and waits for it: make this call once outside "
+                    "capture first", fn);
     const int n = H->n;
     const int64_t nnz = (int64_t)H->d_aci.n;
     int launches = 0;
     if (!H->amap_ready) {
         DevBuf<int8_t> act;                       // every panel of a 1 x 1 x 1 grid is held
-        if ((H->d_amap.n != (size_t)nnz && (H->d_amap.alloc(nnz) || H->d_arow.alloc(nnz))) || act.alloc(H->nsupers)) return -1;
+        if (grow(H, H->d_amap, nnz, true, false, fn) || grow(H, H->d_arow, nnz, true, false, fn) || act.alloc(H->nsupers)) return -1;
         CU(cudaMemsetAsync(act.p, 1, act.bytes(), s));
         launches += launch_refill_slots(H->dev, n, H->d_arp.p, H->d_aci.p, H->d_rmap.p, H->d_cperm.p, act.p, H->d_amap.p, H->d_arow.p, s);
         CU(cudaStreamSynchronize(s));
         CU(cudaGetLastError());
         H->amap_ready = true;
     }
-    factors_replaced(H);
-    H->uploaded = false;
+    H->captured = H->captured || cap;
     if (stream_enter(H, caller)) return -1;
+    if (factors_replaced(H)) return -1;           // d_info's reset goes into the caller's stream order
+    H->uploaded = false;
     CU(cudaMemsetAsync(H->val.p, 0, H->val.bytes(), s));
     const Refill r{n, nnz, (const val_t *)val, H->d_amap.p, H->d_arow.p, H->d_aci.p, H->d_R.p, H->d_C.p, H->d_aval.p};
     launches += batched ? launch_refill(H->bdev, r, s) : launch_refill(H->dev, r, s);
@@ -3130,35 +3225,86 @@ static int refill_impl(slu_b200_handle_t H, bool batched, const double *val, voi
     return 0;
 }
 
+// factor / batch_factor on the caller's stream: the same level loop, with the info flags and d_tiny reset by a kernel and
+// every member's info written to info (device memory) and d_info by another.  No host wait, copy or allocation: capturable.
+// member_info stays INFO_PENDING until a host-synchronous call settles it.
+static int factor_device_impl(slu_b200_handle_t H, bool batched, int32_t *info, void *stream, const char *fn)
+{
+    if (!H || !info) return fail("%s: null argument", fn);
+    if (check(H, fn, scaled_need(batched) | UPLOADED)) return -1;
+    if (check_device_ptr(H, info, fn, "info")) return -1;
+    const cudaStream_t caller = (cudaStream_t)stream, s = H->stream;
+    const int cap = capturing(H, caller, fn);
+    if (cap < 0) return -1;
+    H->captured = H->captured || cap;
+    const int B = batched ? H->batch : 1;
+    if (stream_enter(H, caller)) return -1;
+    if (factors_replaced(H)) return -1;
+    int64_t launches = launch_factor_begin(H->d_flags.p, B, H->d_tiny.p, s);
+    const int64_t l = batched ? factor_levels(H, H->bdev, false, false, false) : factor_levels(H, H->dev, false, false, false);
+    if (l < 0) return -1;
+    launches += l + launch_factor_info(H->d_flags.p, B, info, H->d_info.p, H->d_epoch.p, s);
+    CU(cudaGetLastError());
+    if (stream_leave(H, caller)) return -1;
+    H->st.t_factor_s = 0;
+    H->st.gpu_launches = launches;
+    std::fill(H->member_info.begin(), H->member_info.end(), INFO_PENDING);
+    H->status_on_device = true;
+    return 0;
+}
+
 // solve / solve_trans (scaled = false: F's ordering) and solve_scaled (A's ordering) on device x, with the host twins' layout
-// and checks; the same device work, with device-to-device copies in place of the H2D and D2H ones.  1 x 1 x 1 grids.
+// and checks; the same device work, with device-to-device copies in place of the H2D and D2H ones.  1 x 1 x 1 grids.  After
+// a device factorization the host has not seen the members' info: the guard turns the x of every member whose d_info is not
+// 0 into NaN.
 static int solve_device_impl(slu_b200_handle_t H, bool batched, bool scaled, double *xd, int ldx, int nrhs, int trans, void *stream,
                              const char *fn)
 {
     if (!H || !xd) return fail("%s: null argument", fn);
-    if (check(H, fn, scaled_need(batched) | (scaled ? SCALED : 0) | FACTORED)) return -1;
+    if (check(H, fn, scaled_need(batched) | (scaled ? SCALED : 0) | FACTORED | DEVICE_ORDERED)) return -1;
     if (trans < 0 || trans > 2) return fail("%s: trans = %d, must be 0 (A x = b), 1 (A^T x = b) or 2 (A^H x = b)", fn, trans);
     const int B = batched ? H->batch : 1, n = H->n;
     if (nrhs < 1 || ldx < n) return fail("%s: bad nrhs / ldx", fn);
     if ((int64_t)n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
     if (check_device_ptr(H, xd, fn, "x")) return -1;
-    const size_t len = (size_t)n * nrhs * B;
-    if ((H->d_x.n < len && H->d_x.alloc(len)) || ((scaled || !batched) && H->d_x2.n < len && H->d_x2.alloc(len))) return -1;
     const cudaStream_t caller = (cudaStream_t)stream, s = H->stream;
+    const int cap = capturing(H, caller, fn);
+    if (cap < 0) return -1;
+    const size_t len = (size_t)n * nrhs * B;
+    if (grow(H, H->d_x, len, false, cap, fn) || ((scaled || !batched) && grow(H, H->d_x2, len, false, cap, fn))) return -1;
+    H->captured = H->captured || cap;
     if (stream_enter(H, caller)) return -1;
     // b goes where each solve takes it: scaled_in, d_x2 for solve_dev, d_x for the batched passes
     val_t *in = scaled ? scaled_in(H, batched) : batched ? H->d_x.p : H->d_x2.p, *result = scaled ? H->d_x2.p : H->d_x.p;
     const size_t w = (size_t)n * sizeof(val_t), pitch = (size_t)ldx * sizeof(val_t);
     CU(cudaMemcpy2DAsync(in, w, xd, pitch, w, (size_t)nrhs * B, cudaMemcpyDeviceToDevice, s));
-    const int launches = scaled ? solve_scaled_dev(H, batched, nrhs, trans)
-                                : batched ? solve_passes(H, H->bdev, nrhs, trans) : solve_dev(H, nrhs, trans, &result);
+    int launches = scaled ? solve_scaled_dev(H, batched, nrhs, trans)
+                          : batched ? solve_passes(H, H->bdev, nrhs, trans) : solve_dev(H, nrhs, trans, &result);
     if (launches < 0) return -1;
+    launches += launch_solve_guard(result, H->d_info.p, (int64_t)n * nrhs, B, s);
     CU(cudaMemcpy2DAsync(xd, pitch, result, w, w, (size_t)nrhs * B, cudaMemcpyDeviceToDevice, s));
     CU(cudaGetLastError());
     if (stream_leave(H, caller)) return -1;
     H->st.reserved[4] = 0;
     H->st.reserved[5] = (double)launches;
     return 0;
+}
+
+int slu_b200_get_device(slu_b200_handle_t H, int *device)
+{
+    if (!H || !device) return fail(SLU_API "get_device: null argument");
+    *device = H->device;
+    return 0;
+}
+
+int slu_b200_factor_device(slu_b200_handle_t H, int32_t *info, void *stream)
+{
+    return factor_device_impl(H, false, info, stream, SLU_API "factor_device");
+}
+
+int slu_b200_batch_factor_device(slu_b200_handle_t H, int32_t *info, void *stream)
+{
+    return factor_device_impl(H, true, info, stream, SLU_API "batch_factor_device");
 }
 
 int slu_b200_refill(slu_b200_handle_t H, const double *val, void *stream)
@@ -3227,6 +3373,7 @@ int slu_b200_batch_schur_expand(slu_b200_handle_t H, double *x, int ldx, int nrh
 int slu_b200_get_stats(slu_b200_handle_t H, slu_b200_stats_t *out)
 {
     if (!H || !out) return fail("null argument");
+    if (settle(H)) return -1;
     *out = H->st;
     return 0;
 }

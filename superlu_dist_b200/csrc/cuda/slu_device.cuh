@@ -247,6 +247,13 @@ struct Refill {
 };
 int launch_refill(const DeviceLU &d, const Refill &r, cudaStream_t s);
 int launch_refill(const BatchedLU &d, const Refill &r, cudaStream_t s);
+// the status of a factorization on the device (slu_b200_factor_device and its batched / z twins), 1 launch each.  begin:
+// flags[0 .. members) = INT_MAX, the error slot flags[members] = 0, *tiny = 0.  info: out[j] = status[j] = -1 if the error
+// slot is not 0, else 0 or member j's first zero pivot (flags[j], 1-based), and ++*epoch.  guard: x holds members blocks of len elements;
+// the block of every member whose status is not 0 becomes quiet NaN.
+int launch_factor_begin(int *flags, int members, unsigned long long *tiny, cudaStream_t s);
+int launch_factor_info(const int *flags, int members, int32_t *out, int32_t *status, unsigned long long *epoch, cudaStream_t s);
+int launch_solve_guard(val_t *x, const int32_t *status, int64_t len, int members, cudaStream_t s);
 // the vector transforms of slu_b200_solve_scaled, over (entries, members) with members blocks of n x nrhs (scale: n per
 // member): scatter dst[map[i]] = scale[i] src[i], else gather dst[i] = scale[i] src[map[i]]
 int launch_permute_scale(val_t *dst, const val_t *src, const int32_t *map, const double *scale, int n, int nrhs, int members,

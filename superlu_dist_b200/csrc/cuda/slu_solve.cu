@@ -21,6 +21,8 @@
 #include "slu_kernels_common.cuh"
 #include "slu_scalar.cuh"
 
+#include <algorithm>
+#include <climits>
 #include <type_traits>
 
 namespace SLU_NS {
@@ -611,6 +613,66 @@ static int launch_refill_t(const LU &d, const Refill &r, cudaStream_t s)
 }
 int launch_refill(const DeviceLU &d, const Refill &r, cudaStream_t s) { return launch_refill_t(d, r, s); }
 int launch_refill(const BatchedLU &d, const Refill &r, cudaStream_t s) { return launch_refill_t(d, r, s); }
+
+// ---- the status of a factorization on the device (slu_b200_factor_device) ----
+// flags = [members] info slots (INT_MAX: no zero pivot) and the error slot after them; one CTA strides over the members
+constexpr int STATUS_THREADS = 256;
+__global__ void __launch_bounds__(STATUS_THREADS) factor_begin_kernel(int *__restrict__ flags, int members, unsigned long long *__restrict__ tiny)
+{
+    for (int j = threadIdx.x; j <= members; j += STATUS_THREADS) flags[j] = j < members ? INT_MAX : 0;
+    if (threadIdx.x == 0) *tiny = 0;
+}
+
+int launch_factor_begin(int *flags, int members, unsigned long long *tiny, cudaStream_t s)
+{
+    factor_begin_kernel<<<1, STATUS_THREADS, 0, s>>>(flags, members, tiny);
+    return 1;
+}
+
+// info of member j: -1 when a Schur-update destination was missing (the error slot counts them), else 0 or the 1-based column
+// of the first exact zero pivot; one more factorization in *epoch
+__global__ void __launch_bounds__(STATUS_THREADS) factor_info_kernel(const int *__restrict__ flags, int members, int32_t *__restrict__ out,
+                                                                   int32_t *__restrict__ status, unsigned long long *__restrict__ epoch)
+{
+    const bool err = flags[members] != 0;
+    if (threadIdx.x == 0) ++*epoch;
+    for (int j = threadIdx.x; j < members; j += STATUS_THREADS) {
+        const int f = flags[j];
+        const int32_t v = err ? -1 : f == INT_MAX ? 0 : f;
+        out[j] = v;
+        status[j] = v;
+    }
+}
+
+int launch_factor_info(const int *flags, int members, int32_t *out, int32_t *status, unsigned long long *epoch, cudaStream_t s)
+{
+    factor_info_kernel<<<1, STATUS_THREADS, 0, s>>>(flags, members, out, status, epoch);
+    return 1;
+}
+
+// grid (element tiles, members): member blockIdx.y's block of len elements becomes quiet NaN (both parts in complex) where its
+// status is not 0; the other members' blocks are not touched
+__global__ void __launch_bounds__(STATUS_THREADS) solve_guard_kernel(val_t *__restrict__ x, const int32_t *__restrict__ status, int64_t len)
+{
+    const int64_t m = blockIdx.y;
+    if (status[m] == 0) return;
+    const double q = __longlong_as_double(0x7ff8000000000000LL);
+    val_t v;
+#ifdef SLU_COMPLEX
+    v = make_double2(q, q);
+#else
+    v = q;
+#endif
+    for (int64_t i = (int64_t)blockIdx.x * STATUS_THREADS + threadIdx.x; i < len; i += (int64_t)gridDim.x * STATUS_THREADS) x[m * len + i] = v;
+}
+
+int launch_solve_guard(val_t *x, const int32_t *status, int64_t len, int members, cudaStream_t s)
+{
+    if (len <= 0 || members <= 0) return 0;
+    const unsigned tiles = (unsigned)std::min<int64_t>((len + STATUS_THREADS - 1) / STATUS_THREADS, 1024);
+    solve_guard_kernel<<<dim3(tiles, (unsigned)members), STATUS_THREADS, 0, s>>>(x, status, len);
+    return 1;
+}
 
 // thread = entry i of the member blockIdx.y, every right-hand side
 template <bool SCATTER>
