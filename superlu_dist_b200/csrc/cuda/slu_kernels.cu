@@ -326,7 +326,9 @@ __device__ __forceinline__ int pk(int k) { return (k & ~7) | ((k & 3) << 1) | ((
 //   L case: vectors = sub-diagonal rows of panel k, T(p,c) = U_kk(p,c)            (non-unit)
 //   U case: vectors = packed columns of U(k,:),    T(p,c) = L_kk(c,p) (transposed, unit)
 // The 16x16 diagonal blocks are inverted once per supernode by diag_inv_kernel; everything else is
-// substitution, so the only departure from the reference's dtrsm is inside a 16x16 block.
+// substitution.  Inside a block, R = Y_j - sum is multiplied by the inverse and then corrected once,
+// X = R inv + (R - (R inv) T_jj) inv: the product with an explicit inverse alone has a backward error that
+// grows with cond(T_jj) on consistent right-hand sides, the correction brings it to substitution's.
 // ------------------------------------------------------------------------------------------------
 template <class LU>
 __global__ void __launch_bounds__(64) diag_inv_kernel(LU dd, Batch b, double *dinv)
@@ -405,6 +407,7 @@ constexpr int TRSM_THREADS = 128, TRSM_KC = 64;
 constexpr int TRSM_LD = TRSM_STRIP + 4;   // == 4 (mod 16) doubles: conflict-free A fragments
 constexpr int TRSM_LDT = TRSM_KC + 8;     // == 8 (mod 16): conflict-free B fragments
 static_assert(TRSM_STRIP == 32 && TRSM_THREADS == 128 && TRSM_KC % 16 == 0, "trsm_kernel thread mapping");
+static_assert(2 * 16 * TRSM_LD <= 16 * TRSM_LDT, "X and R - X T_jj of a block fit in one T buffer");
 static size_t trsm_smem(int max_ns)
 {
     return sizeof(double) * ((size_t)((max_ns + 15) & ~15) * TRSM_LD + 2 * 16 * TRSM_LDT);
@@ -491,14 +494,21 @@ __global__ void __launch_bounds__(TRSM_THREADS, 2) trsm_kernel(LU dd, Batch b, c
     const double *const tb = Tb + (8 * nt + g) * TRSM_LDT + 2 * t;         // B fragment of k8 slice q: tb + 8 q
     int buf = 0;
     for (int j0 = 0; j0 < ns; j0 += 16) {
-        const double *ib = inv + (size_t)(j0 >> 4) * 512;   // loaded ahead: the latency hides behind the update
-        double bi[2][2];
+        // inv(T_jj) and T_jj itself, loaded ahead: the latency hides behind the update.  T_jj is padded with the
+        // identity beyond jb as diag_inv_kernel pads it; in the U case its diagonal is 1 (the stored one holds U's pivots).
+        const double *ib = inv + (size_t)(j0 >> 4) * 512;
+        const int jb = min(16, ns - j0);
+        double bi[2][2], bt[2][2];
 #pragma unroll
         for (int kk = 0; kk < 2; ++kk)
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int p = 8 * kk + 4 * h + t, c = 8 * nt + g;
                 bi[kk][h] = UCASE ? ib[256 + p * 16 + c] : ib[c * 16 + p];
+                double v = (p == c) ? 1.0 : 0.0;
+                if (c < jb && (UCASE ? p < c : p <= c))
+                    v = UCASE ? T[(size_t)(j0 + p) * lda + j0 + c] : T[(size_t)(j0 + c) * lda + j0 + p];
+                bt[kk][h] = v;
             }
         double acc[4][4];
 #pragma unroll
@@ -528,18 +538,35 @@ __global__ void __launch_bounds__(TRSM_THREADS, 2) trsm_kernel(LU dd, Batch b, c
 #pragma unroll
         for (int e = 0; e < 4; ++e) sum[e] = (acc[0][e] + acc[1][e]) + (acc[2][e] + acc[3][e]);
         const double2 y0 = *d0, y1 = *d1;
-        *d0 = make_double2(y0.x - sum[0], y0.y - sum[2]);
-        *d1 = make_double2(y1.x - sum[1], y1.y - sum[3]);
-        __syncthreads();   // the product with inv(T_jj) reads both column halves of the block
-        double o[4] = {0.0, 0.0, 0.0, 0.0};
+        const double r[4] = {y0.x - sum[0], y1.x - sum[1], y0.y - sum[2], y1.y - sum[3]};   // R = Y_j - sum, kept
+        *d0 = make_double2(r[0], r[2]);
+        *d1 = make_double2(r[1], r[3]);
+        __syncthreads();   // each product with a 16-row right factor reads both column halves of the block
+        // X = R inv, then the correction X += (R - X T_jj) inv; X and R - X T_jj pass between the warps through the
+        // T buffer that the sweep is not fetching into (it is refilled only after the next block's first barrier).
+        double *const xw = Tb + (buf ^ 1) * 16 * TRSM_LDT, *const cw = xw + 16 * TRSM_LD;
+        const size_t dofs = (size_t)(8 * nt + 2 * t) * TRSM_LD + 16 * mt + 2 * g;
+        const size_t aofs = (size_t)t * TRSM_LD + 16 * mt + 2 * g;
+        auto mul16 = [&](double (&acc)[4], const double *a0, const double (&b)[2][2]) {
 #pragma unroll
-        for (int kk = 0; kk < 2; ++kk) {
-            const double2 lo = *reinterpret_cast<const double2 *>(ya + (size_t)(j0 + 8 * kk) * TRSM_LD);
-            const double2 hi = *reinterpret_cast<const double2 *>(ya + (size_t)(j0 + 8 * kk + 4) * TRSM_LD);
-            const double a[4] = {lo.x, lo.y, hi.x, hi.y};
-            dmma1688(o, a, bi[kk]);
-        }
+            for (int kk = 0; kk < 2; ++kk) {
+                const double2 lo = *reinterpret_cast<const double2 *>(a0 + (size_t)(8 * kk) * TRSM_LD);
+                const double2 hi = *reinterpret_cast<const double2 *>(a0 + (size_t)(8 * kk + 4) * TRSM_LD);
+                const double a[4] = {lo.x, lo.y, hi.x, hi.y};
+                dmma1688(acc, a, b[kk]);
+            }
+        };
+        double o[4] = {0.0, 0.0, 0.0, 0.0};
+        mul16(o, ya + (size_t)j0 * TRSM_LD, bi);
+        *reinterpret_cast<double2 *>(xw + dofs) = make_double2(o[0], o[2]);
+        *reinterpret_cast<double2 *>(xw + dofs + TRSM_LD) = make_double2(o[1], o[3]);
         __syncthreads();
+        double xt[4] = {0.0, 0.0, 0.0, 0.0};
+        mul16(xt, xw + aofs, bt);
+        *reinterpret_cast<double2 *>(cw + dofs) = make_double2(r[0] - xt[0], r[2] - xt[2]);
+        *reinterpret_cast<double2 *>(cw + dofs + TRSM_LD) = make_double2(r[1] - xt[1], r[3] - xt[3]);
+        __syncthreads();
+        mul16(o, cw + aofs, bi);
         *d0 = make_double2(o[0], o[2]);
         *d1 = make_double2(o[1], o[3]);
     }

@@ -239,7 +239,8 @@ int launch_diag_inv(const BatchedLU &d, const Batch &b, int64_t ctas, zd *dinv, 
 //   L case: vectors = sub-diagonal rows of panel k, T(p,c) = U_kk(p,c)            (non-unit)
 //   U case: vectors = packed columns of U(k,:),    T(p,c) = L_kk(c,p) (transposed, unit)
 // A CTA keeps a strip of 32 vectors in shared memory (Ys[c][s]); 256 threads = 32 vectors x 8 column lanes, each
-// thread owns columns cl and cl + 8 of the current 16-column block.
+// thread owns columns cl and cl + 8 of the current 16-column block.  Each block is multiplied by the inverse of
+// T_jj and corrected once with it, as in slu_kernels.cu.
 // ------------------------------------------------------------------------------------------------
 constexpr int TZ_LD = TRSM_STRIP + 1;
 
@@ -299,19 +300,48 @@ __global__ void __launch_bounds__(256) trsm_kernel(LU dd, Batch b, const zd *din
 #pragma unroll
         for (int h = 0; h < 2; ++h) Tmp[(cl + 8 * h) * TZ_LD + s] = acc[h];
         __syncthreads();
-        // (2) Y(s, j0 + c) = sum_q tmp(s, q) Inv(q, c)
+        // (2) x(s, c) = sum_q tmp(s, q) Inv(q, c), then one correction step x += (tmp - x T_jj) Inv: the product with
+        // an explicit inverse alone has a backward error that grows with cond(T_jj) on consistent right-hand sides
         const zd *ib = inv + (size_t)(j0 >> 4) * 512;
+        const int jb = min(16, ns - j0);
         zd out[2] = {zmake(0.0, 0.0), zmake(0.0, 0.0)};
+        auto mul_inv = [&]() {
 #pragma unroll
-        for (int q = 0; q < 16; ++q) {
-            const zd y = Tmp[q * TZ_LD + s];
+            for (int q = 0; q < 16; ++q) {
+                const zd y = Tmp[q * TZ_LD + s];
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int c = cl + 8 * h;
-                const zd t = UCASE ? __ldg(ib + 256 + q * 16 + c) : __ldg(ib + c * 16 + q);
-                zaddmul(out[h], y, t);
+                for (int h = 0; h < 2; ++h) {
+                    const int c = cl + 8 * h;
+                    const zd t = UCASE ? __ldg(ib + 256 + q * 16 + c) : __ldg(ib + c * 16 + q);
+                    zaddmul(out[h], y, t);
+                }
             }
+        };
+        mul_inv();
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int c = j0 + cl + 8 * h;
+            if (c < ns) Ys[c * TZ_LD + s] = out[h];
         }
+        __syncthreads();
+        // tmp - x T_jj, T_jj(q, c) for q <= c < jb; in the U case its diagonal is 1 (the stored one holds U's pivots)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int c = cl + 8 * h;
+            zd r = zmake(0.0, 0.0);
+            if (c < jb) {
+                r = acc[h];
+                for (int q = 0; q <= c; ++q) {
+                    const zd x = Ys[(j0 + q) * TZ_LD + s];
+                    if (UCASE && q == c) r = zmake(r.x - x.x, r.y - x.y);
+                    else zsubmul(r, x, UCASE ? __ldg(T + (size_t)(j0 + q) * lda + j0 + c)
+                                             : __ldg(T + (size_t)(j0 + c) * lda + j0 + q));
+                }
+            }
+            Tmp[c * TZ_LD + s] = r;   // every thread read its tmp in (2), before the barrier above
+        }
+        __syncthreads();
+        mul_inv();
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int c = j0 + cl + 8 * h;

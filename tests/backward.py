@@ -180,6 +180,46 @@ def trsm_u_input(family, ns, nc, seed, z=False):
     return lo, b
 
 
+# Consistent right-hand sides: B = X T formed in extended precision and rounded, X uniform in [-1, 1], the kind of B a
+# factorization hands the panel TRSM (B = L U_kk with moderate L).  A random B makes X as large as the conditioning of T
+# allows, and then even a product with an explicit inverse of T_jj passes; with a consistent B that product has a
+# backward error that grows with cond(T_jj), while substitution's does not.  One column is planted per chosen 16-column
+# block (the first, a middle and the last, possibly partial, one) at in-block offsets 1, 7 and 14, rotated by ns mod 3.
+DELTAS = [1e-4, 1e-8, 1e-12]
+CWIDTHS = [w for w in WIDTHS if w >= 16]
+ZCWIDTHS = [w for w in ZWIDTHS if w >= 16]
+CVECS = 33   # crosses the 32-vector TRSM strip
+
+
+def consistent_positions(ns):
+    nb = (ns + 15) // 16
+    offs = np.roll((1, 7, 14), ns % 3)
+    return sorted({min(16 * blk + int(o), ns - 1) for blk, o in zip(sorted({0, nb // 2, nb - 1}), offs)})
+
+
+def trsm_l_consistent(ns, m, delta, positions, seed, z=False):
+    """(U, B) of X U = B: U upper, off-diagonal uniform in [-1, 1], pivots of modulus in [1, 2] (random phase in complex)
+    but delta (times the phase) at `positions`"""
+    rng = np.random.default_rng(seed)
+    u = np.triu(_rand(rng, (ns, ns), z, "uniform"), 1)
+    d = rng.uniform(1.0, 2.0, ns)
+    d[list(positions)] = delta
+    u = u + np.diag(d * np.exp(2j * np.pi * rng.uniform(size=ns)) if z else d * rng.choice([-1.0, 1.0], ns))
+    x = _rand(rng, (m, ns), z, "uniform")
+    return u, (ext(x) @ ext(u)).astype(u.dtype)
+
+
+def trsm_u_consistent(ns, nc, delta, positions, seed, z=False):
+    """(L, B) of L X = B: L unit lower, multipliers uniform in [-1, 1], those of the columns at `positions` times
+    delta^-1/2 (the multipliers below a pivot of delta in a factor whose |L| |U| stays moderate)"""
+    rng = np.random.default_rng(seed)
+    lo = np.tril(_rand(rng, (ns, ns), z, "uniform"), -1)
+    lo[:, list(positions)] *= delta ** -0.5
+    lo = lo + np.eye(ns)
+    x = _rand(rng, (ns, nc), z, "uniform")
+    return lo, (ext(lo) @ ext(x)).astype(lo.dtype)
+
+
 GEMM_SHAPES = [(1, 1, 1), (33, 31, 7), (96, 97, 17), (128, 130, 100), (257, 131, 137), (200, 97, 256), (129, 300, 513)]
 GEMM_FAMILIES = ["random", "cancel", "scaled"]
 
@@ -240,15 +280,22 @@ def _inv_unit_lower16(lo):
     return x
 
 
-def trsm_blocked(t, b, unit):
-    """trsm_kernel's algorithm in NumPy: Y <- Y T^-1 blocked by 16 columns, Y_j <- (Y_j - sum_{p<j} Y_p T_pj) inv(T_jj)
-    with the explicit 16 x 16 inverses of diag_inv_kernel.  unit: T = L^T of a unit lower L (the U case)."""
+def trsm_blocked(t, b, unit, refine=1):
+    """trsm_kernel's algorithm in NumPy: Y <- Y T^-1 blocked by 16 columns; with R = Y_j - sum_{p<j} Y_p T_pj and the
+    explicit 16 x 16 inverse of diag_inv_kernel, X = R inv(T_jj), then `refine` correction steps X += (R - X T_jj) inv.
+    unit: T = L^T of a unit lower L (the U case; the diagonal of T is taken as 1).  refine=0 is the plain product with
+    the inverse, which is not backward stable on consistent right-hand sides: kept to show that the tests see it."""
     ns = t.shape[0]
     y = b.copy()
     for j0 in range(0, ns, 16):
         j1 = min(ns, j0 + 16)
-        inv = _inv_unit_lower16(t[j0:j1, j0:j1].T).T if unit else _inv_upper16(t[j0:j1, j0:j1])
-        y[:, j0:j1] = (y[:, j0:j1] - y[:, :j0] @ t[:j0, j0:j1]) @ inv
+        tjj = np.triu(t[j0:j1, j0:j1], 1) + np.eye(j1 - j0) if unit else np.triu(t[j0:j1, j0:j1])
+        inv = _inv_unit_lower16(tjj.T).T if unit else _inv_upper16(tjj)
+        r = y[:, j0:j1] - y[:, :j0] @ t[:j0, j0:j1]
+        x = r @ inv
+        for _ in range(refine):
+            x = x + (r - x @ tjj) @ inv
+        y[:, j0:j1] = x
     return y
 
 
@@ -401,6 +448,94 @@ SHIFT_N, SHIFT_KW = 12, dict(N=12, leaf=8, relax=16, maxsup=128)
 def shift_sigma():
     from test_inertia_cpu import gap_shifts, spectrum
     return gap_shifts(spectrum(SHIFT_N), 7)[3]
+
+
+# Planted factors: F = fl(L0 U0) with moderate L0 and U0 on the panel pattern, so that every panel TRSM of the
+# factorization of F gets a consistent right-hand side; small pivots are planted in the widest supernodes (PLANTED_DELTA).
+# "w512": fem 8^3 x 3 relaxed into supernodes of 512, 384, 288 and 256 columns (panels up to 768 rows).
+PLANTED = {"top256": PROBLEMS["top256"], "fem6": PROBLEMS["fem6"],
+           "w512": dict(N=8, leaf=8, relax=512, maxsup=512, fem=3)}
+ZPLANTED = {"z200": ZPROBLEMS["z200"]}
+PLANTED_DELTA = 1e-6     # a computed pivot of delta perturbs what follows by ~ u / delta: keep the others planted
+PLANTED_MULT = 1e4       # the multipliers of the scaled columns (their U rows scaled by its inverse)
+PLANTED_NODES = 3        # the widest supernodes get the planted pivots
+
+
+def planted_nodes(prob, count=PLANTED_NODES):
+    ns = np.diff(np.asarray(prob.xsup))
+    return sorted(np.argsort(-ns, kind="stable")[:count].tolist())
+
+
+def plant_factors(prob, delta=PLANTED_DELTA, mult=PLANTED_MULT, seed=0, nodes=None):
+    """L0 (unit lower) and U0 (upper) on the panel pattern of layer 0: entries uniform in [-1, 1] scaled by 1 / sqrt of
+    the supernode's width, pivots of modulus in [1, 2] with random signs (phases in complex).  In each supernode of
+    `nodes` (default: the widest), at the positions consistent_positions(ns) picks: a pivot of delta (an ill-conditioned
+    U_kk for the L-panel TRSM); and two columns on, multipliers scaled by mult and the U row beside the pivot by 1 / mult
+    (an ill-conditioned L_kk for the U-panel TRSM; that column of L0 times that row of U0 stays O(1)).  Writes
+    F = fl(L0 U0) into layer 0 and checks that no entry of F falls outside the panels.  -> F as CSR."""
+    lay = prob.layers[0]
+    z = np.iscomplexobj(lay.lval)
+    rng = np.random.default_rng(seed)
+    lrow, lcol, urow, ucol = panel_coords(prob, lay)
+    xsup = np.asarray(prob.xsup)
+    n = prob.n
+    width = np.diff(xsup)[np.searchsorted(xsup, np.arange(n), side="right") - 1]
+    lk, uk = lrow >= 0, urow >= 0
+    rows = np.concatenate([lrow[lk], urow[uk]])
+    cols = np.concatenate([lcol[lk], ucol[uk]])
+    vals = _rand(rng, len(rows), z, "uniform") / np.sqrt(width[np.minimum(rows, cols)])
+    piv = rng.uniform(1.0, 2.0, n) * (np.exp(2j * np.pi * rng.uniform(size=n)) if z else rng.choice([-1.0, 1.0], n))
+    lscale, uscale = np.ones(n), np.ones(n)
+    for k in (planted_nodes(prob) if nodes is None else nodes):
+        f, ns = int(xsup[k]), int(xsup[k + 1] - xsup[k])
+        for p in consistent_positions(ns):
+            piv[f + p] *= delta
+            q = f + (p + 2) % ns
+            lscale[q], uscale[q] = mult, 1.0 / mult
+    low, dia = rows > cols, rows == cols
+    vals = np.where(low, vals * lscale[cols], vals * uscale[rows])
+    vals[dia] = piv[rows[dia]]
+    L0 = _csr(np.concatenate([rows[low], np.arange(n)]), np.concatenate([cols[low], np.arange(n)]),
+              np.concatenate([vals[low], np.ones(n, vals.dtype)]), n)
+    U0 = _csr(rows[~low], cols[~low], vals[~low], n)
+    F = (ext(L0) @ ext(U0)).astype(vals.dtype).tocsr()
+    assert np.isin(_keys(F)[0], rows.astype(np.int64) * n + cols).all(), "an entry of L0 U0 falls outside the panels"
+    lay.lval[lk] = np.asarray(F[lrow[lk], lcol[lk]]).ravel()
+    lay.uval[uk] = np.asarray(F[urow[uk], ucol[uk]]).ravel()
+    return F
+
+
+def to_csr(F, perm):
+    """The CSR (rowptr, colind, values) of A = P^T F P, perm[old] = new: what fill_csr takes to put F into the panels"""
+    perm = np.asarray(perm)
+    A = F.tocsr()[perm][:, perm].tocsr()
+    A.sort_indices()
+    return A.indptr.astype(np.int32), A.indices.astype(np.int32), A.data
+
+
+def panel_trsm_ratios(prob, L, Uf, refine, nodes=None):
+    """The panel TRSMs of a factorization restated on its factors: for supernode k with columns f..l, X_L U_kk = B_L and
+    L_kk X_U = B_U with X_L, X_U the L rows below and the U columns right of the diagonal block, and B formed from them
+    in extended precision; trsm_blocked(refine) solves.  -> the largest ratio / kernel_bound(ns) of each case"""
+    xsup = np.asarray(prob.xsup)
+    L, Uf = L.tocsc(), Uf.tocsr()
+    worst = [0.0, 0.0]
+    for k in (range(prob.nsupers) if nodes is None else nodes):
+        f, l = int(xsup[k]), int(xsup[k + 1])
+        ukk = Uf[f:l, f:l].toarray()
+        lkk = L[f:l, f:l].toarray()
+        xl = L[l:, f:l].tocsr()
+        xl = xl[np.diff(xl.indptr) > 0].toarray()
+        xu = Uf[f:l, l:].tocsc()
+        xu = xu[:, np.diff(xu.indptr) > 0].toarray()
+        bound = kernel_bound(l - f, prob.dtype)
+        if len(xl):
+            b = (ext(xl) @ ext(ukk)).astype(xl.dtype)
+            worst[0] = max(worst[0], trsm_l_ratio(ukk, b, trsm_blocked(ukk, b, False, refine)) / bound)
+        if xu.shape[1]:
+            b = (ext(lkk) @ ext(xu)).astype(xu.dtype)
+            worst[1] = max(worst[1], trsm_u_ratio(lkk, b, trsm_blocked(lkk.T, b.T, True, refine).T) / bound)
+    return tuple(worst)
 
 
 def kkt_matrix():
