@@ -540,6 +540,34 @@ int slu_b200_batch_solve_scaled_device(slu_b200_handle_t h, double *x, int ldx, 
  * a graph that uses it is alive is the caller's error, as with any CUDA library workspace. */
 int slu_b200_factor_device(slu_b200_handle_t h, int32_t *info, void *stream);
 int slu_b200_batch_factor_device(slu_b200_handle_t h, int32_t *info, void *stream);
+/* ---- iterative refinement and condition estimation on the caller's CUDA stream, capturable into the same graph.
+ * gsrfs_device / batch_gsrfs_device: slu_b200_gsrfs / _batch_gsrfs (A x = b on the factors and scalings of the last scaled
+ * fill or refill and the A it kept) with b, x, berr and the nullable ferr and steps in device memory, in the host twins'
+ * layouts (outputs: one value per (member, column), member-major); they compute what the host twins compute.
+ * gscon_device / batch_gscon_device: slu_b200_gscon / _batch_gscon (dlacn2 on F after a fill and a factorization) with anorm
+ * and rcond in device memory, one value per member; norm '1', 'O' or 'I'.
+ * Preconditions, pointer checks, stream order and refusals are those of solve_device / solve_scaled_device above: 1 x 1 x 1
+ * grids, no Schur handles, gsrfs_device needs a scaled fill; factors pending from factor_device are taken as they are.  No
+ * host wait, PCIe copy or allocation, except where a buffer grows: the first call of each kind, or a gsrfs_device with more
+ * right-hand sides than any before, allocates and must be made once outside capture (under capture it is refused before
+ * anything is enqueued, leaving the capture valid).  The loops run on the device: each is a conditional WHILE node of a CUDA
+ * graph whose body decides, on the device, whether it runs again (the estimator's body runs its solve in one of two IF
+ * nodes), with the host loops' kernels, so the device loops take the same decisions on the same vectors.  Called under
+ * capture, the nodes go into the caller's graph; called eagerly, the handle launches a graph of the same sequence that it
+ * captured at the first such call (one per kind, batched, nrhs and ferr; captured again when a buffer it holds moved).  That
+ * first eager call of each kind, nrhs and ferr instantiates its graph, which may wait for the device once.
+ * A member whose status is not 0 (a zero pivot from factor_device, which the host has not seen): x, berr, ferr and rcond
+ * NaN, steps 0, its columns never refined; the other members are unaffected.  An estimate that does not finish in 64 solves
+ * (where the host calls fail) gives NaN ferr / rcond for the members still waiting.  gscon_device: rcond 0 for anorm 0 or
+ * +inf, NaN for a negative or NaN anorm (refused by the host call).  stats.reserved[4] = 0, [5] = the launches enqueued
+ * outside the loops plus one pass of each loop body (both IF bodies); gscon_device sets [6] and [7] to 0.
+ * Needs a CUDA driver of version 12.4 or later (conditional nodes); an older one is refused, naming its version. */
+int slu_b200_gsrfs_device(slu_b200_handle_t h, const double *b, int ldb, double *x, int ldx, int nrhs, double *berr,
+                          double *ferr, int32_t *steps, void *stream);
+int slu_b200_batch_gsrfs_device(slu_b200_handle_t h, const double *b, int ldb, double *x, int ldx, int nrhs, double *berr,
+                                double *ferr, int32_t *steps, void *stream);
+int slu_b200_gscon_device(slu_b200_handle_t h, char norm, const double *anorm, double *rcond, void *stream);
+int slu_b200_batch_gscon_device(slu_b200_handle_t h, char norm, const double *anorm, double *rcond, void *stream);
 /* the CUDA device the handle was created on (options.device, or the current device when that was < 0): where the
  * device-memory arguments of the calls above must live */
 int slu_b200_get_device(slu_b200_handle_t h, int *device);
@@ -649,6 +677,14 @@ int slu_b200_z_batch_solve_scaled_device(slu_b200_zhandle_t h, double *x, int ld
 int slu_b200_z_factor_device(slu_b200_zhandle_t h, int32_t *info, void *stream);
 int slu_b200_z_batch_factor_device(slu_b200_zhandle_t h, int32_t *info, void *stream);
 int slu_b200_z_get_device(slu_b200_zhandle_t h, int *device);
+/* as slu_b200_gsrfs_device / _gscon_device and their batched twins: b and x interleaved doublecomplex on the device (ldb, ldx
+ * count complex elements); berr, ferr, anorm and rcond real */
+int slu_b200_z_gsrfs_device(slu_b200_zhandle_t h, const double *b, int ldb, double *x, int ldx, int nrhs, double *berr,
+                            double *ferr, int32_t *steps, void *stream);
+int slu_b200_z_batch_gsrfs_device(slu_b200_zhandle_t h, const double *b, int ldb, double *x, int ldx, int nrhs,
+                                  double *berr, double *ferr, int32_t *steps, void *stream);
+int slu_b200_z_gscon_device(slu_b200_zhandle_t h, char norm, const double *anorm, double *rcond, void *stream);
+int slu_b200_z_batch_gscon_device(slu_b200_zhandle_t h, char norm, const double *anorm, double *rcond, void *stream);
 int slu_b200_z_get_stats(slu_b200_zhandle_t h, slu_b200_stats_t *out);
 int slu_b200_z_plan(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, slu_b200_stats_t *stats);
 void slu_b200_z_destroy(slu_b200_zhandle_t h);

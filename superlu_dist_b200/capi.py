@@ -173,6 +173,12 @@ def lib():
         getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     for f in ("slu_b200_get_device", "slu_b200_z_get_device"):
         getattr(L, f).argtypes = [C.c_void_p, C.c_void_p]
+    for f in ("gsrfs_device", "batch_gsrfs_device"):
+        for pre in ("slu_b200_", "slu_b200_z_"):
+            getattr(L, pre + f).argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 4
+    for f in ("gscon_device", "batch_gscon_device"):
+        for pre in ("slu_b200_", "slu_b200_z_"):
+            getattr(L, pre + f).argtypes = [C.c_void_p, C.c_char, C.c_void_p, C.c_void_p, C.c_void_p]
     _lib = L
     return L
 
@@ -278,6 +284,44 @@ def _solve_device(name, complex_, h, b, n, batch, trans):
     nrhs = 1 if b.dim() == nd else b.shape[-2]
     _check(_fn(name, complex_)(h, C.c_void_p(x.data_ptr()), n, nrhs, _TRANS[trans], stream))
     return x
+
+
+def _refine_device(name, complex_, h, b, x, n, batch, ferr):
+    """slu_b200_[z_][batch_]gsrfs_device on CUDA tensors b and x of solve_scaled's shapes, on the current stream of their
+    device -> (new refined x, berr float64, steps int32, ferr float64 or None), the outputs of shape b.shape[:-1]"""
+    import torch
+    lead = () if batch is None else (batch,)
+    nd = len(lead) + 1
+    if (not _is_tensor(x) or tuple(b.shape) != tuple(x.shape) or b.dim() not in (nd, nd + 1) or tuple(b.shape[:len(lead)]) != lead
+            or b.shape[-1] != n):
+        raise ValueError(f"b and x must both be CUDA tensors of shape {lead + (n,)} or {lead + ('nrhs', n)}")
+    b, stream = _device_args(b, complex_, None, "b")
+    x, _ = _device_args(x, complex_, None, "x")
+    if x.device != b.device:
+        raise ValueError(f"x is on {x.device}, b on {b.device}")
+    x = x.clone()
+    nrhs = 1 if b.dim() == nd else b.shape[-2]
+    shape = tuple(b.shape[:-1])
+    berr = torch.empty(shape, dtype=torch.float64, device=b.device)
+    steps = torch.empty(shape, dtype=torch.int32, device=b.device)
+    fe = torch.empty(shape, dtype=torch.float64, device=b.device) if ferr else None
+    _check(_fn(name, complex_)(h, C.c_void_p(b.data_ptr()), n, C.c_void_p(x.data_ptr()), n, nrhs, C.c_void_p(berr.data_ptr()),
+                               None if fe is None else C.c_void_p(fe.data_ptr()), C.c_void_p(steps.data_ptr()), stream))
+    return x, berr, steps, fe
+
+
+def _rcond_device(name, complex_, h, anorm, norm, count):
+    """slu_b200_[z_][batch_]gscon_device with anorm a float64 CUDA tensor (a scalar broadcast to count values) on the current
+    stream of its device -> rcond, a float64 CUDA tensor (count,)"""
+    import torch
+    nb = _norm_byte(norm)
+    if not anorm.is_cuda or anorm.dtype != torch.float64 or anorm.numel() not in (1, count):
+        raise ValueError(f"anorm must be a float64 CUDA tensor of 1 or {count} values")
+    a = anorm.reshape(-1).expand(count).contiguous()
+    out = torch.empty(count, dtype=torch.float64, device=a.device)
+    stream = C.c_void_p(torch.cuda.current_stream(a.device).cuda_stream)
+    _check(_fn(name, complex_)(h, nb, C.c_void_p(a.data_ptr()), C.c_void_p(out.data_ptr()), stream))
+    return out
 
 
 def _handle_device(complex_, h):
@@ -523,7 +567,12 @@ class Handle:
         """Iterative refinement of x for A x = b on the factors of a scaled fill and the A it kept (slu_b200_gsrfs), as
         pdgsrfs; b and x: (n,) or (nrhs, n) in A's ordering, x typically from solve_scaled.  -> (refined x, berr, steps,
         ferr or None): berr the componentwise backward error of the refined x, steps the refinement steps, ferr dgerfs's
-        forward error bound (ferr=False skips its estimate), one per right-hand side ((nrhs,) arrays, scalars for (n,))"""
+        forward error bound (ferr=False skips its estimate), one per right-hand side ((nrhs,) arrays, scalars for (n,)).
+        Torch CUDA tensors b and x are refined on the device, on the current stream of their device, without a host wait
+        (slu_b200_gsrfs_device): x is a new tensor, berr (float64), steps (int32) and ferr (float64) CUDA tensors of shape
+        b.shape[:-1]."""
+        if _is_tensor(b):
+            return _refine_device("gsrfs_device", self.z_, self.h, b, x, self.prob.n, None, ferr)
         bb = np.ascontiguousarray(b, self._dtype())
         xx = np.array(x, self._dtype(), order="C", copy=True)
         if bb.shape != xx.shape or bb.ndim not in (1, 2) or bb.shape[-1] != self.prob.n:
@@ -550,7 +599,11 @@ class Handle:
 
     def rcond(self, anorm, norm="1"):
         """Reciprocal condition number estimate on the resident factors (slu_b200_gscon / slu_b200_z_gscon), as LAPACK's
-        gecon: (1 / est ||F^-1||) / anorm with anorm = ||A|| in the same norm, '1' (or 'O') or 'I'."""
+        gecon: (1 / est ||F^-1||) / anorm with anorm = ||A|| in the same norm, '1' (or 'O') or 'I'.  A float64 CUDA tensor
+        anorm (one value) is estimated on the device, on the current stream of its device (slu_b200_gscon_device): rcond is
+        then a 0-d CUDA tensor."""
+        if _is_tensor(anorm):
+            return _rcond_device("gscon_device", self.z_, self.h, anorm, norm, 1).reshape(())
         out = C.c_double(0.0)
         _check(_fn("gscon", self.z_)(self.h, _norm_byte(norm), float(anorm), C.byref(out)))
         return out.value
@@ -733,7 +786,10 @@ class BatchHandle:
 
     def refine(self, b, x, ferr=True):
         """Handle.refine for every member (slu_b200_batch_gsrfs); b and x: (batch, n) or (batch, nrhs, n) in A's ordering.
-        -> (refined x, berr, steps, ferr or None) with berr, steps, ferr of shape (batch,) or (batch, nrhs)"""
+        -> (refined x, berr, steps, ferr or None) with berr, steps, ferr of shape (batch,) or (batch, nrhs).  Torch CUDA
+        tensors take the device (slu_b200_batch_gsrfs_device), as Handle.refine."""
+        if _is_tensor(b):
+            return _refine_device("batch_gsrfs_device", self.z_, self.h, b, x, self.prob.n, self.batch, ferr)
         bb = np.ascontiguousarray(b, self._dtype())
         xx = np.array(x, self._dtype(), order="C", copy=True)
         if bb.shape != xx.shape or bb.ndim not in (2, 3) or bb.shape[0] != self.batch or bb.shape[-1] != self.prob.n:
@@ -770,7 +826,10 @@ class BatchHandle:
 
     def rcond(self, anorm, norm="1"):
         """Every member's reciprocal condition number estimate (slu_b200_batch_gscon), as Handle.rcond; anorm: (batch,)
-        norms of the members, or one value for all.  -> float64 array (batch,)"""
+        norms of the members, or one value for all.  -> float64 array (batch,).  A float64 CUDA tensor anorm takes the
+        device (slu_b200_batch_gscon_device), as Handle.rcond: rcond is then a CUDA tensor (batch,)."""
+        if _is_tensor(anorm):
+            return _rcond_device("batch_gscon_device", self.z_, self.h, anorm, norm, self.batch)
         a = np.ascontiguousarray(np.broadcast_to(np.asarray(anorm, np.float64), (self.batch,)))
         out = np.zeros(self.batch, np.float64)
         _check(_fn("batch_gscon", self.z_)(self.h, _norm_byte(norm), a.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p)))

@@ -80,6 +80,10 @@
 #define slu_b200_factor_device slu_b200_z_factor_device
 #define slu_b200_batch_factor_device slu_b200_z_batch_factor_device
 #define slu_b200_get_device slu_b200_z_get_device
+#define slu_b200_gsrfs_device slu_b200_z_gsrfs_device
+#define slu_b200_batch_gsrfs_device slu_b200_z_batch_gsrfs_device
+#define slu_b200_gscon_device slu_b200_z_gscon_device
+#define slu_b200_batch_gscon_device slu_b200_z_batch_gscon_device
 #define SLU_API "slu_b200_z_"     // name prefix of the exported calls, for error messages
 #else
 #define SLU_API "slu_b200_"
@@ -379,6 +383,24 @@ struct slu_b200_handle_s {
     unsigned long long epoch = 0, si_epoch = 0;
     // a call on the caller's stream has been captured into a CUDA graph: the buffers those calls use are pinned (grow)
     bool captured = false;
+    bool loop_captured = false;           // one of them was gsrfs_device or gscon_device: their buffers are pinned too (grow_loop)
+    // gsrfs_device / gscon_device: their outputs before the copies to the caller (berr then ferr, steps; rcond) and anorm,
+    // max_i |x_i| per column as bits, the estimator loop's {kase, rounds}; the side streams the bodies of the conditional
+    // nodes are captured on (one per nesting depth); the executable graphs of the eager calls, each with the key it was
+    // captured for and the buffer addresses it holds (captured again when one of them moved)
+    DevBuf<double> d_rout, d_canorm, d_crcond;
+    DevBuf<int32_t> d_rsteps;
+    DevBuf<unsigned long long> d_rxmax;
+    DevBuf<int> d_cloop;
+    cudaStream_t s_body[2] = {nullptr, nullptr};
+    struct LoopGraph {
+        std::array<int, 4> key;
+        std::vector<uintptr_t> bufs;
+        cudaGraph_t graph;
+        cudaGraphExec_t exec;
+        int launches;
+    };
+    std::vector<LoopGraph> loop_graphs;
 };
 
 namespace {
@@ -519,6 +541,16 @@ int grow(const slu_b200_handle_s *H, DevBuf<T> &b, size_t len, bool exact, bool 
         return fail("%s would allocate device buffers while the stream is capturing a CUDA graph: make this call once outside "
                     "capture first", fn);
     if (pin_check(H, true, fn)) return -1;
+    return b.alloc(len);
+}
+
+// The growth of the buffers that only the graphs of gsrfs_device and gscon_device hold besides the host calls gsrfs and gscon
+// (the refinement's and the estimator's): pinned once one of those calls was captured (loop_captured).
+template <class T>
+int grow_loop(const slu_b200_handle_s *H, DevBuf<T> &b, size_t len, bool capturing, const char *fn)
+{
+    if (b.n >= len) return 0;
+    if (capturing || H->loop_captured) return grow(H, b, len, false, capturing, fn);
     return b.alloc(len);
 }
 
@@ -1765,6 +1797,11 @@ void slu_b200_destroy(slu_b200_handle_t H)
     if (H->stream2) cudaStreamDestroy(H->stream2);
     if (H->s_down) cudaStreamDestroy(H->s_down);
     if (H->s_up) cudaStreamDestroy(H->s_up);
+    for (auto s : H->s_body) if (s) cudaStreamDestroy(s);
+    for (auto &g : H->loop_graphs) {
+        cudaGraphExecDestroy(g.exec);
+        cudaGraphDestroy(g.graph);
+    }
     for (auto e : H->ev_up) if (e) cudaEventDestroy(e);
     for (auto e : H->ev_panel) if (e) cudaEventDestroy(e);
     for (auto e : H->ev_bulk) if (e) cudaEventDestroy(e);
@@ -2596,16 +2633,25 @@ int slu_b200_batch_solve_trans(slu_b200_handle_t H, double *xh, int ldx, int nrh
 constexpr int COND_MAX_ROUNDS = 64;     // dlacn2 makes at most 11 solves; lock-step at most doubles that
 
 }  // extern "C"
+// The estimator's buffers for `members` vectors of n elements (pinned once a call on the caller's stream was captured: grow)
+static int cond_buffers(slu_b200_handle_t H, int n, int members, bool capturing, const char *fn)
+{
+    const size_t len = (size_t)n * members;
+    const size_t parts = (size_t)((n + COND_CHUNK - 1) / COND_CHUNK) * members;
+    if (VAL_DOUBLES == 1 && grow_loop(H, H->d_csgn, len, capturing, fn)) return -1;     // the real repeated-sign test
+    if (grow_loop(H, H->d_cstate, members, capturing, fn) || grow_loop(H, H->d_cpart, parts, capturing, fn) ||
+        grow_loop(H, H->d_ccount, 2, capturing, fn))
+        return -1;
+    return 0;
+}
+
 // The rounds of dlacn2 / zlacn2 over `members` vectors of n elements, shared by gscon and the forward error bound of gsrfs:
 // v holds the pending vectors; apply(kase, &x) enqueues the operator of kase on them and points x at the result.  Ends when
 // no member waits; the estimates are then in d_cstate.  *rounds counts the applications.
 template <class Apply>
 static int cond_rounds(slu_b200_handle_t H, int n, int members, val_t *v, Apply apply, int *rounds, const char *fn)
 {
-    const size_t len = (size_t)n * members;
-    const size_t parts = (size_t)((n + COND_CHUNK - 1) / COND_CHUNK) * members;
-    if (VAL_DOUBLES == 1 && H->d_csgn.n < len && H->d_csgn.alloc(len)) return -1;     // the real repeated-sign test
-    if (H->d_cstate.n < (size_t)members && (H->d_cstate.alloc(members) || H->d_cpart.alloc(parts) || H->d_ccount.alloc(2))) return -1;
+    if (cond_buffers(H, n, members, false, fn)) return -1;
     cudaStream_t s = H->stream;
     launch_cond_init(H->d_cstate.p, v, n, members, s);
     for (int kase = 1;;) {
@@ -2648,7 +2694,7 @@ static int gscon_impl(slu_b200_handle_t H, char norm, const double *anorm, doubl
     }
     if (any) {
         const size_t len = (size_t)n * B;
-        if (batched && H->d_cv.n < len && H->d_cv.alloc(len)) return -1;
+        if (batched && grow_loop(H, H->d_cv, len, false, fn)) return -1;
         if (grow(H, H->d_x, len, false, false, fn) || (!batched && grow(H, H->d_x2, len, false, false, fn))) return -1;
         cudaStream_t s = H->stream;
         val_t *v = batched ? H->d_cv.p : H->d_x2.p;       // the pending vectors
@@ -3045,6 +3091,16 @@ int slu_b200_batch_solve_scaled(slu_b200_handle_t H, double *x, int ldx, int nrh
 // residual kernel over every (row, column, member), the decide kernel and one read of the count of columns still active, then
 // one scaled solve of the whole block of residuals and the update.  ferr: dlacn2 through cond_rounds, each (member, column)
 // one estimator member: kase 1 solves with A^T (A^H) and multiplies by W, kase 2 multiplies by W and solves with A.
+// The refinement's buffers for cols columns of len elements in all (pinned after a captured call: grow)
+static int refine_buffers(slu_b200_handle_t H, size_t len, int cols, bool ferr, bool capturing, const char *fn)
+{
+    if (grow(H, H->d_x, len, false, capturing, fn) || grow(H, H->d_x2, len, false, capturing, fn) || grow_loop(H, H->d_rb, len, capturing, fn) ||
+        grow_loop(H, H->d_rx, len, capturing, fn) || grow_loop(H, H->d_rst, cols, capturing, fn) || grow_loop(H, H->d_ract, 1, capturing, fn))
+        return -1;
+    if (ferr && (grow_loop(H, H->d_rw, len, capturing, fn) || grow_loop(H, H->d_cv, len, capturing, fn))) return -1;
+    return 0;
+}
+
 static int gsrfs_impl(slu_b200_handle_t H, bool batched, const double *bh, int ldb, double *xh, int ldx, int nrhs, double *berr,
                       double *ferr, int32_t *steps, const char *fn)
 {
@@ -3056,10 +3112,7 @@ static int gsrfs_impl(slu_b200_handle_t H, bool batched, const double *bh, int l
     if ((int64_t)n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
     const int cols = B * nrhs;
     const size_t len = (size_t)n * cols;
-    if (grow(H, H->d_x, len, false, false, fn) || grow(H, H->d_x2, len, false, false, fn) || (H->d_rb.n < len && H->d_rb.alloc(len)) ||
-        (H->d_rx.n < len && H->d_rx.alloc(len)) || (H->d_rst.n < (size_t)cols && H->d_rst.alloc(cols)) ||
-        (!H->d_ract.p && H->d_ract.alloc(1)) || (ferr && ((H->d_rw.n < len && H->d_rw.alloc(len)) || (H->d_cv.n < len && H->d_cv.alloc(len)))))
-        return -1;
+    if (refine_buffers(H, len, cols, ferr != nullptr, false, fn)) return -1;
     cudaStream_t s = H->stream;
     const double t0 = now_s();
     const size_t w = (size_t)n * sizeof(val_t);
@@ -3288,6 +3341,331 @@ static int solve_device_impl(slu_b200_handle_t H, bool batched, bool scaled, dou
     H->st.reserved[4] = 0;
     H->st.reserved[5] = (double)launches;
     return 0;
+}
+
+// ---- iterative refinement and condition estimation on the caller's stream (gsrfs_device, gscon_device and their twins).
+// The host loops of gsrfs and gscon read a counter back after every step or round to decide whether to go on.  Here the
+// decision stays on the device: each loop is a conditional WHILE node whose body ends with a kernel that sets the node's
+// handle from the same counter, and the estimator's body runs the solve of the round's kase in one of two IF nodes.  The
+// residual, decide, update, solve and estimator-step kernels are those of the host loops, so the device loops take the same
+// decisions on the same vectors.  One enqueue path serves both ways a call runs: under the caller's capture (the handle's
+// stream joins it in stream_enter) the nodes go straight into the caller's graph; an eager call captures the same sequence
+// on the handle's stream once, caches the executable graph and launches it, with only the copies of the caller's pointers
+// outside it.  Conditional nodes cannot be children of a child graph node, hence the nodes are added to the capture itself:
+// each body graph is captured on a side stream of the handle (one per nesting depth), swapped in for H->stream while the
+// body's solves are enqueued.
+}  // extern "C"
+
+// conditional graph nodes need a driver of CUDA 12.4 or later; read once
+static int conditional_nodes_check(const char *fn)
+{
+    static int version = 0;
+    if (version == 0) CU(cudaDriverGetVersion(&version));
+    if (version < 12040)
+        return fail("%s needs a CUDA driver of version 12.4 or later for conditional graph nodes (this driver is %d.%d)", fn,
+                    version / 1000, version % 1000 / 10);
+    return 0;
+}
+
+// a new conditional handle in the graph being captured on H->stream
+static int cond_handle(slu_b200_handle_t H, cudaGraphConditionalHandle *h)
+{
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    cudaGraph_t g = nullptr;
+    CU(cudaStreamGetCaptureInfo(H->stream, &cs, nullptr, &g, nullptr, nullptr));
+    if (cs != cudaStreamCaptureStatusActive) return fail("the handle's stream is not capturing a CUDA graph");
+    CU(cudaGraphConditionalHandleCreate(h, g, 0, 0));
+    return 0;
+}
+
+// A conditional node of `type` on handle h after the current dependencies of the capture on H->stream, its body captured from
+// body() (which enqueues on H->stream and returns < 0 on an error) on side stream s_body[depth]; the node becomes the
+// capture's next dependency.  H->stream is restored on every path.
+template <class Body>
+static int add_conditional(slu_b200_handle_t H, cudaGraphConditionalNodeType type, cudaGraphConditionalHandle h, int depth, Body body)
+{
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    cudaGraph_t g = nullptr;
+    const cudaGraphNode_t *deps = nullptr;
+    size_t ndeps = 0;
+    CU(cudaStreamGetCaptureInfo(H->stream, &cs, nullptr, &g, &deps, &ndeps));
+    cudaGraphNodeParams p{};
+    p.type = cudaGraphNodeTypeConditional;
+    p.conditional.handle = h;
+    p.conditional.type = type;
+    p.conditional.size = 1;
+    cudaGraphNode_t node = nullptr;
+    CU(cudaGraphAddNode(&node, g, deps, ndeps, &p));
+    const cudaStream_t outer = H->stream, side = H->s_body[depth];
+    CU(cudaStreamBeginCaptureToGraph(side, p.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
+    H->stream = side;
+    const int rc = body();
+    H->stream = outer;
+    cudaGraph_t captured = nullptr;
+    const cudaError_t e = cudaStreamEndCapture(side, &captured);
+    if (rc < 0) return -1;
+    if (e != cudaSuccess) return fail("cudaStreamEndCapture (conditional node body): %s", cudaGetErrorString(e));
+    CU(cudaStreamUpdateCaptureDependencies(outer, &node, 1, cudaStreamSetCaptureDependencies));
+    return 0;
+}
+
+// The rounds of cond_rounds as a WHILE node: cond_init, then per round the IF node of the round's kase (apply(kase, &x), the
+// counter reset and the step kernels of that kase; launch_cond_step takes its kase as an argument) and the decision.  Enqueued
+// on H->stream, which is capturing.  Returns the launches (each body counted once), < 0 on an error.
+template <class Apply>
+static int cond_loop(slu_b200_handle_t H, int n, int members, val_t *v, Apply apply)
+{
+    int launches = launch_cond_init(H->d_cstate.p, v, n, members, H->stream);
+    cudaGraphConditionalHandle w;
+    if (cond_handle(H, &w)) return -1;
+    launches += launch_cond_continue(H->d_ccount.p, H->d_cloop.p, 1, COND_MAX_ROUNDS, w, H->stream);
+    const int rc = add_conditional(H, cudaGraphCondTypeWhile, w, 0, [&]() -> int {
+        cudaGraphConditionalHandle k[2];
+        if (cond_handle(H, &k[0]) || cond_handle(H, &k[1])) return -1;
+        launches += launch_cond_select(H->d_cloop.p, k[0], k[1], H->stream);
+        for (int kase = 1; kase <= 2; ++kase)
+            if (add_conditional(H, cudaGraphCondTypeIf, k[kase - 1], 1, [&]() -> int {
+                    val_t *x = nullptr;
+                    const int l = apply(kase, &x);
+                    if (l < 0) return -1;
+                    CU(cudaMemsetAsync(H->d_ccount.p, 0, 2 * sizeof(int), H->stream));
+                    launches += l + launch_cond_step(H->d_cstate.p, kase, x, v, H->d_csgn.p, H->d_cpart.p, H->d_ccount.p, n, members, H->stream);
+                    return 0;
+                }))
+                return -1;
+        launches += launch_cond_continue(H->d_ccount.p, H->d_cloop.p, 0, COND_MAX_ROUNDS, w, H->stream);
+        return 0;
+    });
+    return rc < 0 ? -1 : launches;
+}
+
+// Runs enqueue() (a call's device work on H->stream, returning its launches) after stream_enter.  Under the caller's capture
+// (cap) it goes into the caller's graph.  Otherwise the graph captured from it for this key is launched on H->stream, captured
+// and instantiated first if there is none or if one of the buffer addresses it holds (bufs) has changed since.
+template <class Enqueue>
+static int run_loop(slu_b200_handle_t H, bool cap, const std::array<int, 4> &key, const std::vector<uintptr_t> &bufs, Enqueue enqueue)
+{
+    if (cap) return enqueue();
+    auto it = std::find_if(H->loop_graphs.begin(), H->loop_graphs.end(), [&](const slu_b200_handle_s::LoopGraph &g) { return g.key == key; });
+    if (it != H->loop_graphs.end() && it->bufs != bufs) {        // a buffer moved: capture again
+        cudaGraphExecDestroy(it->exec);
+        cudaGraphDestroy(it->graph);
+        H->loop_graphs.erase(it);
+        it = H->loop_graphs.end();
+    }
+    if (it == H->loop_graphs.end()) {
+        CU(cudaStreamBeginCapture(H->stream, cudaStreamCaptureModeThreadLocal));
+        const int launches = enqueue();
+        cudaGraph_t graph = nullptr;
+        const cudaError_t e = cudaStreamEndCapture(H->stream, &graph);
+        if (launches < 0 || e != cudaSuccess) {
+            if (graph) cudaGraphDestroy(graph);
+            return launches < 0 ? -1 : fail("cudaStreamEndCapture: %s", cudaGetErrorString(e));
+        }
+        cudaGraphExec_t exec = nullptr;
+        const cudaError_t ei = cudaGraphInstantiate(&exec, graph, 0);
+        if (ei != cudaSuccess) {
+            cudaGraphDestroy(graph);
+            return fail("cudaGraphInstantiate: %s", cudaGetErrorString(ei));
+        }
+        H->loop_graphs.push_back({key, bufs, graph, exec, launches});
+        it = H->loop_graphs.end() - 1;
+    }
+    CU(cudaGraphLaunch(it->exec, H->stream));
+    return it->launches;
+}
+
+// the side streams of the conditional bodies, created outside capture by a call's first use
+static int body_streams(slu_b200_handle_t H, bool cap, const char *fn)
+{
+    if (H->s_body[0]) return 0;
+    if (cap) return fail("%s would create streams while the stream is capturing a CUDA graph: make this call once outside capture first", fn);
+    for (auto &s : H->s_body) CU(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+    return 0;
+}
+
+// gsrfs's loop for x in d_rx and b in d_rb, results in d_rx, d_rout (berr, then ferr) and d_rsteps: pdgsrfs's steps in a WHILE
+// node, then (ferr) dgerfs's estimate in cond_loop, the finish kernels and the guard of x.  Enqueued on H->stream, capturing.
+static int gsrfs_loop(slu_b200_handle_t H, bool batched, int nrhs, bool ferr)
+{
+    const int B = batched ? H->batch : 1, n = H->n, cols = B * nrhs;
+    const size_t len = (size_t)n * cols;
+    const RefineArgs a{n, nrhs, B, (int64_t)H->d_aci.n, H->d_arp.p, H->d_aci.p, H->d_aval.p, H->d_rb.p, H->d_rst.p, ferr ? H->d_rw.p : nullptr};
+    val_t *x = H->d_rx.p;
+    int launches = launch_refine_init(H->d_rst.p, H->d_info.p, nrhs, B, H->stream);
+    launches += launch_refine_residual(a, x, scaled_in(H, batched), H->stream);
+    CU(cudaMemsetAsync(H->d_ract.p, 0, sizeof(int), H->stream));
+    launches += launch_refine_decide(a, H->d_ract.p, H->stream);
+    cudaGraphConditionalHandle w;
+    if (cond_handle(H, &w)) return -1;
+    launches += launch_refine_continue(H->d_ract.p, w, H->stream);
+    if (add_conditional(H, cudaGraphCondTypeWhile, w, 0, [&]() -> int {
+            const int l = solve_scaled_dev(H, batched, nrhs, 0);    // dx = A^-1 r in d_x2
+            if (l < 0) return -1;
+            launches += l + launch_refine_update(a, x, H->d_x2.p, H->stream) + launch_refine_residual(a, x, scaled_in(H, batched), H->stream);
+            CU(cudaMemsetAsync(H->d_ract.p, 0, sizeof(int), H->stream));
+            launches += launch_refine_decide(a, H->d_ract.p, H->stream) + launch_refine_continue(H->d_ract.p, w, H->stream);
+            return 0;
+        }))
+        return -1;
+    if (ferr) {
+        const double *W = H->d_rw.p;
+        auto apply = [&](int kase, val_t **res) -> int {          // as gsrfs_impl's
+            val_t *in = scaled_in(H, batched);
+            *res = H->d_x2.p;
+            int l;
+            if (kase == 2) {                                    // A^-1 diag(W) v
+                l = launch_refine_scale(in, H->d_cv.p, W, (int64_t)len, H->stream);
+                const int ls = solve_scaled_dev(H, batched, nrhs, 0);
+                if (ls < 0) return -1;
+                l += ls;
+            } else {                                            // diag(W) A^-T v
+                CU(cudaMemcpyAsync(in, H->d_cv.p, len * sizeof(val_t), cudaMemcpyDeviceToDevice, H->stream));
+                l = solve_scaled_dev(H, batched, nrhs, VAL_DOUBLES == 2 ? 2 : 1);
+                if (l < 0) return -1;
+                l += launch_refine_scale(*res, *res, W, (int64_t)len, H->stream);
+            }
+            return l;
+        };
+        const int l = cond_loop(H, n, cols, H->d_cv.p, apply);
+        if (l < 0) return -1;
+        launches += l;
+        CU(cudaMemsetAsync(H->d_rxmax.p, 0, (size_t)cols * sizeof(unsigned long long), H->stream));
+        launches += launch_refine_xmax(a, x, H->d_rxmax.p, H->stream);
+    }
+    launches += launch_refine_finish(a, H->d_cstate.p, H->d_rxmax.p, H->d_info.p, H->d_rout.p, ferr ? H->d_rout.p + cols : nullptr,
+                                     H->d_rsteps.p, H->stream);
+    launches += launch_solve_guard(x, H->d_info.p, (int64_t)n * nrhs, B, H->stream);
+    return launches;
+}
+
+// gscon's rounds for every member, anorm in d_canorm, rcond into d_crcond (the operator of gscon_impl).  Capturing, on H->stream.
+static int gscon_loop(slu_b200_handle_t H, bool batched, bool one)
+{
+    const int B = batched ? H->batch : 1, n = H->n;
+    const size_t len = (size_t)n * B;
+    val_t *v = batched ? H->d_cv.p : H->d_x2.p;
+    auto apply = [&](int kase, val_t **x) -> int {
+        const int trans = (kase == 1) == one ? 0 : (VAL_DOUBLES == 2 ? 2 : 1);
+        *x = H->d_x.p;
+        if (!batched) return solve_dev(H, 1, trans, x);
+        CU(cudaMemcpyAsync(*x, v, len * sizeof(val_t), cudaMemcpyDeviceToDevice, H->stream));
+        return solve_passes(H, H->bdev, 1, trans);
+    };
+    const int l = cond_loop(H, n, B, v, apply);
+    if (l < 0) return -1;
+    return l + launch_cond_rcond(H->d_cstate.p, H->d_canorm.p, H->d_info.p, B, H->d_crcond.p, H->stream);
+}
+extern "C" {
+
+// gsrfs / batch_gsrfs on device b, x and outputs, ordered on the caller's stream (see the section comment above)
+static int gsrfs_device_impl(slu_b200_handle_t H, bool batched, const double *bd, int ldb, double *xd, int ldx, int nrhs, double *berr,
+                             double *ferr, int32_t *steps, void *stream, const char *fn)
+{
+    if (!H || !bd || !xd || !berr) return fail("%s: null argument (b, x and berr are required)", fn);
+    if (check(H, fn, scaled_need(batched) | SCALED | FACTORED | DEVICE_ORDERED)) return -1;
+    const int B = batched ? H->batch : 1, n = H->n;
+    if (nrhs < 1) return fail("%s: nrhs = %d, must be >= 1", fn, nrhs);
+    if (ldb < n || ldx < n) return fail("%s: ldb = %d and ldx = %d must be >= n = %d", fn, ldb, ldx, n);
+    if ((int64_t)n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
+    if (check_device_ptr(H, bd, fn, "b") || check_device_ptr(H, xd, fn, "x") || check_device_ptr(H, berr, fn, "berr") ||
+        (ferr && check_device_ptr(H, ferr, fn, "ferr")) || (steps && check_device_ptr(H, steps, fn, "steps")))
+        return -1;
+    if (conditional_nodes_check(fn)) return -1;
+    const cudaStream_t caller = (cudaStream_t)stream;
+    const int cap = capturing(H, caller, fn);
+    if (cap < 0) return -1;
+    const int cols = B * nrhs;
+    const size_t len = (size_t)n * cols;
+    if (refine_buffers(H, len, cols, ferr != nullptr, cap, fn) || (ferr && (cond_buffers(H, n, cols, cap, fn) || grow_loop(H, H->d_rxmax, cols, cap, fn))) ||
+        grow_loop(H, H->d_cloop, 2, cap, fn) || grow_loop(H, H->d_rout, 2 * (size_t)cols, cap, fn) || grow_loop(H, H->d_rsteps, cols, cap, fn) ||
+        body_streams(H, cap, fn))
+        return -1;
+    H->captured = H->captured || cap;
+    H->loop_captured = H->loop_captured || cap;
+    if (stream_enter(H, caller)) return -1;
+    const size_t w = (size_t)n * sizeof(val_t);
+    CU(cudaMemcpy2DAsync(H->d_rb.p, w, bd, (size_t)ldb * sizeof(val_t), w, (size_t)cols, cudaMemcpyDeviceToDevice, H->stream));
+    CU(cudaMemcpy2DAsync(H->d_rx.p, w, xd, (size_t)ldx * sizeof(val_t), w, (size_t)cols, cudaMemcpyDeviceToDevice, H->stream));
+    const std::vector<uintptr_t> bufs = {
+        (uintptr_t)H->d_x.p, (uintptr_t)H->d_x2.p, (uintptr_t)H->d_rb.p, (uintptr_t)H->d_rx.p, (uintptr_t)H->d_rst.p, (uintptr_t)H->d_ract.p,
+        (uintptr_t)H->d_rw.p, (uintptr_t)H->d_cv.p, (uintptr_t)H->d_csgn.p, (uintptr_t)H->d_cstate.p, (uintptr_t)H->d_cpart.p,
+        (uintptr_t)H->d_ccount.p, (uintptr_t)H->d_cloop.p, (uintptr_t)H->d_rout.p, (uintptr_t)H->d_rsteps.p, (uintptr_t)H->d_rxmax.p,
+        (uintptr_t)H->d_arp.p, (uintptr_t)H->d_aci.p, (uintptr_t)H->d_aci.n, (uintptr_t)H->d_aval.p, (uintptr_t)H->d_R.p,
+        (uintptr_t)H->d_C.p, (uintptr_t)H->d_rmap.p, (uintptr_t)H->d_cperm.p, (uintptr_t)H->d_info.p};
+    const int launches = run_loop(H, cap, {0, batched, nrhs, ferr != nullptr}, bufs, [&] { return gsrfs_loop(H, batched, nrhs, ferr != nullptr); });
+    if (launches < 0) return -1;
+    cudaStream_t s = H->stream;
+    CU(cudaMemcpy2DAsync(xd, (size_t)ldx * sizeof(val_t), H->d_rx.p, w, w, (size_t)cols, cudaMemcpyDeviceToDevice, s));
+    CU(cudaMemcpyAsync(berr, H->d_rout.p, (size_t)cols * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    if (ferr) CU(cudaMemcpyAsync(ferr, H->d_rout.p + cols, (size_t)cols * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    if (steps) CU(cudaMemcpyAsync(steps, H->d_rsteps.p, (size_t)cols * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
+    CU(cudaGetLastError());
+    if (stream_leave(H, caller)) return -1;
+    H->st.reserved[4] = 0;
+    H->st.reserved[5] = (double)launches;
+    return 0;
+}
+
+// gscon / batch_gscon with device anorm and rcond (one per member), ordered on the caller's stream
+static int gscon_device_impl(slu_b200_handle_t H, bool batched, char norm, const double *anorm, double *rcond, void *stream, const char *fn)
+{
+    if (!H || !anorm || !rcond) return fail("%s: null argument", fn);
+    if (check(H, fn, scaled_need(batched) | FACTORED | DEVICE_ORDERED)) return -1;
+    const bool one = norm == '1' || norm == 'O' || norm == 'o';
+    if (!one && norm != 'I' && norm != 'i')
+        return fail("%s: norm must be '1', 'O' or 'I' (got character code %d)", fn, (int)(unsigned char)norm);
+    if (check_device_ptr(H, anorm, fn, "anorm") || check_device_ptr(H, rcond, fn, "rcond")) return -1;
+    if (conditional_nodes_check(fn)) return -1;
+    const cudaStream_t caller = (cudaStream_t)stream;
+    const int cap = capturing(H, caller, fn);
+    if (cap < 0) return -1;
+    const int B = batched ? H->batch : 1, n = H->n;
+    const size_t len = (size_t)n * B;
+    if (grow(H, H->d_x, len, false, cap, fn) || (batched ? grow_loop(H, H->d_cv, len, cap, fn) : grow(H, H->d_x2, len, false, cap, fn)) || cond_buffers(H, n, B, cap, fn) ||
+        grow_loop(H, H->d_cloop, 2, cap, fn) || grow_loop(H, H->d_canorm, B, cap, fn) || grow_loop(H, H->d_crcond, B, cap, fn) ||
+        body_streams(H, cap, fn))
+        return -1;
+    H->captured = H->captured || cap;
+    H->loop_captured = H->loop_captured || cap;
+    if (stream_enter(H, caller)) return -1;
+    CU(cudaMemcpyAsync(H->d_canorm.p, anorm, (size_t)B * sizeof(double), cudaMemcpyDeviceToDevice, H->stream));
+    const std::vector<uintptr_t> bufs = {
+        (uintptr_t)H->d_x.p, (uintptr_t)H->d_x2.p, (uintptr_t)H->d_cv.p, (uintptr_t)H->d_csgn.p, (uintptr_t)H->d_cstate.p,
+        (uintptr_t)H->d_cpart.p, (uintptr_t)H->d_ccount.p, (uintptr_t)H->d_cloop.p, (uintptr_t)H->d_canorm.p, (uintptr_t)H->d_crcond.p,
+        (uintptr_t)H->d_info.p};
+    const int launches = run_loop(H, cap, {1, batched, 1, one}, bufs, [&] { return gscon_loop(H, batched, one); });
+    if (launches < 0) return -1;
+    CU(cudaMemcpyAsync(rcond, H->d_crcond.p, (size_t)B * sizeof(double), cudaMemcpyDeviceToDevice, H->stream));
+    CU(cudaGetLastError());
+    if (stream_leave(H, caller)) return -1;
+    H->st.reserved[4] = 0;
+    H->st.reserved[5] = (double)launches;
+    H->st.reserved[6] = 0;
+    H->st.reserved[7] = 0;
+    return 0;
+}
+
+int slu_b200_gsrfs_device(slu_b200_handle_t H, const double *b, int ldb, double *x, int ldx, int nrhs, double *berr, double *ferr,
+                          int32_t *steps, void *stream)
+{
+    return gsrfs_device_impl(H, false, b, ldb, x, ldx, nrhs, berr, ferr, steps, stream, SLU_API "gsrfs_device");
+}
+
+int slu_b200_batch_gsrfs_device(slu_b200_handle_t H, const double *b, int ldb, double *x, int ldx, int nrhs, double *berr, double *ferr,
+                                int32_t *steps, void *stream)
+{
+    return gsrfs_device_impl(H, true, b, ldb, x, ldx, nrhs, berr, ferr, steps, stream, SLU_API "batch_gsrfs_device");
+}
+
+int slu_b200_gscon_device(slu_b200_handle_t H, char norm, const double *anorm, double *rcond, void *stream)
+{
+    return gscon_device_impl(H, false, norm, anorm, rcond, stream, SLU_API "gscon_device");
+}
+
+int slu_b200_batch_gscon_device(slu_b200_handle_t H, char norm, const double *anorm, double *rcond, void *stream)
+{
+    return gscon_device_impl(H, true, norm, anorm, rcond, stream, SLU_API "batch_gscon_device");
 }
 
 int slu_b200_get_device(slu_b200_handle_t H, int *device)

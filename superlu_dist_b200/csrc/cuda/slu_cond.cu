@@ -215,6 +215,68 @@ __global__ void __launch_bounds__(COND_THREADS) cond_next_kernel(const CondState
     }
 }
 
+// ---- the loop on the device (gscon_device, gsrfs_device's ferr): conditional graph nodes in place of the host's reads ----
+
+// after a round (first = 0): the next kase by the host loop's rule (the other kase if a member waits for it, else the same
+// one if a member waits for it, else 0) and one round more; first = 1: kase 1, 0 rounds.  The WHILE handle w continues while
+// a kase is left and fewer than max_rounds rounds ran (the host loop fails there; the members still waiting get NaN).
+__global__ void cond_continue_kernel(const int *counts, int *loop, int first, int max_rounds, cudaGraphConditionalHandle w)
+{
+    int kase = 1, rounds = 0;
+    if (!first) {
+        kase = loop[0];
+        rounds = loop[1] + 1;
+        if (counts[2 - kase] > 0) kase = 3 - kase;
+        else if (counts[kase - 1] == 0) kase = 0;
+    }
+    loop[0] = kase;
+    loop[1] = rounds;
+    cudaGraphSetConditional(w, kase != 0 && rounds < max_rounds ? 1u : 0u);
+}
+
+// at the head of each round: the IF node of the round's kase runs
+__global__ void cond_select_kernel(const int *loop, cudaGraphConditionalHandle k1, cudaGraphConditionalHandle k2)
+{
+    cudaGraphSetConditional(k1, loop[0] == 1 ? 1u : 0u);
+    cudaGraphSetConditional(k2, loop[0] == 2 ? 1u : 0u);
+}
+
+// one thread per member: rcond as gscon's host side: anorm 0 or +inf -> 0, (1 / est) / anorm where est is finite and not 0,
+// else 0.  NaN where the member's status is not 0, anorm is negative or NaN (which the host call refuses), or the estimate
+// stopped at the round cap.
+__global__ void __launch_bounds__(COND_THREADS) cond_rcond_kernel(const CondState *st, const double *anorm, const int32_t *status, int members,
+                                                                  double *rcond)
+{
+    const int m = blockIdx.x * COND_THREADS + threadIdx.x;
+    if (m >= members) return;
+    const double a = anorm[m], q = __longlong_as_double(0x7ff8000000000000LL);
+    const CondState s = st[m];
+    double r;
+    if (status[m] != 0 || !(a >= 0.0)) r = q;
+    else if (a == 0.0 || isinf(a)) r = 0.0;
+    else if (s.kase != 0) r = q;
+    else r = isfinite(s.est) && s.est != 0.0 ? (1.0 / s.est) / a : 0.0;
+    rcond[m] = r;
+}
+
+int launch_cond_continue(const int *counts, int *loop, int first, int max_rounds, cudaGraphConditionalHandle w, cudaStream_t s)
+{
+    cond_continue_kernel<<<1, 1, 0, s>>>(counts, loop, first, max_rounds, w);
+    return 1;
+}
+
+int launch_cond_select(const int *loop, cudaGraphConditionalHandle k1, cudaGraphConditionalHandle k2, cudaStream_t s)
+{
+    cond_select_kernel<<<1, 1, 0, s>>>(loop, k1, k2);
+    return 1;
+}
+
+int launch_cond_rcond(const CondState *st, const double *anorm, const int32_t *status, int members, double *rcond, cudaStream_t s)
+{
+    cond_rcond_kernel<<<(members + COND_THREADS - 1) / COND_THREADS, COND_THREADS, 0, s>>>(st, anorm, status, members, rcond);
+    return 1;
+}
+
 int launch_cond_init(CondState *st, val_t *v, int n, int members, cudaStream_t s)
 {
     cond_init_kernel<<<dim3((n + COND_CHUNK - 1) / COND_CHUNK, members), COND_THREADS, 0, s>>>(st, v, n);

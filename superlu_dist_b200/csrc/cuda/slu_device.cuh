@@ -277,6 +277,13 @@ int launch_cond_init(CondState *st, val_t *v, int n, int members, cudaStream_t s
 // part: members * ceil(n / COND_CHUNK) entries
 int launch_cond_step(CondState *st, int kase, const val_t *x, val_t *v, val_t *sgn, CondPart *part, int *counts, int n, int members,
                      cudaStream_t s);
+// The estimator loop on the device (gscon_device, gsrfs_device's ferr), in conditional graph nodes.  loop = {kase of the next
+// round, rounds so far}.  continue: first = 1 starts the loop (kase 1, 0 rounds); else one round more and the next kase from
+// counts as the host loop takes it; the WHILE handle w = a kase is left and fewer than max_rounds rounds ran.  select: the
+// IF handles k1 / k2 = the round's kase.  rcond: (1 / est) / anorm per member, as gscon.  1 launch each.
+int launch_cond_continue(const int *counts, int *loop, int first, int max_rounds, cudaGraphConditionalHandle w, cudaStream_t s);
+int launch_cond_select(const int *loop, cudaGraphConditionalHandle k1, cudaGraphConditionalHandle k2, cudaStream_t s);
+int launch_cond_rcond(const CondState *st, const double *anorm, const int32_t *status, int members, double *rcond, cudaStream_t s);
 
 // slu_refine.cu (double) / slu_refine_z.cu (doublecomplex): the step kernels of iterative refinement (slu_b200_gsrfs), pdgsrfs's
 // loop per column.  One RefineState per column, members x nrhs of them, member-major; vectors: members blocks of n x nrhs.
@@ -303,6 +310,14 @@ int launch_refine_decide(const RefineArgs &a, int *active, cudaStream_t s);
 int launch_refine_update(const RefineArgs &a, val_t *x, const val_t *dx, cudaStream_t s);
 // dst[t] = W[t] src[t], t < len
 int launch_refine_scale(val_t *dst, const val_t *src, const double *W, int64_t len, cudaStream_t s);
+// The refinement loop on the device (gsrfs_device), in conditional graph nodes.  init: pdgsrfs's start state of every column,
+// inactive where the member's status is not 0.  continue: the WHILE handle h = *active > 0.  xmax: max_i |x_i| of every
+// column as bits into xmax (zeroed by the caller).  finish: berr, steps and (ferr non-null) dgerfs's ferr per column.
+int launch_refine_init(RefineState *st, const int32_t *status, int nrhs, int members, cudaStream_t s);
+int launch_refine_continue(const int *active, cudaGraphConditionalHandle h, cudaStream_t s);
+int launch_refine_xmax(const RefineArgs &a, const val_t *x, unsigned long long *xmax, cudaStream_t s);
+int launch_refine_finish(const RefineArgs &a, const CondState *est, const unsigned long long *xmax, const int32_t *status, double *berr,
+                         double *ferr, int32_t *steps, cudaStream_t s);
 
 #ifndef SLU_COMPLEX
 // slu_ozaki.cu: the Schur update of wide supernodes on wgmma (int8 slices, exact int32 accumulation in registers)

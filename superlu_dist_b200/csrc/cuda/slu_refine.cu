@@ -113,6 +113,57 @@ __global__ void __launch_bounds__(REF_THREADS) refine_scale_kernel(val_t *dst, c
     if (t < len) dst[t] = ref_scale(W[t], src[t]);
 }
 
+// ---- the loop on the device (slu_b200_gsrfs_device): the host reads nothing between steps, conditional graph nodes loop --
+
+constexpr int XMAX_PER_THREAD = 8;
+
+__device__ __forceinline__ double ref_nan() { return __longlong_as_double(0x7ff8000000000000LL); }
+
+// pdgsrfs's start (lstres = 3, count = 0) for every column; the columns of a member whose status is not 0 start inactive
+__global__ void __launch_bounds__(REF_THREADS) refine_init_kernel(RefineState *st, const int32_t *status, int nrhs, int cols)
+{
+    const int c = blockIdx.x * REF_THREADS + threadIdx.x;
+    if (c < cols) st[c] = RefineState{3.0, 0.0, 0ull, 0, status[c / nrhs] == 0};
+}
+
+// the refinement's WHILE node runs another step while a column is active
+__global__ void refine_continue_kernel(const int *active, cudaGraphConditionalHandle h)
+{
+    cudaGraphSetConditional(h, *active > 0 ? 1u : 0u);
+}
+
+// max_i |x_i| per column: a CTA reduces XMAX_PER_THREAD * REF_THREADS rows of column blockIdx.y, then one integer atomicMax
+// on the bits of the non-negative result, so the maximum does not depend on the order
+__global__ void __launch_bounds__(REF_THREADS) refine_xmax_kernel(int n, const val_t *__restrict__ x, unsigned long long *xmax)
+{
+    const int64_t c = blockIdx.y;
+    const val_t *xc = x + c * n;
+    unsigned long long m = 0;
+    for (int k = 0; k < XMAX_PER_THREAD; ++k) {
+        const int i = (blockIdx.x * XMAX_PER_THREAD + k) * REF_THREADS + threadIdx.x;
+        if (i < n) m = max(m, ref_bits(ref_abs1(xc[i])));
+    }
+    for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_down_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0 && m) atomicMax(xmax + c, m);
+}
+
+// per column: berr and steps of the loop, and dgerfs's ferr = est / max_i |x_i| (est where x = 0), as gsrfs's host side.
+// A member whose status is not 0: NaN berr and ferr, 0 steps; a column whose estimate stopped at the round cap: NaN ferr.
+__global__ void __launch_bounds__(REF_THREADS) refine_finish_kernel(RefineArgs a, const CondState *est, const unsigned long long *xmax,
+                                                                     const int32_t *status, double *berr, double *ferr, int32_t *steps)
+{
+    const int c = blockIdx.x * REF_THREADS + threadIdx.x;
+    if (c >= a.nrhs * a.members) return;
+    const RefineState s = a.st[c];
+    const bool ok = status[c / a.nrhs] == 0;
+    berr[c] = ok ? s.berr : ref_nan();
+    steps[c] = ok ? s.count : 0;
+    if (!ferr) return;
+    const CondState e = est[c];
+    const double xm = __longlong_as_double((long long)xmax[c]);
+    ferr[c] = !ok || e.kase != 0 ? ref_nan() : xm != 0.0 ? e.est / xm : e.est;
+}
+
 static dim3 refine_grid(const RefineArgs &a) { return dim3((unsigned)(((int64_t)a.n * a.nrhs + REF_THREADS - 1) / REF_THREADS), (unsigned)a.members); }
 
 int launch_refine_residual(const RefineArgs &a, const val_t *x, val_t *r, cudaStream_t s)
@@ -137,6 +188,34 @@ int launch_refine_scale(val_t *dst, const val_t *src, const double *W, int64_t l
 {
     if (len <= 0) return 0;
     refine_scale_kernel<<<(unsigned)((len + REF_THREADS - 1) / REF_THREADS), REF_THREADS, 0, s>>>(dst, src, W, len);
+    return 1;
+}
+
+int launch_refine_init(RefineState *st, const int32_t *status, int nrhs, int members, cudaStream_t s)
+{
+    const int cols = nrhs * members;
+    refine_init_kernel<<<(cols + REF_THREADS - 1) / REF_THREADS, REF_THREADS, 0, s>>>(st, status, nrhs, cols);
+    return 1;
+}
+
+int launch_refine_continue(const int *active, cudaGraphConditionalHandle h, cudaStream_t s)
+{
+    refine_continue_kernel<<<1, 1, 0, s>>>(active, h);
+    return 1;
+}
+
+int launch_refine_xmax(const RefineArgs &a, const val_t *x, unsigned long long *xmax, cudaStream_t s)
+{
+    const int per = XMAX_PER_THREAD * REF_THREADS;
+    refine_xmax_kernel<<<dim3((unsigned)((a.n + per - 1) / per), (unsigned)(a.nrhs * a.members)), REF_THREADS, 0, s>>>(a.n, x, xmax);
+    return 1;
+}
+
+int launch_refine_finish(const RefineArgs &a, const CondState *est, const unsigned long long *xmax, const int32_t *status, double *berr,
+                         double *ferr, int32_t *steps, cudaStream_t s)
+{
+    const int cols = a.nrhs * a.members;
+    refine_finish_kernel<<<(cols + REF_THREADS - 1) / REF_THREADS, REF_THREADS, 0, s>>>(a, est, xmax, status, berr, ferr, steps);
     return 1;
 }
 
