@@ -5,12 +5,15 @@ computes H = F^-T at every stored position of L + U, supernode by supernode from
 destination of supernode K lies in a supernode after K):
 
     M      = H(R, C)                          gathered from the panels of the later supernodes
-    H(R,K) = -M U_KC^T U_KK^-T
+    P_RK   = -M U_KC^T
+    H(R,K) =  P_RK U_KK^-T
     H(K,C) = -L_KK^-T L_RK^T M
-    H(K,K) =  L_KK^-T (U_KK^-T - L_RK^T H(R,K))
+    H(K,K) =  L_KK^-T (I - L_RK^T P_RK) U_KK^-T  ( = L_KK^-T (U_KK^-T - L_RK^T H(R,K)) )
 
 R = the sub-diagonal rows of L panel K, C = the packed columns of U panel K.  A^-1(i, j) = H(perm[j], perm[i]).
-Only tests import this module."""
+Every solve is a LAPACK substitution.  H(K,K) is solved from both sides, as slu_selinv.cu does: the explicit U_KK^-T of
+the second form is not backward stable for L_KK^T H(K,K) U_KK^T = I - L_RK^T H(R,K) U_KK^T when U_KK is ill-conditioned
+(pivots replaced by a threshold put it past its bound in tests/backward.py).  Only tests import this module."""
 import numpy as np
 import scipy.linalg as sla
 
@@ -121,10 +124,11 @@ def selinv(prob, layer):
         Ukc = P.upanel(layer.uval, k)
         R, C = P.lrows[k][ns:], P.ucols[k]
         M = P.gather(hl, hu, R, C) if len(R) and len(C) else np.zeros((len(R), len(C)), layer.lval.dtype)
-        Hrk = -sla.solve_triangular(Ukk, (M @ Ukc.T).T, lower=False).T if len(R) else np.zeros((0, ns))
+        Prk = -(M @ Ukc.T)
+        Hrk = sla.solve_triangular(Ukk, Prk.T, lower=False).T if len(R) else np.zeros((0, ns), Prk.dtype)
         Hkc = -sla.solve_triangular(Lkk, Lrk.T @ M, trans="T", lower=True, unit_diagonal=True)
-        Uinv_t = sla.solve_triangular(Ukk, np.eye(ns), trans="T", lower=False)
-        Hkk = sla.solve_triangular(Lkk, Uinv_t - Lrk.T @ Hrk, trans="T", lower=True, unit_diagonal=True)
+        Y = sla.solve_triangular(Lkk, np.eye(ns) - Lrk.T @ Prk, trans="T", lower=True, unit_diagonal=True)
+        Hkk = sla.solve_triangular(Ukk, Y.T, lower=False).T
         Hp = P.lpanel(hl, k)            # a view: writes land in hl
         Hp[:ns] = Hkk
         Hp[ns:] = Hrk

@@ -225,13 +225,16 @@ __global__ void __launch_bounds__(SI_NT, SELINV_MIN_CTAS<LU>) selinv_gemm_kernel
 
 // ------------------------------------------------------------------------------------------------
 // In-place back substitution with an upper triangular T of the supernode's diagonal block, one vector per thread, 16
-// unknowns at a time: the already solved unknowns are subtracted, then the 16 x 16 block inverse of diag_inv_kernel is
-// applied.  COLS = 0: the rows x of L panel K of H, T = U_KK (x <- x U_KK^-T, i.e. U_KK x^T = x^T); COLS = 1: the ns
-// columns of H(K,K) and the ncols columns of H(K,C), T = L_KK^T (unit; its block inverse is inv(L_bb) read transposed).
-// In doublecomplex the block inverses are read transposed exactly as in double, never conjugated.
+// unknowns at a time: the already solved unknowns are subtracted, giving R, then the 16 x 16 block inverse of
+// diag_inv_kernel is applied and corrected once, Z = inv R + inv (R - T_jj (inv R)), as trsm_kernel does.  COLS = 0: the
+// rows x of L panel K of H, T = U_KK (x <- x U_KK^-T, i.e. U_KK x^T = x^T); COLS = 1: the ns columns of H(K,K) and the
+// ncols columns of H(K,C), T = L_KK^T (unit; its block inverse is inv(L_bb) read transposed).  In doublecomplex the
+// block inverses and T_jj are read transposed exactly as in double, never conjugated.
 // ------------------------------------------------------------------------------------------------
+// The minimum of one CTA per SM only changes ptxas's register target: without it the correction step's 32 live values
+// spilled in the batched double COLS = 0 and doublecomplex COLS = 1 instantiations.
 template <int COLS, class LU>
-__global__ void __launch_bounds__(SELINV_VECS) selinv_trsm_kernel(LU dd, Batch b, const val_t *__restrict__ dinv,
+__global__ void __launch_bounds__(SELINV_VECS, 1) selinv_trsm_kernel(LU dd, Batch b, const val_t *__restrict__ dinv,
                                                                    val_t *__restrict__ hv)
 {
     if (blockIdx.x >= b.prefix[b.count]) return;
@@ -264,11 +267,35 @@ __global__ void __launch_bounds__(SELINV_VECS) selinv_trsm_kernel(LU dd, Batch b
                 acc[r] = vfnma(tv, z, acc[r]);
             }
         }
+        // Z = inv R, then one correction step Z += inv (R - T_jj Z) with the block's own entries (unit diagonal for
+        // L_KK^T): the product with the explicit inverse alone has a backward error that grows with cond(T_jj)
         const val_t *bi = inv + (size_t)blk * 512 + (COLS ? 256 : 0);
+        auto tjj = [&](int r, int c) -> val_t {      // T_jj(r, c), c > r
+            return COLS ? D[(int64_t)(p0 + r) * lda + p0 + c] : D[(int64_t)(p0 + c) * lda + p0 + r];
+        };
+        val_t z[16];
+#pragma unroll
+        for (int r = 0; r < 16; ++r) {
+            z[r] = vzero();
+            if (r >= w) continue;
+#pragma unroll
+            for (int c = 0; c < 16; ++c) z[r] = vfma(COLS ? bi[r * 16 + c] : bi[c * 16 + r], acc[c], z[r]);
+        }
 #pragma unroll
         for (int r = 0; r < 16; ++r) {
             if (r >= w) break;
-            val_t y = vzero();
+            val_t s = COLS ? vsub(acc[r], z[r]) : vfnma(D[(int64_t)(p0 + r) * lda + p0 + r], z[r], acc[r]);
+#pragma unroll
+            for (int c = r + 1; c < 16; ++c) {
+                if (c >= w) break;
+                s = vfnma(tjj(r, c), z[c], s);
+            }
+            acc[r] = s;
+        }
+#pragma unroll
+        for (int r = 0; r < 16; ++r) {
+            if (r >= w) break;
+            val_t y = z[r];
 #pragma unroll
             for (int c = 0; c < 16; ++c) y = vfma(COLS ? bi[r * 16 + c] : bi[c * 16 + r], acc[c], y);
             x[(int64_t)(p0 + r) * stride] = y;

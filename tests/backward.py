@@ -16,6 +16,7 @@ write to a position that no product touches fails.  In doublecomplex |.| is the 
     gemm_sub (C - A B)         C_out - (C - A B)              |C| + |A| |B|           2 (k + 1) u
     factorization              F - L U on pattern(F, L U)     |L| |U|                 4 k_max u
     solve, op = N / T / H      b - op(L U) x, per row         op(|L| |U|) |x|         4 k_max u
+    selected inversion         per step of each supernode: the table of the last section
 
 u = 2^-53.  k_max is the largest panel height (nsupr) of the problem.  The bounds are fixed formulas in u: none is
 tuned to what a GPU returns.  Pivots replaced by +-thresh (static pivoting) are excluded from the factorization ratio
@@ -545,3 +546,134 @@ def kkt_matrix():
 
 
 KKT_THRESH = 0.625   # above the smallest pivots of the matched, scaled KKT matrix (0.57..): some are replaced
+
+
+# ------------------------------------------------------------------------------------------------ selected inversion
+# H = F^-T supernode by supernode (oracle/selinv.py, slu_selinv.cu).  For supernode K with sub-diagonal rows R (m of them),
+# packed U columns C (ncols) and M = H(R, C) gathered from the returned H, each step solves its own equations:
+#
+#    step     residual R                                           scale D                                          bound
+#    H(R,K)   H(R,K) U_KK^T + M U_KC^T                             |H(R,K)| |U_KK|^T + |M| |U_KC|^T                  4 (ns + ncols) u
+#    H(K,C)   L_KK^T H(K,C) + L_RK^T M                             |L_KK|^T |H(K,C)| + |L_RK|^T |M|                  4 (ns + m) u
+#    H(K,K)   L_KK^T H(K,K) U_KK^T - I + L_RK^T H(R,K) U_KK^T      |L_KK|^T |H(K,K)| |U_KK|^T + I                    8 (ns + m) u
+#                                                                  + |L_RK|^T (|H(R,K)| |U_KK|^T + |M| |U_KC|^T)
+#
+# Each is a product of length ncols or m (its rounding is covered by the terms with M or L_RK) and one triangular solve of
+# length ns (a substitution's backward error is within the terms with the solved block); H(K,K) takes two solves and the
+# product that forms its right-hand side, hence twice the constant.  Doubled in complex, as every bound here.  H(K,C) is
+# checked where it is stored: row i of column j from the column's skyline start on (rows above it are not kept, and
+# L_KK^T, upper triangular, takes the stored rows from the stored rows only).
+SELINV_STEPS = ("H(R,K)", "H(K,C)", "H(K,K)")
+
+
+def _selinv_node(P, lval, uval, k):
+    """(ns, Lkk unit lower, Ukk upper, Lrk, Ukc dense-packed, R, C) of supernode k of the factors lval / uval"""
+    f, ns = int(P.xsup[k]), int(P.xsup[k + 1] - P.xsup[k])
+    Lp = P.lpanel(lval, k)
+    return (ns, np.tril(Lp[:ns], -1) + np.eye(ns), np.triu(Lp[:ns]), Lp[ns:], P.upanel(uval, k),
+            P.lrows[k][ns:], P.ucols[k])
+
+
+def _gather_m(P, hl, hu, R, C):
+    return P.gather(hl, hu, R, C) if len(R) and len(C) else np.zeros((len(R), len(C)), hl.dtype)
+
+
+def selinv_ratios(prob, layer, hl, hu):
+    """The three steps of every supernode of the factors in `layer`, on H as returned (hl, hu shaped like layer.lval /
+    layer.uval) -> (the largest ratio / bound of each step, the largest ratio of each step)"""
+    from oracle.selinv import _Panels
+    P = _Panels(prob, layer)
+    cf = cfactor(layer.lval.dtype)
+    scaled, raw = np.zeros(3), np.zeros(3)
+    for k in np.nonzero(layer.held)[0]:
+        ns, Lkk, Ukk, Lrk, Ukc, R, C = _selinv_node(P, layer.lval, layer.uval, k)
+        f, m, nc = int(P.xsup[k]), len(R), len(C)
+        Hp = P.lpanel(hl, k)
+        Hkk, Hrk = Hp[:ns], Hp[ns:]
+        Hkc = P.upanel(hu, k)
+        M = _gather_m(P, hl, hu, R, C)
+        eM, eUkc, eLrk, eUkk, eLkk, eHrk = ext(M), ext(Ukc), ext(Lrk), ext(Ukk), ext(Lkk), ext(Hrk)
+        aM, aUkc, aLrk, aUkk, aLkk, aHrk = (np.abs(a) for a in (M, Ukc, Lrk, Ukk, Lkk, Hrk))
+        # H(R,K)
+        HU = eHrk @ eUkk.T
+        steps = [(HU + eM @ eUkc.T, aHrk @ aUkk.T + aM @ aUkc.T, 4 * (ns + nc))]
+        # H(K,C), on the stored rows of each column
+        stored = np.arange(ns)[:, None] >= (P.ufst[k] - f)[None, :]
+        r = eLkk.T @ ext(Hkc) + eLrk.T @ eM
+        d = aLkk.T @ np.abs(Hkc) + aLrk.T @ aM
+        steps.append((np.where(stored, r, 0), np.where(stored, d, 0), 4 * (ns + m)))
+        # H(K,K)
+        r = eLkk.T @ ext(Hkk) @ eUkk.T - np.eye(ns) + eLrk.T @ HU
+        d = aLkk.T @ np.abs(Hkk) @ aUkk.T + np.eye(ns) + aLrk.T @ (aHrk @ aUkk.T + aM @ aUkc.T)
+        steps.append((r, d, 8 * (ns + m)))
+        for s, (r, d, c) in enumerate(steps):
+            q = ratio(r, d)
+            raw[s] = max(raw[s], q)
+            scaled[s] = max(scaled[s], q / (c * cf * U))
+    return scaled, raw
+
+
+def _back_blocked(t, b, unit, inv_of, refine):
+    """T Z = B for an upper triangle T (unit: its diagonal taken as 1), B's columns the vectors: selinv_trsm_kernel's
+    sweep, 16 unknowns at a time from the last block (partial where 16 does not divide ns) up, R = B_j - sum_{p > j} T_jp Z_p, then
+    Z_j = inv(T_jj) R with the explicit block inverse inv_of(T_jj), and `refine` steps Z_j += inv (R - T_jj Z_j)"""
+    ns = t.shape[0]
+    z = b.copy()
+    for p0 in range(((ns - 1) // 16) * 16, -1, -16):
+        p1 = min(ns, p0 + 16)
+        tjj = np.triu(t[p0:p1, p0:p1], 1) + np.eye(p1 - p0) if unit else np.triu(t[p0:p1, p0:p1])
+        inv = inv_of(tjj)
+        r = z[p0:p1] - t[p0:p1, p1:] @ z[p1:]
+        x = inv @ r
+        for _ in range(refine):
+            x = x + inv @ (r - tjj @ x)
+        z[p0:p1] = x
+    return z
+
+
+def selinv_blocked(prob, layer, refine=1):
+    """The sweep of slu_selinv.cu in NumPy, on the factors in `layer` -> (hl, hu) as oracle.selinv.selinv returns them.
+    Per supernode, the products P = -M U_KC^T, H(K,C) = -L_RK^T M and H(K,K) = I - L_RK^T P, then every row x of
+    [H(K,K); P] solves x U_KK^T = x and every column y of [H(K,K) H(K,C)] solves L_KK^T y = y, each by _back_blocked with
+    diag_inv_kernel's 16 x 16 inverses (U_bb's, and L_bb's transposed).  refine=0 is the plain product with the inverse,
+    refine=1 adds the correction step: for the sensitivity tests of test_selinv_backward_cpu.py only."""
+    from oracle.selinv import _Panels
+    P = _Panels(prob, layer)
+    hl, hu = np.zeros_like(layer.lval), np.zeros_like(layer.uval)
+    for k in np.nonzero(layer.held)[0][::-1]:
+        ns, Lkk, Ukk, Lrk, Ukc, R, C = _selinv_node(P, layer.lval, layer.uval, k)
+        f, klst = int(P.xsup[k]), int(P.xsup[k + 1])
+        M = _gather_m(P, hl, hu, R, C)
+        Prk = -(M @ Ukc.T)
+        Hkc = -(Lrk.T @ M)
+        Hkk = np.eye(ns, dtype=hl.dtype) - Lrk.T @ Prk
+        rows = _back_blocked(Ukk, np.vstack([Hkk, Prk]).T, False, _inv_upper16, refine).T
+        cols = _back_blocked(Lkk.T, np.hstack([rows[:ns], Hkc]), True, lambda t: _inv_unit_lower16(t.T).T, refine)
+        Hp = P.lpanel(hl, k)
+        Hp[:ns] = cols[:, :ns]
+        Hp[ns:] = rows[ns:]
+        o = int(layer.uval_off[k])
+        for j in range(len(C)):
+            fst, seg = int(P.ufst[k][j]), int(P.useg[k][j])
+            hu[o + seg:o + seg + klst - fst] = cols[fst - f:, ns + j]
+    return hl, hu
+
+
+def pivot_logdet(prob, layer):
+    """(sign or phase, log |det F|, its tolerance, the phase's tolerance) from the pivots of `layer`: log |u_ii| summed
+    exactly (math.fsum) and the count of negative pivots, or in complex exp(i theta) with theta = fsum(arg u_ii) mod
+    2 pi.  A sum of n correctly rounded terms x_i in any order is within n u sum |x_i| of the exact sum of the terms
+    (n - 1 additions, each off by at most u times a partial sum, plus the rounding of each term); a bound in max |x_i|
+    alone does not hold for a sequential sum, whose partial sums grow to n max |x_i|."""
+    import math
+    from oracle.inertia import pivots
+    d = pivots(prob, layer)
+    logs = np.log(np.abs(d))
+    n = len(d)
+    la = math.fsum(logs.tolist())
+    tol = n * U * float(np.abs(logs).sum())
+    if not np.iscomplexobj(d):
+        return (-1.0 if np.count_nonzero(d < 0) % 2 else 1.0), la, tol, 0.0
+    arg = np.angle(d)
+    theta = math.remainder(math.fsum(arg.tolist()), 2 * math.pi)
+    return np.exp(1j * theta), la, tol, n * U * (float(np.abs(arg).sum()) + 2 * math.pi)
