@@ -568,6 +568,37 @@ int slu_b200_batch_gsrfs_device(slu_b200_handle_t h, const double *b, int ldb, d
                                 double *ferr, int32_t *steps, void *stream);
 int slu_b200_gscon_device(slu_b200_handle_t h, char norm, const double *anorm, double *rcond, void *stream);
 int slu_b200_batch_gscon_device(slu_b200_handle_t h, char norm, const double *anorm, double *rcond, void *stream);
+/* ---- gradients on the caller's CUDA stream, capturable into the same graph: the pieces of d log|det A| / dA and of the
+ * adjoint of x = A^-1 b, in A's own ordering and on the pattern of the last scaled fill (the order refill takes).
+ * selinv_device / batch_selinv_device: slu_b200_selinv / _batch_selinv ordered on the stream, with no host wait and no
+ * timing.  The missed-destination check stays on the device: a member of a sweep that missed one gets NaN from
+ * logdet_grad_device, and the next host-synchronous call reads the check before it lets selinv_get use the inverse.  The
+ * first selected inversion on a handle allocates the second arena and uploads the plan (refused under capture); the arena is
+ * never moved afterwards.
+ * logdet_device / batch_logdet_device: slu_b200_logdet / _batch_logdet into logabs[members] and sign[members] in device
+ * memory, bit for bit the host call's values.
+ * logdet_grad_device / batch_logdet_grad_device: grad[j nnz + e] = coef[j] R_i C_j H(perm[perm_r[i]], perm[j]) for entry e =
+ * (i, j) of the scaled fill's CSR pattern, H the inverse of the last selinv or selinv_device (F^-T), R and C member j's
+ * scalings: coef[j] A_j^-T(i, j), the gradient of log |det A_j| times coef[j].  coef: one value per member in device memory.
+ * Refused when the host knows the inverse is stale (a later fill, refill, upload or factorization).
+ * solve_grad_device / batch_solve_grad_device: grad[j nnz + e] = -sum_k lam_j(i, k) x_j(col, k) for entry e = (i, col) of the
+ * same pattern: the gradient of a loss with respect to A's values when x = A^-1 b and lam = A^-T dL/dx (solve_scaled_device
+ * with trans 1).  lam and x: n x nrhs column-major per member, ldl / ldx elements apart per column, member-major.  A first
+ * call with more right-hand sides than any before allocates a staging buffer (refused under capture).
+ * Every call: the preconditions, pointer checks, stream order and refusals of solve_scaled_device (a scaled fill, factors from
+ * factor or pending from factor_device, 1 x 1 x 1 grids, no Schur handles); the first gradient call after a scaled fill builds
+ * the refill's slot map if no refill did (allocates and waits once; refused under capture).  A member whose status is not 0
+ * gets NaN results; the other members are unaffected.  stats.reserved[4] = 0, [5] = the launches enqueued. */
+int slu_b200_selinv_device(slu_b200_handle_t h, void *stream);
+int slu_b200_batch_selinv_device(slu_b200_handle_t h, void *stream);
+int slu_b200_logdet_device(slu_b200_handle_t h, double *logabs, double *sign, void *stream);
+int slu_b200_batch_logdet_device(slu_b200_handle_t h, double *logabs, double *sign, void *stream);
+int slu_b200_logdet_grad_device(slu_b200_handle_t h, const double *coef, double *grad, void *stream);
+int slu_b200_batch_logdet_grad_device(slu_b200_handle_t h, const double *coef, double *grad, void *stream);
+int slu_b200_solve_grad_device(slu_b200_handle_t h, const double *lam, int ldl, const double *x, int ldx, int nrhs,
+                               double *grad, void *stream);
+int slu_b200_batch_solve_grad_device(slu_b200_handle_t h, const double *lam, int ldl, const double *x, int ldx, int nrhs,
+                                     double *grad, void *stream);
 /* the CUDA device the handle was created on (options.device, or the current device when that was < 0): where the
  * device-memory arguments of the calls above must live */
 int slu_b200_get_device(slu_b200_handle_t h, int *device);
@@ -685,6 +716,20 @@ int slu_b200_z_batch_gsrfs_device(slu_b200_zhandle_t h, const double *b, int ldb
                                   double *berr, double *ferr, int32_t *steps, void *stream);
 int slu_b200_z_gscon_device(slu_b200_zhandle_t h, char norm, const double *anorm, double *rcond, void *stream);
 int slu_b200_z_batch_gscon_device(slu_b200_zhandle_t h, char norm, const double *anorm, double *rcond, void *stream);
+/* as slu_b200_selinv_device / _logdet_device / _logdet_grad_device / _solve_grad_device and their batched twins: sign holds
+ * 2 x members doubles (exp(i theta) as (re, im)); coef, grad, lam and x interleaved doublecomplex (ldl, ldx count complex
+ * elements).  logdet_grad: grad = coef[j] R_i C_j conj(H(...)), coef[j] A_j^-H(i, j); solve_grad: grad = -sum_k lam_j(i, k)
+ * conj(x_j(col, k)) with lam = A^-H dL/dx (trans 2) */
+int slu_b200_z_selinv_device(slu_b200_zhandle_t h, void *stream);
+int slu_b200_z_batch_selinv_device(slu_b200_zhandle_t h, void *stream);
+int slu_b200_z_logdet_device(slu_b200_zhandle_t h, double *logabs, double *sign, void *stream);
+int slu_b200_z_batch_logdet_device(slu_b200_zhandle_t h, double *logabs, double *sign, void *stream);
+int slu_b200_z_logdet_grad_device(slu_b200_zhandle_t h, const double *coef, double *grad, void *stream);
+int slu_b200_z_batch_logdet_grad_device(slu_b200_zhandle_t h, const double *coef, double *grad, void *stream);
+int slu_b200_z_solve_grad_device(slu_b200_zhandle_t h, const double *lam, int ldl, const double *x, int ldx, int nrhs,
+                                 double *grad, void *stream);
+int slu_b200_z_batch_solve_grad_device(slu_b200_zhandle_t h, const double *lam, int ldl, const double *x, int ldx, int nrhs,
+                                       double *grad, void *stream);
 int slu_b200_z_get_stats(slu_b200_zhandle_t h, slu_b200_stats_t *out);
 int slu_b200_z_plan(const slu_b200_lu_view_t *lu, const slu_b200_options_t *opt, slu_b200_stats_t *stats);
 void slu_b200_z_destroy(slu_b200_zhandle_t h);

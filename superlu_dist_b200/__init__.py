@@ -8,4 +8,12 @@ fixtures dumped from the reference (``dumpio``).  Nothing here computes a factor
 """
 from .problem import LUProblem  # noqa: F401
 
-__all__ = ["LUProblem"]
+__all__ = ["LUProblem", "autograd"]
+
+
+def __getattr__(name):
+    # superlu_dist_b200.autograd imports torch: loaded on first use
+    if name == "autograd":
+        import importlib
+        return importlib.import_module(".autograd", __name__)
+    raise AttributeError(f"module {__name__!r} has no attribute {name!r}")

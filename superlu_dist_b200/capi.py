@@ -179,6 +179,13 @@ def lib():
     for f in ("gscon_device", "batch_gscon_device"):
         for pre in ("slu_b200_", "slu_b200_z_"):
             getattr(L, pre + f).argtypes = [C.c_void_p, C.c_char, C.c_void_p, C.c_void_p, C.c_void_p]
+    # gradients on the caller's stream
+    for pre in ("slu_b200_", "slu_b200_z_", "slu_b200_batch_", "slu_b200_z_batch_"):
+        getattr(L, pre + "selinv_device").argtypes = [C.c_void_p, C.c_void_p]
+        getattr(L, pre + "logdet_device").argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        getattr(L, pre + "logdet_grad_device").argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        getattr(L, pre + "solve_grad_device").argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int,
+                                                          C.c_void_p, C.c_void_p]
     _lib = L
     return L
 
@@ -346,6 +353,75 @@ def _factor_device(name, complex_, h, info, count):
     return info
 
 
+def _stream(complex_, h):
+    """(torch device of the handle, raw cudaStream_t of its current stream)"""
+    import torch
+    dev = torch.device("cuda", _handle_device(complex_, h))
+    return dev, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
+def _selinv_device(name, complex_, h):
+    """slu_b200_[z_][batch_]selinv_device on the current stream of the handle's device"""
+    _, stream = _stream(complex_, h)
+    _check(_fn(name, complex_)(h, stream))
+
+
+def _logdet_device(name, complex_, h, count):
+    """slu_b200_[z_][batch_]logdet_device -> (sign, logabs) CUDA tensors (count,): sign float64, or complex128 of modulus 1"""
+    import torch
+    dev, stream = _stream(complex_, h)
+    la = torch.empty(count, dtype=torch.float64, device=dev)
+    sg = torch.empty(count, dtype=torch.complex128 if complex_ else torch.float64, device=dev)
+    _check(_fn(name, complex_)(h, C.c_void_p(la.data_ptr()), C.c_void_p(sg.data_ptr()), stream))
+    return sg, la
+
+
+def _logdet_grad(name, complex_, h, coef, count, nnz):
+    """slu_b200_[z_][batch_]logdet_grad_device with coef a CUDA tensor of count values -> grad, a CUDA tensor (count, nnz)"""
+    import torch
+    if not _is_tensor(coef) or coef.numel() != count:
+        raise ValueError(f"coef must be a CUDA tensor of {count} values")
+    c, stream = _device_args(coef.reshape(count), complex_, None, "coef")
+    g = torch.empty((count, nnz), dtype=c.dtype, device=c.device)
+    _check(_fn(name, complex_)(h, C.c_void_p(c.data_ptr()), C.c_void_p(g.data_ptr()), stream))
+    return g
+
+
+def _solve_grad(name, complex_, h, lam, x, n, batch, nnz):
+    """slu_b200_[z_][batch_]solve_grad_device on CUDA tensors lam and x of solve_scaled's shapes -> grad, a CUDA tensor (nnz,)
+    or (batch, nnz)"""
+    import torch
+    lead = () if batch is None else (batch,)
+    nd = len(lead) + 1
+    if (not (_is_tensor(lam) and _is_tensor(x)) or tuple(lam.shape) != tuple(x.shape) or lam.dim() not in (nd, nd + 1)
+            or tuple(lam.shape[:len(lead)]) != lead or lam.shape[-1] != n):
+        raise ValueError(f"lam and x must both be CUDA tensors of shape {lead + (n,)} or {lead + ('nrhs', n)}")
+    lam, stream = _device_args(lam, complex_, None, "lam")
+    x, _ = _device_args(x, complex_, None, "x")
+    nrhs = 1 if lam.dim() == nd else lam.shape[-2]
+    g = torch.empty(lead + (nnz,), dtype=lam.dtype, device=lam.device)
+    _check(_fn(name, complex_)(h, C.c_void_p(lam.data_ptr()), n, C.c_void_p(x.data_ptr()), n, nrhs, C.c_void_p(g.data_ptr()),
+                               stream))
+    return g
+
+
+class _Generation:
+    """A counter of the writes to a handle's values or factors: every upload, fill, refill and factorization bumps it and
+    records its name, so that a gradient computed later can tell that the factors it needs are gone
+    (superlu_dist_b200.autograd)."""
+    generation = 0
+    moved_by = None
+    fill_generation = 0            # the generation of the last upload or fill: the scaling it set stays until the next one
+    fill_perm_r = None             # the perm_r of the last scaled fill (None: the identity)
+
+    def _moved(self, name, perm_r=None):
+        self.generation += 1
+        self.moved_by = name
+        if name == "upload" or name.startswith("fill"):
+            self.fill_generation = self.generation
+            self.fill_perm_r = perm_r
+
+
 def device_count():
     return lib().slu_b200_device_count()
 
@@ -475,7 +551,7 @@ def nccl_unique_id():
     return bytes(buf)
 
 
-class Handle:
+class Handle(_Generation):
     """slu_b200_handle_t: create (analysis + HBM allocation) / upload / factor / download."""
 
     def __init__(self, prob, z=0, **opt):
@@ -488,9 +564,11 @@ class Handle:
         _check(_fn("create", self.z_)(C.byref(self.h), C.byref(self.view), C.byref(self.opt)))
 
     def upload(self):
+        self._moved("upload")
         _check(_fn("upload", self.z_)(self.h))
 
     def factor(self):
+        self._moved("factor")
         info = C.c_int(0)
         _check(_fn("factor", self.z_)(self.h, C.byref(info)))
         return info.value
@@ -500,10 +578,12 @@ class Handle:
         CUDA tensor (1,): 0, the 1-based column of the first exact zero pivot, or -1 (missing Schur-update destinations),
         written in stream order.  info: a caller-owned tensor to write instead (what a captured CUDA graph needs).  Solves
         on torch tensors follow without a wait; host calls wait for the status and refuse as after factor()."""
+        self._moved("factor_device")
         return _factor_device("factor_device", self.z_, self.h, info, 1)
 
     def factor_host(self):
         """upload + factor + download with the transfers overlapped (slu_b200_factor_host)."""
+        self._moved("factor_host")
         info = C.c_int(0)
         _check(_fn("factor_host", self.z_)(self.h, C.byref(info)))
         return info.value
@@ -514,6 +594,7 @@ class Handle:
     def fill_csr(self, rowptr, colind, val, perm):
         """Device-side distribution (slu_b200_fill_csr): P A P^T scattered into the HBM panels by a kernel; replaces
         upload().  perm[old] = new.  val is complex128 for a complex problem (slu_b200_z_fill_csr)."""
+        self._moved("fill_csr")
         rp = np.ascontiguousarray(rowptr, np.int32)
         ci = np.ascontiguousarray(colind, np.int32)
         v = np.ascontiguousarray(val, self._dtype())
@@ -528,6 +609,7 @@ class Handle:
         factors into R and C.  Replaces upload().  -> dict rowcnd, colcnd, amax, equed (0 none, 1 rows, 2 columns, 3 both),
         norm_inf (||F||_inf, for rcond(norm_inf, 'I')), max_abs"""
         rp, ci, pm, pr, Rv, Cv = _scaled_args(rowptr, colind, perm, perm_r, R, C, [(self.prob.n,)])
+        self._moved("fill_csr_scaled", pr)
         v = np.ascontiguousarray(val, self._dtype())
         out = np.zeros(6)
         _check(_fn("fill_csr_scaled", self.z_)(self.h, len(rp) - 1, _ptr(rp), _ptr(ci), _ptr(v), _ptr(pr), _ptr(pm), _ptr(Rv),
@@ -540,6 +622,7 @@ class Handle:
         float64 (complex128 for a complex problem), in that fill's CSR entry order.  F is written with the kept perm_r, perm,
         R and C (no equilibration), ordered after the work on the current stream of val's device, which waits for it in turn:
         val may be overwritten right after.  factor() follows as after any fill."""
+        self._moved("refill")
         v, stream = _device_args(val, self.z_, [(getattr(self, "_nnz", val.shape[0]),)], "val")
         _check(_fn("refill", self.z_)(self.h, C.c_void_p(v.data_ptr()), stream))
 
@@ -649,6 +732,28 @@ class Handle:
         _check(_fn("inertia", self.z_)(self.h, cnt.ctypes.data_as(C.c_void_p), C.byref(dfc)))
         return int(cnt[0]), int(cnt[1]), int(cnt[2]), dfc.value
 
+    def selinv_device(self):
+        """selinv() ordered on the current stream of the handle's device, with no host wait (slu_b200_selinv_device)"""
+        _selinv_device("selinv_device", self.z_, self.h)
+
+    def logdet_device(self):
+        """logdet() on the device (slu_b200_logdet_device) -> (sign, logabs): 0-d CUDA tensors, NaN where factor_device found
+        a zero pivot"""
+        sg, la = _logdet_device("logdet_device", self.z_, self.h, 1)
+        return sg.reshape(()), la.reshape(())
+
+    def logdet_grad(self, coef):
+        """coef * A^-T on A's pattern (coef * A^-H in complex), in the last scaled fill's entry order, from the inverse of the
+        last selinv / selinv_device (slu_b200_logdet_grad_device).  coef: a CUDA tensor of one value (float64 / complex128)
+        -> a CUDA tensor (nnz,)"""
+        return _logdet_grad("logdet_grad_device", self.z_, self.h, coef, 1, self._nnz).reshape(-1)
+
+    def solve_grad(self, lam, x):
+        """-lam x^T sampled on A's pattern (-lam x^H in complex), in the last scaled fill's entry order
+        (slu_b200_solve_grad_device): the gradient with respect to A's values of a loss of x = A^-1 b, with lam = A^-T dL/dx
+        (solve_scaled(dL/dx, 'T'); 'H' in complex).  lam and x: CUDA tensors (n,) or (nrhs, n) -> a CUDA tensor (nnz,)"""
+        return _solve_grad("solve_grad_device", self.z_, self.h, lam, x, self.prob.n, None, self._nnz)
+
     def _dtype(self):
         return np.complex128 if self.z_ else np.float64
 
@@ -708,7 +813,7 @@ class SchurHandle(Handle):
         return self._pass("schur_expand", y)
 
 
-class BatchHandle:
+class BatchHandle(_Generation):
     """A batched handle (slu_b200_batch_*): `batch` matrices with the sparsity pattern of `prob` (layer 0, 1 x 1 x 1
     grid), factored and solved together.  The analysis is shared; each member has its own values.  A complex128 `prob`
     takes the doublecomplex twins (slu_b200_z_batch_*): values, right-hand sides and solutions are then complex128."""
@@ -727,6 +832,7 @@ class BatchHandle:
 
     def fill_csr(self, rowptr, colind, vals, perm):
         """One CSR pattern and perm[old] = new for every member; vals: (batch, nnz), row j = member j's values."""
+        self._moved("fill_csr")
         rp = np.ascontiguousarray(rowptr, np.int32)
         ci = np.ascontiguousarray(colind, np.int32)
         v = np.ascontiguousarray(vals, self._dtype())
@@ -742,6 +848,7 @@ class BatchHandle:
         arrays (batch,) with the keys of Handle.fill_csr_scaled (equed int32)"""
         n, B = self.prob.n, self.batch
         rp, ci, pm, pr, Rv, Cv = _scaled_args(rowptr, colind, perm, perm_r, R, C, [(n,), (B, n)])
+        self._moved("fill_csr_scaled", pr)
         per = [x.ndim == 2 for x in (Rv, Cv) if x is not None]
         if len(set(per)) > 1:
             raise ValueError("R and C must both be shared (n,) or both per member (batch, n)")
@@ -759,6 +866,7 @@ class BatchHandle:
     def refill(self, vals):
         """Handle.refill for every member (slu_b200_batch_refill): vals a torch CUDA tensor (batch, nnz); each member keeps
         its own R and C"""
+        self._moved("refill")
         nnz = getattr(self, "_nnz", vals.shape[-1])
         v, stream = _device_args(vals, self.z_, [(self.batch, nnz)], "vals")
         _check(_fn("batch_refill", self.z_)(self.h, C.c_void_p(v.data_ptr()), stream))
@@ -801,6 +909,7 @@ class BatchHandle:
 
     def factor(self):
         """-> int32 array (batch,): 0, or the 1-based column of the member's first exact zero pivot."""
+        self._moved("factor")
         info = np.zeros(self.batch, np.int32)
         _check(_fn("batch_factor", self.z_)(self.h, info.ctypes.data_as(C.c_void_p)))
         return info
@@ -808,6 +917,7 @@ class BatchHandle:
     def factor_device(self, info=None):
         """factor() on the device for every member (slu_b200_batch_factor_device), as Handle.factor_device -> an int32 CUDA
         tensor (batch,)"""
+        self._moved("factor_device")
         return _factor_device("batch_factor_device", self.z_, self.h, info, self.batch)
 
     def solve(self, b, trans="N"):
@@ -875,10 +985,28 @@ class BatchHandle:
         _check(_fn("batch_inertia", self.z_)(self.h, cnt.ctypes.data_as(C.c_void_p), dfc.ctypes.data_as(C.c_void_p)))
         return cnt[:, 0].copy(), cnt[:, 1].copy(), cnt[:, 2].copy(), dfc
 
+    def selinv_device(self):
+        """selinv() of every member on the current stream, with no host wait (slu_b200_batch_selinv_device)"""
+        _selinv_device("batch_selinv_device", self.z_, self.h)
+
+    def logdet_device(self):
+        """logdet() on the device (slu_b200_batch_logdet_device) -> (sign, logabs): CUDA tensors (batch,)"""
+        return _logdet_device("batch_logdet_device", self.z_, self.h, self.batch)
+
+    def logdet_grad(self, coef):
+        """Handle.logdet_grad for every member (slu_b200_batch_logdet_grad_device): coef a CUDA tensor (batch,) -> (batch, nnz)"""
+        return _logdet_grad("batch_logdet_grad_device", self.z_, self.h, coef, self.batch, self._nnz)
+
+    def solve_grad(self, lam, x):
+        """Handle.solve_grad for every member (slu_b200_batch_solve_grad_device): lam and x (batch, n) or (batch, nrhs, n) ->
+        (batch, nnz)"""
+        return _solve_grad("batch_solve_grad_device", self.z_, self.h, lam, x, self.prob.n, self.batch, self._nnz)
+
     def fill_affine(self, rowptr, colind, terms, coef, perm):
         """An affine family on one CSR pattern (slu_b200_batch_fill_affine): member j's values are
         sum_t coef[j, t] * terms[t], computed on the device.  terms: (T, nnz), coef: (batch, T), float64 (complex128 for a
         complex problem); perm[old] = new as in fill_csr."""
+        self._moved("fill_affine")
         rp = np.ascontiguousarray(rowptr, np.int32)
         ci = np.ascontiguousarray(colind, np.int32)
         tv = np.ascontiguousarray(terms, self._dtype())

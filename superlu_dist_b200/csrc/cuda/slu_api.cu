@@ -84,6 +84,14 @@
 #define slu_b200_batch_gsrfs_device slu_b200_z_batch_gsrfs_device
 #define slu_b200_gscon_device slu_b200_z_gscon_device
 #define slu_b200_batch_gscon_device slu_b200_z_batch_gscon_device
+#define slu_b200_selinv_device slu_b200_z_selinv_device
+#define slu_b200_batch_selinv_device slu_b200_z_batch_selinv_device
+#define slu_b200_logdet_device slu_b200_z_logdet_device
+#define slu_b200_batch_logdet_device slu_b200_z_batch_logdet_device
+#define slu_b200_logdet_grad_device slu_b200_z_logdet_grad_device
+#define slu_b200_batch_logdet_grad_device slu_b200_z_batch_logdet_grad_device
+#define slu_b200_solve_grad_device slu_b200_z_solve_grad_device
+#define slu_b200_batch_solve_grad_device slu_b200_z_batch_solve_grad_device
 #define SLU_API "slu_b200_z_"     // name prefix of the exported calls, for error messages
 #else
 #define SLU_API "slu_b200_"
@@ -401,6 +409,16 @@ struct slu_b200_handle_s {
         int launches;
     };
     std::vector<LoopGraph> loop_graphs;
+    // the gradient calls (selinv_device, logdet_device, logdet_grad_device, solve_grad_device): the status of the last device
+    // selected inversion per member and its record {factorization count inverted, missed destinations} (si_dev: the inverse
+    // came from selinv_device, settle reads the record); logdet_device's partials and result; solve_grad_device's row-major
+    // copies of lambda and x
+    DevBuf<int32_t> d_si_status;
+    DevBuf<unsigned long long> d_si_rec;
+    bool si_dev = false;
+    DevBuf<double> d_lpart, d_lres;
+    DevBuf<phase_t> d_lph;
+    DevBuf<val_t> d_gstage;
 };
 
 namespace {
@@ -478,6 +496,12 @@ int settle(slu_b200_handle_s *H)
     std::copy(info.begin(), info.end(), H->member_info.begin());
     H->st.tiny_pivots = (int64_t)tiny;
     H->status_on_device = false;
+    if (H->si_dev) {                       // the inverse of selinv_device: the count it inverted, and whether it missed destinations
+        unsigned long long rec[2] = {0, 0};
+        CU(cudaMemcpy(rec, H->d_si_rec.p, sizeof rec, cudaMemcpyDeviceToHost));
+        H->si_epoch = rec[0];
+        if (rec[1]) H->si_ready = false;
+    }
     if (H->captured && H->epoch != H->si_epoch) H->si_ready = false;
     return 0;
 }
@@ -2336,14 +2360,9 @@ static int selinv_plan(slu_b200_handle_s *H)
     return H->d_si_pool.upload(pool);
 }
 
-// The sweep on device LU d (H->dev, or H->bdev for every member of a batched handle: the same launches with gridDim.y =
-// members).  The destination maps are value-independent and built on H->dev for all members, as in slu_b200_batch_factor.
-// fn names the call in the messages.
-}  // extern "C"
-template <class LU>
-static int selinv_sweep(slu_b200_handle_t H, const LU &d, int members, const char *fn, double out[4])
+// The plan and the second arena, on the first selected inversion of the handle (allocates)
+static int selinv_alloc(slu_b200_handle_t H, int members, const char *fn)
 {
-    H->si_ready = false;
     if (H->si_levels.empty() && selinv_plan(H)) return -1;
     if (!H->d_hinv.p && H->d_hinv.alloc((size_t)H->member_len * members)) {
         cudaGetLastError();
@@ -2352,12 +2371,19 @@ static int selinv_sweep(slu_b200_handle_t H, const LU &d, int members, const cha
         return fail("%s: the inverse needs a second arena of %.2f GB beside the factors, which does not fit (%s); "
                     "the factors are unchanged", fn, 1e-9 * sizeof(val_t) * H->member_len * members, why.c_str());
     }
+    return 0;
+}
+}  // extern "C"
+
+// The sweep's launches on H->stream, dev.err counting the missed destinations -> the launches; *flops as selinv's out[1] for
+// one member
+template <class LU>
+static int selinv_enqueue(slu_b200_handle_t H, const LU &d, double *flops)
+{
     cudaStream_t s = H->stream;
     const int64_t *p64 = H->d_pool_i64.p, *sp = H->d_si_pool.p;
     val_t *hv = H->d_hinv.p;
-    double flops = 0;
     int launches = 0;
-    const double t0 = now_s();
     CU(cudaMemsetAsync(H->dev.err, 0, sizeof(int), s));
     for (size_t li = H->levels.size(); li-- > 0;) {
         const LevelPlan &L = H->levels[li];
@@ -2373,9 +2399,26 @@ static int selinv_sweep(slu_b200_handle_t H, const LU &d, int members, const cha
         for (int t = 0; t < L.count; ++t) {
             const NodeDesc &nd = H->nodes[H->h_pool_i32[L.nodes_off + t]];
             const double m = nd.m, n = nd.ncols, ns = nd.ns;
-            flops += 4.0 * m * n * ns + 2.0 * m * ns * ns + (nd.nsupr + ns + n) * ns * ns;
+            *flops += 4.0 * m * n * ns + 2.0 * m * ns * ns + (nd.nsupr + ns + n) * ns * ns;
         }
     }
+    return launches;
+}
+
+// The sweep on device LU d (H->dev, or H->bdev for every member of a batched handle: the same launches with gridDim.y =
+// members), then a wait for the missed-destination count.  The destination maps are value-independent and built on H->dev
+// for all members, as in slu_b200_batch_factor.  fn names the call in the messages.
+template <class LU>
+static int selinv_sweep(slu_b200_handle_t H, const LU &d, int members, const char *fn, double out[4])
+{
+    H->si_ready = false;
+    H->si_dev = false;
+    if (selinv_alloc(H, members, fn)) return -1;
+    cudaStream_t s = H->stream;
+    double flops = 0;
+    const double t0 = now_s();
+    const int launches = selinv_enqueue(H, d, &flops);
+    if (launches < 0) return -1;
     int bad = 0;
     CU(cudaMemcpyAsync(&bad, H->dev.err, sizeof(int), cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
@@ -3236,6 +3279,23 @@ static int capturing(slu_b200_handle_t H, cudaStream_t caller, const char *fn)
     return cs != cudaStreamCaptureStatusNone;
 }
 
+// The refill's slot map of the kept A (d_amap, d_arow), once per scaled fill: allocates and waits for it -> its launches
+static int build_amap(slu_b200_handle_t H, const char *fn)
+{
+    if (H->amap_ready) return 0;
+    const int64_t nnz = (int64_t)H->d_aci.n;
+    const cudaStream_t s = H->stream;
+    DevBuf<int8_t> act;                       // every panel of a 1 x 1 x 1 grid is held
+    if (grow(H, H->d_amap, nnz, true, false, fn) || grow(H, H->d_arow, nnz, true, false, fn) || act.alloc(H->nsupers)) return -1;
+    CU(cudaMemsetAsync(act.p, 1, act.bytes(), s));
+    const int launches = launch_refill_slots(H->dev, H->n, H->d_arp.p, H->d_aci.p, H->d_rmap.p, H->d_cperm.p, act.p, H->d_amap.p,
+                                             H->d_arow.p, s);
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    H->amap_ready = true;
+    return launches;
+}
+
 // New values of the last scaled fill's pattern, val on the device (batch x nnz on a batched handle): the arena zeroed, then
 // F = Pc Pr Dr A Dc Pc^T with the kept perm_r, perm, R and C, bit for bit the scaled fill's values; val also replaces the
 // kept A.  The first refill after a scaled fill builds the slot map (allocates, and waits for it once).
@@ -3252,16 +3312,8 @@ static int refill_impl(slu_b200_handle_t H, bool batched, const double *val, voi
                     "capture first", fn);
     const int n = H->n;
     const int64_t nnz = (int64_t)H->d_aci.n;
-    int launches = 0;
-    if (!H->amap_ready) {
-        DevBuf<int8_t> act;                       // every panel of a 1 x 1 x 1 grid is held
-        if (grow(H, H->d_amap, nnz, true, false, fn) || grow(H, H->d_arow, nnz, true, false, fn) || act.alloc(H->nsupers)) return -1;
-        CU(cudaMemsetAsync(act.p, 1, act.bytes(), s));
-        launches += launch_refill_slots(H->dev, n, H->d_arp.p, H->d_aci.p, H->d_rmap.p, H->d_cperm.p, act.p, H->d_amap.p, H->d_arow.p, s);
-        CU(cudaStreamSynchronize(s));
-        CU(cudaGetLastError());
-        H->amap_ready = true;
-    }
+    int launches = build_amap(H, fn);
+    if (launches < 0) return -1;
     H->captured = H->captured || cap;
     if (stream_enter(H, caller)) return -1;
     if (factors_replaced(H)) return -1;           // d_info's reset goes into the caller's stream order
@@ -3341,6 +3393,189 @@ static int solve_device_impl(slu_b200_handle_t H, bool batched, bool scaled, dou
     H->st.reserved[4] = 0;
     H->st.reserved[5] = (double)launches;
     return 0;
+}
+
+// ---- gradients on the caller's stream (selinv_device, logdet_device, logdet_grad_device, solve_grad_device and their twins).
+// The checks of solve_scaled_device; no host wait or PCIe copy, except in the allocating first calls (the second arena and the
+// plan of the first selected inversion, the refill's slot map, the staging buffer of a wider solve_grad), which are refused
+// under capture.  The result of a member whose status is not 0 (its factorization, or a selected inversion that missed a
+// destination) is NaN.
+
+// selinv's sweep ordered on the caller's stream.  The missed-destination count stays on the device: selinv_status_kernel
+// turns it into the status logdet_grad_device reads, and the next host-synchronous call reads it (settle) before it trusts
+// the inverse.
+static int selinv_device_impl(slu_b200_handle_t H, bool batched, void *stream, const char *fn)
+{
+    if (!H) return fail("%s: null argument", fn);
+    if (check(H, fn, scaled_need(batched) | SCALED | FACTORED | DEVICE_ORDERED)) return -1;
+    const cudaStream_t caller = (cudaStream_t)stream, s = H->stream;
+    const int cap = capturing(H, caller, fn);
+    if (cap < 0) return -1;
+    const int B = batched ? H->batch : 1;
+    if (!H->d_hinv.p || H->si_levels.empty() || !H->d_si_status.p) {
+        if (cap)
+            return fail("%s: the first selected inversion on a handle allocates the inverse's arena and plan: make this call once "
+                        "outside capture first", fn);
+        if (selinv_alloc(H, B, fn) || H->d_si_status.alloc((size_t)B) || H->d_si_rec.alloc(2)) return -1;
+    }
+    H->captured = H->captured || cap;
+    if (stream_enter(H, caller)) return -1;
+    H->si_ready = false;
+    double flops = 0;
+    int launches = batched ? selinv_enqueue(H, H->bdev, &flops) : selinv_enqueue(H, H->dev, &flops);
+    if (launches < 0) return -1;
+    launches += launch_selinv_status(H->dev.err, H->d_info.p, B, H->d_epoch.p, H->d_si_status.p, H->d_si_rec.p, s);
+    CU(cudaGetLastError());
+    if (stream_leave(H, caller)) return -1;
+    H->si_ready = true;
+    H->si_dev = true;
+    H->status_on_device = true;           // the next host-synchronous call settles the record before it reads the inverse
+    H->st.reserved[4] = 0;
+    H->st.reserved[5] = (double)launches;
+    return 0;
+}
+
+// logdet's reduction into the handle's buffers, then logabs[members] and sign[members * VAL_DOUBLES] on the device
+static int logdet_device_impl(slu_b200_handle_t H, bool batched, double *logabs, double *sign, void *stream, const char *fn)
+{
+    if (!H || !logabs || !sign) return fail("%s: null argument", fn);
+    if (check(H, fn, scaled_need(batched) | SCALED | FACTORED | DEVICE_ORDERED)) return -1;
+    if (check_device_ptr(H, logabs, fn, "logabs") || check_device_ptr(H, sign, fn, "sign")) return -1;
+    const cudaStream_t caller = (cudaStream_t)stream, s = H->stream;
+    const int cap = capturing(H, caller, fn);
+    if (cap < 0) return -1;
+    const int B = batched ? H->batch : 1;
+    const int count = (int)H->znodes[0].size();
+    const size_t nparts = (size_t)(count + SELINV_VECS - 1) / SELINV_VECS;
+    if (grow(H, H->d_lpart, nparts * B, false, cap, fn) || grow(H, H->d_lph, nparts * B, false, cap, fn) ||
+        grow(H, H->d_lres, (size_t)(1 + VAL_DOUBLES) * B, false, cap, fn))
+        return -1;
+    H->captured = H->captured || cap;
+    if (stream_enter(H, caller)) return -1;
+    const int32_t *nodes = H->d_pool_i32.p + H->z_nodes_off[0];
+    int launches = batched ? launch_selinv_logdet(H->bdev, nodes, count, H->d_lpart.p, H->d_lph.p, H->d_lres.p, s)
+                           : launch_selinv_logdet(H->dev, nodes, count, H->d_lpart.p, H->d_lph.p, H->d_lres.p, s);
+    launches += launch_logdet_out(H->d_lres.p, H->d_info.p, B, logabs, sign, s);
+    CU(cudaGetLastError());
+    if (stream_leave(H, caller)) return -1;
+    H->st.reserved[4] = 0;
+    H->st.reserved[5] = (double)launches;
+    return 0;
+}
+
+// grad[members x nnz] = coef[j] R_i C_j H(slot of entry (i, j)) (conj(H) in doublecomplex): the inverse of the last selinv or
+// selinv_device gathered through the refill's slot map onto the kept A's pattern, in the scaled fill's entry order
+static int logdet_grad_impl(slu_b200_handle_t H, bool batched, const double *coef, double *grad, void *stream, const char *fn)
+{
+    if (!H || !coef || !grad) return fail("%s: null argument", fn);
+    if (check(H, fn, scaled_need(batched) | SCALED | FACTORED | DEVICE_ORDERED)) return -1;
+    if (!H->si_ready)
+        return fail("%s needs %s or %s on the current factors first (a later fill, refill, upload or factorization invalidates "
+                    "the inverse)", fn, batched ? SLU_API "batch_selinv_device" : SLU_API "selinv_device",
+                    batched ? SLU_API "batch_selinv" : SLU_API "selinv");
+    if (check_device_ptr(H, coef, fn, "coef") || check_device_ptr(H, grad, fn, "grad")) return -1;
+    const cudaStream_t caller = (cudaStream_t)stream, s = H->stream;
+    const int cap = capturing(H, caller, fn);
+    if (cap < 0) return -1;
+    if (cap && !H->amap_ready)
+        return fail("%s: the first gradient or refill after a scaled fill builds the slot map and waits for it: make this call "
+                    "once outside capture first", fn);
+    int launches = build_amap(H, fn);
+    if (launches < 0) return -1;
+    H->captured = H->captured || cap;
+    if (stream_enter(H, caller)) return -1;
+    const LogdetGrad a{H->n, (int64_t)H->d_aci.n, H->d_amap.p, H->d_arow.p, H->d_aci.p, H->d_R.p, H->d_C.p, H->d_hinv.p,
+                       (const val_t *)coef, H->si_dev ? H->d_si_status.p : H->d_info.p, (val_t *)grad};
+    launches += batched ? launch_logdet_grad(H->bdev, a, s) : launch_logdet_grad(H->dev, a, s);
+    CU(cudaGetLastError());
+    if (stream_leave(H, caller)) return -1;
+    H->st.reserved[4] = 0;
+    H->st.reserved[5] = (double)launches;
+    return 0;
+}
+
+// grad[members x nnz] = -sum_k lam(i, k) conj(x(j, k)) on the kept A's pattern; lam and x: members blocks of n x nrhs
+// column-major, ldl / ldx apart per column, as the device solves take them.  nrhs > 1 goes through row-major copies in
+// d_gstage, so that each entry reads its nrhs values of lam and of x as two contiguous runs.
+static int solve_grad_impl(slu_b200_handle_t H, bool batched, const double *lam, int ldl, const double *x, int ldx, int nrhs,
+                           double *grad, void *stream, const char *fn)
+{
+    if (!H || !lam || !x || !grad) return fail("%s: null argument", fn);
+    if (check(H, fn, scaled_need(batched) | SCALED | FACTORED | DEVICE_ORDERED)) return -1;
+    const int B = batched ? H->batch : 1, n = H->n;
+    if (nrhs < 1 || ldl < n || ldx < n) return fail("%s: bad nrhs / ldl / ldx", fn);
+    if ((int64_t)n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
+    if (check_device_ptr(H, lam, fn, "lam") || check_device_ptr(H, x, fn, "x") || check_device_ptr(H, grad, fn, "grad")) return -1;
+    const cudaStream_t caller = (cudaStream_t)stream, s = H->stream;
+    const int cap = capturing(H, caller, fn);
+    if (cap < 0) return -1;
+    if (cap && !H->amap_ready)
+        return fail("%s: the first gradient or refill after a scaled fill builds the slot map and waits for it: make this call "
+                    "once outside capture first", fn);
+    const size_t len = (size_t)n * nrhs * B;
+    if (nrhs > 1 && grow(H, H->d_gstage, 2 * len, false, cap, fn)) return -1;
+    int launches = build_amap(H, fn);
+    if (launches < 0) return -1;
+    H->captured = H->captured || cap;
+    if (stream_enter(H, caller)) return -1;
+    SolveGrad a{(int64_t)H->d_aci.n, nrhs, 0, H->d_arow.p, H->d_aci.p, (const val_t *)lam, (const val_t *)x, ldl, ldx, 1,
+                H->d_info.p, (val_t *)grad};
+    if (nrhs > 1) {
+        launches += launch_grad_stage(H->d_gstage.p, a.lam, n, nrhs, ldl, B, s);
+        launches += launch_grad_stage(H->d_gstage.p + len, a.x, n, nrhs, ldx, B, s);
+        a.lam = H->d_gstage.p;
+        a.x = H->d_gstage.p + len;
+        a.lms = a.xms = (int64_t)n * nrhs;
+        a.rs = nrhs;
+    }
+    launches += launch_solve_grad(a, B, s);
+    CU(cudaGetLastError());
+    if (stream_leave(H, caller)) return -1;
+    H->st.reserved[4] = 0;
+    H->st.reserved[5] = (double)launches;
+    return 0;
+}
+
+int slu_b200_selinv_device(slu_b200_handle_t H, void *stream)
+{
+    return selinv_device_impl(H, false, stream, SLU_API "selinv_device");
+}
+
+int slu_b200_batch_selinv_device(slu_b200_handle_t H, void *stream)
+{
+    return selinv_device_impl(H, true, stream, SLU_API "batch_selinv_device");
+}
+
+int slu_b200_logdet_device(slu_b200_handle_t H, double *logabs, double *sign, void *stream)
+{
+    return logdet_device_impl(H, false, logabs, sign, stream, SLU_API "logdet_device");
+}
+
+int slu_b200_batch_logdet_device(slu_b200_handle_t H, double *logabs, double *sign, void *stream)
+{
+    return logdet_device_impl(H, true, logabs, sign, stream, SLU_API "batch_logdet_device");
+}
+
+int slu_b200_logdet_grad_device(slu_b200_handle_t H, const double *coef, double *grad, void *stream)
+{
+    return logdet_grad_impl(H, false, coef, grad, stream, SLU_API "logdet_grad_device");
+}
+
+int slu_b200_batch_logdet_grad_device(slu_b200_handle_t H, const double *coef, double *grad, void *stream)
+{
+    return logdet_grad_impl(H, true, coef, grad, stream, SLU_API "batch_logdet_grad_device");
+}
+
+int slu_b200_solve_grad_device(slu_b200_handle_t H, const double *lam, int ldl, const double *x, int ldx, int nrhs, double *grad,
+                               void *stream)
+{
+    return solve_grad_impl(H, false, lam, ldl, x, ldx, nrhs, grad, stream, SLU_API "solve_grad_device");
+}
+
+int slu_b200_batch_solve_grad_device(slu_b200_handle_t H, const double *lam, int ldl, const double *x, int ldx, int nrhs,
+                                     double *grad, void *stream)
+{
+    return solve_grad_impl(H, true, lam, ldl, x, ldx, nrhs, grad, stream, SLU_API "batch_solve_grad_device");
 }
 
 // ---- iterative refinement and condition estimation on the caller's stream (gsrfs_device, gscon_device and their twins).

@@ -379,6 +379,44 @@ int launch_selinv_trsm(const BatchedLU &d, const Batch &b, int64_t ctas, int col
 int launch_selinv_logdet(const BatchedLU &d, const int32_t *nodes, int count, double *part, phase_t *pph, double *out, cudaStream_t s);
 int launch_selinv_get(const BatchedLU &d, const val_t *hv, int n, const int32_t *rowptr, const int32_t *colind, const int32_t *perm,
                       val_t *out, int *err, cudaStream_t s);
+// slu_grad.cu (double) / slu_grad_z.cu (doublecomplex): the gradient kernels (slu_b200_solve_grad_device, _logdet_grad_device
+// and their twins), 1 launch each.  stage: dst[(m n + i) nrhs + k] = src[(m nrhs + k) ld + i] for members blocks of n x nrhs
+// column-major values.
+int launch_grad_stage(val_t *dst, const val_t *src, int n, int nrhs, int ld, int members, cudaStream_t s);
+// g[m nnz + e] = -sum_k lam_m(row[e], k) conj(x_m(colind[e], k)) on the kept A's pattern; element (i, k) of member m at
+// lam[m lms + i rs + k] (x: xms); NaN for every entry of a member whose status is not 0.  members = gridDim.y
+struct SolveGrad {
+    int64_t nnz;
+    int nrhs, pad;
+    const int32_t *row, *colind;
+    const val_t *lam, *x;
+    int64_t lms, xms, rs;
+    const int32_t *status;
+    val_t *grad;                       // members x nnz, member-major
+};
+int launch_solve_grad(const SolveGrad &a, int members, cudaStream_t s);
+// g[m nnz + e] = coef[m] ((R_i h) C_j), h = H[slot[e]] of member m (conj(H) in doublecomplex); NaN for every entry of a member
+// whose status is not 0 and for an entry without a slot
+struct LogdetGrad {
+    int n;
+    int64_t nnz;
+    const int64_t *slot;
+    const int32_t *row, *colind;
+    const double *R, *C;               // members x n
+    const val_t *hv;                   // member 0's H arena (the members' d.val_stride elements apart)
+    const val_t *coef;                 // [members]
+    const int32_t *status;
+    val_t *grad;                       // members x nnz, member-major
+};
+int launch_logdet_grad(const DeviceLU &d, const LogdetGrad &a, cudaStream_t s);
+int launch_logdet_grad(const BatchedLU &d, const LogdetGrad &a, cudaStream_t s);
+// after a device selected inversion: status[j] = -1 if *err (missed destinations) is not 0, else info[j]; rec[0] = *epoch,
+// rec[1] = *err
+int launch_selinv_status(const int *err, const int32_t *info, int members, const unsigned long long *epoch, int32_t *status,
+                         unsigned long long *rec, cudaStream_t s);
+// logabs[j] and sign[j VAL_DOUBLES ...] from launch_selinv_logdet's out (members x (1 + VAL_DOUBLES)), NaN where status[j] is
+// not 0
+int launch_logdet_out(const double *res, const int32_t *status, int members, double *logabs, double *sign, cudaStream_t s);
 // inertia (slu_b200_inertia, _batch_inertia) over the listed supernodes' pivots u_ii: per member cnt[3 j ...] = the pivots with
 // Re u_ii < 0, the others, those with |u_ii| <= thresh; def[j] = max |Im u_ii| / |u_ii| (0 in double).  pcnt / pdef: members x
 // ceil(count / SELINV_VECS) partials (3 counts each).  2 launches.
