@@ -533,7 +533,8 @@ int slu_b200_batch_solve_scaled_device(slu_b200_handle_t h, double *x, int ldx, 
  * outside capture first.  A graph holds the addresses of the handle's buffers: from the first captured call on, a call that
  * would reallocate one of them (a solve, gscon or gsrfs with more right-hand sides than any before, a scaled fill with
  * another nnz) is refused, naming the captured graph, until slu_b200_destroy; an upload or plain fill keeps the kept A's
- * buffers instead of freeing them.  A replay runs on the stream it is launched on, not on the handle's stream: a
+ * buffers instead of freeing them.  A buffer that no call has allocated yet is in no graph: a later call outside capture
+ * allocates it (gscon after a captured gsrfs_device without ferr, gsrfs after a captured gscon_device).  A replay runs on the stream it is launched on, not on the handle's stream: a
  * host-synchronous call after a replay needs the caller to have synchronised that stream first (the status it reads is
  * then the replay's, and a selinv inverse from before a replayed factorization is refused as after slu_b200_factor); a
  * call on the same stream is ordered after the replay without that.  Destroying the handle while

@@ -556,7 +556,8 @@ int pin_check(const slu_b200_handle_s *H, bool moves, const char *fn)
 }
 
 // Every growth of those buffers (exact: resized to len, else grown to at least len).  capturing: the call is being captured,
-// where an allocation is not allowed: it is refused before anything is enqueued.
+// where an allocation is not allowed: it is refused before anything is enqueued.  A buffer never allocated is held by no
+// graph: its first allocation is refused only under capture.
 template <class T>
 int grow(const slu_b200_handle_s *H, DevBuf<T> &b, size_t len, bool exact, bool capturing, const char *fn)
 {
@@ -564,7 +565,7 @@ int grow(const slu_b200_handle_s *H, DevBuf<T> &b, size_t len, bool exact, bool 
     if (capturing)
         return fail("%s would allocate device buffers while the stream is capturing a CUDA graph: make this call once outside "
                     "capture first", fn);
-    if (pin_check(H, true, fn)) return -1;
+    if (b.p && pin_check(H, true, fn)) return -1;
     return b.alloc(len);
 }
 
@@ -2224,28 +2225,82 @@ static int solve_dev(slu_b200_handle_t H, int nrhs, int trans, val_t **result)
     return launches;
 }
 
-// Every solve on host vectors: solve, solve_trans, schur_condense / expand and their batched twins (fn, with what they need
-// of the handle).  x: one n x nrhs block per member (ldx >= n), block j at x + j * ldx * nrhs: b on entry, the result on
-// return.  The complete unbatched solve is solve_dev (b in d_x2), everything else the passes in place in d_x.
+// x in A's ordering: b' = the row-permuted, scaled b into the solve's input (one scatter launch), the plain solve, x = the
+// scaled, permuted-back solution (one gather launch).  trans 0: b'[rmap[i]] = R[i] b[i], x[j] = C[j] y[perm[j]]; trans 1 / 2:
+// b'[perm[j]] = C[j] b[j], x[i] = R[i] y[rmap[i]] (the scalings are real, so F^H needs nothing more than F^T).
+// Where solve_scaled_dev takes b: d_x2 on a batched handle, d_x on an unbatched one (the scatter writes b' where the plain
+// solve takes its right-hand side)
+static val_t *scaled_in(slu_b200_handle_t H, bool batched) { return batched ? H->d_x2.p : H->d_x.p; }
+
+// The device part of solve_scaled: b in scaled_in(H), x in d_x2 (both buffers hold batch x n x nrhs).  Enqueued on H->stream,
+// not synchronised.  Returns the kernel launches, < 0 on an error.
+static int solve_scaled_dev(slu_b200_handle_t H, bool batched, int nrhs, int trans)
+{
+    const int B = batched ? H->batch : 1, n = H->n;
+    cudaStream_t s = H->stream;
+    val_t *in = scaled_in(H, batched), *b = batched ? H->d_x.p : H->d_x2.p;
+    int launches = launch_permute_scale(b, in, trans ? H->d_cperm.p : H->d_rmap.p, trans ? H->d_C.p : H->d_R.p, n, nrhs, B, true, s);
+    val_t *y = H->d_x.p;
+    if (batched) {
+        launches += solve_passes(H, H->bdev, nrhs, trans);
+    } else {
+        const int l = solve_dev(H, nrhs, trans, &y);
+        if (l < 0) return -1;
+        launches += l;
+    }
+    launches += launch_permute_scale(H->d_x2.p, y, trans ? H->d_rmap.p : H->d_cperm.p, trans ? H->d_R.p : H->d_C.p, n, nrhs, B, false, s);
+    return launches;
+}
+
+// The checks of every solve on x (ldx >= n, nrhs columns per member), after null pointers: what the call needs of the handle
+// (check), trans, nrhs / ldx and, where limit, n * nrhs below 2^31 per member
+static int solve_check(slu_b200_handle_t H, const char *fn, unsigned need, int trans, int nrhs, int ldx, bool limit)
+{
+    if (check(H, fn, need)) return -1;
+    if (trans < 0 || trans > 2) return fail("%s: trans = %d, must be 0 (A x = b), 1 (A^T x = b) or 2 (A^H x = b)", fn, trans);
+    if (nrhs < 1 || ldx < H->n) return fail("%s: bad nrhs / ldx", fn);
+    if (limit && (int64_t)H->n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
+    return 0;
+}
+
+// The buffers solve_enqueue uses for len elements in all
+static int solve_buffers(slu_b200_handle_t H, bool batched, bool scaled, size_t len, bool capturing, const char *fn)
+{
+    return grow(H, H->d_x, len, false, capturing, fn) || ((scaled || !batched) && grow(H, H->d_x2, len, false, capturing, fn)) ? -1 : 0;
+}
+
+// Every solve: b (one n x nrhs block per member at pitch ldb, in memory of `kind`'s source) copied where the device solve
+// takes it, then that solve on H->stream: scaled, solve_scaled_dev (b in scaled_in, x in d_x2); the complete unbatched solve,
+// solve_dev (b in d_x2, x where it says); else the passes in place in d_x.  Returns the kernel launches and points *x at the
+// solution, < 0 on an error.
+static int solve_enqueue(slu_b200_handle_t H, bool batched, bool scaled, int passes, const double *b, int ldb, int nrhs, int trans,
+                         cudaMemcpyKind kind, val_t **x)
+{
+    const bool full = !scaled && !batched && passes == PASS_BOTH;
+    const size_t w = (size_t)H->n * sizeof(val_t), cols = (size_t)nrhs * (batched ? H->batch : 1);
+    *x = scaled ? H->d_x2.p : H->d_x.p;
+    CU(cudaMemcpy2DAsync(scaled ? scaled_in(H, batched) : full ? H->d_x2.p : H->d_x.p, w, b, (size_t)ldb * sizeof(val_t), w, cols, kind,
+                         H->stream));
+    if (scaled) return solve_scaled_dev(H, batched, nrhs, trans);
+    if (full) return solve_dev(H, nrhs, trans, x);
+    return batched ? solve_passes(H, H->bdev, nrhs, trans, passes) : solve_passes(H, H->dev, nrhs, trans, passes);
+}
+
+// Every solve on host vectors: solve, solve_trans, solve_scaled (need has SCALED), schur_condense / expand and their batched
+// twins (fn, with what they need of the handle).  x: one n x nrhs block per member (ldx >= n), block j at x + j * ldx * nrhs:
+// b on entry, the result on return.
 static int solve_host(slu_b200_handle_t H, const char *fn, unsigned need, double *xh, int ldx, int nrhs, int trans, int passes)
 {
     if (!H || !xh) return fail("null argument");
-    if (check(H, fn, need)) return -1;
-    if (trans < 0 || trans > 2) return fail("%s: trans = %d, must be 0 (A x = b), 1 (A^T x = b) or 2 (A^H x = b)", fn, trans);
-    const bool batched = H->batch > 0, full = !batched && passes == PASS_BOTH;
+    const bool batched = H->batch > 0, scaled = (need & SCALED) != 0;
+    if (solve_check(H, fn, need, trans, nrhs, ldx, batched || scaled)) return -1;
     const int B = batched ? H->batch : 1, n = H->n;
-    if (nrhs < 1 || ldx < n) return fail("%s: bad nrhs / ldx", fn);
-    if (batched && (int64_t)n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
-    const size_t len = (size_t)n * nrhs * B;
-    if (grow(H, H->d_x, len, false, false, fn) || (!batched && grow(H, H->d_x2, len, false, false, fn))) return -1;
+    if (solve_buffers(H, batched, scaled, (size_t)n * nrhs * B, false, fn)) return -1;
     cudaStream_t s = H->stream;
     double t0 = now_s();
-    val_t *result = H->d_x.p;
+    val_t *result = nullptr;
     // the blocks are B * nrhs columns at pitch ldx: one 2D copy each way
-    CU(cudaMemcpy2DAsync(full ? H->d_x2.p : result, (size_t)n * sizeof(val_t), xh, (size_t)ldx * sizeof(val_t), (size_t)n * sizeof(val_t),
-                         (size_t)nrhs * B, cudaMemcpyHostToDevice, s));
-    const int launches = full ? solve_dev(H, nrhs, trans, &result)
-                              : batched ? solve_passes(H, H->bdev, nrhs, trans, passes) : solve_passes(H, H->dev, nrhs, trans, passes);
+    const int launches = solve_enqueue(H, batched, scaled, passes, xh, ldx, nrhs, trans, cudaMemcpyHostToDevice, &result);
     if (launches < 0) return -1;
     CU(cudaMemcpy2DAsync(xh, (size_t)ldx * sizeof(val_t), result, (size_t)n * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs * B,
                          cudaMemcpyDeviceToHost, s));
@@ -2689,18 +2744,22 @@ static int cond_buffers(slu_b200_handle_t H, int n, int members, bool capturing,
 }
 
 // The rounds of dlacn2 / zlacn2 over `members` vectors of n elements, shared by gscon and the forward error bound of gsrfs:
-// v holds the pending vectors; apply(kase, &x) enqueues the operator of kase on them and points x at the result.  Ends when
-// no member waits; the estimates are then in d_cstate.  *rounds counts the applications.
+// v holds the pending vectors; apply(kase, &x) enqueues the operator of kase on them, points x at the result and returns its
+// launches (< 0 on an error).  Ends when no member waits; the estimates are then in d_cstate.  *rounds counts the
+// applications.  Returns the launches of the applications, < 0 on an error.
 template <class Apply>
 static int cond_rounds(slu_b200_handle_t H, int n, int members, val_t *v, Apply apply, int *rounds, const char *fn)
 {
     if (cond_buffers(H, n, members, false, fn)) return -1;
     cudaStream_t s = H->stream;
     launch_cond_init(H->d_cstate.p, v, n, members, s);
+    int launches = 0;
     for (int kase = 1;;) {
         if (*rounds == COND_MAX_ROUNDS) return fail("%s: the estimator did not finish in %d solves", fn, *rounds);
         val_t *x = nullptr;
-        if (apply(kase, &x) < 0) return -1;
+        const int l = apply(kase, &x);
+        if (l < 0) return -1;
+        launches += l;
         CU(cudaMemsetAsync(H->d_ccount.p, 0, 2 * sizeof(int), s));
         launch_cond_step(H->d_cstate.p, kase, x, v, H->d_csgn.p, H->d_cpart.p, H->d_ccount.p, n, members, s);
         int waiting[2] = {0, 0};                      // members waiting for kase 1 / kase 2
@@ -2711,11 +2770,35 @@ static int cond_rounds(slu_b200_handle_t H, int n, int members, val_t *v, Apply 
         else if (waiting[kase - 1] == 0) break;
     }
     CU(cudaGetLastError());
-    return 0;
+    return launches;
+}
+
+// gscon's buffers: the solve's, the pending vectors (gscon_v), the estimator's, anorm and rcond of every member
+static int gscon_buffers(slu_b200_handle_t H, bool batched, bool capturing, const char *fn)
+{
+    const int B = batched ? H->batch : 1;
+    const size_t len = (size_t)H->n * B;
+    return grow(H, H->d_x, len, false, capturing, fn) || (batched ? grow_loop(H, H->d_cv, len, capturing, fn) : grow(H, H->d_x2, len, false, capturing, fn)) ||
+           cond_buffers(H, H->n, B, capturing, fn) || grow_loop(H, H->d_canorm, B, capturing, fn) || grow_loop(H, H->d_crcond, B, capturing, fn) ? -1 : 0;
+}
+
+// gscon's pending vectors
+static val_t *gscon_v(slu_b200_handle_t H, bool batched) { return batched ? H->d_cv.p : H->d_x2.p; }
+
+// gscon's operator for cond_rounds and cond_loop: the solve of kase (kase 1 with F for norm '1', with F^T / F^H for 'I'; kase
+// 2 the other) of every member's pending vector, the result in *x.  Returns the launches, < 0 on an error.
+static int gscon_apply(slu_b200_handle_t H, bool batched, bool one, int kase, val_t **x)
+{
+    const int trans = (kase == 1) == one ? 0 : (VAL_DOUBLES == 2 ? 2 : 1);
+    *x = H->d_x.p;
+    if (!batched) return solve_dev(H, 1, trans, x);
+    CU(cudaMemcpyAsync(*x, H->d_cv.p, (size_t)H->n * H->batch * sizeof(val_t), cudaMemcpyDeviceToDevice, H->stream));
+    return solve_passes(H, H->bdev, 1, trans);
 }
 extern "C" {
 
-// the preconditions of the matching solve are checked by the caller; B = 1 member on an unbatched handle
+// the preconditions of the matching solve are checked by the caller; B = 1 member on an unbatched handle.  rcond from
+// cond_rcond_kernel, as gscon_device's.
 static int gscon_impl(slu_b200_handle_t H, char norm, const double *anorm, double *rcond, const char *fn)
 {
     const bool batched = H->batch > 0;
@@ -2736,25 +2819,15 @@ static int gscon_impl(slu_b200_handle_t H, char norm, const double *anorm, doubl
         any = any || (anorm[j] > 0.0 && std::isfinite(anorm[j]));
     }
     if (any) {
-        const size_t len = (size_t)n * B;
-        if (batched && grow_loop(H, H->d_cv, len, false, fn)) return -1;
-        if (grow(H, H->d_x, len, false, false, fn) || (!batched && grow(H, H->d_x2, len, false, false, fn))) return -1;
+        if (gscon_buffers(H, batched, false, fn)) return -1;
         cudaStream_t s = H->stream;
-        val_t *v = batched ? H->d_cv.p : H->d_x2.p;       // the pending vectors
-        auto apply = [&](int kase, val_t **x) -> int {
-            const int trans = (kase == 1) == one ? 0 : (VAL_DOUBLES == 2 ? 2 : 1);
-            *x = H->d_x.p;
-            if (!batched) return solve_dev(H, 1, trans, x) < 0 ? -1 : 0;
-            CU(cudaMemcpyAsync(*x, v, len * sizeof(val_t), cudaMemcpyDeviceToDevice, s));
-            solve_passes(H, H->bdev, 1, trans);
-            return 0;
-        };
-        if (cond_rounds(H, n, B, v, apply, &rounds, fn)) return -1;
-        std::vector<CondState> st(B);
-        CU(cudaMemcpy(st.data(), H->d_cstate.p, B * sizeof(CondState), cudaMemcpyDeviceToHost));
-        for (int j = 0; j < B; ++j)
-            if (anorm[j] > 0.0 && std::isfinite(anorm[j]) && std::isfinite(st[j].est) && st[j].est != 0.0)
-                rcond[j] = (1.0 / st[j].est) / anorm[j];
+        CU(cudaMemcpyAsync(H->d_canorm.p, anorm, (size_t)B * sizeof(double), cudaMemcpyHostToDevice, s));
+        auto apply = [&](int kase, val_t **x) { return gscon_apply(H, batched, one, kase, x); };
+        if (cond_rounds(H, n, B, gscon_v(H, batched), apply, &rounds, fn) < 0) return -1;
+        launch_cond_rcond(H->d_cstate.p, H->d_canorm.p, H->d_info.p, B, H->d_crcond.p, s);
+        CU(cudaMemcpyAsync(rcond, H->d_crcond.p, (size_t)B * sizeof(double), cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+        CU(cudaGetLastError());
     }
     H->st.reserved[6] = now_s() - t0;
     H->st.reserved[7] = (double)rounds;
@@ -3043,58 +3116,6 @@ static int get_scaling_impl(slu_b200_handle_t H, bool batched, int member, int32
     return 0;
 }
 
-// x in A's ordering: b' = the row-permuted, scaled b into the solve's input (one scatter launch), the plain solve, x = the
-// scaled, permuted-back solution (one gather launch).  trans 0: b'[rmap[i]] = R[i] b[i], x[j] = C[j] y[perm[j]]; trans 1 / 2:
-// b'[perm[j]] = C[j] b[j], x[i] = R[i] y[rmap[i]] (the scalings are real, so F^H needs nothing more than F^T).
-// Where solve_scaled_dev takes b: d_x2 on a batched handle, d_x on an unbatched one (the scatter writes b' where the plain
-// solve takes its right-hand side)
-static val_t *scaled_in(slu_b200_handle_t H, bool batched) { return batched ? H->d_x2.p : H->d_x.p; }
-
-// The device part of solve_scaled: b in scaled_in(H), x in d_x2 (both buffers hold batch x n x nrhs).  Enqueued on H->stream,
-// not synchronised.  Returns the kernel launches, < 0 on an error.
-static int solve_scaled_dev(slu_b200_handle_t H, bool batched, int nrhs, int trans)
-{
-    const int B = batched ? H->batch : 1, n = H->n;
-    cudaStream_t s = H->stream;
-    val_t *in = scaled_in(H, batched), *b = batched ? H->d_x.p : H->d_x2.p;
-    int launches = launch_permute_scale(b, in, trans ? H->d_cperm.p : H->d_rmap.p, trans ? H->d_C.p : H->d_R.p, n, nrhs, B, true, s);
-    val_t *y = H->d_x.p;
-    if (batched) {
-        launches += solve_passes(H, H->bdev, nrhs, trans);
-    } else {
-        const int l = solve_dev(H, nrhs, trans, &y);
-        if (l < 0) return -1;
-        launches += l;
-    }
-    launches += launch_permute_scale(H->d_x2.p, y, trans ? H->d_rmap.p : H->d_cperm.p, trans ? H->d_R.p : H->d_C.p, n, nrhs, B, false, s);
-    return launches;
-}
-
-static int solve_scaled_impl(slu_b200_handle_t H, bool batched, double *xh, int ldx, int nrhs, int trans, const char *fn)
-{
-    if (!H || !xh) return fail("null argument");
-    if (check(H, fn, scaled_need(batched) | SCALED | FACTORED)) return -1;
-    if (trans < 0 || trans > 2) return fail("%s: trans = %d, must be 0 (A x = b), 1 (A^T x = b) or 2 (A^H x = b)", fn, trans);
-    const int B = batched ? H->batch : 1, n = H->n;
-    if (nrhs < 1 || ldx < n) return fail("%s: bad nrhs / ldx", fn);
-    if ((int64_t)n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
-    const size_t len = (size_t)n * nrhs * B;
-    if (grow(H, H->d_x, len, false, false, fn) || grow(H, H->d_x2, len, false, false, fn)) return -1;
-    cudaStream_t s = H->stream;
-    double t0 = now_s();
-    CU(cudaMemcpy2DAsync(scaled_in(H, batched), (size_t)n * sizeof(val_t), xh, (size_t)ldx * sizeof(val_t), (size_t)n * sizeof(val_t),
-                         (size_t)nrhs * B, cudaMemcpyHostToDevice, s));
-    const int launches = solve_scaled_dev(H, batched, nrhs, trans);
-    if (launches < 0) return -1;
-    CU(cudaMemcpy2DAsync(xh, (size_t)ldx * sizeof(val_t), H->d_x2.p, (size_t)n * sizeof(val_t), (size_t)n * sizeof(val_t), (size_t)nrhs * B,
-                         cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    CU(cudaGetLastError());
-    H->st.reserved[4] = now_s() - t0;
-    H->st.reserved[5] = (double)launches;
-    return 0;
-}
-
 int slu_b200_fill_csr_scaled(slu_b200_handle_t H, int n, const int32_t *rowptr, const int32_t *colind, const double *val,
                              const int32_t *perm_r, const int32_t *perm, const double *R, const double *C, int flags, double out[6])
 {
@@ -3108,7 +3129,7 @@ int slu_b200_get_scaling(slu_b200_handle_t H, int32_t *perm_r, double *R, double
 
 int slu_b200_solve_scaled(slu_b200_handle_t H, double *x, int ldx, int nrhs, int trans)
 {
-    return solve_scaled_impl(H, false, x, ldx, nrhs, trans, SLU_API "solve_scaled");
+    return solve_host(H, SLU_API "solve_scaled", scaled_need(false) | SCALED | FACTORED, x, ldx, nrhs, trans, PASS_BOTH);
 }
 
 int slu_b200_batch_fill_csr_scaled(slu_b200_handle_t H, int n, const int32_t *rowptr, const int32_t *colind, const double *val,
@@ -3126,7 +3147,7 @@ int slu_b200_batch_get_scaling(slu_b200_handle_t H, int member, double *R, doubl
 
 int slu_b200_batch_solve_scaled(slu_b200_handle_t H, double *x, int ldx, int nrhs, int trans)
 {
-    return solve_scaled_impl(H, true, x, ldx, nrhs, trans, SLU_API "batch_solve_scaled");
+    return solve_host(H, SLU_API "batch_solve_scaled", scaled_need(true) | SCALED | FACTORED, x, ldx, nrhs, trans, PASS_BOTH);
 }
 
 // ---- iterative refinement with error bounds: pdgsrfs (pdgsrfs.c:198-251) for op(A) = A in A's own ordering, on the factors
@@ -3134,92 +3155,131 @@ int slu_b200_batch_solve_scaled(slu_b200_handle_t H, double *x, int ldx, int nrh
 // residual kernel over every (row, column, member), the decide kernel and one read of the count of columns still active, then
 // one scaled solve of the whole block of residuals and the update.  ferr: dlacn2 through cond_rounds, each (member, column)
 // one estimator member: kase 1 solves with A^T (A^H) and multiplies by W, kase 2 multiplies by W and solves with A.
-// The refinement's buffers for cols columns of len elements in all (pinned after a captured call: grow)
+
+// The checks of gsrfs and gsrfs_device after null pointers: what they need of the handle, nrhs, ldb / ldx, n * nrhs
+static int gsrfs_check(slu_b200_handle_t H, const char *fn, unsigned need, int ldb, int ldx, int nrhs)
+{
+    if (check(H, fn, need)) return -1;
+    const int n = H->n;
+    if (nrhs < 1) return fail("%s: nrhs = %d, must be >= 1", fn, nrhs);
+    if (ldb < n || ldx < n) return fail("%s: ldb = %d and ldx = %d must be >= n = %d", fn, ldb, ldx, n);
+    if ((int64_t)n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
+    return 0;
+}
+
+// The refinement's buffers for cols columns of len elements in all, with ferr the estimator's (pinned after a capture: grow)
 static int refine_buffers(slu_b200_handle_t H, size_t len, int cols, bool ferr, bool capturing, const char *fn)
 {
     if (grow(H, H->d_x, len, false, capturing, fn) || grow(H, H->d_x2, len, false, capturing, fn) || grow_loop(H, H->d_rb, len, capturing, fn) ||
-        grow_loop(H, H->d_rx, len, capturing, fn) || grow_loop(H, H->d_rst, cols, capturing, fn) || grow_loop(H, H->d_ract, 1, capturing, fn))
+        grow_loop(H, H->d_rx, len, capturing, fn) || grow_loop(H, H->d_rst, cols, capturing, fn) || grow_loop(H, H->d_ract, 1, capturing, fn) ||
+        grow_loop(H, H->d_rout, 2 * (size_t)cols, capturing, fn) || grow_loop(H, H->d_rsteps, cols, capturing, fn))
         return -1;
-    if (ferr && (grow_loop(H, H->d_rw, len, capturing, fn) || grow_loop(H, H->d_cv, len, capturing, fn))) return -1;
-    return 0;
+    return ferr && (grow_loop(H, H->d_rw, len, capturing, fn) || grow_loop(H, H->d_cv, len, capturing, fn) ||
+                    cond_buffers(H, H->n, cols, capturing, fn) || grow_loop(H, H->d_rxmax, cols, capturing, fn)) ? -1 : 0;
+}
+
+// The pieces of the refinement of x in d_rx for b in d_rb, shared by gsrfs (the host reads d_ract between refine_check and
+// refine_step) and gsrfs_loop (a WHILE node).  Each enqueues on H->stream and returns its launches, < 0 on an error.
+static RefineArgs refine_args(slu_b200_handle_t H, bool batched, int nrhs, bool ferr)
+{
+    return RefineArgs{H->n, nrhs, batched ? H->batch : 1, (int64_t)H->d_aci.n, H->d_arp.p, H->d_aci.p, H->d_aval.p, H->d_rb.p, H->d_rst.p,
+                      ferr ? H->d_rw.p : nullptr};
+}
+
+// pdgsrfs's start state of every column (lstres = 3, count = 0); inactive where the member's status is not 0
+static int refine_init(slu_b200_handle_t H, const RefineArgs &a)
+{
+    return launch_refine_init(H->d_rst.p, H->d_info.p, a.nrhs, a.members, H->stream);
+}
+
+// the residual of every active column, then pdgsrfs's test: d_ract = the columns that take another step
+static int refine_check(slu_b200_handle_t H, const RefineArgs &a, bool batched)
+{
+    const int l = launch_refine_residual(a, H->d_rx.p, scaled_in(H, batched), H->stream);
+    CU(cudaMemsetAsync(H->d_ract.p, 0, sizeof(int), H->stream));
+    return l + launch_refine_decide(a, H->d_ract.p, H->stream);
+}
+
+// one step: dx = A^-1 r in d_x2, x += dx on the active columns
+static int refine_step(slu_b200_handle_t H, const RefineArgs &a, bool batched)
+{
+    const int l = solve_scaled_dev(H, batched, a.nrhs, 0);
+    return l < 0 ? -1 : l + launch_refine_update(a, H->d_rx.p, H->d_x2.p, H->stream);
+}
+
+// dgerfs's operator for ferr on the pending vectors v in d_cv, the result in d_x2 (*res): kase 1 diag(W) A^-T v (A^-H in
+// complex), kase 2 A^-1 diag(W) v
+static int refine_ferr_apply(slu_b200_handle_t H, bool batched, int nrhs, int kase, val_t **res)
+{
+    const int64_t len = (int64_t)H->n * nrhs * (batched ? H->batch : 1);
+    val_t *in = scaled_in(H, batched);
+    *res = H->d_x2.p;
+    if (kase == 2) {
+        const int l = launch_refine_scale(in, H->d_cv.p, H->d_rw.p, len, H->stream);
+        const int ls = solve_scaled_dev(H, batched, nrhs, 0);
+        return ls < 0 ? -1 : l + ls;
+    }
+    CU(cudaMemcpyAsync(in, H->d_cv.p, (size_t)len * sizeof(val_t), cudaMemcpyDeviceToDevice, H->stream));
+    const int l = solve_scaled_dev(H, batched, nrhs, VAL_DOUBLES == 2 ? 2 : 1);
+    return l < 0 ? -1 : l + launch_refine_scale(*res, *res, H->d_rw.p, len, H->stream);
+}
+
+// berr, steps and (ferr, the estimate in d_cstate) dgerfs's ferr = est / max_i |x_i| per column into d_rout (berr, ferr), d_rsteps
+static int refine_end(slu_b200_handle_t H, const RefineArgs &a, bool ferr)
+{
+    const int cols = a.nrhs * a.members;
+    int launches = 0;
+    if (ferr) {
+        CU(cudaMemsetAsync(H->d_rxmax.p, 0, (size_t)cols * sizeof(unsigned long long), H->stream));
+        launches += launch_refine_xmax(a, H->d_rx.p, H->d_rxmax.p, H->stream);
+    }
+    return launches + launch_refine_finish(a, H->d_cstate.p, H->d_rxmax.p, H->d_info.p, H->d_rout.p, ferr ? H->d_rout.p + cols : nullptr,
+                                           H->d_rsteps.p, H->stream);
 }
 
 static int gsrfs_impl(slu_b200_handle_t H, bool batched, const double *bh, int ldb, double *xh, int ldx, int nrhs, double *berr,
                       double *ferr, int32_t *steps, const char *fn)
 {
     if (!H || !bh || !xh || !berr) return fail("%s: null argument (b, x and berr are required)", fn);
-    if (check(H, fn, scaled_need(batched) | SCALED | FACTORED)) return -1;
-    const int B = batched ? H->batch : 1, n = H->n;
-    if (nrhs < 1) return fail("%s: nrhs = %d, must be >= 1", fn, nrhs);
-    if (ldb < n || ldx < n) return fail("%s: ldb = %d and ldx = %d must be >= n = %d", fn, ldb, ldx, n);
-    if ((int64_t)n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
-    const int cols = B * nrhs;
-    const size_t len = (size_t)n * cols;
-    if (refine_buffers(H, len, cols, ferr != nullptr, false, fn)) return -1;
+    if (gsrfs_check(H, fn, scaled_need(batched) | SCALED | FACTORED, ldb, ldx, nrhs)) return -1;
+    const int n = H->n, cols = (batched ? H->batch : 1) * nrhs;
+    if (refine_buffers(H, (size_t)n * cols, cols, ferr != nullptr, false, fn)) return -1;
     cudaStream_t s = H->stream;
     const double t0 = now_s();
     const size_t w = (size_t)n * sizeof(val_t);
     CU(cudaMemcpy2DAsync(H->d_rb.p, w, bh, (size_t)ldb * sizeof(val_t), w, (size_t)cols, cudaMemcpyHostToDevice, s));
     CU(cudaMemcpy2DAsync(H->d_rx.p, w, xh, (size_t)ldx * sizeof(val_t), w, (size_t)cols, cudaMemcpyHostToDevice, s));
-    std::vector<RefineState> st(cols, RefineState{3.0, 0.0, 0, 0, 1});   // pdgsrfs: lstres = 3, count = 0
-    CU(cudaMemcpyAsync(H->d_rst.p, st.data(), cols * sizeof(RefineState), cudaMemcpyHostToDevice, s));
-    const RefineArgs a{n, nrhs, B, (int64_t)H->d_aci.n, H->d_arp.p, H->d_aci.p, H->d_aval.p, H->d_rb.p, H->d_rst.p,
-                       ferr ? H->d_rw.p : nullptr};
-    val_t *in = scaled_in(H, batched), *x = H->d_rx.p;
-    int launches = 0;
+    const RefineArgs a = refine_args(H, batched, nrhs, ferr != nullptr);
+    int launches = refine_init(H, a);       // d_info is 0 for every member here (FACTORED)
     for (int step = 0;; ++step) {
         if (step > REFINE_ITMAX) return fail("%s: the refinement did not stop after %d steps", fn, REFINE_ITMAX);
-        launches += launch_refine_residual(a, x, in, s);
-        CU(cudaMemsetAsync(H->d_ract.p, 0, sizeof(int), s));
-        launches += launch_refine_decide(a, H->d_ract.p, s);
+        const int lc = refine_check(H, a, batched);
+        if (lc < 0) return -1;
+        launches += lc;
         int active = 0;
         CU(cudaMemcpyAsync(&active, H->d_ract.p, sizeof(int), cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
         if (active == 0) break;
-        const int l = solve_scaled_dev(H, batched, nrhs, 0);    // dx = A^-1 r in d_x2
-        if (l < 0) return -1;
-        launches += l + launch_refine_update(a, x, H->d_x2.p, s);
+        const int ls = refine_step(H, a, batched);
+        if (ls < 0) return -1;
+        launches += ls;
     }
     if (ferr) {
         int rounds = 0;
-        val_t *v = H->d_cv.p;
-        const double *W = H->d_rw.p;
-        auto apply = [&](int kase, val_t **res) -> int {
-            *res = H->d_x2.p;
-            int l;
-            if (kase == 2) {                                    // A^-1 diag(W) v
-                launches += launch_refine_scale(in, v, W, (int64_t)len, s);
-                l = solve_scaled_dev(H, batched, nrhs, 0);
-            } else {                                            // diag(W) A^-T v
-                CU(cudaMemcpyAsync(in, v, len * sizeof(val_t), cudaMemcpyDeviceToDevice, s));
-                l = solve_scaled_dev(H, batched, nrhs, VAL_DOUBLES == 2 ? 2 : 1);
-                launches += launch_refine_scale(*res, *res, W, (int64_t)len, s);
-            }
-            if (l < 0) return -1;
-            launches += l;
-            return 0;
-        };
-        if (cond_rounds(H, n, cols, v, apply, &rounds, fn)) return -1;
+        auto apply = [&](int kase, val_t **res) { return refine_ferr_apply(H, batched, nrhs, kase, res); };
+        const int l = cond_rounds(H, n, cols, H->d_cv.p, apply, &rounds, fn);
+        if (l < 0) return -1;
+        launches += l;
     }
-    CU(cudaMemcpy2DAsync(xh, (size_t)ldx * sizeof(val_t), x, w, w, (size_t)cols, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(st.data(), H->d_rst.p, cols * sizeof(RefineState), cudaMemcpyDeviceToHost, s));
-    std::vector<CondState> est(ferr ? cols : 0);
-    if (ferr) CU(cudaMemcpyAsync(est.data(), H->d_cstate.p, cols * sizeof(CondState), cudaMemcpyDeviceToHost, s));
+    const int le = refine_end(H, a, ferr != nullptr);
+    if (le < 0) return -1;
+    launches += le;
+    CU(cudaMemcpy2DAsync(xh, (size_t)ldx * sizeof(val_t), H->d_rx.p, w, w, (size_t)cols, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(berr, H->d_rout.p, (size_t)cols * sizeof(double), cudaMemcpyDeviceToHost, s));
+    if (ferr) CU(cudaMemcpyAsync(ferr, H->d_rout.p + cols, (size_t)cols * sizeof(double), cudaMemcpyDeviceToHost, s));
+    if (steps) CU(cudaMemcpyAsync(steps, H->d_rsteps.p, (size_t)cols * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     CU(cudaGetLastError());
-    for (int c = 0; c < cols; ++c) {
-        berr[c] = st[c].berr;
-        if (steps) steps[c] = st[c].count;
-        if (!ferr) continue;
-        double xmax = 0.0;                                      // dgerfs: divide by max |x_i| unless it is 0 (cabs1 in complex)
-        const double *xc = xh + (size_t)c * ldx * VAL_DOUBLES;
-        for (int i = 0; i < n; ++i) {
-            double ai = std::fabs(xc[(size_t)i * VAL_DOUBLES]);
-            if (VAL_DOUBLES == 2) ai += std::fabs(xc[(size_t)i * VAL_DOUBLES + 1]);
-            xmax = std::max(xmax, ai);
-        }
-        ferr[c] = xmax != 0.0 ? est[c].est / xmax : est[c].est;
-    }
     H->st.reserved[4] = now_s() - t0;
     H->st.reserved[5] = (double)launches;
     return 0;
@@ -3254,8 +3314,10 @@ static int check_device_ptr(slu_b200_handle_t H, const void *p, const char *fn, 
     return 0;
 }
 
-static int stream_enter(slu_b200_handle_t H, cudaStream_t caller)
+// cap: the call is being captured (capturing), which pins the handle's buffers from now on
+static int stream_enter(slu_b200_handle_t H, cudaStream_t caller, bool cap)
 {
+    H->captured = H->captured || cap;
     CU(cudaEventRecord(H->ev_in, caller));
     CU(cudaStreamWaitEvent(H->stream, H->ev_in, 0));
     return 0;
@@ -3263,6 +3325,7 @@ static int stream_enter(slu_b200_handle_t H, cudaStream_t caller)
 
 static int stream_leave(slu_b200_handle_t H, cudaStream_t caller)
 {
+    CU(cudaGetLastError());
     CU(cudaEventRecord(H->ev_out, H->stream));
     CU(cudaStreamWaitEvent(caller, H->ev_out, 0));
     return 0;
@@ -3270,7 +3333,7 @@ static int stream_leave(slu_b200_handle_t H, cudaStream_t caller)
 
 // Whether the caller's stream is capturing a CUDA graph: 1 yes, 0 no, < 0 an error.  Every call on the caller's stream asks
 // before it enqueues anything, refuses under capture what would allocate or wait on the host, and marks the handle as
-// captured (pin_check) once it is sure to enqueue.
+// captured (pin_check) in stream_enter, once it is sure to enqueue.
 static int capturing(slu_b200_handle_t H, cudaStream_t caller, const char *fn)
 {
     cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
@@ -3314,14 +3377,12 @@ static int refill_impl(slu_b200_handle_t H, bool batched, const double *val, voi
     const int64_t nnz = (int64_t)H->d_aci.n;
     int launches = build_amap(H, fn);
     if (launches < 0) return -1;
-    H->captured = H->captured || cap;
-    if (stream_enter(H, caller)) return -1;
+    if (stream_enter(H, caller, cap)) return -1;
     if (factors_replaced(H)) return -1;           // d_info's reset goes into the caller's stream order
     H->uploaded = false;
     CU(cudaMemsetAsync(H->val.p, 0, H->val.bytes(), s));
     const Refill r{n, nnz, (const val_t *)val, H->d_amap.p, H->d_arow.p, H->d_aci.p, H->d_R.p, H->d_C.p, H->d_aval.p};
     launches += batched ? launch_refill(H->bdev, r, s) : launch_refill(H->dev, r, s);
-    CU(cudaGetLastError());
     if (stream_leave(H, caller)) return -1;
     H->st.t_upload_s = 0;
     H->st.reserved[4] = 0;
@@ -3341,15 +3402,13 @@ static int factor_device_impl(slu_b200_handle_t H, bool batched, int32_t *info, 
     const cudaStream_t caller = (cudaStream_t)stream, s = H->stream;
     const int cap = capturing(H, caller, fn);
     if (cap < 0) return -1;
-    H->captured = H->captured || cap;
     const int B = batched ? H->batch : 1;
-    if (stream_enter(H, caller)) return -1;
+    if (stream_enter(H, caller, cap)) return -1;
     if (factors_replaced(H)) return -1;
     int64_t launches = launch_factor_begin(H->d_flags.p, B, H->d_tiny.p, s);
     const int64_t l = batched ? factor_levels(H, H->bdev, false, false, false) : factor_levels(H, H->dev, false, false, false);
     if (l < 0) return -1;
     launches += l + launch_factor_info(H->d_flags.p, B, info, H->d_info.p, H->d_epoch.p, s);
-    CU(cudaGetLastError());
     if (stream_leave(H, caller)) return -1;
     H->st.t_factor_s = 0;
     H->st.gpu_launches = launches;
@@ -3366,29 +3425,20 @@ static int solve_device_impl(slu_b200_handle_t H, bool batched, bool scaled, dou
                              const char *fn)
 {
     if (!H || !xd) return fail("%s: null argument", fn);
-    if (check(H, fn, scaled_need(batched) | (scaled ? SCALED : 0) | FACTORED | DEVICE_ORDERED)) return -1;
-    if (trans < 0 || trans > 2) return fail("%s: trans = %d, must be 0 (A x = b), 1 (A^T x = b) or 2 (A^H x = b)", fn, trans);
-    const int B = batched ? H->batch : 1, n = H->n;
-    if (nrhs < 1 || ldx < n) return fail("%s: bad nrhs / ldx", fn);
-    if ((int64_t)n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
+    if (solve_check(H, fn, scaled_need(batched) | (scaled ? SCALED : 0) | FACTORED | DEVICE_ORDERED, trans, nrhs, ldx, true)) return -1;
     if (check_device_ptr(H, xd, fn, "x")) return -1;
+    const int B = batched ? H->batch : 1, n = H->n;
     const cudaStream_t caller = (cudaStream_t)stream, s = H->stream;
     const int cap = capturing(H, caller, fn);
     if (cap < 0) return -1;
-    const size_t len = (size_t)n * nrhs * B;
-    if (grow(H, H->d_x, len, false, cap, fn) || ((scaled || !batched) && grow(H, H->d_x2, len, false, cap, fn))) return -1;
-    H->captured = H->captured || cap;
-    if (stream_enter(H, caller)) return -1;
-    // b goes where each solve takes it: scaled_in, d_x2 for solve_dev, d_x for the batched passes
-    val_t *in = scaled ? scaled_in(H, batched) : batched ? H->d_x.p : H->d_x2.p, *result = scaled ? H->d_x2.p : H->d_x.p;
-    const size_t w = (size_t)n * sizeof(val_t), pitch = (size_t)ldx * sizeof(val_t);
-    CU(cudaMemcpy2DAsync(in, w, xd, pitch, w, (size_t)nrhs * B, cudaMemcpyDeviceToDevice, s));
-    int launches = scaled ? solve_scaled_dev(H, batched, nrhs, trans)
-                          : batched ? solve_passes(H, H->bdev, nrhs, trans) : solve_dev(H, nrhs, trans, &result);
+    if (solve_buffers(H, batched, scaled, (size_t)n * nrhs * B, cap, fn)) return -1;
+    if (stream_enter(H, caller, cap)) return -1;
+    val_t *result = nullptr;
+    int launches = solve_enqueue(H, batched, scaled, PASS_BOTH, xd, ldx, nrhs, trans, cudaMemcpyDeviceToDevice, &result);
     if (launches < 0) return -1;
     launches += launch_solve_guard(result, H->d_info.p, (int64_t)n * nrhs, B, s);
-    CU(cudaMemcpy2DAsync(xd, pitch, result, w, w, (size_t)nrhs * B, cudaMemcpyDeviceToDevice, s));
-    CU(cudaGetLastError());
+    const size_t w = (size_t)n * sizeof(val_t);
+    CU(cudaMemcpy2DAsync(xd, (size_t)ldx * sizeof(val_t), result, w, w, (size_t)nrhs * B, cudaMemcpyDeviceToDevice, s));
     if (stream_leave(H, caller)) return -1;
     H->st.reserved[4] = 0;
     H->st.reserved[5] = (double)launches;
@@ -3418,14 +3468,12 @@ static int selinv_device_impl(slu_b200_handle_t H, bool batched, void *stream, c
                         "outside capture first", fn);
         if (selinv_alloc(H, B, fn) || H->d_si_status.alloc((size_t)B) || H->d_si_rec.alloc(2)) return -1;
     }
-    H->captured = H->captured || cap;
-    if (stream_enter(H, caller)) return -1;
+    if (stream_enter(H, caller, cap)) return -1;
     H->si_ready = false;
     double flops = 0;
     int launches = batched ? selinv_enqueue(H, H->bdev, &flops) : selinv_enqueue(H, H->dev, &flops);
     if (launches < 0) return -1;
     launches += launch_selinv_status(H->dev.err, H->d_info.p, B, H->d_epoch.p, H->d_si_status.p, H->d_si_rec.p, s);
-    CU(cudaGetLastError());
     if (stream_leave(H, caller)) return -1;
     H->si_ready = true;
     H->si_dev = true;
@@ -3450,13 +3498,11 @@ static int logdet_device_impl(slu_b200_handle_t H, bool batched, double *logabs,
     if (grow(H, H->d_lpart, nparts * B, false, cap, fn) || grow(H, H->d_lph, nparts * B, false, cap, fn) ||
         grow(H, H->d_lres, (size_t)(1 + VAL_DOUBLES) * B, false, cap, fn))
         return -1;
-    H->captured = H->captured || cap;
-    if (stream_enter(H, caller)) return -1;
+    if (stream_enter(H, caller, cap)) return -1;
     const int32_t *nodes = H->d_pool_i32.p + H->z_nodes_off[0];
     int launches = batched ? launch_selinv_logdet(H->bdev, nodes, count, H->d_lpart.p, H->d_lph.p, H->d_lres.p, s)
                            : launch_selinv_logdet(H->dev, nodes, count, H->d_lpart.p, H->d_lph.p, H->d_lres.p, s);
     launches += launch_logdet_out(H->d_lres.p, H->d_info.p, B, logabs, sign, s);
-    CU(cudaGetLastError());
     if (stream_leave(H, caller)) return -1;
     H->st.reserved[4] = 0;
     H->st.reserved[5] = (double)launches;
@@ -3482,12 +3528,10 @@ static int logdet_grad_impl(slu_b200_handle_t H, bool batched, const double *coe
                     "once outside capture first", fn);
     int launches = build_amap(H, fn);
     if (launches < 0) return -1;
-    H->captured = H->captured || cap;
-    if (stream_enter(H, caller)) return -1;
+    if (stream_enter(H, caller, cap)) return -1;
     const LogdetGrad a{H->n, (int64_t)H->d_aci.n, H->d_amap.p, H->d_arow.p, H->d_aci.p, H->d_R.p, H->d_C.p, H->d_hinv.p,
                        (const val_t *)coef, H->si_dev ? H->d_si_status.p : H->d_info.p, (val_t *)grad};
     launches += batched ? launch_logdet_grad(H->bdev, a, s) : launch_logdet_grad(H->dev, a, s);
-    CU(cudaGetLastError());
     if (stream_leave(H, caller)) return -1;
     H->st.reserved[4] = 0;
     H->st.reserved[5] = (double)launches;
@@ -3516,8 +3560,7 @@ static int solve_grad_impl(slu_b200_handle_t H, bool batched, const double *lam,
     if (nrhs > 1 && grow(H, H->d_gstage, 2 * len, false, cap, fn)) return -1;
     int launches = build_amap(H, fn);
     if (launches < 0) return -1;
-    H->captured = H->captured || cap;
-    if (stream_enter(H, caller)) return -1;
+    if (stream_enter(H, caller, cap)) return -1;
     SolveGrad a{(int64_t)H->d_aci.n, nrhs, 0, H->d_arow.p, H->d_aci.p, (const val_t *)lam, (const val_t *)x, ldl, ldx, 1,
                 H->d_info.p, (val_t *)grad};
     if (nrhs > 1) {
@@ -3529,7 +3572,6 @@ static int solve_grad_impl(slu_b200_handle_t H, bool batched, const double *lam,
         a.rs = nrhs;
     }
     launches += launch_solve_grad(a, B, s);
-    CU(cudaGetLastError());
     if (stream_leave(H, caller)) return -1;
     H->st.reserved[4] = 0;
     H->st.reserved[5] = (double)launches;
@@ -3719,75 +3761,43 @@ static int body_streams(slu_b200_handle_t H, bool cap, const char *fn)
     return 0;
 }
 
-// gsrfs's loop for x in d_rx and b in d_rb, results in d_rx, d_rout (berr, then ferr) and d_rsteps: pdgsrfs's steps in a WHILE
-// node, then (ferr) dgerfs's estimate in cond_loop, the finish kernels and the guard of x.  Enqueued on H->stream, capturing.
+// gsrfs's loop for x in d_rx and b in d_rb, results in d_rx, d_rout (berr, then ferr) and d_rsteps: gsrfs's pieces, the steps
+// in a WHILE node and (ferr) dgerfs's estimate in cond_loop, then the guard of x.  Enqueued on H->stream, capturing.
 static int gsrfs_loop(slu_b200_handle_t H, bool batched, int nrhs, bool ferr)
 {
-    const int B = batched ? H->batch : 1, n = H->n, cols = B * nrhs;
-    const size_t len = (size_t)n * cols;
-    const RefineArgs a{n, nrhs, B, (int64_t)H->d_aci.n, H->d_arp.p, H->d_aci.p, H->d_aval.p, H->d_rb.p, H->d_rst.p, ferr ? H->d_rw.p : nullptr};
-    val_t *x = H->d_rx.p;
-    int launches = launch_refine_init(H->d_rst.p, H->d_info.p, nrhs, B, H->stream);
-    launches += launch_refine_residual(a, x, scaled_in(H, batched), H->stream);
-    CU(cudaMemsetAsync(H->d_ract.p, 0, sizeof(int), H->stream));
-    launches += launch_refine_decide(a, H->d_ract.p, H->stream);
+    const RefineArgs a = refine_args(H, batched, nrhs, ferr);
+    int launches = refine_init(H, a);
+    const int lc = refine_check(H, a, batched);
+    if (lc < 0) return -1;
+    launches += lc;
     cudaGraphConditionalHandle w;
     if (cond_handle(H, &w)) return -1;
     launches += launch_refine_continue(H->d_ract.p, w, H->stream);
     if (add_conditional(H, cudaGraphCondTypeWhile, w, 0, [&]() -> int {
-            const int l = solve_scaled_dev(H, batched, nrhs, 0);    // dx = A^-1 r in d_x2
+            const int ls = refine_step(H, a, batched);
+            const int l = ls < 0 ? -1 : refine_check(H, a, batched);
             if (l < 0) return -1;
-            launches += l + launch_refine_update(a, x, H->d_x2.p, H->stream) + launch_refine_residual(a, x, scaled_in(H, batched), H->stream);
-            CU(cudaMemsetAsync(H->d_ract.p, 0, sizeof(int), H->stream));
-            launches += launch_refine_decide(a, H->d_ract.p, H->stream) + launch_refine_continue(H->d_ract.p, w, H->stream);
+            launches += ls + l + launch_refine_continue(H->d_ract.p, w, H->stream);
             return 0;
         }))
         return -1;
     if (ferr) {
-        const double *W = H->d_rw.p;
-        auto apply = [&](int kase, val_t **res) -> int {          // as gsrfs_impl's
-            val_t *in = scaled_in(H, batched);
-            *res = H->d_x2.p;
-            int l;
-            if (kase == 2) {                                    // A^-1 diag(W) v
-                l = launch_refine_scale(in, H->d_cv.p, W, (int64_t)len, H->stream);
-                const int ls = solve_scaled_dev(H, batched, nrhs, 0);
-                if (ls < 0) return -1;
-                l += ls;
-            } else {                                            // diag(W) A^-T v
-                CU(cudaMemcpyAsync(in, H->d_cv.p, len * sizeof(val_t), cudaMemcpyDeviceToDevice, H->stream));
-                l = solve_scaled_dev(H, batched, nrhs, VAL_DOUBLES == 2 ? 2 : 1);
-                if (l < 0) return -1;
-                l += launch_refine_scale(*res, *res, W, (int64_t)len, H->stream);
-            }
-            return l;
-        };
-        const int l = cond_loop(H, n, cols, H->d_cv.p, apply);
+        auto apply = [&](int kase, val_t **res) { return refine_ferr_apply(H, batched, nrhs, kase, res); };
+        const int l = cond_loop(H, H->n, a.nrhs * a.members, H->d_cv.p, apply);
         if (l < 0) return -1;
         launches += l;
-        CU(cudaMemsetAsync(H->d_rxmax.p, 0, (size_t)cols * sizeof(unsigned long long), H->stream));
-        launches += launch_refine_xmax(a, x, H->d_rxmax.p, H->stream);
     }
-    launches += launch_refine_finish(a, H->d_cstate.p, H->d_rxmax.p, H->d_info.p, H->d_rout.p, ferr ? H->d_rout.p + cols : nullptr,
-                                     H->d_rsteps.p, H->stream);
-    launches += launch_solve_guard(x, H->d_info.p, (int64_t)n * nrhs, B, H->stream);
-    return launches;
+    const int le = refine_end(H, a, ferr);
+    if (le < 0) return -1;
+    return launches + le + launch_solve_guard(H->d_rx.p, H->d_info.p, (int64_t)H->n * nrhs, a.members, H->stream);
 }
 
-// gscon's rounds for every member, anorm in d_canorm, rcond into d_crcond (the operator of gscon_impl).  Capturing, on H->stream.
+// gscon's rounds for every member, anorm in d_canorm, rcond into d_crcond.  Capturing, on H->stream.
 static int gscon_loop(slu_b200_handle_t H, bool batched, bool one)
 {
-    const int B = batched ? H->batch : 1, n = H->n;
-    const size_t len = (size_t)n * B;
-    val_t *v = batched ? H->d_cv.p : H->d_x2.p;
-    auto apply = [&](int kase, val_t **x) -> int {
-        const int trans = (kase == 1) == one ? 0 : (VAL_DOUBLES == 2 ? 2 : 1);
-        *x = H->d_x.p;
-        if (!batched) return solve_dev(H, 1, trans, x);
-        CU(cudaMemcpyAsync(*x, v, len * sizeof(val_t), cudaMemcpyDeviceToDevice, H->stream));
-        return solve_passes(H, H->bdev, 1, trans);
-    };
-    const int l = cond_loop(H, n, B, v, apply);
+    const int B = batched ? H->batch : 1;
+    auto apply = [&](int kase, val_t **x) { return gscon_apply(H, batched, one, kase, x); };
+    const int l = cond_loop(H, H->n, B, gscon_v(H, batched), apply);
     if (l < 0) return -1;
     return l + launch_cond_rcond(H->d_cstate.p, H->d_canorm.p, H->d_info.p, B, H->d_crcond.p, H->stream);
 }
@@ -3798,11 +3808,8 @@ static int gsrfs_device_impl(slu_b200_handle_t H, bool batched, const double *bd
                              double *ferr, int32_t *steps, void *stream, const char *fn)
 {
     if (!H || !bd || !xd || !berr) return fail("%s: null argument (b, x and berr are required)", fn);
-    if (check(H, fn, scaled_need(batched) | SCALED | FACTORED | DEVICE_ORDERED)) return -1;
+    if (gsrfs_check(H, fn, scaled_need(batched) | SCALED | FACTORED | DEVICE_ORDERED, ldb, ldx, nrhs)) return -1;
     const int B = batched ? H->batch : 1, n = H->n;
-    if (nrhs < 1) return fail("%s: nrhs = %d, must be >= 1", fn, nrhs);
-    if (ldb < n || ldx < n) return fail("%s: ldb = %d and ldx = %d must be >= n = %d", fn, ldb, ldx, n);
-    if ((int64_t)n * nrhs > INT_MAX) return fail("%s: n * nrhs must stay below 2^31 per member", fn);
     if (check_device_ptr(H, bd, fn, "b") || check_device_ptr(H, xd, fn, "x") || check_device_ptr(H, berr, fn, "berr") ||
         (ferr && check_device_ptr(H, ferr, fn, "ferr")) || (steps && check_device_ptr(H, steps, fn, "steps")))
         return -1;
@@ -3811,14 +3818,10 @@ static int gsrfs_device_impl(slu_b200_handle_t H, bool batched, const double *bd
     const int cap = capturing(H, caller, fn);
     if (cap < 0) return -1;
     const int cols = B * nrhs;
-    const size_t len = (size_t)n * cols;
-    if (refine_buffers(H, len, cols, ferr != nullptr, cap, fn) || (ferr && (cond_buffers(H, n, cols, cap, fn) || grow_loop(H, H->d_rxmax, cols, cap, fn))) ||
-        grow_loop(H, H->d_cloop, 2, cap, fn) || grow_loop(H, H->d_rout, 2 * (size_t)cols, cap, fn) || grow_loop(H, H->d_rsteps, cols, cap, fn) ||
-        body_streams(H, cap, fn))
+    if (refine_buffers(H, (size_t)n * cols, cols, ferr != nullptr, cap, fn) || grow_loop(H, H->d_cloop, 2, cap, fn) || body_streams(H, cap, fn))
         return -1;
-    H->captured = H->captured || cap;
     H->loop_captured = H->loop_captured || cap;
-    if (stream_enter(H, caller)) return -1;
+    if (stream_enter(H, caller, cap)) return -1;
     const size_t w = (size_t)n * sizeof(val_t);
     CU(cudaMemcpy2DAsync(H->d_rb.p, w, bd, (size_t)ldb * sizeof(val_t), w, (size_t)cols, cudaMemcpyDeviceToDevice, H->stream));
     CU(cudaMemcpy2DAsync(H->d_rx.p, w, xd, (size_t)ldx * sizeof(val_t), w, (size_t)cols, cudaMemcpyDeviceToDevice, H->stream));
@@ -3835,7 +3838,6 @@ static int gsrfs_device_impl(slu_b200_handle_t H, bool batched, const double *bd
     CU(cudaMemcpyAsync(berr, H->d_rout.p, (size_t)cols * sizeof(double), cudaMemcpyDeviceToDevice, s));
     if (ferr) CU(cudaMemcpyAsync(ferr, H->d_rout.p + cols, (size_t)cols * sizeof(double), cudaMemcpyDeviceToDevice, s));
     if (steps) CU(cudaMemcpyAsync(steps, H->d_rsteps.p, (size_t)cols * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
-    CU(cudaGetLastError());
     if (stream_leave(H, caller)) return -1;
     H->st.reserved[4] = 0;
     H->st.reserved[5] = (double)launches;
@@ -3855,15 +3857,10 @@ static int gscon_device_impl(slu_b200_handle_t H, bool batched, char norm, const
     const cudaStream_t caller = (cudaStream_t)stream;
     const int cap = capturing(H, caller, fn);
     if (cap < 0) return -1;
-    const int B = batched ? H->batch : 1, n = H->n;
-    const size_t len = (size_t)n * B;
-    if (grow(H, H->d_x, len, false, cap, fn) || (batched ? grow_loop(H, H->d_cv, len, cap, fn) : grow(H, H->d_x2, len, false, cap, fn)) || cond_buffers(H, n, B, cap, fn) ||
-        grow_loop(H, H->d_cloop, 2, cap, fn) || grow_loop(H, H->d_canorm, B, cap, fn) || grow_loop(H, H->d_crcond, B, cap, fn) ||
-        body_streams(H, cap, fn))
-        return -1;
-    H->captured = H->captured || cap;
+    const int B = batched ? H->batch : 1;
+    if (gscon_buffers(H, batched, cap, fn) || grow_loop(H, H->d_cloop, 2, cap, fn) || body_streams(H, cap, fn)) return -1;
     H->loop_captured = H->loop_captured || cap;
-    if (stream_enter(H, caller)) return -1;
+    if (stream_enter(H, caller, cap)) return -1;
     CU(cudaMemcpyAsync(H->d_canorm.p, anorm, (size_t)B * sizeof(double), cudaMemcpyDeviceToDevice, H->stream));
     const std::vector<uintptr_t> bufs = {
         (uintptr_t)H->d_x.p, (uintptr_t)H->d_x2.p, (uintptr_t)H->d_cv.p, (uintptr_t)H->d_csgn.p, (uintptr_t)H->d_cstate.p,
@@ -3872,7 +3869,6 @@ static int gscon_device_impl(slu_b200_handle_t H, bool batched, char norm, const
     const int launches = run_loop(H, cap, {1, batched, 1, one}, bufs, [&] { return gscon_loop(H, batched, one); });
     if (launches < 0) return -1;
     CU(cudaMemcpyAsync(rcond, H->d_crcond.p, (size_t)B * sizeof(double), cudaMemcpyDeviceToDevice, H->stream));
-    CU(cudaGetLastError());
     if (stream_leave(H, caller)) return -1;
     H->st.reserved[4] = 0;
     H->st.reserved[5] = (double)launches;
